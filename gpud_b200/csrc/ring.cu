@@ -52,7 +52,13 @@ struct WinParams {
   double inv_w;        // 1.0 / W
   int n_list;          // > 0: process only windows w_list[0..n_list) of every field (generic instantiation)
   int w_list[2];
-  int w_skip[2];       // windows the specialised launch leaves to the generic one (-1 = none)
+  int w_skip[2];       // windows the aligned loop leaves to the generic code (-1 = none)
+  int n_tail;          // > 0: the launch reduces the w_skip[0..n_tail) windows of every field itself, after its aligned units
+  // work cursor (zeroed before every launch): cursor[0] hands out the launch's units, cursor[1] its tail units.  Claim k is the
+  // run of run_len consecutive units starting at k * run_len while k < n_runs, after that the single unit n_runs * run_len + (k - n_runs)
+  unsigned long long* cursor;
+  int run_len;
+  int64_t n_runs;
   // RANGE instantiations only (whole-range order statistic, select.cu): the pass classifies every sample against the field's
   // pivot pair lo <= hi and parks the keys strictly between them in the field's list
   const double* piv;           // [F][2]: lo, hi
@@ -319,13 +325,26 @@ constexpr int kPrefetchPairs = GPUD_PREFETCH_PAIRS;      // register pairs of th
 // cap, spills) 1.85.  The rest of the window is loaded by fetch_rest() at the top of the trip that consumes it.
 constexpr int kHotCtasPerSM = 2;
 
+#ifdef GPUD_EXPERIMENT_FINISH
+// EXPERIMENT (`-DGPUD_EXPERIMENT_FINISH`, tools/exp_warp_finish.py): every warp of the hot instantiation records its %globaltimer at
+// entry and at exit and the number of windows it reduced, so the spread of warp finish times within one launch can be read back.
+constexpr int kExpMaxWarps = 4096;
+__device__ unsigned long long g_exp_finish[kExpMaxWarps][3];   // {start ns, end ns, windows}
+__device__ __forceinline__ unsigned long long global_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+  return t;
+}
+#endif
+
+// The warp loop of k_window_reduce: reduces the units it claims from the work cursor until the cursor runs out and returns how
+// many it reduced.  TAIL: the units are the w_skip[0..n_tail) windows of every field (claimed from cursor[1]).
 // TMA: the window lands in a per-warp stage buffer through one cp.async.bulk (UBLKCP) instead of 16 LDG.128 per lane into registers;
 // pass 1 reads it with conflict-free LDS.128 and the copy of the next window is issued as soon as pass 1 is done with the buffer.
 // Only for the hot shape (ALIGNED, JF >= 0); 13 warps per SM in one CTA (the stage buffers take the room of the second CTA's rows).
-template <bool ALIGNED, int JF, bool RANGE, bool TMA = false>
-__global__ void __launch_bounds__((TMA ? kTmaWarps : kWarpsPerBlock) * 32, TMA ? 1 : ((ALIGNED && JF >= 0) ? kHotCtasPerSM : 2)) k_window_reduce(const WinParams p) {
+template <bool ALIGNED, int JF, bool RANGE, bool TMA, bool TAIL>
+__device__ __forceinline__ int window_loop(const WinParams& p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  constexpr int WPB = TMA ? kTmaWarps : kWarpsPerBlock;
   constexpr int kPerWarp = kWarpSmemBytes + (TMA ? kStageBytesTma : 0);
   __shared__ __align__(8) unsigned long long s_bars[TMA ? kTmaWarps : 1];
   const int lane = threadIdx.x & 31;
@@ -345,30 +364,65 @@ __global__ void __launch_bounds__((TMA ? kTmaWarps : kWarpsPerBlock) * 32, TMA ?
   unsigned* s32 = reinterpret_cast<unsigned*>(cand);                                            // 128 B scratch, reused before the gather
   reinterpret_cast<unsigned long long*>(wbase + kPadRowOff)[lane] = kPadStored;                 // the pad row, written once
   uint4* my_row4 = reinterpret_cast<uint4*>(sk + lane * kRowU64);   // one uint4 = two keys {lo0, hi0, lo1, hi1}
-  const int64_t n_units = p.n_list > 0 ? (int64_t)p.F * p.n_list : (int64_t)p.F * p.nw;
   const unsigned lt_mask = (1u << lane) - 1u;
 
-  // (field, slot) advance incrementally: one division per kernel instead of one per window
-  const int per_f = p.n_list > 0 ? p.n_list : p.nw;
-  const int64_t stride = (int64_t)gridDim.x * WPB;
-  const int df = (int)(stride / per_f), ds = (int)(stride - (int64_t)df * per_f);
-  int64_t u = (int64_t)blockIdx.x * WPB + warp;
-  int uf = (int)(u / per_f), uslot = (int)(u - (int64_t)uf * per_f);
+  // Units are handed out by the work cursor in address order (unit = field * per_f + slot), so the windows in flight stay one
+  // front that sweeps the ring, and a warp that is done early takes more instead of idling while the slowest one finishes.
+  // A run is walked in order: the 256-byte block two neighbouring windows share is read again by the same warp a moment later,
+  // while it is still in L2.  The runs end before the last units, which go out one at a time so that all warps finish together.
+  const int per_f = TAIL ? p.n_tail : (p.n_list > 0 ? p.n_list : p.nw);
+  const int64_t n_units = (int64_t)p.F * per_f;
+  const int run_len = TAIL ? 1 : p.run_len;
+  const int64_t n_runs = TAIL ? 0 : p.n_runs;
+  unsigned long long* const cursor = p.cursor + (TAIL ? 1 : 0);
+  int64_t u = 0, u_end = 0;          // the rest of the warp's run; (field, slot) of u advance incrementally
+  int uf = 0, uslot = 0;
+  // lane 0: the next claim, asked for at the top of the trip that reduces the last unit of the run, so the atomic's round trip
+  // runs under that trip's pass 1.  (Asking a whole run ahead was no faster and leaves a claimed run idle behind a busy warp.)
+  unsigned long long claim = 0;
+  bool asked = false;
+  auto ask = [&]() {
+    if (lane == 0) claim = atomicAdd(cursor, 1ull);
+    asked = true;
+  };
+  auto take_run = [&]() -> bool {
+    if (!asked) ask();
+    asked = false;
+    const int64_t k = (int64_t)__shfl_sync(kFull, claim, 0);
+    u = k < n_runs ? k * run_len : n_runs * run_len + (k - n_runs);
+    u_end = min(u + (k < n_runs ? run_len : 1), n_units);
+    if (u >= n_units) return false;
+    uf = (int)(u / per_f);
+    uslot = (int)(u - (int64_t)uf * per_f);
+    return true;
+  };
+  int n_done = 0;
 
   constexpr int PF = (ALIGNED && JF >= 0) ? kPrefetchPairs : 16;
   double2 v[16];                 // the window in flight: loaded for the NEXT unit while the current one is post-processed
   double thr_next = 0.0, lo_next = 0.0, hi_next = 0.0;
+  auto load_unaligned = [&](const WinUnit& q) {
+    const double* __restrict__ base = p.ring + (int64_t)q.f * p.cap;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int t0 = 64 * j + 2 * lane;
+      v[j] = make_double2(0.0, 0.0);
+      if (t0 < q.m) { int64_t a = q.p0 + t0; if (a >= p.cap) a -= p.cap; v[j].x = __ldcs(base + a); }
+      if (t0 + 1 < q.m) { int64_t a = q.p0 + t0 + 1; if (a >= p.cap) a -= p.cap; v[j].y = __ldcs(base + a); }
+    }
+  };
   // fetch the next non-skipped unit of this warp (if any) and issue its first kPrefetchPairs loads.  Alternatives that were
   // slower: choosing the next unit BEFORE pass 1 (its address/threshold registers live through pass 1) and issuing each
-  // pair's load inside pass 1 right after the pair is consumed.
+  // pair's load inside pass 1 right after the pair is consumed.  TAIL loads nothing ahead: a warp reduces at most a few tail
+  // units, and without a window in flight during the post-processing the tail loop fits the hot kernel's 128 registers.
   auto fetch = [&](WinUnit& q) -> bool {
     for (;;) {
-      if (u >= n_units) return false;
+      if (u >= u_end && !take_run()) return false;
       q.f = uf;
-      q.w = p.n_list > 0 ? p.w_list[uslot] : uslot;
-      u += stride; uf += df; uslot += ds;
-      if (uslot >= per_f) { uslot -= per_f; ++uf; }
-      if (p.n_list > 0 || (q.w != p.w_skip[0] && q.w != p.w_skip[1])) break;
+      q.w = TAIL ? p.w_skip[uslot] : (p.n_list > 0 ? p.w_list[uslot] : uslot);
+      ++u;
+      if (++uslot == per_f) { uslot = 0; ++uf; }
+      if (TAIL || p.n_list > 0 || (q.w != p.w_skip[0] && q.w != p.w_skip[1])) break;
     }
     const int64_t c0 = (int64_t)q.w * p.W;
     q.m = JF >= 0 ? p.W : (int)min((int64_t)p.W, p.count - c0);
@@ -391,19 +445,14 @@ __global__ void __launch_bounds__((TMA ? kTmaWarps : kWarpsPerBlock) * 32, TMA ?
         v[j] = make_double2(0.0, 0.0);
         if (64 * j + 2 * lane < q.m) v[j] = ld_stream(b2 + 32 * j);   // element t0+1 == m is masked in pass 1 (the ring has slack)
       }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int t0 = 64 * j + 2 * lane;
-        v[j] = make_double2(0.0, 0.0);
-        if (t0 < q.m) { int64_t a = q.p0 + t0; if (a >= p.cap) a -= p.cap; v[j].x = __ldcs(base + a); }
-        if (t0 + 1 < q.m) { int64_t a = q.p0 + t0 + 1; if (a >= p.cap) a -= p.cap; v[j].y = __ldcs(base + a); }
-      }
+    } else if (!TAIL) {
+      load_unaligned(q);
     }
     return true;
   };
 
   auto fetch_rest = [&](const WinUnit& q) {
+    if (TAIL) load_unaligned(q);
     if (PF >= 16 || TMA) return;
     const double2* __restrict__ b2 = reinterpret_cast<const double2*>(p.ring + (int64_t)q.f * p.cap + q.p0) + lane;
 #pragma unroll
@@ -418,6 +467,8 @@ __global__ void __launch_bounds__((TMA ? kTmaWarps : kWarpsPerBlock) * 32, TMA ?
   WinUnit cur, nxt;
   bool have = fetch(cur);
   while (have) {
+    ++n_done;
+    if (u >= u_end && !asked) ask();                 // the run ends with this unit
     fetch_rest(cur);
     if (TMA) { mbar_wait(bar_a, tma_parity); tma_parity ^= 1; }      // the window has landed in the stage buffer
     const int f = cur.f, w = cur.w, m = cur.m;
@@ -739,6 +790,29 @@ __global__ void __launch_bounds__((TMA ? kTmaWarps : kWarpsPerBlock) * 32, TMA ?
     }
     cur = nxt;
   }
+  return n_done;
+}
+
+// The trailing partial window and the window that wraps the physical end of the ring (w_skip) need the generic code; an aligned
+// launch reduces them itself once its cursor has run out (n_tail > 0), through the same loop instantiated for them.
+template <bool ALIGNED, int JF, bool RANGE, bool TMA = false>
+__global__ void __launch_bounds__((TMA ? kTmaWarps : kWarpsPerBlock) * 32, TMA ? 1 : ((ALIGNED && JF >= 0) ? kHotCtasPerSM : 2)) k_window_reduce(const WinParams p) {
+#ifdef GPUD_EXPERIMENT_FINISH
+  const unsigned long long exp_t0 = global_ns();
+#endif
+  int n_done = window_loop<ALIGNED, JF, RANGE, TMA, false>(p);
+  if constexpr (ALIGNED && !TMA) {
+    if (p.n_tail > 0) n_done += window_loop<false, -1, RANGE, false, true>(p);
+  }
+#ifdef GPUD_EXPERIMENT_FINISH
+  const int exp_warp = blockIdx.x * (TMA ? kTmaWarps : kWarpsPerBlock) + (threadIdx.x >> 5);
+  if (ALIGNED && JF >= 0 && !RANGE && !TMA && (threadIdx.x & 31) == 0 && exp_warp < kExpMaxWarps) {
+    g_exp_finish[exp_warp][0] = exp_t0;
+    g_exp_finish[exp_warp][1] = global_ns();
+    g_exp_finish[exp_warp][2] = (unsigned long long)n_done;
+  }
+#endif
+  (void)n_done;
 }
 
 #ifdef GPUD_EXPERIMENT_TMA
@@ -1022,6 +1096,7 @@ struct gpud_ring {
   double* d_res[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
   uint32_t* d_nover = nullptr;
   double* d_part = nullptr;
+  unsigned long long* d_cursor = nullptr;   // window-kernel work cursors: [0..1] gpud_ring_reduce, [2..3] the range pass
   int64_t reduced_nw = -1;
   cudaStream_t own_stream = nullptr, stream = nullptr;
   double* h_stage[2] = {nullptr, nullptr};
@@ -1089,6 +1164,7 @@ extern "C" int32_t gpud_ring_create(gpud_ctx* ctx, int32_t dev, const gpud_ring_
   for (int i = 0; i < 5 && e == cudaSuccess; ++i) e = cudaMalloc(&r->d_res[i], res_bytes);
   if (e == cudaSuccess) e = cudaMalloc(&r->d_nover, (size_t)r->F * r->nw_max * sizeof(uint32_t));
   if (e == cudaSuccess) e = cudaMalloc(&r->d_part, res_bytes);
+  if (e == cudaSuccess) e = cudaMalloc(&r->d_cursor, 4 * sizeof(unsigned long long));
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&r->own_stream, cudaStreamNonBlocking);
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&r->copy_stream, cudaStreamNonBlocking);
   r->stage_rows = std::max<int64_t>(1, (int64_t)(kStageBytes / (sizeof(double) * r->F)));
@@ -1126,6 +1202,7 @@ extern "C" int32_t gpud_ring_destroy(gpud_ring* r) {
   cudaSetDevice(r->dev);
   if (r->own_stream) cudaStreamSynchronize(r->own_stream);
   cudaFree(r->d_ring); cudaFree(r->d_sample); cudaFree(r->d_pwl); cudaFree(r->d_thr); cudaFree(r->d_pw); cudaFree(r->d_nover); cudaFree(r->d_part);
+  cudaFree(r->d_cursor);
   for (auto& p : r->d_res) cudaFree(p);
   for (auto& p : r->d_rng) cudaFree(p);
   cudaFree(r->d_rng_nover);
@@ -1262,14 +1339,28 @@ extern "C" int32_t gpud_ring_counts(gpud_ring* r, int64_t* total, int64_t* count
 
 // Launch the window kernel(s).  The bulk goes to the aligned 128-bit instantiation (specialised for the window shape when
 // W >> 6 is 15 or 16, i.e. W in 960..1024); the window that wraps the physical end of the ring and a trailing partial
-// window go to the generic run-time instantiation, which also serves rings whose start is odd.
+// window go through the generic run-time code at the end of the same launch.  The generic instantiation on its own serves
+// rings whose start is odd.
+#ifndef GPUD_RUN_WINDOWS
+#define GPUD_RUN_WINDOWS 8
+#endif
+constexpr int kRunWindows = GPUD_RUN_WINDOWS;   // windows per claim of the work cursor while the ring is far from done
+
+// Claims of kRunWindows units, then single units for the last warps x kRunWindows / 2: when the runs are gone the warps are on
+// average half a run from the end of theirs, and the single units fill that in.
+static void set_schedule(WinParams& p, int64_t units, int64_t warps) {
+  p.run_len = kRunWindows;
+  p.n_runs = kRunWindows > 1 ? std::max<int64_t>(0, (units - warps * kRunWindows / 2) / kRunWindows) : 0;
+}
+
 #ifdef GPUD_EXPERIMENT_TMA
 template <int JF, bool RANGE>
-static cudaError_t launch_one_tma(gpud_ring* r, const WinParams& p, int64_t units) {
+static cudaError_t launch_one_tma(gpud_ring* r, WinParams p, int64_t units) {
   constexpr int kSmem = kTmaWarps * (kWarpSmemBytes + kStageBytesTma);
   cudaError_t e = cudaFuncSetAttribute(k_window_reduce<true, JF, RANGE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
   if (e != cudaSuccess) return e;
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((units + kTmaWarps - 1) / kTmaWarps, (int64_t)r->sm_count - (r->cta_reserve ? 1 : 0)));
+  set_schedule(p, units, (int64_t)grid * kTmaWarps);
   k_window_reduce<true, JF, RANGE, true><<<grid, kTmaWarps * 32, kSmem, r->stream>>>(p);
   return cudaGetLastError();
 }
@@ -1286,12 +1377,13 @@ static cudaError_t launch_inplace(gpud_ring* r, const WinParams& p, int64_t unit
 #endif  // GPUD_EXPERIMENT_TMA
 
 template <bool ALIGNED, int JF, bool RANGE>
-static cudaError_t launch_one(gpud_ring* r, const WinParams& p, int64_t units) {
+static cudaError_t launch_one(gpud_ring* r, WinParams p, int64_t units) {
   // persistent grid: 2 CTAs of 8 warps per SM, a whole number of waves
   // 72 KB of dynamic shared memory per CTA (8 warps x (32 x 272 B key rows + candidate list)): opt in above 48 KB
   cudaError_t e = cudaFuncSetAttribute(k_window_reduce<ALIGNED, JF, RANGE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBlockSmemBytes);
   if (e != cudaSuccess) return e;
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((units + kWarpsPerBlock - 1) / kWarpsPerBlock, (int64_t)r->sm_count * ((ALIGNED && JF >= 0) ? kHotCtasPerSM : 2) - r->cta_reserve));
+  set_schedule(p, units, (int64_t)grid * kWarpsPerBlock);
   k_window_reduce<ALIGNED, JF, RANGE><<<grid, kWarpsPerBlock * 32, kBlockSmemBytes, r->stream>>>(p);
   return cudaGetLastError();
 }
@@ -1307,6 +1399,8 @@ static int32_t launch_windows(gpud_ring* r, WinParams p) {
   p.n_list = 0;
   p.w_list[0] = p.w_list[1] = -1;
   p.w_skip[0] = p.w_skip[1] = -1;
+  p.n_tail = 0;
+  GPUD_CUDA(r->ctx, cudaMemsetAsync(p.cursor, 0, 2 * sizeof(unsigned long long), r->stream));
   const int64_t units = (int64_t)p.F * p.nw;
   if ((p.start & 1) || ((p.W & 1) && p.nw > 1)) {          // some window would start on an odd element: 64-bit loads everywhere
     GPUD_CUDA(r->ctx, (launch_one<false, -1, RANGE>(r, p, units)));
@@ -1320,22 +1414,31 @@ static int32_t launch_windows(gpud_ring* r, WinParams p) {
   if (special && (p.count % p.W) != 0 && (n_skip == 0 || p.w_skip[0] != p.nw - 1)) p.w_skip[n_skip++] = p.nw - 1;   // trailing partial window
   cudaError_t e;
 #ifdef GPUD_EXPERIMENT_TMA
-  if (special && r->inplace_landing && !RANGE && (p.W & 1) == 0) e = launch_inplace(r, p, units);
-  else if (special && r->tma_landing && jf == 15 && !RANGE) e = launch_one_tma<15, false>(r, p, units);
-  else if (special && r->tma_landing && jf == 16) e = launch_one_tma<16, RANGE>(r, p, units);
+  const bool inplace = special && r->inplace_landing && !RANGE && (p.W & 1) == 0;
+  const bool tma = special && r->tma_landing && (jf == 16 || !RANGE);
+  const bool tail_launch = inplace || tma;                 // the landing variants leave w_skip to a second launch
+  if (inplace) e = launch_inplace(r, p, units);
+  else if (tma && jf == 15) e = launch_one_tma<15, false>(r, p, units);
+  else if (tma) e = launch_one_tma<16, RANGE>(r, p, units);
   else
 #endif
-  if (special && jf == 15 && !RANGE) e = launch_one<true, 15, false>(r, p, units);   // the range pass always runs W' = 1024 (jf = 16)
-  else if (special && jf == 16) e = launch_one<true, 16, RANGE>(r, p, units);
-  else e = launch_one<true, -1, RANGE>(r, p, units);
+  {
+    p.n_tail = n_skip;
+    if (special && jf == 15 && !RANGE) e = launch_one<true, 15, false>(r, p, units);   // the range pass always runs W' = 1024 (jf = 16)
+    else if (special && jf == 16) e = launch_one<true, 16, RANGE>(r, p, units);
+    else e = launch_one<true, -1, RANGE>(r, p, units);
+  }
   GPUD_CUDA(r->ctx, e);
-  if (n_skip > 0) {
+#ifdef GPUD_EXPERIMENT_TMA
+  if (tail_launch && n_skip > 0) {
     p.n_list = n_skip;
     p.w_list[0] = p.w_skip[0];
     p.w_list[1] = p.w_skip[1];
     p.w_skip[0] = p.w_skip[1] = -1;
+    p.cursor += 1;
     GPUD_CUDA(r->ctx, (launch_one<false, -1, RANGE>(r, p, (int64_t)p.F * n_skip)));
   }
+#endif
   return GPUD_OK;
 }
 
@@ -1351,6 +1454,7 @@ extern "C" int32_t gpud_ring_reduce(gpud_ring* r) {
   p.q64 = pow(1.0 - r->alpha, 64.0); p.alpha = r->alpha;
   p.out_min = r->d_res[GPUD_OP_MIN]; p.out_max = r->d_res[GPUD_OP_MAX]; p.out_mean = r->d_res[GPUD_OP_MEAN];
   p.out_p99 = r->d_res[GPUD_OP_P99]; p.out_nover = r->d_nover; p.part = r->d_part; p.do_select = 1;
+  p.cursor = r->d_cursor;
   cudaEventRecord(r->ev_k[0], r->stream);
   { int32_t rc = launch_windows<false>(r, p); if (rc) return rc; }
   cudaEventRecord(r->ev_k[1], r->stream);
@@ -1373,6 +1477,19 @@ extern "C" int32_t gpud_ring_kernel_ms(gpud_ring* r, float* reduce_ms, float* ca
   GPUD_CUDA(r->ctx, cudaEventElapsedTime(carry_ms, r->ev_k[1], r->ev_k[2]));
   return GPUD_OK;
 }
+
+#ifdef GPUD_EXPERIMENT_FINISH
+// Copies the per-warp {start ns, end ns, windows} records of the hot launches since the last call into out[n_warps][3] and clears them.
+extern "C" int32_t gpud_exp_warp_finish(gpud_ring* r, unsigned long long* out, int32_t n_warps) {
+  if (!r || !out || n_warps < 1 || n_warps > kExpMaxWarps) return GPUD_E_INVALID;
+  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
+  GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));
+  GPUD_CUDA(r->ctx, cudaMemcpyFromSymbol(out, g_exp_finish, (size_t)n_warps * 3 * sizeof(unsigned long long)));
+  static const unsigned long long zeros[kExpMaxWarps][3] = {};
+  GPUD_CUDA(r->ctx, cudaMemcpyToSymbol(g_exp_finish, zeros, sizeof(zeros)));
+  return GPUD_OK;
+}
+#endif
 
 extern "C" int32_t gpud_ring_sync(gpud_ring* r) {
   if (!r) return GPUD_E_INVALID;
@@ -1455,6 +1572,7 @@ int32_t gpud_ring_range_pass(gpud_ring* r, const gpud_range_view* v) {
   p.q_num = r->q_num; p.q_den = r->q_den; p.thr = r->d_thr; p.pw = r->d_pw; p.q64 = pow(1.0 - r->alpha, 64.0); p.alpha = r->alpha;
   p.out_min = r->d_rng[0]; p.out_max = r->d_rng[1]; p.out_mean = r->d_rng[2]; p.out_p99 = nullptr; p.out_nover = r->d_rng_nover;
   p.part = r->d_rng[4]; p.do_select = 0;
+  p.cursor = r->d_cursor + 2;
   p.piv = v->piv; p.w_cls = v->w_cls; p.lists = v->lists; p.fill = v->fill; p.list_cap = v->list_cap;
   { int32_t rc = v->sampled ? launch_windows<true>(r, p) : launch_windows<false>(r, p); if (rc) return rc; }
   const int m_last = (int)(v->n - (int64_t)(v->nw - 1) * v->Wp);
