@@ -1,7 +1,7 @@
 # Builds libgpud_b200.so (sm_90a only) and the oracle.  `python -c "import __graft_entry__ as g; g.build()"` calls this.
 NVCC ?= /usr/local/cuda/bin/nvcc
 ARCH := -gencode arch=compute_90a,code=sm_90a
-NVFLAGS := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xcompiler -Wall -Xptxas -v $(if $(EXPERIMENT_TMA),-DGPUD_EXPERIMENT_TMA)
+NVFLAGS := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xcompiler -Wall -Xptxas -v
 SRC := gpud_b200/csrc
 OBJS := $(SRC)/api.o $(SRC)/ring.o $(SRC)/select.o $(SRC)/kmsg_scan.o $(SRC)/ib_scan.o $(SRC)/fabric.o $(SRC)/catalog.o $(SRC)/host_component.o $(SRC)/component_abi.o $(SRC)/kmsg_stateful.o $(SRC)/poller.o $(SRC)/store_sqlite.o
 LIB := gpud_b200/libgpud_b200.so

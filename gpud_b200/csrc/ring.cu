@@ -14,7 +14,6 @@
 //   threshold `>`   components/accelerator/nvidia/temperature/component.go:228,240
 #include <math.h>
 #include <stdarg.h>
-#include <stdlib.h>
 
 #include <algorithm>
 
@@ -38,7 +37,6 @@ struct WinParams {
   int q_num, q_den;
   const double* thr;   // [F]
   const double* pw;    // [127]: (1-alpha)^e for e = -63..63
-  const double* pwl;   // [32]: (1-alpha)^(W - 32 l - 32) (in-place kernel)
   double q64;          // (1-alpha)^64
   double alpha;
   double* out_min;
@@ -50,7 +48,8 @@ struct WinParams {
   int do_select;       // 0: skip the order statistic (range reduce uses the radix select instead)
   int k_full;          // k-th largest rank of a full window (m == W), precomputed on the host
   double inv_w;        // 1.0 / W
-  int n_list;          // > 0: process only windows w_list[0..n_list) of every field (generic instantiation)
+  // Always 0 / -1.  window_loop still tests them: without the test, ptxas (CUDA 12.9) grows the hot instantiations by ~40 % and spills.
+  int n_list;          // > 0 would mean: reduce only windows w_list[0..n_list) of every field
   int w_list[2];
   int w_skip[2];       // windows the aligned loop leaves to the generic code (-1 = none)
   int n_tail;          // > 0: the launch reduces the w_skip[0..n_tail) windows of every field itself, after its aligned units
@@ -231,18 +230,15 @@ __device__ __forceinline__ int elem_index(int row, int col) { return 64 * (col >
 // per row gives every lane one key of that row and the few lanes that hold a hit claim a slot with a predicated
 // shared-memory atomic - straight-line code, four rows in flight per trip.
 // Returns the number of hits (may exceed kCandMax; only the first kCandMax are stored).
-// INPLACE: the rows are not stored anywhere - "row r, entry i" is element 64 (i >> 1) + 2 ((r + (i >> 1)) & 31) + (i & 1) of the
-// linear window buffer (k_window_reduce_inplace); the row list then holds 16 r and the pad row is reached through a flag bit.
-template <bool HI_ONLY, int ROWW = kRowU64, bool INPLACE = false>
+template <bool HI_ONLY>
 __device__ __forceinline__ int gather_rows(unsigned char* wbase, unsigned rows, unsigned Lh, unsigned Ll, int lane, unsigned lt_mask) {
-  constexpr int kPadOff = 32 * ROWW * 8, kCndOff = kPadOff + 256, kLstOff = kCndOff + (kCandMax + 4) * 8;   // the scratch follows the rows
   const int n_rows = __popc(rows);
-  unsigned* row_off = reinterpret_cast<unsigned*>(wbase + kLstOff);
-  if ((rows >> lane) & 1u) row_off[__popc(rows & lt_mask)] = INPLACE ? (unsigned)lane : (unsigned)lane * (ROWW * 8);
-  if (lane < 4) row_off[n_rows + lane] = INPLACE ? 0x80000000u : kPadOff;
+  unsigned* row_off = reinterpret_cast<unsigned*>(wbase + kRowListOff);
+  if ((rows >> lane) & 1u) row_off[__popc(rows & lt_mask)] = (unsigned)lane * (kRowU64 * 8);
+  if (lane < 4) row_off[n_rows + lane] = kPadRowOff;
   __syncwarp();
-  const unsigned col = (unsigned)__cvta_generic_to_shared(wbase) + (INPLACE ? (unsigned)((lane >> 1) * 512 + (lane & 1) * 8) : (unsigned)(lane * 8));
-  uint2* cand = reinterpret_cast<uint2*>(wbase + kCndOff);
+  const unsigned col = (unsigned)__cvta_generic_to_shared(wbase) + (unsigned)(lane * 8);
+  uint2* cand = reinterpret_cast<uint2*>(wbase + kCandOff);
   const unsigned long long Lp = ((unsigned long long)Lh << 32) | Ll;
   const unsigned X = (Lh & 0x80000000u) ? 0u : 0x7fffffffu;
   const int Y = (int)(Lh ^ 0x80000000u);
@@ -251,11 +247,7 @@ __device__ __forceinline__ int gather_rows(unsigned char* wbase, unsigned rows, 
   // equal keys that would overflow the candidate list ends the walk after the trip that passes 32 (the caller falls back).
 #pragma unroll 1
   for (int i = 0; i < n_rows && cnt <= 32; i += 4) {
-    uint4 o4 = *reinterpret_cast<const uint4*>(row_off + i);                         // broadcast
-    if (INPLACE) {
-      auto at = [&](unsigned r) { return (r & 0x80000000u) ? (unsigned)(kPadOff + lane * 8) - (unsigned)((lane >> 1) * 512 + (lane & 1) * 8) : 16u * ((r + (unsigned)(lane >> 1)) & 31u); };
-      o4 = make_uint4(at(o4.x), at(o4.y), at(o4.z), at(o4.w));
-    }
+    const uint4 o4 = *reinterpret_cast<const uint4*>(row_off + i);                   // broadcast
     unsigned lo[4], hi[4];
     asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(lo[0]), "=r"(hi[0]) : "r"(col + o4.x));
     asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(lo[1]), "=r"(hi[1]) : "r"(col + o4.y));
@@ -296,20 +288,39 @@ __device__ __forceinline__ unsigned warp_kth_largest_smem(unsigned v, int k, uns
   return __reduce_min_sync(kFull, (int)(0u - neg_rank) < k ? v : 0xffffffffu);
 }
 
+// Low word of the window's exact maximum (MAX) or minimum key, given its high word eh and each lane's extreme high word lane_h:
+// the low words of the row entries whose high word is eh, over the rows of the lanes whose extreme is eh.
+template <bool MAX>
+__device__ __forceinline__ unsigned extreme_lo(const unsigned long long* sk, unsigned lane_h, unsigned eh, int m, int lane) {
+  unsigned rows = __ballot_sync(kFull, lane_h == eh);
+  unsigned el = MAX ? 0u : 0xffffffffu;
+  const unsigned raw_eh = raw_hi_of(eh);
+  if (__popc(rows) > 6) {
+    // tie-heavy window (integer readings, flat gauges): most rows hold the extreme high word, so every lane scans its own
+    // row instead of the warp visiting the rows one by one
+    rows = 0u;
+#pragma unroll 4
+    for (int i = 0; i < 32; ++i) {
+      const unsigned long long kv = sk[lane * kRowU64 + i];
+      if ((unsigned)(kv >> 32) == raw_eh && elem_index(lane, i) < m) {
+        const unsigned l = true_lo(eh, (unsigned)kv);
+        el = MAX ? max(el, l) : min(el, l);
+      }
+    }
+  }
+  while (rows) {
+    const int row = __ffs(rows) - 1;
+    rows &= rows - 1;
+    const unsigned long long kv = sk[row * kRowU64 + lane];
+    if ((unsigned)(kv >> 32) == raw_eh && elem_index(row, lane) < m) {   // the index test screens padding
+      const unsigned l = true_lo(eh, (unsigned)kv);
+      el = MAX ? max(el, l) : min(el, l);
+    }
+  }
+  return MAX ? __reduce_max_sync(kFull, el) : __reduce_min_sync(kFull, el);
+}
+
 struct WinUnit { int f, w, m; int64_t p0; };
-// ---- cp.async.bulk landing (TMA instantiations): one bulk copy per window into the warp's stage buffer, completion on an mbarrier ----
-__device__ __forceinline__ void mbar_init(unsigned a, int cnt) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(a), "r"(cnt)); }
-__device__ __forceinline__ void mbar_expect(unsigned a, int bytes) { asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(a), "r"(bytes) : "memory"); }
-__device__ __forceinline__ void bulk_g2s(unsigned dst, const void* src, int bytes, unsigned mbar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(mbar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(unsigned a, int parity) {
-  unsigned ok = 0;
-  while (!ok)
-    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(ok) : "r"(a), "r"(parity) : "memory");
-}
-constexpr int kStageBytesTma = 8192;                       // one window of <= 1024 doubles
-constexpr int kTmaWarps = 13;                              // 13 x (row area + stage) = 226.7 KB: one CTA per SM
 // streaming 128-bit load: read-only path, no L1 allocation, 256-byte L2 sector promotion
 __device__ __forceinline__ double2 ld_stream(const double2* p) {
   double2 r;
@@ -323,7 +334,7 @@ constexpr int kPrefetchPairs = GPUD_PREFETCH_PAIRS;      // register pairs of th
 // H100 SXM (400 W limit), survey stream, kernel ms for 4 GiB: 8 pairs + 2 CTAs/SM (112 registers, no spill) 1.53; 12 pairs + 2 CTAs
 // 1.53; 16 pairs + 2 CTAs 2.95 (the 128-register cap spills ~530 B per thread); 16 pairs + 1 CTA 1.62; 8 pairs + 3 CTAs (80-register
 // cap, spills) 1.85.  The rest of the window is loaded by fetch_rest() at the top of the trip that consumes it.
-constexpr int kHotCtasPerSM = 2;
+constexpr int kCtasPerSM = 2;                            // k_window_reduce occupancy: its launch bounds and its persistent grid
 
 #ifdef GPUD_EXPERIMENT_FINISH
 // EXPERIMENT (`-DGPUD_EXPERIMENT_FINISH`, tools/exp_warp_finish.py): every warp of the hot instantiation records its %globaltimer at
@@ -339,26 +350,12 @@ __device__ __forceinline__ unsigned long long global_ns() {
 
 // The warp loop of k_window_reduce: reduces the units it claims from the work cursor until the cursor runs out and returns how
 // many it reduced.  TAIL: the units are the w_skip[0..n_tail) windows of every field (claimed from cursor[1]).
-// TMA: the window lands in a per-warp stage buffer through one cp.async.bulk (UBLKCP) instead of 16 LDG.128 per lane into registers;
-// pass 1 reads it with conflict-free LDS.128 and the copy of the next window is issued as soon as pass 1 is done with the buffer.
-// Only for the hot shape (ALIGNED, JF >= 0); 13 warps per SM in one CTA (the stage buffers take the room of the second CTA's rows).
-template <bool ALIGNED, int JF, bool RANGE, bool TMA, bool TAIL>
+template <bool ALIGNED, int JF, bool RANGE, bool TAIL>
 __device__ __forceinline__ int window_loop(const WinParams& p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
-  constexpr int kPerWarp = kWarpSmemBytes + (TMA ? kStageBytesTma : 0);
-  __shared__ __align__(8) unsigned long long s_bars[TMA ? kTmaWarps : 1];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
-  unsigned char* wbase = smem_raw + (size_t)warp * kPerWarp + (TMA ? kStageBytesTma : 0);     // stage buffer first (128-byte aligned), rows after it
-  const unsigned stage_a = (unsigned)__cvta_generic_to_shared(smem_raw + (size_t)warp * kPerWarp);
-  const double2* stage2 = reinterpret_cast<const double2*>(smem_raw + (size_t)warp * kPerWarp) + lane;
-  const unsigned bar_a = (unsigned)__cvta_generic_to_shared(s_bars + (TMA ? warp : 0));
-  int tma_parity = 0;
-  if (TMA) {
-    if (lane == 0) mbar_init(bar_a, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    __syncthreads();
-  }
+  unsigned char* wbase = smem_raw + (size_t)warp * kWarpSmemBytes;
   unsigned long long* sk = reinterpret_cast<unsigned long long*>(wbase);                        // [32][kRowU64] key rows
   uint2* cand = reinterpret_cast<uint2*>(wbase + kCandOff);                                     // [kCandMax + 4]
   unsigned* s32 = reinterpret_cast<unsigned*>(cand);                                            // 128 B scratch, reused before the gather
@@ -431,12 +428,7 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
     const double* __restrict__ base = p.ring + (int64_t)q.f * p.cap;
     thr_next = __ldg(p.thr + q.f);
     if (RANGE) { lo_next = __ldg(p.piv + 2 * q.f); hi_next = __ldg(p.piv + 2 * q.f + 1); }
-    if (TMA) {
-      if (lane == 0) {                                               // one 8 W-byte bulk copy; the mbarrier flips when all of it has landed
-        mbar_expect(bar_a, q.m * 8);
-        bulk_g2s(stage_a, base + q.p0, q.m * 8, bar_a);
-      }
-    } else if (ALIGNED) {
+    if (ALIGNED) {
       const double2* __restrict__ b2 = reinterpret_cast<const double2*>(base + q.p0) + lane;
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
@@ -453,7 +445,7 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
 
   auto fetch_rest = [&](const WinUnit& q) {
     if (TAIL) load_unaligned(q);
-    if (PF >= 16 || TMA) return;
+    if (PF >= 16) return;
     const double2* __restrict__ b2 = reinterpret_cast<const double2*>(p.ring + (int64_t)q.f * p.cap + q.p0) + lane;
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
@@ -470,7 +462,6 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
     ++n_done;
     if (u >= u_end && !asked) ask();                 // the run ends with this unit
     fetch_rest(cur);
-    if (TMA) { mbar_wait(bar_a, tma_parity); tma_parity ^= 1; }      // the window has landed in the stage buffer
     const int f = cur.f, w = cur.w, m = cur.m;
     const int J = (m + 63) >> 6;                     // register pairs that hold at least one valid element
     const int Jfull = JF >= 0 ? JF : (m >> 6);       // register pairs in which every lane's two elements are valid
@@ -491,7 +482,6 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
       if (JF >= 0 ? (j < JF) : (j < Jfull)) {  // whole register pair valid (compile-time when JF >= 0, else warp-uniform)
-        if (TMA) v[j] = stage2[32 * j];          // LDS.128, lane-consecutive: conflict-free
         const double x0 = v[j].x, x1 = v[j].y;
         const int h0 = __double2hiint(x0), h1 = __double2hiint(x1);
         sum0 += x0; sum1 += x1;
@@ -510,7 +500,6 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
       } else if (JF >= 0 ? (j == JF) : (j < J)) {   // the one partially valid pair
         const int t0 = 64 * j + 2 * lane;
         const bool q0 = t0 < m, q1 = t0 + 1 < m;
-        if (TMA) v[j] = stage2[32 * j];          // bytes past the window are stale: masked by q0 / q1
         const double x0 = q0 ? v[j].x : 0.0, x1 = q1 ? v[j].y : 0.0;
         const unsigned h0 = q0 ? (unsigned)__double2hiint(x0) : 0xffffffffu, h1 = q1 ? (unsigned)__double2hiint(x1) : 0xffffffffu;   // padding = kPadStored
         sum0 += x0; sum1 += x1;
@@ -599,26 +588,7 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
     } else if (lo_zero) {
       wmin.lo = true_lo(wmin.hi, 0u);
     } else {
-      unsigned rows = __ballot_sync(kFull, nh == wmin.hi);
-      unsigned nl = 0xffffffffu;
-      const unsigned raw_min_hi = raw_hi_of(wmin.hi);
-      if (__popc(rows) > 6) {
-        // tie-heavy window (integer readings, flat gauges): most rows hold the minimum high word, so every lane scans its own
-        // row instead of the warp visiting the rows one by one
-        rows = 0u;
-#pragma unroll 4
-        for (int i = 0; i < 32; ++i) {
-          const unsigned long long kv = sk[lane * kRowU64 + i];
-          if ((unsigned)(kv >> 32) == raw_min_hi && elem_index(lane, i) < m) nl = min(nl, true_lo(wmin.hi, (unsigned)kv));
-        }
-      }
-      while (rows) {
-        const int row = __ffs(rows) - 1;
-        rows &= rows - 1;
-        const unsigned long long kv = sk[row * kRowU64 + lane];
-        if ((unsigned)(kv >> 32) == raw_min_hi && elem_index(row, lane) < m) nl = min(nl, true_lo(wmin.hi, (unsigned)kv));   // the index test screens padding
-      }
-      wmin.lo = __reduce_min_sync(kFull, nl);
+      wmin.lo = extreme_lo<false>(sk, nh, wmin.hi, m, lane);
     }
 
     K64 ans, wmax;
@@ -710,24 +680,7 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
       if (lo_zero) {
         wmax.lo = true_lo(wmax.hi, 0u);
       } else {
-        unsigned rows = __ballot_sync(kFull, mh == wmax.hi);
-        unsigned ml = 0u;
-        const unsigned raw_max_hi = raw_hi_of(wmax.hi);
-        if (__popc(rows) > 6) {
-          rows = 0u;
-#pragma unroll 4
-          for (int i = 0; i < 32; ++i) {
-            const unsigned long long kv = sk[lane * kRowU64 + i];
-            if ((unsigned)(kv >> 32) == raw_max_hi && elem_index(lane, i) < m) ml = max(ml, true_lo(wmax.hi, (unsigned)kv));
-          }
-        }
-        while (rows) {
-          const int row = __ffs(rows) - 1;
-          rows &= rows - 1;
-          const unsigned long long kv = sk[row * kRowU64 + lane];
-          if ((unsigned)(kv >> 32) == raw_max_hi && elem_index(row, lane) < m) ml = max(ml, true_lo(wmax.hi, (unsigned)kv));
-        }
-        wmax.lo = __reduce_max_sync(kFull, ml);
+        wmax.lo = extreme_lo<true>(sk, mh, wmax.hi, m, lane);
       }
       unsigned n_eh = 0, n_el = 0, n_in = 0;
       if (__any_sync(kFull, inmask != 0u)) {
@@ -795,18 +748,18 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
 
 // The trailing partial window and the window that wraps the physical end of the ring (w_skip) need the generic code; an aligned
 // launch reduces them itself once its cursor has run out (n_tail > 0), through the same loop instantiated for them.
-template <bool ALIGNED, int JF, bool RANGE, bool TMA = false>
-__global__ void __launch_bounds__((TMA ? kTmaWarps : kWarpsPerBlock) * 32, TMA ? 1 : ((ALIGNED && JF >= 0) ? kHotCtasPerSM : 2)) k_window_reduce(const WinParams p) {
+template <bool ALIGNED, int JF, bool RANGE>
+__global__ void __launch_bounds__(kWarpsPerBlock * 32, kCtasPerSM) k_window_reduce(const WinParams p) {
 #ifdef GPUD_EXPERIMENT_FINISH
   const unsigned long long exp_t0 = global_ns();
 #endif
-  int n_done = window_loop<ALIGNED, JF, RANGE, TMA, false>(p);
-  if constexpr (ALIGNED && !TMA) {
-    if (p.n_tail > 0) n_done += window_loop<false, -1, RANGE, false, true>(p);
+  int n_done = window_loop<ALIGNED, JF, RANGE, false>(p);
+  if constexpr (ALIGNED) {
+    if (p.n_tail > 0) n_done += window_loop<false, -1, RANGE, true>(p);
   }
 #ifdef GPUD_EXPERIMENT_FINISH
-  const int exp_warp = blockIdx.x * (TMA ? kTmaWarps : kWarpsPerBlock) + (threadIdx.x >> 5);
-  if (ALIGNED && JF >= 0 && !RANGE && !TMA && (threadIdx.x & 31) == 0 && exp_warp < kExpMaxWarps) {
+  const int exp_warp = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
+  if (ALIGNED && JF >= 0 && !RANGE && (threadIdx.x & 31) == 0 && exp_warp < kExpMaxWarps) {
     g_exp_finish[exp_warp][0] = exp_t0;
     g_exp_finish[exp_warp][1] = global_ns();
     g_exp_finish[exp_warp][2] = (unsigned long long)n_done;
@@ -814,221 +767,6 @@ __global__ void __launch_bounds__((TMA ? kTmaWarps : kWarpsPerBlock) * 32, TMA ?
 #endif
   (void)n_done;
 }
-
-#ifdef GPUD_EXPERIMENT_TMA
-// ---------------------------------------------------------------------------------------------
-// K2+K4, in-place variant (EXPERIMENT, GPUD_WINDOW_LANDING=inplace): the window lands in the warp's 8 KB buffer through ONE
-// cp.async.bulk and is processed where it landed - no register landing zone, no second copy into a row array - so an SM holds 20-24
-// warps instead of 16.  The linear buffer dictates the element -> lane map: lane l owns the CONTIGUOUS elements 32 l .. 32 l + 31
-// ("row" l = bytes [256 l, 256 l + 256)), which makes a row read (lane i reads entry i) conflict-free as it stands, and pass 1 / the
-// own-row scans conflict-free when lane l starts at pair (or entry) l and walks cyclically.  Only full windows of an even W in
-// 960 .. 1024 (the hot shape); everything else stays with k_window_reduce.
-// ---------------------------------------------------------------------------------------------
-#ifndef GPUD_INPLACE_WARPS
-#define GPUD_INPLACE_WARPS 20
-#endif
-constexpr int kIpWarps = GPUD_INPLACE_WARPS;
-constexpr int kIpRow = 32;                                        // u64 per row: the window itself
-constexpr int kIpPadOff = 32 * kIpRow * 8;                        // 8192
-constexpr int kIpCandOff = kIpPadOff + 256;
-constexpr int kIpListOff = kIpCandOff + (kCandMax + 4) * 8;
-constexpr int kIpWarpBytes = kIpListOff + 36 * 4 + 16;            // 9152
-
-__global__ void __launch_bounds__(kIpWarps * 32, 1) k_window_reduce_inplace(const WinParams p) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  __shared__ __align__(8) unsigned long long s_bars[kIpWarps];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  unsigned char* wbase = smem_raw + (size_t)warp * kIpWarpBytes;
-  unsigned long long* sk = reinterpret_cast<unsigned long long*>(wbase);                        // [32][32]: element t at sk[t]
-  uint2* cand = reinterpret_cast<uint2*>(wbase + kIpCandOff);
-  unsigned* s32 = reinterpret_cast<unsigned*>(cand);
-  const unsigned stage_a = (unsigned)__cvta_generic_to_shared(wbase);
-  const unsigned bar_a = (unsigned)__cvta_generic_to_shared(s_bars + warp);
-  const unsigned lt_mask = (1u << lane) - 1u;
-  const int m = p.W;                                                                             // every window here is full
-  reinterpret_cast<unsigned long long*>(wbase + kIpPadOff)[lane] = kPadStored;                  // the pad row
-  for (int t = m + lane; t < 1024; t += 32) sk[t] = kPadStored;                                  // entries past the window: never touched by the copy
-  if (lane == 0) mbar_init(bar_a, 1);
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  __syncthreads();
-
-  const int per_f = p.nw;
-  const int64_t n_units = (int64_t)p.F * p.nw;
-  const int64_t stride = (int64_t)gridDim.x * kIpWarps;
-  const int df = (int)(stride / per_f), ds = (int)(stride - (int64_t)df * per_f);
-  int64_t u = (int64_t)blockIdx.x * kIpWarps + warp;
-  int uf = (int)(u / per_f), uslot = (int)(u - (int64_t)uf * per_f);
-  double thr_next = 0.0;
-  auto fetch = [&](WinUnit& q) -> bool {
-    for (;;) {
-      if (u >= n_units) return false;
-      q.f = uf; q.w = uslot;
-      u += stride; uf += df; uslot += ds;
-      if (uslot >= per_f) { uslot -= per_f; ++uf; }
-      if (q.w != p.w_skip[0] && q.w != p.w_skip[1]) break;
-    }
-    q.p0 = p.start + (int64_t)q.w * p.W;
-    if (q.p0 >= p.cap) q.p0 -= p.cap;
-    thr_next = __ldg(p.thr + q.f);
-    if (lane == 0) {
-      mbar_expect(bar_a, m * 8);
-      bulk_g2s(stage_a, p.ring + (int64_t)q.f * p.cap + q.p0, m * 8, bar_a);
-    }
-    return true;
-  };
-  // lane l, pair j <-> 16-byte chunk 32 j + ((l + j) & 31): consecutive samples stay spread over the lanes (the pigeonhole bounds need
-  // that), pass 1 reads 32 distinct chunks of a 512-byte span per step, and a row's 16 chunks hit every 16-byte bank group twice
-  const double a1 = 1.0 - p.alpha;
-  const double w_first = __ldg(p.pw + (62 - 2 * lane + 63));        // (1-alpha)^(62 - 2 c) for c = lane: weight of pair 0 inside its 64-block
-  const double w_step = __ldg(p.pw + (-2 + 63)), w_wrap = __ldg(p.pw + (62 + 63));   // c -> c + 1: x (1-alpha)^-2; c wraps 31 -> 0: x (1-alpha)^62
-  const double tail_w = __ldg(p.pw + (m - 1024 + 63));               // the Horner below weighs sample t by (1-alpha)^(1023 - t)
-  auto elem_at = [&](int row, int i) { return 64 * (i >> 1) + 2 * ((row + (i >> 1)) & 31) + (i & 1); };   // chronological index of (row, entry)
-
-  WinUnit cur;
-  int parity = 0;
-  bool have = fetch(cur);
-  while (have) {
-    mbar_wait(bar_a, parity);
-    parity ^= 1;
-    const int f = cur.f, w = cur.w;
-    const double thr = thr_next;
-    // ---- pass 1 ----
-    double sum0 = 0.0, sum1 = 0.0, acc = 0.0, wq = w_first;
-    unsigned nov = 0, lor = 0u;
-    int a_smax = (int)0x80000000;
-    unsigned b_umin = 0xffffffffu, c_umax = 0u;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int c = (lane + j) & 31;
-      const bool ok = 64 * j + 2 * c < m;                            // W is even: a pair is valid or not as a whole
-      const double2 v = *reinterpret_cast<const double2*>(wbase + 512 * j + 16 * c);
-      const double x0 = ok ? v.x : 0.0, x1 = ok ? v.y : 0.0;
-      sum0 += x0; sum1 += x1;
-      acc = fma(acc, p.q64, fma(x0, a1, x1) * wq);
-      wq *= (c == 31) ? w_wrap : w_step;
-      if (ok) {
-        const int h0 = __double2hiint(x0), h1 = __double2hiint(x1);
-        count_gt_f64(nov, x0, thr);
-        count_gt_f64(nov, x1, thr);
-        a_smax = max(a_smax, max(h0, h1));
-        b_umin = min(b_umin, min((unsigned)h0, (unsigned)h1));
-        c_umax = max(c_umax, max((unsigned)h0, (unsigned)h1));
-        lor |= (unsigned)__double2loint(x0) | (unsigned)__double2loint(x1);
-      }
-    }
-    const double e_lane = acc, lane_w = tail_w;
-    const unsigned rmh = a_smax >= 0 ? (unsigned)a_smax : b_umin;
-    const unsigned mh = key_hi_of(rmh);
-    const bool lane_empty = c_umax == 0u && b_umin == 0xffffffffu;
-    const unsigned nh = lane_empty ? 0xffffffffu : key_hi_of((c_umax & 0x80000000u) ? c_umax : b_umin);
-
-    double ep = e_lane * lane_w, sum = sum0 + sum1;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      sum += __shfl_xor_sync(kFull, sum, o);
-      ep += __shfl_xor_sync(kFull, ep, o);
-    }
-    ep *= p.alpha;
-    nov = __reduce_add_sync(kFull, nov);
-    const bool lo_zero = __reduce_or_sync(kFull, lor) == 0u;
-
-    // ---- exact minimum ----
-    K64 wmin;
-    wmin.hi = __reduce_min_sync(kFull, nh);
-    if (lo_zero) {
-      wmin.lo = true_lo(wmin.hi, 0u);
-    } else {
-      unsigned rows = __ballot_sync(kFull, nh == wmin.hi);
-      unsigned nl = 0xffffffffu;
-      const unsigned raw_min_hi = raw_hi_of(wmin.hi);
-      if (__popc(rows) > 6) {
-        rows = 0u;
-#pragma unroll 4
-        for (int i = 0; i < 32; ++i) {
-          const int t = elem_at(lane, i);
-          const unsigned long long kv = sk[t];
-          if ((unsigned)(kv >> 32) == raw_min_hi && t < m) nl = min(nl, true_lo(wmin.hi, (unsigned)kv));
-        }
-      }
-      while (rows) {
-        const int row = __ffs(rows) - 1;
-        rows &= rows - 1;
-        const int t = elem_at(row, lane);
-        const unsigned long long kv = sk[t];
-        if ((unsigned)(kv >> 32) == raw_min_hi && t < m) nl = min(nl, true_lo(wmin.hi, (unsigned)kv));
-      }
-      wmin.lo = __reduce_min_sync(kFull, nl);
-    }
-
-    // ---- exact order statistic + maximum (same scheme as k_window_reduce) ----
-    const int k = p.k_full;
-    K64 ans, wmax;
-    ans.hi = ans.lo = 0u;
-    bool done = false;
-    if (k <= 32) {
-      const unsigned Lh = warp_kth_largest_smem(mh, k, s32, lane);
-      if (lo_zero) {
-        const unsigned rows = __ballot_sync(kFull, mh > Lh);
-        const int cnt = rows ? gather_rows<true, kIpRow, true>(wbase, rows, Lh + 1u, 0u, lane, lt_mask) : 0;
-        if (cnt < k) { ans.hi = Lh; ans.lo = true_lo(Lh, 0u); done = true; }
-        else if (cnt <= 32) { K64 unused; ans = select_from_candidates(cand, cnt, k, lane, &unused); done = true; }
-        if (done) { wmax.hi = __reduce_max_sync(kFull, mh); wmax.lo = true_lo(wmax.hi, 0u); }
-      } else {
-        const int cnt = gather_rows<true, kIpRow, true>(wbase, __ballot_sync(kFull, mh >= Lh), Lh, 0u, lane, lt_mask);
-        if (cnt <= 32) { ans = select_from_candidates(cand, cnt, k, lane, &wmax); done = true; }
-      }
-      __syncwarp();
-    }
-    if (!done) {
-      unsigned ml = 0u;
-#pragma unroll 4
-      for (int i = 0; i < 32; ++i) {
-        const unsigned long long kv = sk[elem_at(lane, i)];
-        if ((unsigned)(kv >> 32) == rmh) ml = max(ml, true_lo(mh, (unsigned)kv));
-      }
-      wmax = warp_max_k64(mh, ml);
-      bool solved = false;
-      if (k <= 32) {
-        unsigned sh = mh, sl = ml;
-        warp_sort_desc_k64(sh, sl, lane);
-        const unsigned Lh = __shfl_sync(kFull, sh, k - 1), Ll = __shfl_sync(kFull, sl, k - 1);
-        const int cnt = gather_rows<false, kIpRow, true>(wbase, __ballot_sync(kFull, k_gt(mh, ml, Lh, Ll)), Lh, Ll, lane, lt_mask);
-        if (cnt < k) { ans.hi = Lh; ans.lo = Ll; solved = true; }
-        else if (cnt <= 32) { K64 unused; ans = select_from_candidates(cand, cnt, k, lane, &unused); solved = true; }
-        __syncwarp();
-      }
-      if (!solved) {
-        unsigned long long pref = 0ull;
-        int kk2 = k;
-#pragma unroll 1
-        for (int b = 63; b >= 0; --b) {
-          const unsigned long long trial = pref | (1ull << b);
-          const unsigned long long himask = ~((1ull << b) - 1ull);
-          unsigned c = 0;
-#pragma unroll 4
-          for (int i = 0; i < 32; ++i) c += ((true_key(sk[elem_at(lane, i)]) & himask) == trial) ? 1u : 0u;
-          c = __reduce_add_sync(kFull, c);
-          if ((int)c >= kk2) pref = trial; else kk2 -= (int)c;
-        }
-        ans.hi = (unsigned)(pref >> 32);
-        ans.lo = (unsigned)pref;
-      }
-    }
-    __syncwarp();                              // every lane is done with the buffer: the next window may land in it
-    if (lane == 0) {
-      const int64_t o = (int64_t)f * p.nw + w;
-      p.out_min[o] = k64_to_f64(wmin);
-      p.out_max[o] = k64_to_f64(wmax);
-      p.out_mean[o] = sum * p.inv_w;
-      if (p.do_select) p.out_p99[o] = k64_to_f64(ans);
-      p.out_nover[o] = nov;
-      p.part[o] = ep;
-    }
-    have = fetch(cur);
-  }
-}
-
-#endif  // GPUD_EXPERIMENT_TMA
 
 // ---------------------------------------------------------------------------------------------
 // K3 carry: E_w = (1-alpha)^{m_w} E_{w-1} + P_w, E_{-1} = x[0] (oldest sample).  One 128-thread CTA per field:
@@ -1108,9 +846,7 @@ struct gpud_ring {
   double* d_sample = nullptr;      // [F][smp_slots]: column c with c % 2^smp_shift == 2^smp_shift / 2 lives at slot c >> smp_shift (kept by the append kernel)
   int smp_shift = 0;
   int64_t smp_slots = 0;
-  double* d_pwl = nullptr;         // [32]: (1-alpha)^(W - 32 l - 32), the lane weights of the in-place kernel's EMA partial
   int sm_count = 132;
-  bool inplace_landing = false, tma_landing = false;   // only ever set in a GPUD_EXPERIMENT_TMA build
   int cta_reserve = 0;           // CTA slots the persistent window grid leaves free for kernels of other streams (gpud_ring_set_cta_reserve)
   double* d_rng[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};   // range-reduce scratch: per-window min,max,mean,ema,partials
   size_t rng_bytes[5] = {0, 0, 0, 0, 0};
@@ -1147,9 +883,6 @@ extern "C" int32_t gpud_ring_create(gpud_ctx* ctx, int32_t dev, const gpud_ring_
   r->ctx = ctx; r->dev = dev; r->F = cfg->n_fields; r->W = cfg->window; r->cap = cfg->capacity; r->alpha = alpha;
   r->q_num = qn; r->q_den = qd;
   r->sm_count = ctx->sm_count;
-#ifdef GPUD_EXPERIMENT_TMA   /* `make EXPERIMENT_TMA=1`: the two cp.async.bulk landing variants (DESIGN.md) */
-  { const char* env = getenv("GPUD_WINDOW_LANDING"); r->tma_landing = env && !strcmp(env, "tma"); r->inplace_landing = env && !strcmp(env, "inplace"); }
-#endif
   r->nw_max = (r->cap + r->W - 1) / r->W;
   const size_t ring_bytes = (size_t)r->F * r->cap * sizeof(double) + 64;   // slack: the 16-byte load of a window's last odd element
   const size_t res_bytes = (size_t)r->F * r->nw_max * sizeof(double);
@@ -1186,12 +919,6 @@ extern "C" int32_t gpud_ring_create(gpud_ctx* ctx, int32_t dev, const gpud_ring_
   for (int ex = -63; ex <= 63; ++ex) pw[ex + 63] = pow(1.0 - alpha, (double)ex);
   GPUD_CUDA(ctx, cudaMemcpy(r->d_thr, thr.data(), r->F * sizeof(double), cudaMemcpyHostToDevice));
   GPUD_CUDA(ctx, cudaMemcpy(r->d_pw, pw.data(), 127 * sizeof(double), cudaMemcpyHostToDevice));
-  {
-    std::vector<double> pwl(32);
-    for (int l = 0; l < 32; ++l) pwl[l] = pow(1.0 - alpha, (double)(r->W - 32 * l - 32));
-    GPUD_CUDA(ctx, cudaMalloc(&r->d_pwl, 32 * sizeof(double)));
-    GPUD_CUDA(ctx, cudaMemcpy(r->d_pwl, pwl.data(), 32 * sizeof(double), cudaMemcpyHostToDevice));
-  }
   GPUD_CUDA(ctx, cudaDeviceSynchronize());
   *out = r;
   return GPUD_OK;
@@ -1201,7 +928,7 @@ extern "C" int32_t gpud_ring_destroy(gpud_ring* r) {
   if (!r) return GPUD_E_INVALID;
   cudaSetDevice(r->dev);
   if (r->own_stream) cudaStreamSynchronize(r->own_stream);
-  cudaFree(r->d_ring); cudaFree(r->d_sample); cudaFree(r->d_pwl); cudaFree(r->d_thr); cudaFree(r->d_pw); cudaFree(r->d_nover); cudaFree(r->d_part);
+  cudaFree(r->d_ring); cudaFree(r->d_sample); cudaFree(r->d_thr); cudaFree(r->d_pw); cudaFree(r->d_nover); cudaFree(r->d_part);
   cudaFree(r->d_cursor);
   for (auto& p : r->d_res) cudaFree(p);
   for (auto& p : r->d_rng) cudaFree(p);
@@ -1337,10 +1064,10 @@ extern "C" int32_t gpud_ring_counts(gpud_ring* r, int64_t* total, int64_t* count
 }
 
 
-// Launch the window kernel(s).  The bulk goes to the aligned 128-bit instantiation (specialised for the window shape when
-// W >> 6 is 15 or 16, i.e. W in 960..1024); the window that wraps the physical end of the ring and a trailing partial
-// window go through the generic run-time code at the end of the same launch.  The generic instantiation on its own serves
-// rings whose start is odd.
+// Launch the window kernel: one launch per reduce.  The bulk goes to the aligned 128-bit instantiation (specialised for the
+// window shape when W >> 6 is 15 or 16, i.e. W in 960..1024); the window that wraps the physical end of the ring and a trailing
+// partial window go through the generic run-time code at the end of the same launch.  The generic instantiation on its own
+// serves rings in which some window starts on an odd element.
 #ifndef GPUD_RUN_WINDOWS
 #define GPUD_RUN_WINDOWS 8
 #endif
@@ -1353,36 +1080,13 @@ static void set_schedule(WinParams& p, int64_t units, int64_t warps) {
   p.n_runs = kRunWindows > 1 ? std::max<int64_t>(0, (units - warps * kRunWindows / 2) / kRunWindows) : 0;
 }
 
-#ifdef GPUD_EXPERIMENT_TMA
-template <int JF, bool RANGE>
-static cudaError_t launch_one_tma(gpud_ring* r, WinParams p, int64_t units) {
-  constexpr int kSmem = kTmaWarps * (kWarpSmemBytes + kStageBytesTma);
-  cudaError_t e = cudaFuncSetAttribute(k_window_reduce<true, JF, RANGE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-  if (e != cudaSuccess) return e;
-  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((units + kTmaWarps - 1) / kTmaWarps, (int64_t)r->sm_count - (r->cta_reserve ? 1 : 0)));
-  set_schedule(p, units, (int64_t)grid * kTmaWarps);
-  k_window_reduce<true, JF, RANGE, true><<<grid, kTmaWarps * 32, kSmem, r->stream>>>(p);
-  return cudaGetLastError();
-}
-
-static cudaError_t launch_inplace(gpud_ring* r, const WinParams& p, int64_t units) {
-  constexpr int kSmem = kIpWarps * kIpWarpBytes;
-  cudaError_t e = cudaFuncSetAttribute(k_window_reduce_inplace, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-  if (e != cudaSuccess) return e;
-  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((units + kIpWarps - 1) / kIpWarps, (int64_t)r->sm_count - (r->cta_reserve ? 1 : 0)));
-  k_window_reduce_inplace<<<grid, kIpWarps * 32, kSmem, r->stream>>>(p);
-  return cudaGetLastError();
-}
-
-#endif  // GPUD_EXPERIMENT_TMA
-
 template <bool ALIGNED, int JF, bool RANGE>
 static cudaError_t launch_one(gpud_ring* r, WinParams p, int64_t units) {
-  // persistent grid: 2 CTAs of 8 warps per SM, a whole number of waves
+  // persistent grid: kCtasPerSM CTAs of kWarpsPerBlock warps per SM, a whole number of waves
   // 72 KB of dynamic shared memory per CTA (8 warps x (32 x 272 B key rows + candidate list)): opt in above 48 KB
   cudaError_t e = cudaFuncSetAttribute(k_window_reduce<ALIGNED, JF, RANGE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBlockSmemBytes);
   if (e != cudaSuccess) return e;
-  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((units + kWarpsPerBlock - 1) / kWarpsPerBlock, (int64_t)r->sm_count * ((ALIGNED && JF >= 0) ? kHotCtasPerSM : 2) - r->cta_reserve));
+  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((units + kWarpsPerBlock - 1) / kWarpsPerBlock, (int64_t)r->sm_count * kCtasPerSM - r->cta_reserve));
   set_schedule(p, units, (int64_t)grid * kWarpsPerBlock);
   k_window_reduce<ALIGNED, JF, RANGE><<<grid, kWarpsPerBlock * 32, kBlockSmemBytes, r->stream>>>(p);
   return cudaGetLastError();
@@ -1406,39 +1110,16 @@ static int32_t launch_windows(gpud_ring* r, WinParams p) {
     GPUD_CUDA(r->ctx, (launch_one<false, -1, RANGE>(r, p, units)));
     return GPUD_OK;
   }
-  int n_skip = 0;
   const int64_t c_wrap = p.cap - p.start;                 // chronological index of the sample stored at physical column 0
-  if (p.start > 0 && c_wrap < p.count && (c_wrap % p.W) != 0) p.w_skip[n_skip++] = (int)(c_wrap / p.W);
+  if (p.start > 0 && c_wrap < p.count && (c_wrap % p.W) != 0) p.w_skip[p.n_tail++] = (int)(c_wrap / p.W);
   const int jf = p.W >> 6;
   const bool special = (jf == 15 || jf == 16) && p.nw > 1;
-  if (special && (p.count % p.W) != 0 && (n_skip == 0 || p.w_skip[0] != p.nw - 1)) p.w_skip[n_skip++] = p.nw - 1;   // trailing partial window
+  if (special && (p.count % p.W) != 0 && (p.n_tail == 0 || p.w_skip[0] != p.nw - 1)) p.w_skip[p.n_tail++] = p.nw - 1;   // trailing partial window
   cudaError_t e;
-#ifdef GPUD_EXPERIMENT_TMA
-  const bool inplace = special && r->inplace_landing && !RANGE && (p.W & 1) == 0;
-  const bool tma = special && r->tma_landing && (jf == 16 || !RANGE);
-  const bool tail_launch = inplace || tma;                 // the landing variants leave w_skip to a second launch
-  if (inplace) e = launch_inplace(r, p, units);
-  else if (tma && jf == 15) e = launch_one_tma<15, false>(r, p, units);
-  else if (tma) e = launch_one_tma<16, RANGE>(r, p, units);
-  else
-#endif
-  {
-    p.n_tail = n_skip;
-    if (special && jf == 15 && !RANGE) e = launch_one<true, 15, false>(r, p, units);   // the range pass always runs W' = 1024 (jf = 16)
-    else if (special && jf == 16) e = launch_one<true, 16, RANGE>(r, p, units);
-    else e = launch_one<true, -1, RANGE>(r, p, units);
-  }
+  if (special && jf == 15 && !RANGE) e = launch_one<true, 15, false>(r, p, units);   // the range pass always runs W' = 1024 (jf = 16)
+  else if (special && jf == 16) e = launch_one<true, 16, RANGE>(r, p, units);
+  else e = launch_one<true, -1, RANGE>(r, p, units);
   GPUD_CUDA(r->ctx, e);
-#ifdef GPUD_EXPERIMENT_TMA
-  if (tail_launch && n_skip > 0) {
-    p.n_list = n_skip;
-    p.w_list[0] = p.w_skip[0];
-    p.w_list[1] = p.w_skip[1];
-    p.w_skip[0] = p.w_skip[1] = -1;
-    p.cursor += 1;
-    GPUD_CUDA(r->ctx, (launch_one<false, -1, RANGE>(r, p, (int64_t)p.F * n_skip)));
-  }
-#endif
   return GPUD_OK;
 }
 
@@ -1450,7 +1131,7 @@ extern "C" int32_t gpud_ring_reduce(gpud_ring* r) {
   WinParams p;
   p.ring = r->d_ring; p.cap = r->cap; p.start = ring_start(r); p.count = count;
   p.W = r->W; p.F = r->F; p.nw = (int)((count + r->W - 1) / r->W);
-  p.q_num = r->q_num; p.q_den = r->q_den; p.thr = r->d_thr; p.pw = r->d_pw; p.pwl = r->d_pwl;
+  p.q_num = r->q_num; p.q_den = r->q_den; p.thr = r->d_thr; p.pw = r->d_pw;
   p.q64 = pow(1.0 - r->alpha, 64.0); p.alpha = r->alpha;
   p.out_min = r->d_res[GPUD_OP_MIN]; p.out_max = r->d_res[GPUD_OP_MAX]; p.out_mean = r->d_res[GPUD_OP_MEAN];
   p.out_p99 = r->d_res[GPUD_OP_P99]; p.out_nover = r->d_nover; p.part = r->d_part; p.do_select = 1;
