@@ -44,10 +44,6 @@ constexpr int kModeMask = 0xff;
 #ifndef GPUD_MATCH_BLOCKS
 #define GPUD_MATCH_BLOCKS 5                  // resident 128-thread blocks per SM the match kernel is compiled for (register budget)
 #endif
-#ifndef GPUD_MATCH_LANES
-#define GPUD_MATCH_LANES 1
-#endif
-constexpr unsigned kMatchLanes = GPUD_MATCH_LANES;        // candidates per warp in k_scan_match
 #ifndef GPUD_FILTER_BLOCKS
 #define GPUD_FILTER_BLOCKS 3
 #endif
@@ -392,6 +388,7 @@ __global__ void __launch_bounds__(256, kFilterBlocks) k_scan_filter(ScanBuf b, u
         const unsigned t = ((w[k] ^ 0x0a0a0a0au) & c7f) + c7f;
         unsigned z = ~(t | w[k]) & 0x80808080u;                                 // 0x80 in every byte that is '\n'
         if (MODE == GPUD_SCAN_RAW_KMSG) {                                      // ... not followed by ' ' (continuation line)
+          // (a '\n' in the buffer's last byte is followed by 0 here, not ' ': it stays a separator)
           const unsigned x1 = __funnelshift_r(w[k], w[k + 1], 8);
           const unsigned ts = ((x1 ^ 0x20202020u) & c7f) + c7f;
           z &= ts | x1;
@@ -399,9 +396,6 @@ __global__ void __launch_bounds__(256, kFilterBlocks) k_scan_filter(ScanBuf b, u
         sep128 = __dp4a(z, 0x01010101u, sep128);
       }
       unsigned sep = sep128 >> 7;
-      if (MODE == GPUD_SCAN_RAW_KMSG) {
-        // a '\n' in the last byte of the buffer has no follower: it is a separator (x1's byte there is 0, not ' ') - nothing to fix
-      }
       // ---- anchors (rare): handled by the whole warp, one flagged lane at a time, so no lane works alone ----
       unsigned hit_lanes = __ballot_sync(kFull, hit);
       while (hit_lanes) {
@@ -787,18 +781,9 @@ __device__ bool pattern_ok(uint8_t kind, uint32_t care, uint32_t val, uint32_t i
   return (intrinfo & care) == val;
 }
 
-// normalizeUnit(log unit) == normalizeUnit(alias) for any alias (xid.go:3174-3218)
-__device__ bool unit_matches_norm(const gpud_t_rule& r, const char* norm) {
-  if (norm[0] == 0) return false;
-  for (int a = 0; a < r.n_alias; ++a) {
-    int i = 0;
-    while (r.alias[a][i] && r.alias[a][i] == norm[i]) ++i;
-    if (r.alias[a][i] == 0 && norm[i] == 0) return true;
-  }
-  return false;
-}
-// the same test on whole words: alias rows and `norm` are NUL-padded to GPUD_T_ALIAS_LEN, so two strings are equal iff their 12 words
-// are - twelve independent loads per alias instead of a chain of dependent byte loads (the finish kernel's top stall line)
+// normalizeUnit(log unit) == normalizeUnit(alias) for any alias (xid.go:3174-3218), on whole words: alias rows and `norm` are
+// NUL-padded to GPUD_T_ALIAS_LEN, so two strings are equal iff their 12 words are - twelve independent loads per alias instead of a
+// chain of dependent byte loads (the finish kernel's top stall line)
 static_assert(offsetof(gpud_t_rule, alias) % 4 == 0 && sizeof(gpud_t_rule) % 4 == 0 && offsetof(gpud_tables, rules) % 4 == 0 && GPUD_T_ALIAS_LEN % 4 == 0,
               "alias rows are read as 32-bit words");
 __device__ __forceinline__ bool unit_matches_words(const gpud_t_rule& r, const unsigned* norm_words) {
@@ -822,64 +807,62 @@ __device__ void normalize_unit(const char* unit, char* norm) {          // TrimS
   }
   norm[n] = 0;
 }
-__device__ bool unit_matches(const gpud_t_rule& r, const char* unit) {
-  char norm[GPUD_T_ALIAS_LEN];
-  int n = 0;
-  // TrimSpace + ToUpper + '-'->'_' + keep [A-Z0-9_]
-  for (int i = 0; unit[i] && n < GPUD_T_ALIAS_LEN - 1; ++i) {
-    int c = (unsigned char)unit[i];
-    if (c >= 'a' && c <= 'z') c -= 32;
-    if (c == '-') c = '_';
-    if ((c >= 'A' && c <= 'Z') || (c >= '0' && c <= '9') || c == '_') norm[n++] = (char)c;
-  }
-  norm[n] = 0;
-  if (n == 0) return false;
-  for (int a = 0; a < r.n_alias; ++a) {
-    int i = 0;
-    while (r.alias[a][i] && r.alias[a][i] == norm[i]) ++i;
-    if (r.alias[a][i] == 0 && norm[i] == 0) return true;
-  }
-  return false;
-}
 
-// detailFromNVLinkInfo (xid.go:2954-2995); returns false when the base code is unknown
-__device__ bool classify_extended(const gpud_tables* T, gpud_xid_hit* h) {
-  const int xid = h->code;
-  if (xid <= 0 || xid >= GPUD_T_MAX_XID || !T->xid[xid].present) return false;
-  const gpud_t_detail base = T->xid[xid];
-  gpud_t_detail d = base;
-  int variant = 0;
-  bool found = false;
-  for (int i = 0; i < T->n_by_status && !found; ++i)      // getDetailWithSubCodeAndStatus (xid.go:97-107)
-    if (T->by_status[i].xid == xid && T->by_status[i].sub_code == h->sub_code && T->by_status[i].error_status == h->error_status) {
-      d = T->by_status[i].d; variant = T->by_status[i].variant; found = true;
-    }
-  if (!found && T->has_sub_map[xid]) {                    // getDetailWithSubCode (xid.go:79-93)
-    for (int pass = 0; pass < 2 && !found; ++pass) {
-      const int want = pass == 0 ? h->sub_code : 0;
-      for (int i = 0; i < T->n_by_sub && !found; ++i)
-        if (T->by_sub[i].xid == xid && T->by_sub[i].sub_code == want) { d = T->by_sub[i].d; variant = T->by_sub[i].variant; found = true; }
-    }
+// detailFromNVLinkInfo (xid.go:2954-2995) of an extended hit whose base code exists, one WARP per hit - the whole warp calls it:
+// the three table searches (sub-code + status override, sub-code detail, the 94 NVLink rules with their alias lists) are spread
+// over the lanes and the first match in table order is the minimum matching index (a single thread spent about as long on the
+// sequential loops as on the whole regex automaton).  Lane 0 merges and stores the result.
+__device__ __forceinline__ void detail_from_nvlink_info(const gpud_tables* __restrict__ T, gpud_xid_hit* h, int lane) {
+  const int xid = h->code, sub = h->sub_code;
+  const uint32_t st = h->error_status, intr = h->intrinfo;
+  char unit[40];
+  __align__(4) char norm[GPUD_T_ALIAS_LEN];
+  for (int i = 0; i < 40; ++i) unit[i] = h->unit_name[i];
+  unit[39] = 0;
+  for (int i = 0; i < GPUD_T_ALIAS_LEN; ++i) norm[i] = 0;         // NUL-padded: compared word by word below
+  normalize_unit(unit, norm);
+  const unsigned* norm_words = reinterpret_cast<const unsigned*>(norm);
+  int i_status = 0x7fffffff, i_sub = 0x7fffffff, i_sub0 = 0x7fffffff, i_rule = 0x7fffffff;
+  for (int i = lane; i < T->n_by_status; i += 32)
+    if (i < i_status && T->by_status[i].xid == xid && T->by_status[i].sub_code == sub && T->by_status[i].error_status == st) i_status = i;
+  for (int i = lane; i < T->n_by_sub; i += 32) {
+    if (T->by_sub[i].xid != xid) continue;
+    if (i < i_sub && T->by_sub[i].sub_code == sub) i_sub = i;
+    if (i < i_sub0 && T->by_sub[i].sub_code == 0) i_sub0 = i;
   }
-  h->rule_index = -1;
-  for (int i = 0; i < T->n_rules; ++i) {                  // lookupNVLinkRule (xid.go:3099-3114), table order
+  for (int i = lane; i < T->n_rules; i += 32) {
     const gpud_t_rule& r = T->rules[i];
-    if (r.xid != xid || r.error_status != h->error_status) continue;
-    if (!unit_matches(r, h->unit_name)) continue;
-    if (pattern_ok(r.v2_kind, r.v2_care, r.v2_val, h->intrinfo) || pattern_ok(r.v1_kind, r.v1_care, r.v1_val, h->intrinfo)) {
-      h->rule_index = i;
+    if (i >= i_rule || r.xid != xid || r.error_status != st) continue;
+    if (!unit_matches_words(r, norm_words)) continue;
+    if (pattern_ok(r.v2_kind, r.v2_care, r.v2_val, intr) || pattern_ok(r.v1_kind, r.v1_care, r.v1_val, intr)) i_rule = i;
+  }
+  i_status = __reduce_min_sync(kFull, i_status);
+  i_sub = __reduce_min_sync(kFull, i_sub);
+  i_sub0 = __reduce_min_sync(kFull, i_sub0);
+  i_rule = __reduce_min_sync(kFull, i_rule);
+  if (lane == 0) {
+    const gpud_t_detail base = T->xid[xid];
+    gpud_t_detail d = base;
+    int variant = 0;
+    if (i_status != 0x7fffffff) { d = T->by_status[i_status].d; variant = T->by_status[i_status].variant; }          // xid.go:97-107
+    else if (T->has_sub_map[xid]) {                                                                                   // xid.go:79-93
+      const int k = i_sub != 0x7fffffff ? i_sub : i_sub0;
+      if (k != 0x7fffffff) { d = T->by_sub[k].d; variant = T->by_sub[k].variant; }
+    }
+    h->rule_index = -1;
+    if (i_rule != 0x7fffffff) {                                                                                       // xid.go:3099-3114
+      const gpud_t_rule& r = T->rules[i_rule];
+      h->rule_index = i_rule;
       h->flags |= GPUD_HIT_HAS_RULE;
       if (r.rule_event != GPUD_EVENT_UNKNOWN) d.event = r.rule_event;
       if (r.rule_n_actions > 0) { d.n_actions = 1; d.actions[0] = r.rule_action; d.actions[1] = d.actions[2] = d.actions[3] = 0; }
-      break;
     }
+    const int log_ev = h->severity_fatal ? GPUD_EVENT_FATAL : GPUD_EVENT_WARNING;   // eventTypeFromLogSeverity
+    if (log_ev > d.event) d.event = (int8_t)log_ev;
+    if (d.n_actions < 0) { d.n_actions = base.n_actions; for (int i = 0; i < 4; ++i) d.actions[i] = base.actions[i]; }
+    set_detail(h, d);
+    h->detail_variant = variant;
   }
-  const int log_ev = h->severity_fatal ? GPUD_EVENT_FATAL : GPUD_EVENT_WARNING;   // eventTypeFromLogSeverity
-  if (log_ev > d.event) d.event = (int8_t)log_ev;
-  if (d.n_actions < 0) { d.n_actions = base.n_actions; for (int i = 0; i < 4; ++i) d.actions[i] = base.actions[i]; }
-  set_detail(h, d);
-  h->detail_variant = variant;
-  return true;
 }
 
 __device__ bool classify_plain_xid(const gpud_tables* T, gpud_xid_hit* h) {   // GetDetail (xid.go:74-77)
@@ -932,7 +915,7 @@ __device__ bool xid_match_unit(const ScanBuf& g, int64_t s, int64_t e, const gpu
       copy_span(b, m2.unit_s, m2.unit_e, h->unit_name, 40, nullptr);
       if (h->unit_name_len >= 40) h->flags |= GPUD_HIT_DEV_TRUNCATED;   // inline copy cut; no catalog alias is that long
       if (h->code > 0 && h->code < GPUD_T_MAX_XID && T->xid[h->code].present) {   // detailFromNVLinkInfo needs only the base code to
-        h->event_type = kPendingExtended;                                            // exist; the table searches run warp-wide in k_classify_ext_coop
+        h->event_type = kPendingExtended;                                            // exist; the table searches run warp-wide in k_scan_finish
         h->dev_off = m2.dev_s; h->dev_len = (int32_t)(m2.dev_e - m2.dev_s);
         copy_span(b, m2.dev_s, m2.dev_e, h->device, 40, "PCI:");      // kmsg.go:206-208
         if (h->dev_len + 4 > 39) h->flags |= GPUD_HIT_DEV_TRUNCATED;
@@ -1214,7 +1197,7 @@ __global__ void __launch_bounds__(256) k_cand_scatter(const unsigned long long* 
   }
 }
 
-__global__ void __launch_bounds__(128, GPUD_MATCH_BLOCKS) k_scan_match(ScanBuf b, int mode, int lanes_min, const unsigned long long* __restrict__ cands_in,
+__global__ void __launch_bounds__(128, GPUD_MATCH_BLOCKS) k_scan_match(ScanBuf b, int mode, const unsigned long long* __restrict__ cands_in,
                                                      const unsigned long long* __restrict__ side, unsigned long long side_cap,
                                                      const unsigned long long* __restrict__ n_cand, unsigned long long cand_cap,
                                                      const uint32_t* __restrict__ chunk_local, const unsigned long long* __restrict__ tile_base, const gpud_tables* __restrict__ T,
@@ -1234,7 +1217,6 @@ __global__ void __launch_bounds__(128, GPUD_MATCH_BLOCKS) k_scan_match(ScanBuf b
   const unsigned lane = threadIdx.x & 31;
   const unsigned long long n_warps = ((unsigned long long)gridDim.x * blockDim.x) >> 5;
   unsigned long long per_warp = (n + n_warps - 1) / n_warps;
-  if (per_warp < (unsigned long long)lanes_min) per_warp = (unsigned long long)lanes_min;
   if (per_warp > 32) per_warp = 32;
   if (lane >= per_warp) return;
   const unsigned long long slot0 = (((unsigned long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5) * per_warp + lane;
@@ -1338,7 +1320,7 @@ __global__ void __launch_bounds__(128, GPUD_MATCH_BLOCKS) k_scan_match(ScanBuf b
     // every pattern starts with this family's anchor literal and `a` is the unit's first such anchor: start there
     const bool ok = (fam == kFamS) ? sxid_match_unit(b, a, ue, T, &h) : xid_match_unit(b, a0, ue, T, &h);
     if (!ok) return false;
-    h.unit_index = 0;                              // filled by k_scan_unit_index (one warp per hit, cooperative count)
+    h.unit_index = 0;                              // filled by k_scan_finish (one warp per hit, cooperative count)
     h.unit_offset = us;
     h.kmsg_priority = (int32_t)k_prio;
     h.kmsg_seq = k_seq;
@@ -1394,11 +1376,8 @@ __device__ __forceinline__ void unit_index_of_hit(const ScanBuf& b, int mode, co
   if (lane == 0) hits[hi].unit_index = (int64_t)(before + cnt);
 }
 
-// detailFromNVLinkInfo for the extended hits of a scan, one WARP per hit: the three table searches (sub-code + status
-// override, sub-code detail, the 94 NVLink rules with their alias lists) are spread over the lanes and the first match in
-// table order is the minimum matching index - the same answer as the sequential loops of classify_extended(), which a
-// single thread of the match kernel spent about as long on as on the whole regex automaton.
-// The same warp first numbers the hit's unit (unit_index_of_hit), so one launch finishes every hit of the scan.
+// One warp per hit: the hit's unit number (unit_index_of_hit), then detailFromNVLinkInfo for an extended hit, so one launch
+// finishes every hit of the scan.
 __global__ void __launch_bounds__(256) k_scan_finish(ScanBuf b, int mode, const uint32_t* __restrict__ chunk_local, const unsigned long long* __restrict__ tile_base,
                                                       const gpud_tables* __restrict__ T, gpud_xid_hit* hits, const unsigned long long* __restrict__ n_hits,
                                                       unsigned long long hit_cap) {
@@ -1412,72 +1391,34 @@ __global__ void __launch_bounds__(256) k_scan_finish(ScanBuf b, int mode, const 
     const int event_type = h->event_type;                            // asked for together with the unit offset (the store below would pin it behind)
     unit_index_of_hit(b, mode, chunk_local, tile_base, hits, hi, lane);
     if (event_type != kPendingExtended) continue;                    // warp-uniform
-    const int xid = h->code, sub = h->sub_code;
-    const uint32_t st = h->error_status, intr = h->intrinfo;
-    char unit[40];
-    __align__(4) char norm[GPUD_T_ALIAS_LEN];
-    for (int i = 0; i < 40; ++i) unit[i] = h->unit_name[i];
-    unit[39] = 0;
-    for (int i = 0; i < GPUD_T_ALIAS_LEN; ++i) norm[i] = 0;         // NUL-padded: compared word by word below
-    normalize_unit(unit, norm);
-    const unsigned* norm_words = reinterpret_cast<const unsigned*>(norm);
-    int i_status = 0x7fffffff, i_sub = 0x7fffffff, i_sub0 = 0x7fffffff, i_rule = 0x7fffffff;
-    for (int i = lane; i < T->n_by_status; i += 32)
-      if (i < i_status && T->by_status[i].xid == xid && T->by_status[i].sub_code == sub && T->by_status[i].error_status == st) i_status = i;
-    for (int i = lane; i < T->n_by_sub; i += 32) {
-      if (T->by_sub[i].xid != xid) continue;
-      if (i < i_sub && T->by_sub[i].sub_code == sub) i_sub = i;
-      if (i < i_sub0 && T->by_sub[i].sub_code == 0) i_sub0 = i;
-    }
-    for (int i = lane; i < T->n_rules; i += 32) {
-      const gpud_t_rule& r = T->rules[i];
-      if (i >= i_rule || r.xid != xid || r.error_status != st) continue;
-      if (!unit_matches_words(r, norm_words)) continue;
-      if (pattern_ok(r.v2_kind, r.v2_care, r.v2_val, intr) || pattern_ok(r.v1_kind, r.v1_care, r.v1_val, intr)) i_rule = i;
-    }
-    i_status = __reduce_min_sync(kFull, i_status);
-    i_sub = __reduce_min_sync(kFull, i_sub);
-    i_sub0 = __reduce_min_sync(kFull, i_sub0);
-    i_rule = __reduce_min_sync(kFull, i_rule);
-    if (lane == 0) {
-      const gpud_t_detail base = T->xid[xid];
-      gpud_t_detail d = base;
-      int variant = 0;
-      if (i_status != 0x7fffffff) { d = T->by_status[i_status].d; variant = T->by_status[i_status].variant; }          // xid.go:97-107
-      else if (T->has_sub_map[xid]) {                                                                                   // xid.go:79-93
-        const int k = i_sub != 0x7fffffff ? i_sub : i_sub0;
-        if (k != 0x7fffffff) { d = T->by_sub[k].d; variant = T->by_sub[k].variant; }
-      }
-      h->rule_index = -1;
-      if (i_rule != 0x7fffffff) {                                                                                       // xid.go:3099-3114
-        const gpud_t_rule& r = T->rules[i_rule];
-        h->rule_index = i_rule;
-        h->flags |= GPUD_HIT_HAS_RULE;
-        if (r.rule_event != GPUD_EVENT_UNKNOWN) d.event = r.rule_event;
-        if (r.rule_n_actions > 0) { d.n_actions = 1; d.actions[0] = r.rule_action; d.actions[1] = d.actions[2] = d.actions[3] = 0; }
-      }
-      const int log_ev = h->severity_fatal ? GPUD_EVENT_FATAL : GPUD_EVENT_WARNING;   // eventTypeFromLogSeverity
-      if (log_ev > d.event) d.event = (int8_t)log_ev;
-      if (d.n_actions < 0) { d.n_actions = base.n_actions; for (int i = 0; i < 4; ++i) d.actions[i] = base.actions[i]; }
-      set_detail(h, d);
-      h->detail_variant = variant;
-    }
+    detail_from_nvlink_info(T, h, lane);
     __syncwarp();
   }
 }
 
+// gpud_xid_classify: one warp per hit, so extended hits take the scan's own table searches.  Every branch is decided by the hit,
+// i.e. the same for the whole warp.
 __global__ void k_classify(const gpud_tables* __restrict__ T, gpud_xid_hit* hits, int64_t n) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int lane = threadIdx.x & 31;
+  const int64_t i = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (i >= n) return;
-  gpud_xid_hit h = hits[i];
-  if (h.kind != GPUD_KIND_XID && h.kind != GPUD_KIND_SXID) return;   // the extra matchers carry no catalog detail
-  h.unit_name[39] = 0;
-  bool ok;
-  if (h.kind == GPUD_KIND_SXID) ok = classify_sxid(T, &h);
-  else if (h.flags & GPUD_HIT_EXTENDED) { h.sub_code = (int32_t)((h.intrinfo >> 20) & 0x3F); ok = classify_extended(T, &h); }
-  else ok = classify_plain_xid(T, &h);
-  if (!ok) { h.event_type = GPUD_EVENT_UNKNOWN; h.n_actions = -1; h.rule_index = -1; h.detail_variant = 0; }
-  hits[i] = h;
+  gpud_xid_hit* h = hits + i;
+  const int kind = h->kind, xid = h->code;
+  if (kind != GPUD_KIND_XID && kind != GPUD_KIND_SXID) return;       // the extra matchers carry no catalog detail
+  const bool extended = kind == GPUD_KIND_XID && (h->flags & GPUD_HIT_EXTENDED);
+  bool ok = true;
+  if (lane == 0) {
+    h->unit_name[39] = 0;
+    if (kind == GPUD_KIND_SXID) ok = classify_sxid(T, h);
+    else if (extended) h->sub_code = (int32_t)((h->intrinfo >> 20) & 0x3F);
+    else ok = classify_plain_xid(T, h);
+  }
+  if (extended) {
+    ok = xid > 0 && xid < GPUD_T_MAX_XID && T->xid[xid].present;
+    __syncwarp();                                                    // lane 0's sub_code is visible to the whole warp
+    if (ok) detail_from_nvlink_info(T, h, lane);
+  }
+  if (lane == 0 && !ok) { h->event_type = GPUD_EVENT_UNKNOWN; h->n_actions = -1; h->rule_index = -1; h->detail_variant = 0; }
 }
 
 }  // namespace
@@ -1700,7 +1641,7 @@ static int32_t scan_launch(gpud_ctx* ctx, gpud_scan_state* s, const uint8_t* d_b
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_scan_match, 128, 0) != cudaSuccess || nb < 1) nb = 4;
     return nb;
   }();
-  GPUD_CUDA(ctx, launch_chain(!phased, k_scan_match, dim3((unsigned)(ctx->sm_count * match_blocks)), dim3(128), st, b, (int)mode, (int)kMatchLanes,
+  GPUD_CUDA(ctx, launch_chain(!phased, k_scan_match, dim3((unsigned)(ctx->sm_count * match_blocks)), dim3(128), st, b, (int)mode,
                               (const unsigned long long*)s->d_cands, (const unsigned long long*)s->d_side, side_cap, (const unsigned long long*)(s->d_counters + 0),
                               (unsigned long long)s->cand_cap, (const uint32_t*)s->d_chunk_local, (const unsigned long long*)s->d_tile_base, (const gpud_tables*)s->d_tables,
                               s->d_hits, (unsigned long long)s->hit_cap, s->d_counters + 1));
@@ -1882,7 +1823,7 @@ extern "C" int32_t gpud_xid_classify(gpud_ctx* ctx, int32_t dev, gpud_xid_hit* h
   if (rc) return rc;
   GPUD_CUDA(ctx, grow(&s->d_hits, &s->hit_cap, (size_t)std::max<int64_t>(n, 1024)));
   GPUD_CUDA(ctx, cudaMemcpyAsync(s->d_hits, hits, (size_t)n * sizeof(gpud_xid_hit), cudaMemcpyHostToDevice, s->stream));
-  k_classify<<<(unsigned)((n + 127) / 128), 128, 0, s->stream>>>(s->d_tables, s->d_hits, n);
+  k_classify<<<(unsigned)((n + 3) / 4), 128, 0, s->stream>>>(s->d_tables, s->d_hits, n);   // one warp per hit
   GPUD_CUDA(ctx, cudaGetLastError());
   GPUD_CUDA(ctx, cudaMemcpyAsync(hits, s->d_hits, (size_t)n * sizeof(gpud_xid_hit), cudaMemcpyDeviceToHost, s->stream));
   GPUD_CUDA(ctx, cudaStreamSynchronize(s->stream));

@@ -370,6 +370,46 @@ def test_classify_entry(ctx):
             assert h.event_type == d["event_type"] and list(h.actions)[:max(h.n_actions, 0)] == d["actions"]
 
 
+def test_classify_agrees_with_scan(ctx):
+    """gpud_xid_classify gives back the scan's own Xid / SXid hits byte for byte once every field classification writes is cleared:
+    the rule lookup of the ABI entry across the NVLink rule table, against the scan's"""
+    EXTENDED, HAS_RULE = 0x1, 0x8
+    lines = synth.hit_lines() + synth.EDGE_LINES
+    recs = ["%d,%d,%d,-;%s" % (i % 8, 100 + i, 1000 * i, l.replace("\n", "\\x0a")) for i, l in enumerate(lines)]
+    hits = ctx.kmsg_scan("\n".join(lines).encode())[0] + ctx.kmsg_scan("\n".join(recs).encode(), mode=g.SCAN_RAW_KMSG)[0]
+    want = [g.XidHit.from_buffer_copy(bytes(h)) for h in hits if h.kind in (1, 2)]
+    cleared = []
+    for w in want:
+        h = g.XidHit.from_buffer_copy(bytes(w))
+        h.event_type = h.n_actions = 0
+        h.actions[:] = [0, 0, 0, 0]
+        h.rule_index = h.detail_variant = -7
+        h.flags &= ~HAS_RULE
+        if h.flags & EXTENDED:
+            h.sub_code = 0
+        cleared.append(h)
+    for got, w in zip(ctx.classify(cleared), want):
+        assert bytes(got) == bytes(w), (got.as_dict(), w.as_dict())
+    ext = [h for h in want if h.kind == 1 and h.flags & EXTENDED]
+    aliases = {O.normalize_unit(a) for r in O.NVLINK_RULES for a in O.unit_aliases(r["Unit"])}
+    assert any(h.rule_index >= 0 for h in ext)
+    assert any(O.normalize_unit(h.unit_name.decode("latin-1")) not in aliases for h in ext)
+    # extended hits whose base code is not in the catalog: no detail, the sub-code is still derived; actions and flags stay
+    bad = []
+    for code in (0, -3, 133, 191, 192, 200):
+        h = g.XidHit()
+        h.kind, h.code, h.flags, h.intrinfo, h.error_status = 1, code, EXTENDED | 0x4, 0x00a00011, 0
+        h.event_type, h.n_actions, h.rule_index, h.detail_variant = 3, 2, 5, 2
+        h.actions[:] = [3, 1, 2, 4]
+        h.unit_name = b"RLW_REMAP" + b"x" * 31                     # no terminator in the inline copy
+        bad.append(h)
+    for got, h in zip(ctx.classify(bad), bad):
+        w = g.XidHit.from_buffer_copy(bytes(h))
+        w.sub_code, w.event_type, w.n_actions, w.rule_index, w.detail_variant = 10, 0, -1, -1, 0
+        C.memmove(C.addressof(w) + g.XidHit.unit_name.offset + 39, b"\0", 1)
+        assert bytes(got) == bytes(w), (h.code, got.as_dict())
+
+
 # ------------------------------------------------------------------------------------------------ ring
 def _check_windows(got, x, W, thr, alpha=0.0, qn=99, qd=100):
     F = x.shape[1]
