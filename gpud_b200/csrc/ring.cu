@@ -773,6 +773,13 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, kCtasPerSM) k_window_redu
 // rows of 128 consecutive windows are scanned with a decayed Kogge-Stone prefix (S_t += d^off S_{t-off}), the carry
 // crosses rows through shared memory; only the last window can have a different decay.
 // ---------------------------------------------------------------------------------------------
+// w * c + s for a decay weight w >= 0 and a carried value c.  The powers of d = (1-alpha)^W underflow to 0 (alpha = 0.5, W = 1000:
+// d^2 is 0), but an infinite EMA stays infinite under the recurrence however small the weight: 0 * inf would make it NaN.
+// GUARD = false: no weight the kernel uses can be 0 (the host checks d^128), plain fma.
+template <bool GUARD>
+__device__ __forceinline__ double decay_fma(double w, double c, double s) { return (GUARD && w == 0.0 && isinf(c)) ? c + s : fma(w, c, s); }
+
+template <bool GUARD>
 __global__ void __launch_bounds__(128) k_ema_carry(const double* __restrict__ part, const double* __restrict__ ring, int64_t cap,
                                                     int64_t start, int F, int nw, double d_full, double d_last,
                                                     double* __restrict__ out_ema) {
@@ -797,21 +804,21 @@ __global__ void __launch_bounds__(128) k_ema_carry(const double* __restrict__ pa
 #pragma unroll
     for (int i = 0; i < 5; ++i) {
       const double o = __shfl_up_sync(kFull, sacc, 1 << i);
-      if (lane >= (1 << i)) sacc = fma(dp[i], o, sacc);
+      if (lane >= (1 << i)) sacc = decay_fma<GUARD>(dp[i], o, sacc);
     }
     if (lane == 31) s_warp[wid] = sacc;
     __syncthreads();
     // carry of the preceding warps of this row: sum_{v < wid} d^(32 (wid-1-v)) * s_warp[v], applied with d^(lane+1)
     double pre = 0.0;
-    for (int v2 = 0; v2 < wid; ++v2) pre = fma(pre, dp[5], s_warp[v2]);
-    sacc = fma(lane_pow, pre, sacc);
-    const double e = fma(my_pow, s_carry, sacc);
+    for (int v2 = 0; v2 < wid; ++v2) pre = decay_fma<GUARD>(dp[5], pre, s_warp[v2]);
+    sacc = decay_fma<GUARD>(lane_pow, pre, sacc);
+    const double e = decay_fma<GUARD>(my_pow, s_carry, sacc);
     if (w < n_main) O[w] = e;
     __syncthreads();
     if (w == min(n_main, (row + 1) * 128) - 1) s_carry = e;   // the row's last valid window carries into the next row
     __syncthreads();
   }
-  if (t == 0) O[nw - 1] = fma(d_last, s_carry, __ldg(P + nw - 1));
+  if (t == 0) O[nw - 1] = decay_fma<GUARD>(d_last, s_carry, __ldg(P + nw - 1));
 }
 
 }  // namespace
@@ -1113,7 +1120,9 @@ static int32_t launch_windows(gpud_ring* r, WinParams p) {
   const int64_t c_wrap = p.cap - p.start;                 // chronological index of the sample stored at physical column 0
   if (p.start > 0 && c_wrap < p.count && (c_wrap % p.W) != 0) p.w_skip[p.n_tail++] = (int)(c_wrap / p.W);
   const int jf = p.W >> 6;
-  const bool special = (jf == 15 || jf == 16) && p.nw > 1;
+  // <ALIGNED, 15> always treats pair 15 as the partially valid one: W = 960 has no sample there, and the EMA Horner step that
+  // pair still takes would decay the window's partial once too often, so W = 960 runs the generic code
+  const bool special = (jf == 16 || (jf == 15 && (p.W & 63) != 0)) && p.nw > 1;
   if (special && (p.count % p.W) != 0 && (p.n_tail == 0 || p.w_skip[0] != p.nw - 1)) p.w_skip[p.n_tail++] = p.nw - 1;   // trailing partial window
   cudaError_t e;
   if (special && jf == 15 && !RANGE) e = launch_one<true, 15, false>(r, p, units);   // the range pass always runs W' = 1024 (jf = 16)
@@ -1121,6 +1130,15 @@ static int32_t launch_windows(gpud_ring* r, WinParams p) {
   else e = launch_one<true, -1, RANGE>(r, p, units);
   GPUD_CUDA(r->ctx, e);
   return GPUD_OK;
+}
+
+// The carry's smallest decay weight is d^128 (d = (1-alpha)^W); the others are larger powers of d, or d_last >= d.  With the default
+// alpha, d >= e^-2 and d^128 is nowhere near underflow; a larger alpha can drive weights to 0, and then the guarded instantiation
+// keeps an infinite carry infinite (the margin to 2^-1074 covers pow() and the squarings rounding differently on the device).
+static void launch_ema_carry(gpud_ring* r, const double* part, int64_t start, int nw, int W, int m_last, double* out) {
+  const double d_full = pow(1.0 - r->alpha, (double)W), d_last = pow(1.0 - r->alpha, (double)m_last);
+  if (pow(d_full, 128.0) < 0x1p-900) k_ema_carry<true><<<r->F, 128, 0, r->stream>>>(part, r->d_ring, r->cap, start, r->F, nw, d_full, d_last, out);
+  else k_ema_carry<false><<<r->F, 128, 0, r->stream>>>(part, r->d_ring, r->cap, start, r->F, nw, d_full, d_last, out);
 }
 
 extern "C" int32_t gpud_ring_reduce(gpud_ring* r) {
@@ -1140,9 +1158,7 @@ extern "C" int32_t gpud_ring_reduce(gpud_ring* r) {
   { int32_t rc = launch_windows<false>(r, p); if (rc) return rc; }
   cudaEventRecord(r->ev_k[1], r->stream);
   const int m_last = (int)(count - (int64_t)(p.nw - 1) * r->W);
-  k_ema_carry<<<r->F, 128, 0, r->stream>>>(r->d_part, r->d_ring, r->cap, p.start, r->F, p.nw,
-                                                        pow(1.0 - r->alpha, (double)r->W), pow(1.0 - r->alpha, (double)m_last),
-                                                        r->d_res[GPUD_OP_EMA]);
+  launch_ema_carry(r, r->d_part, p.start, p.nw, r->W, m_last, r->d_res[GPUD_OP_EMA]);
   GPUD_CUDA(r->ctx, cudaGetLastError());
   cudaEventRecord(r->ev_k[2], r->stream);
   r->reduced_nw = p.nw;
@@ -1257,8 +1273,7 @@ int32_t gpud_ring_range_pass(gpud_ring* r, const gpud_range_view* v) {
   p.piv = v->piv; p.w_cls = v->w_cls; p.lists = v->lists; p.fill = v->fill; p.list_cap = v->list_cap;
   { int32_t rc = v->sampled ? launch_windows<true>(r, p) : launch_windows<false>(r, p); if (rc) return rc; }
   const int m_last = (int)(v->n - (int64_t)(v->nw - 1) * v->Wp);
-  k_ema_carry<<<r->F, 128, 0, r->stream>>>(r->d_rng[4], r->d_ring, r->cap, v->start, r->F, v->nw, pow(1.0 - r->alpha, (double)v->Wp),
-                                                        pow(1.0 - r->alpha, (double)m_last), r->d_rng[3]);
+  launch_ema_carry(r, r->d_rng[4], v->start, v->nw, v->Wp, m_last, r->d_rng[3]);
   GPUD_CUDA(r->ctx, cudaGetLastError());
   return GPUD_OK;
 }
