@@ -26,14 +26,6 @@ extern "C" int32_t gpud_ctx_create(const int32_t* cuda_devs, int32_t n, gpud_ctx
   ctx->fabric_tables.assign(n, nullptr);
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, ctx->devs[0]) == cudaSuccess) ctx->sm_count = prop.multiProcessorCount;
-  // per-call scratch comes from the stream-ordered pool (cudaMallocAsync); keep up to 256 MiB cached across synchronisations,
-  // otherwise every call that ends in a sync hands its scratch back to the driver and the next one pays for it again
-  for (int i = 0; i < n; ++i) {
-    cudaMemPool_t pool;
-    unsigned long long keep = 256ull << 20;
-    if (cudaDeviceGetDefaultMemPool(&pool, ctx->devs[i]) == cudaSuccess) cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
-    cudaGetLastError();
-  }
   *out = ctx;
   return GPUD_OK;
 }

@@ -14,6 +14,7 @@
 
 struct gpud_scan_state;   // kmsg_scan.cu
 struct gpud_comm_state;   // fabric.cu
+struct gpud_range_state;  // select.cu
 
 struct gpud_ctx {
   std::vector<int> devs;
@@ -27,6 +28,46 @@ struct gpud_ctx {
   unsigned fabric_epoch = 0;            // gathers completed or begun on this ctx's tables (arrival counters expect epoch * n)
   bool fabric_dirty = false;            // the last gather did not finish: counters are re-zeroed before the next one
 };
+
+// The device ring (ring.cu); its whole-range reduce (select.cu) keeps its own state behind `range`.
+struct gpud_ring {
+  gpud_ctx* ctx = nullptr;
+  int dev = 0;
+  int F = 0, W = 0;
+  int64_t cap = 0;
+  double alpha = 0;
+  int q_num = 99, q_den = 100;
+  int64_t total = 0;
+  double* d_ring = nullptr;
+  double* d_thr = nullptr;
+  double* d_pw = nullptr;
+  int64_t nw_max = 0;
+  double* d_res[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
+  uint32_t* d_nover = nullptr;
+  double* d_part = nullptr;
+  unsigned long long* d_cursor = nullptr;   // window-kernel work cursors: [0..1] gpud_ring_reduce, [2..3] the range pass
+  int64_t reduced_nw = -1;
+  cudaStream_t own_stream = nullptr, stream = nullptr;
+  double* h_stage[2] = {nullptr, nullptr};
+  double* d_stage[2] = {nullptr, nullptr};
+  cudaEvent_t ev_stage[2] = {nullptr, nullptr};    // d_stage[i] is free again (its append has run)
+  cudaEvent_t ev_copied[2] = {nullptr, nullptr};   // the H2D into d_stage[i] has landed
+  cudaStream_t copy_stream = nullptr;
+  int64_t stage_rows = 0;
+  double* d_sample = nullptr;      // [F][smp_slots]: column c with c % 2^smp_shift == 2^smp_shift / 2 lives at slot c >> smp_shift (kept by the append kernel)
+  int smp_shift = 0;
+  int64_t smp_slots = 0;
+  int sm_count = 132;
+  int cta_reserve = 0;           // CTA slots the persistent window grid leaves free for kernels of other streams (gpud_ring_set_cta_reserve)
+  gpud_range_state* range = nullptr;                   // created by the first gpud_ring_reduce_range
+  cudaEvent_t ev_k[3] = {nullptr, nullptr, nullptr};   // around the two kernels of the last reduce (bench roofline)
+};
+
+inline int64_t ring_count(const gpud_ring* r) { return r->total < r->cap ? r->total : r->cap; }
+inline int64_t ring_start(const gpud_ring* r) { return r->total <= r->cap ? 0 : r->total % r->cap; }
+
+#define GPUD_MAX_WINDOW 1024           /* longest window of the window kernel: 32 lanes x 32 elements held in registers */
+#define GPUD_RANGE_SAMPLE_MAX 8192     /* keys per field in the sample the range pivots come from: sizes the ring's sample ring */
 
 inline int32_t gpud_fail(gpud_ctx* ctx, int32_t code, const char* fmt, ...) __attribute__((format(printf, 3, 4)));
 inline int32_t gpud_fail(gpud_ctx* ctx, int32_t code, const char* fmt, ...) {
@@ -55,6 +96,18 @@ inline int gpud_dev_slot(gpud_ctx* ctx, int dev) {
   return -1;
 }
 
+// Device scratch that is grown on demand and kept: afterwards *p holds at least `need` elements (*cap counts them).
+template <typename T>
+inline cudaError_t gpud_grow(T** p, size_t* cap, size_t need) {
+  if (need <= *cap) return cudaSuccess;
+  cudaFree(*p);
+  *p = nullptr;
+  *cap = 0;
+  cudaError_t e = cudaMalloc(p, need * sizeof(T));
+  if (e == cudaSuccess) *cap = need;
+  return e;
+}
+
 // ---- device helpers --------------------------------------------------------------------------
 #ifdef __CUDACC__
 // IEEE-754 totalOrder key (oracle/SPEC.md): unsigned compare of the key == totalOrder of the doubles.
@@ -66,34 +119,22 @@ __host__ __device__ __forceinline__ unsigned long long gpud_f64_key(unsigned lon
 __host__ __device__ __forceinline__ unsigned long long gpud_key_f64bits(unsigned long long key) {
   return key ^ ((key >> 63) ? 0x8000000000000000ull : ~0ull);
 }
+// Nearest rank of quantile q = q_num / q_den among n keys (oracle/SPEC.md), counted from the top: k = n - clamp(ceil(n q), 1, n) + 1.
+__host__ __device__ __forceinline__ long long gpud_rank_from_top(long long n, int q_num, int q_den) {
+  long long r = (n * q_num + q_den - 1) / q_den;
+  r = r < 1 ? 1 : (r > n ? n : r);
+  return n - r + 1;
+}
 #endif
 
-// view of a ring range around the per-window pass (ring.cu <-> select.cu)
-#define GPUD_RANGE_SAMPLED_MIN 65536   /* ranges at least this long take the sampled-pivot single pass */
-#define GPUD_RANGE_LIST_CAP 65536      /* keys between the pivots kept per field */
-#define GPUD_RANGE_SAMPLE_MAX 8192     /* keys per field in the sample the pivots come from */
-struct gpud_range_view {
-  const double* ring; int F; int64_t cap, start, n; int Wp, nw;
-  const double *w_min, *w_max, *w_mean, *w_ema; const uint32_t* w_nover;
-  int q_num, q_den; cudaStream_t stream; gpud_ctx* ctx; int dev, sm_count;
-  int sampled;                         // 1: the pass classifies against `piv` and fills `lists`
-  unsigned list_cap;
-  double* piv;                         // [F][2] lo, hi
-  unsigned* fill;                      // [F]
-  uint4* w_cls;                        // [F][nw] {above hi, == hi, == lo, strictly inside}
-  unsigned long long* lists;           // [F][list_cap]
-  const double* sample;                // the ring's own sample ring [F][smp_slots] (ring.cu k_ring_append)
-  int smp_shift; int64_t smp_slots;
-  cudaEvent_t ev[3];
-};
-int32_t gpud_ring_range_prepare(gpud_ring* r, int64_t n, gpud_range_view* v);
-int32_t gpud_ring_range_pass(gpud_ring* r, const gpud_range_view* v);
-void gpud_ring_range_note(gpud_ring* r, bool sampled, unsigned fields_open, const int* reasons /*[GPUD_RANGE_N_OPEN_REASONS]*/);
-void gpud_ring_quantile(gpud_ring* r, int* q_num, int* q_den);
+// ring.cu: the window pass and the EMA carry over chronological samples [start, start + n) of the ring with window Wp, into the
+// caller's buffers w[0..4] = per-window min, max, mean, EMA, EMA partial sums and w_nover, each [F][ceil(n / Wp)].  With piv the
+// pass also classifies every sample against the field's pivots lo = piv[2f], hi = piv[2f + 1]: class counts {above hi, == hi,
+// == lo, strictly inside} per window into w_cls, the keys strictly inside into lists [F][list_cap] behind the counters fill [F].
+int32_t gpud_ring_window_pass(gpud_ring* r, int64_t start, int64_t n, int Wp, double* const w[5], uint32_t* w_nover,
+                              const double* piv, uint4* w_cls, unsigned long long* lists, unsigned* fill, unsigned list_cap);
 
 void gpud_scan_state_free(gpud_scan_state*);
 void gpud_comm_state_free(gpud_comm_state*);
+void gpud_range_state_free(gpud_range_state*);
 void gpud_parallel_memcpy(void* dst, const void* src, size_t n);
-
-// ring.cu: the ring's field count (the pollers check their row width against it before pushing)
-int gpud_ring_n_fields(const gpud_ring* r);

@@ -1481,17 +1481,6 @@ static int32_t scan_state_get(gpud_ctx* ctx, int dev, gpud_scan_state** out) {
   return GPUD_OK;
 }
 
-template <typename T>
-static cudaError_t grow(T** p, size_t* cap, size_t need) {
-  if (need <= *cap) return cudaSuccess;
-  cudaFree(*p);
-  *p = nullptr;
-  *cap = 0;
-  cudaError_t e = cudaMalloc(p, need * sizeof(T));
-  if (e == cudaSuccess) *cap = need;
-  return e;
-}
-
 static const ExtTab& ext_tab() {
   static ExtTab t;
   static bool ready = false;
@@ -1600,13 +1589,13 @@ static int32_t scan_launch(gpud_ctx* ctx, gpud_scan_state* s, const uint8_t* d_b
                            cudaStream_t st) {
   const int64_t n_chunks = std::max<int64_t>(1, (len + kChunk - 1) / kChunk);
   const int64_t n_tiles = (n_chunks + 1023) / 1024;
-  GPUD_CUDA(ctx, grow(&s->d_chunk_sep, &s->chunk_sep_cap, (size_t)n_chunks));
-  GPUD_CUDA(ctx, grow(&s->d_chunk_local, &s->chunk_local_cap, (size_t)n_chunks));
-  GPUD_CUDA(ctx, grow(&s->d_tile_base, &s->tile_cap, (size_t)n_chunks / 1024 + 2));
-  GPUD_CUDA(ctx, grow(&s->d_cands, &s->cand_cap, (size_t)(len / 4 + 1024)));
-  GPUD_CUDA(ctx, grow(&s->d_hits, &s->hit_cap, (size_t)std::max<int64_t>(hit_cap_req, 1024)));
+  GPUD_CUDA(ctx, gpud_grow(&s->d_chunk_sep, &s->chunk_sep_cap, (size_t)n_chunks));
+  GPUD_CUDA(ctx, gpud_grow(&s->d_chunk_local, &s->chunk_local_cap, (size_t)n_chunks));
+  GPUD_CUDA(ctx, gpud_grow(&s->d_tile_base, &s->tile_cap, (size_t)n_chunks / 1024 + 2));
+  GPUD_CUDA(ctx, gpud_grow(&s->d_cands, &s->cand_cap, (size_t)(len / 4 + 1024)));
+  GPUD_CUDA(ctx, gpud_grow(&s->d_hits, &s->hit_cap, (size_t)std::max<int64_t>(hit_cap_req, 1024)));
   GPUD_CUDA(ctx, cudaMemsetAsync(s->d_counters, 0, (4 + 2 * kSortBins) * sizeof(unsigned long long), st));
-  GPUD_CUDA(ctx, grow(&s->d_side, &s->side_cap, std::min<size_t>(s->cand_cap, (size_t)1 << 20)));
+  GPUD_CUDA(ctx, gpud_grow(&s->d_side, &s->side_cap, std::min<size_t>(s->cand_cap, (size_t)1 << 20)));
   if (len == 0) {
     GPUD_CUDA(ctx, cudaMemsetAsync(s->d_chunk_sep, 0, sizeof(uint32_t), st));
   }
@@ -1718,7 +1707,7 @@ extern "C" int32_t gpud_kmsg_scan(gpud_ctx* ctx, int32_t dev, const uint8_t* buf
   gpud_scan_state* s;
   int32_t rc = scan_state_get(ctx, dev, &s);
   if (rc) return rc;
-  GPUD_CUDA(ctx, grow(&s->d_buf, &s->buf_cap, (size_t)len + 64));
+  GPUD_CUDA(ctx, gpud_grow(&s->d_buf, &s->buf_cap, (size_t)len + 64));
   if (len) {
     cudaPointerAttributes attr;
     bool pinned = false;
@@ -1821,7 +1810,7 @@ extern "C" int32_t gpud_xid_classify(gpud_ctx* ctx, int32_t dev, gpud_xid_hit* h
   gpud_scan_state* s;
   int32_t rc = scan_state_get(ctx, dev, &s);
   if (rc) return rc;
-  GPUD_CUDA(ctx, grow(&s->d_hits, &s->hit_cap, (size_t)std::max<int64_t>(n, 1024)));
+  GPUD_CUDA(ctx, gpud_grow(&s->d_hits, &s->hit_cap, (size_t)std::max<int64_t>(n, 1024)));
   GPUD_CUDA(ctx, cudaMemcpyAsync(s->d_hits, hits, (size_t)n * sizeof(gpud_xid_hit), cudaMemcpyHostToDevice, s->stream));
   k_classify<<<(unsigned)((n + 3) / 4), 128, 0, s->stream>>>(s->d_tables, s->d_hits, n);   // one warp per hit
   GPUD_CUDA(ctx, cudaGetLastError());

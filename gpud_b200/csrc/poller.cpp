@@ -134,7 +134,7 @@ extern "C" int32_t gpud_poller_create(gpud_ctx* ctx, int32_t dev, gpud_ring* rin
   if (!ctx || !ring || !out) return GPUD_E_INVALID;
   Nvml* N = nvml();
   if (!N) return gpud_fail(ctx, GPUD_E_UNSUPPORTED, "libnvidia-ml.so.1 not available (no driver on this host)");
-  if (gpud_ring_n_fields(ring) != GPUD_POLL_N_FIELDS) return gpud_fail(ctx, GPUD_E_INVALID, "the gauge poller needs a ring of %d fields (this one has %d)", GPUD_POLL_N_FIELDS, gpud_ring_n_fields(ring));
+  if (ring->F != GPUD_POLL_N_FIELDS) return gpud_fail(ctx, GPUD_E_INVALID, "the gauge poller needs a ring of %d fields (this one has %d)", GPUD_POLL_N_FIELDS, ring->F);
   char bus[32];
   GPUD_CUDA(ctx, cudaDeviceGetPCIBusId(bus, sizeof bus, dev));
   nvmlDevice_t h;
@@ -652,7 +652,7 @@ extern "C" int32_t gpud_poller_poll_fields(gpud_poller* p, gpud_ring* ring, int6
   if (!p || !ring || n_polls < 0 || interval_us < 0) return GPUD_E_INVALID;
   Nvml* N = nvml();
   if (!N || !N->field_values) return GPUD_E_UNSUPPORTED;
-  if (gpud_ring_n_fields(ring) != GPUD_FIELD_ROW_N) return gpud_fail(p->ctx, GPUD_E_INVALID, "the field-row source needs a ring of %d fields (this one has %d)", GPUD_FIELD_ROW_N, gpud_ring_n_fields(ring));
+  if (ring->F != GPUD_FIELD_ROW_N) return gpud_fail(p->ctx, GPUD_E_INVALID, "the field-row source needs a ring of %d fields (this one has %d)", GPUD_FIELD_ROW_N, ring->F);
   if (!p->field_rows) {
     if (cudaMallocHost(&p->field_rows, (size_t)p->cap_rows * GPUD_FIELD_ROW_N * sizeof(uint64_t)) != cudaSuccess) return gpud_fail(p->ctx, GPUD_E_CUDA, "pinned field rows");
   }
@@ -775,7 +775,7 @@ extern "C" int32_t gpud_poller_poll_gpm(gpud_poller* p, gpud_ring* ring, int64_t
   if (!p || !ring || n_polls < 0 || sample_ms < 0) return GPUD_E_INVALID;
   Nvml* N = nvml();
   if (!N || !N->gpm_support || !N->gpm_alloc || !N->gpm_free || !N->gpm_sample || !N->gpm_metrics) return GPUD_E_UNSUPPORTED;
-  if (gpud_ring_n_fields(ring) != GPUD_GPM_N) return gpud_fail(p->ctx, GPUD_E_INVALID, "the GPM source needs a ring of %d fields (this one has %d)", GPUD_GPM_N, gpud_ring_n_fields(ring));
+  if (ring->F != GPUD_GPM_N) return gpud_fail(p->ctx, GPUD_E_INVALID, "the GPM source needs a ring of %d fields (this one has %d)", GPUD_GPM_N, ring->F);
   int32_t sup = 0;
   int32_t r = gpud_poller_gpm_supported(p, &sup);
   if (r) return r;

@@ -21,7 +21,6 @@
 
 namespace {
 
-constexpr int kMaxWindow = 1024;      // 32 lanes x 32 elements held in registers
 #ifndef GPUD_WARPS_PER_BLOCK
 #define GPUD_WARPS_PER_BLOCK 8
 #endif
@@ -598,6 +597,7 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
       // ---- exact order statistic: k-th largest, k = m - ceil(m q) + 1; the maximum falls out of the same candidate set ----
       int k = p.k_full;
       if (JF < 0 && m != p.W) {
+        // gpud_rank_from_top written out: calling it here changes the register allocation of every instantiation, the hot one too
         long long r = ((long long)m * p.q_num + p.q_den - 1) / p.q_den;
         r = r < 1 ? 1 : (r > m ? m : r);
         k = m - (int)r + 1;
@@ -824,63 +824,13 @@ __global__ void __launch_bounds__(128) k_ema_carry(const double* __restrict__ pa
 }  // namespace
 
 // =================================================================================================
-// host side
+// host side (struct gpud_ring: internal.h)
 // =================================================================================================
-struct gpud_ring {
-  gpud_ctx* ctx = nullptr;
-  int dev = 0;
-  int F = 0, W = 0;
-  int64_t cap = 0;
-  double alpha = 0;
-  int q_num = 99, q_den = 100;
-  int64_t total = 0;
-  double* d_ring = nullptr;
-  double* d_thr = nullptr;
-  double* d_pw = nullptr;
-  int64_t nw_max = 0;
-  double* d_res[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  uint32_t* d_nover = nullptr;
-  double* d_part = nullptr;
-  unsigned long long* d_cursor = nullptr;   // window-kernel work cursors: [0..1] gpud_ring_reduce, [2..3] the range pass
-  int64_t reduced_nw = -1;
-  cudaStream_t own_stream = nullptr, stream = nullptr;
-  double* h_stage[2] = {nullptr, nullptr};
-  double* d_stage[2] = {nullptr, nullptr};
-  cudaEvent_t ev_stage[2] = {nullptr, nullptr};    // d_stage[i] is free again (its append has run)
-  cudaEvent_t ev_copied[2] = {nullptr, nullptr};   // the H2D into d_stage[i] has landed
-  cudaStream_t copy_stream = nullptr;
-  int64_t stage_rows = 0;
-  double* d_sample = nullptr;      // [F][smp_slots]: column c with c % 2^smp_shift == 2^smp_shift / 2 lives at slot c >> smp_shift (kept by the append kernel)
-  int smp_shift = 0;
-  int64_t smp_slots = 0;
-  int sm_count = 132;
-  int cta_reserve = 0;           // CTA slots the persistent window grid leaves free for kernels of other streams (gpud_ring_set_cta_reserve)
-  double* d_rng[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};   // range-reduce scratch: per-window min,max,mean,ema,partials
-  size_t rng_bytes[5] = {0, 0, 0, 0, 0};
-  uint32_t* d_rng_nover = nullptr;
-  size_t rng_nover_bytes = 0;
-  uint4* d_rng_cls = nullptr;                          // sampled range pass: per-window class counts
-  size_t rng_cls_bytes = 0;
-  unsigned long long* d_rng_lists = nullptr;           // sampled range pass: per-field lists of the keys between the pivots
-  size_t rng_lists_bytes = 0;
-  double* d_rng_piv = nullptr;                         // [F][2] pivots, then [F] u32 list fill counters
-  size_t rng_piv_bytes = 0;
-  cudaEvent_t ev_rng[3] = {nullptr, nullptr, nullptr}; // start / after the range pass / end of the last sampled reduce_range
-  bool range_timed = false;
-  int range_reasons[GPUD_RANGE_N_OPEN_REASONS] = {0};
-  int range_fields_open = 0;                           // fields the last sampled reduce_range handed to the histogram path
-  int range_nw = 0;                                    // windows of the last reduce_range's pass (rows of d_rng_cls per field)
-  cudaEvent_t ev_k[3] = {nullptr, nullptr, nullptr};   // around the two kernels of the last reduce (bench roofline)
-};
-
-static int64_t ring_count(const gpud_ring* r) { return std::min(r->total, r->cap); }
-static int64_t ring_start(const gpud_ring* r) { return r->total <= r->cap ? 0 : r->total % r->cap; }
-
 extern "C" int32_t gpud_ring_create(gpud_ctx* ctx, int32_t dev, const gpud_ring_cfg* cfg, gpud_ring** out) {
   if (!ctx || !cfg || !out) return GPUD_E_INVALID;
   if (gpud_dev_slot(ctx, dev) < 0) return gpud_fail(ctx, GPUD_E_INVALID, "device %d is not part of this ctx", dev);
-  if (cfg->n_fields < 1 || cfg->window < 1 || cfg->window > kMaxWindow || cfg->capacity < cfg->window || (cfg->capacity & 1))
-    return gpud_fail(ctx, GPUD_E_INVALID, "ring cfg: need n_fields>=1, 1<=window<=%d, capacity even and >= window", kMaxWindow);
+  if (cfg->n_fields < 1 || cfg->window < 1 || cfg->window > GPUD_MAX_WINDOW || cfg->capacity < cfg->window || (cfg->capacity & 1))
+    return gpud_fail(ctx, GPUD_E_INVALID, "ring cfg: need n_fields>=1, 1<=window<=%d, capacity even and >= window", GPUD_MAX_WINDOW);
   double alpha = cfg->ema_alpha > 0 ? cfg->ema_alpha : std::min(2.0 / (cfg->window + 1.0), 0.9999);   // SPEC.md: default clamped
   if (!(alpha > 0.0) || alpha > 0.9999) return gpud_fail(ctx, GPUD_E_INVALID, "ema_alpha must be in (0, 0.9999]");
   int qn = cfg->q_num, qd = cfg->q_den;
@@ -939,10 +889,7 @@ extern "C" int32_t gpud_ring_destroy(gpud_ring* r) {
   cudaFree(r->d_ring); cudaFree(r->d_sample); cudaFree(r->d_thr); cudaFree(r->d_pw); cudaFree(r->d_nover); cudaFree(r->d_part);
   cudaFree(r->d_cursor);
   for (auto& p : r->d_res) cudaFree(p);
-  for (auto& p : r->d_rng) cudaFree(p);
-  cudaFree(r->d_rng_nover);
-  cudaFree(r->d_rng_cls); cudaFree(r->d_rng_lists); cudaFree(r->d_rng_piv);
-  for (auto& ev : r->ev_rng) if (ev) cudaEventDestroy(ev);
+  gpud_range_state_free(r->range);
   for (int i = 0; i < 2; ++i) {
     if (r->h_stage[i]) cudaFreeHost(r->h_stage[i]);
     cudaFree(r->d_stage[i]);
@@ -1060,8 +1007,6 @@ extern "C" int32_t gpud_ring_push_raw(gpud_ring* r, const void* host_rows_v, int
 
 extern "C" int32_t gpud_ring_push(gpud_ring* r, const double* host_rows, int64_t n) { return gpud_ring_push_raw(r, host_rows, n, GPUD_DT_F64); }
 
-int gpud_ring_n_fields(const gpud_ring* r) { return r ? r->F : 0; }
-
 extern "C" int32_t gpud_ring_counts(gpud_ring* r, int64_t* total, int64_t* count, int64_t* n_windows) {
   if (!r) return GPUD_E_INVALID;
   const int64_t c = ring_count(r);
@@ -1102,12 +1047,8 @@ static cudaError_t launch_one(gpud_ring* r, WinParams p, int64_t units) {
 
 template <bool RANGE>
 static int32_t launch_windows(gpud_ring* r, WinParams p) {
-  {
-    long long rr = ((long long)p.W * p.q_num + p.q_den - 1) / p.q_den;
-    rr = rr < 1 ? 1 : (rr > p.W ? p.W : rr);
-    p.k_full = p.W - (int)rr + 1;
-    p.inv_w = 1.0 / (double)p.W;
-  }
+  p.k_full = (int)gpud_rank_from_top(p.W, p.q_num, p.q_den);
+  p.inv_w = 1.0 / (double)p.W;
   p.n_list = 0;
   p.w_list[0] = p.w_list[1] = -1;
   p.w_skip[0] = p.w_skip[1] = -1;
@@ -1142,19 +1083,26 @@ static void launch_ema_carry(gpud_ring* r, const double* part, int64_t start, in
   else k_ema_carry<false><<<r->F, 128, 0, r->stream>>>(part, r->d_ring, r->cap, start, r->F, nw, d_full, d_last, out);
 }
 
+// What both window passes share: the ring, the range [start, start + count) in windows of W, the ring's quantile, thresholds and
+// EMA weights.  The caller fills in the outputs.
+static WinParams win_params(const gpud_ring* r, int64_t start, int64_t count, int W, unsigned long long* cursor) {
+  WinParams p{};
+  p.ring = r->d_ring; p.cap = r->cap; p.start = start; p.count = count;
+  p.W = W; p.F = r->F; p.nw = (int)((count + W - 1) / W);
+  p.q_num = r->q_num; p.q_den = r->q_den; p.thr = r->d_thr; p.pw = r->d_pw;
+  p.q64 = pow(1.0 - r->alpha, 64.0); p.alpha = r->alpha;
+  p.cursor = cursor;
+  return p;
+}
+
 extern "C" int32_t gpud_ring_reduce(gpud_ring* r) {
   if (!r) return GPUD_E_INVALID;
   const int64_t count = ring_count(r);
   if (count == 0) return gpud_fail(r->ctx, GPUD_E_STATE, "ring is empty");
   GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
-  WinParams p;
-  p.ring = r->d_ring; p.cap = r->cap; p.start = ring_start(r); p.count = count;
-  p.W = r->W; p.F = r->F; p.nw = (int)((count + r->W - 1) / r->W);
-  p.q_num = r->q_num; p.q_den = r->q_den; p.thr = r->d_thr; p.pw = r->d_pw;
-  p.q64 = pow(1.0 - r->alpha, 64.0); p.alpha = r->alpha;
+  WinParams p = win_params(r, ring_start(r), count, r->W, r->d_cursor);
   p.out_min = r->d_res[GPUD_OP_MIN]; p.out_max = r->d_res[GPUD_OP_MAX]; p.out_mean = r->d_res[GPUD_OP_MEAN];
   p.out_p99 = r->d_res[GPUD_OP_P99]; p.out_nover = r->d_nover; p.part = r->d_part; p.do_select = 1;
-  p.cursor = r->d_cursor;
   cudaEventRecord(r->ev_k[0], r->stream);
   { int32_t rc = launch_windows<false>(r, p); if (rc) return rc; }
   cudaEventRecord(r->ev_k[1], r->stream);
@@ -1216,101 +1164,15 @@ extern "C" int32_t gpud_ring_read(gpud_ring* r, int32_t op, void* out, int64_t o
   return GPUD_OK;
 }
 
-// ---- range reduce support (select.cu): the window kernel with W' = 1024 over the newest `n` samples, into scratch ----
-// gpud_ring_range_prepare sizes the scratch and fills the view; gpud_ring_range_pass launches the pass (+ the EMA carry) in the
-// mode the view names: plain (per-window min / max / mean / EMA partial / n_over) or sampled (the same, plus every sample
-// classified against the field's pivot pair and the keys between the pivots parked in the field's list).
-static cudaError_t grow(void** ptr, size_t* have, size_t need) {
-  if (need <= *have) return cudaSuccess;
-  cudaFree(*ptr);
-  *ptr = nullptr;
-  *have = 0;
-  cudaError_t e = cudaMalloc(ptr, need);
-  if (e == cudaSuccess) *have = need;
-  return e;
-}
-
-int32_t gpud_ring_range_prepare(gpud_ring* r, int64_t n, gpud_range_view* v) {
-  const int64_t count = ring_count(r);
-  if (n <= 0 || n > count) n = count;
-  const int Wp = (int)std::min<int64_t>(kMaxWindow, n);
-  const int nw = (int)((n + Wp - 1) / Wp);
-  const size_t per = (size_t)r->F * nw;
-  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
-  for (int i = 0; i < 5; ++i) GPUD_CUDA(r->ctx, grow((void**)&r->d_rng[i], &r->rng_bytes[i], per * sizeof(double)));
-  GPUD_CUDA(r->ctx, grow((void**)&r->d_rng_nover, &r->rng_nover_bytes, per * sizeof(uint32_t)));
-  const bool sampled = n >= GPUD_RANGE_SAMPLED_MIN;
-  const unsigned list_cap = (unsigned)std::min<int64_t>(GPUD_RANGE_LIST_CAP, n);
-  if (sampled) {
-    GPUD_CUDA(r->ctx, grow((void**)&r->d_rng_cls, &r->rng_cls_bytes, per * sizeof(uint4)));
-    GPUD_CUDA(r->ctx, grow((void**)&r->d_rng_lists, &r->rng_lists_bytes, (size_t)r->F * list_cap * sizeof(unsigned long long)));
-    GPUD_CUDA(r->ctx, grow((void**)&r->d_rng_piv, &r->rng_piv_bytes, (size_t)r->F * (2 * sizeof(double) + sizeof(unsigned))));
-  }
-  for (auto& ev : r->ev_rng) if (!ev) GPUD_CUDA(r->ctx, cudaEventCreate(&ev));
-  int64_t start = ring_start(r) + (count - n);
-  if (start >= r->cap) start -= r->cap;
-  v->ring = r->d_ring; v->F = r->F; v->cap = r->cap; v->start = start; v->n = n; v->Wp = Wp; v->nw = nw;
-  v->w_min = r->d_rng[0]; v->w_max = r->d_rng[1]; v->w_mean = r->d_rng[2]; v->w_ema = r->d_rng[3]; v->w_nover = r->d_rng_nover;
-  v->q_num = r->q_num; v->q_den = r->q_den; v->stream = r->stream; v->ctx = r->ctx; v->dev = r->dev; v->sm_count = r->sm_count;
-  v->sampled = sampled ? 1 : 0;
-  v->sample = r->d_sample; v->smp_shift = r->smp_shift; v->smp_slots = r->smp_slots;
-  v->list_cap = list_cap;
-  v->piv = sampled ? r->d_rng_piv : nullptr;
-  v->fill = sampled ? reinterpret_cast<unsigned*>(r->d_rng_piv + 2 * (size_t)r->F) : nullptr;
-  v->w_cls = sampled ? r->d_rng_cls : nullptr;
-  v->lists = sampled ? r->d_rng_lists : nullptr;
-  for (int i = 0; i < 3; ++i) v->ev[i] = r->ev_rng[i];
-  r->range_timed = false;
-  r->range_nw = nw;
-  return GPUD_OK;
-}
-
-int32_t gpud_ring_range_pass(gpud_ring* r, const gpud_range_view* v) {
-  WinParams p;
-  p.ring = r->d_ring; p.cap = r->cap; p.start = v->start; p.count = v->n; p.W = v->Wp; p.F = r->F; p.nw = v->nw;
-  p.q_num = r->q_num; p.q_den = r->q_den; p.thr = r->d_thr; p.pw = r->d_pw; p.q64 = pow(1.0 - r->alpha, 64.0); p.alpha = r->alpha;
-  p.out_min = r->d_rng[0]; p.out_max = r->d_rng[1]; p.out_mean = r->d_rng[2]; p.out_p99 = nullptr; p.out_nover = r->d_rng_nover;
-  p.part = r->d_rng[4]; p.do_select = 0;
-  p.cursor = r->d_cursor + 2;
-  p.piv = v->piv; p.w_cls = v->w_cls; p.lists = v->lists; p.fill = v->fill; p.list_cap = v->list_cap;
-  { int32_t rc = v->sampled ? launch_windows<true>(r, p) : launch_windows<false>(r, p); if (rc) return rc; }
-  const int m_last = (int)(v->n - (int64_t)(v->nw - 1) * v->Wp);
-  launch_ema_carry(r, r->d_rng[4], v->start, v->nw, v->Wp, m_last, r->d_rng[3]);
+// The window pass of the whole-range reduce (select.cu); internal.h says what goes in and out.
+int32_t gpud_ring_window_pass(gpud_ring* r, int64_t start, int64_t n, int Wp, double* const w[5], uint32_t* w_nover,
+                              const double* piv, uint4* w_cls, unsigned long long* lists, unsigned* fill, unsigned list_cap) {
+  WinParams p = win_params(r, start, n, Wp, r->d_cursor + 2);
+  p.out_min = w[0]; p.out_max = w[1]; p.out_mean = w[2]; p.out_nover = w_nover; p.part = w[4]; p.do_select = 0;
+  p.piv = piv; p.w_cls = w_cls; p.lists = lists; p.fill = fill; p.list_cap = list_cap;
+  { int32_t rc = piv ? launch_windows<true>(r, p) : launch_windows<false>(r, p); if (rc) return rc; }
+  const int m_last = (int)(n - (int64_t)(p.nw - 1) * Wp);
+  launch_ema_carry(r, w[4], start, p.nw, Wp, m_last, w[3]);
   GPUD_CUDA(r->ctx, cudaGetLastError());
-  return GPUD_OK;
-}
-
-void gpud_ring_range_note(gpud_ring* r, bool sampled, unsigned fields_open, const int* reasons) {
-  r->range_timed = sampled;
-  r->range_fields_open = (int)fields_open;
-  for (int i = 0; i < GPUD_RANGE_N_OPEN_REASONS; ++i) r->range_reasons[i] = reasons[i];
-}
-
-extern "C" int32_t gpud_ring_range_stats(gpud_ring* r, float* pass_ms, float* total_ms, int32_t* fields_by_histogram, int32_t* reasons) {
-  if (!r || !pass_ms || !total_ms || !fields_by_histogram) return GPUD_E_INVALID;
-  if (!r->range_timed) return gpud_fail(r->ctx, GPUD_E_STATE, "the last reduce_range (if any) did not take the sampled single pass");
-  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
-  GPUD_CUDA(r->ctx, cudaEventSynchronize(r->ev_rng[2]));
-  GPUD_CUDA(r->ctx, cudaEventElapsedTime(pass_ms, r->ev_rng[0], r->ev_rng[1]));
-  GPUD_CUDA(r->ctx, cudaEventElapsedTime(total_ms, r->ev_rng[0], r->ev_rng[2]));
-  *fields_by_histogram = r->range_fields_open;
-  if (reasons) for (int i = 0; i < GPUD_RANGE_N_OPEN_REASONS; ++i) reasons[i] = r->range_reasons[i];
-  return GPUD_OK;
-}
-
-void gpud_ring_quantile(gpud_ring* r, int* q_num, int* q_den) { *q_num = r->q_num; *q_den = r->q_den; }
-
-// Test hook (include/gpud_b200_hooks.h): what the last sampled reduce_range left in the ring's scratch - each field's pivots
-// {lo, hi}, its list fill counter (which may exceed the list's capacity) and, when cls is given, its per-window class counts.
-extern "C" int32_t gpudh_ring_range_scratch(gpud_ring* r, double* piv, uint32_t* fill, uint32_t* cls, int64_t* nw) {
-  if (!r || !piv || !fill || !nw) return GPUD_E_INVALID;
-  if (!r->range_timed) return gpud_fail(r->ctx, GPUD_E_STATE, "the last reduce_range (if any) did not take the sampled single pass");
-  const size_t F = (size_t)r->F;
-  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
-  GPUD_CUDA(r->ctx, cudaMemcpyAsync(piv, r->d_rng_piv, 2 * F * sizeof(double), cudaMemcpyDeviceToHost, r->stream));
-  GPUD_CUDA(r->ctx, cudaMemcpyAsync(fill, r->d_rng_piv + 2 * F, F * sizeof(uint32_t), cudaMemcpyDeviceToHost, r->stream));
-  if (cls) GPUD_CUDA(r->ctx, cudaMemcpyAsync(cls, r->d_rng_cls, F * r->range_nw * sizeof(uint4), cudaMemcpyDeviceToHost, r->stream));
-  GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));
-  *nw = r->range_nw;
   return GPUD_OK;
 }

@@ -34,7 +34,7 @@ struct SelState {                      // one per field, device resident
   int nbits;                           // number of fixed bits, from the MSB
   int done;
   unsigned collected;                  // fill counter of the candidate list
-  int pad;
+  int why;                             // GPUD_RANGE_OPEN_*: why k_range_finish left the field open (0: it did not)
 };
 
 __device__ __forceinline__ bool key_matches(unsigned long long key, const SelState& s) {
@@ -68,7 +68,7 @@ __device__ __forceinline__ void for_each_key(const double* __restrict__ base, in
   }
 }
 
-// ---- sampled-pivot single pass (ranges of >= GPUD_RANGE_SAMPLED_MIN samples) -----------------------------------------------------
+// ---- sampled-pivot single pass (ranges of >= kSampledMin samples) ---------------------------------------------------------------
 // One block per field reads a systematic sample of S keys (one 32-byte sector each, the stride apart), and picks two sample order
 // statistics around the wanted rank as the field's pivot pair lo <= hi: for the rank k from the top among n keys the sample rank is
 // about k S / n with a standard deviation of sqrt(S p (1 - p)); five of those to either side (failure odds < 1e-6 per field for
@@ -76,8 +76,9 @@ __device__ __forceinline__ void for_each_key(const double* __restrict__ base, in
 // then counts the keys above hi / equal to hi / equal to lo and parks the keys strictly between the pivots in the field's list
 // (about 10 S p-deviations x n / S keys: 12 Ki of 1 Mi for p99); k_range_finish reads the answer off the counts or selects it
 // from the list.  Any field for which that fails (rank outside the pivots, list overflow, +NaN in the data, -NaN upper pivot) is
-// answered by the histogram path below - results never depend on the sample.
-constexpr int kSampleMax = 8192;
+// answered by the histogram path below - results never depend on the sample.  S <= GPUD_RANGE_SAMPLE_MAX (internal.h).
+constexpr int64_t kSampledMin = 65536; // ranges at least this long take the sampled-pivot single pass
+constexpr unsigned kListCap = 65536;   // keys between the pivots kept per field
 constexpr int kSelThreads = 512;       // block size of k_range_pivots / k_range_finish: latency-bound, one block per field
 
 // The kkA-th and kkB-th largest (1-based) of keys[0..cnt) in shared memory, both at once; kSelThreads threads.  MSB-first 8-bit digits
@@ -270,13 +271,11 @@ __global__ void __launch_bounds__(kSelThreads) k_range_finish(int F, int nw, int
     out[2 * F + f] = sum / (double)n;
     out[3 * F + f] = w_ema[(int64_t)f * nw + nw - 1];
     out_nover[f] = (uint32_t)nov;
-    long long r = (n * q_num + q_den - 1) / q_den;
-    r = r < 1 ? 1 : (r > n ? n : r);
     SelState s;
-    s.kk = (unsigned long long)(n - r + 1);
+    s.kk = (unsigned long long)gpud_rank_from_top(n, q_num, q_den);
     s.cnt = (unsigned long long)n;
     s.collected = 0;
-    s.pad = 0;
+    s.why = 0;
     const unsigned long long diff = kmin ^ kmax;
     int mode = 0;                      // 0: left to the histogram path, 1: answered, 2: select from the list
     int why = GPUD_RANGE_OPEN_SHORT;   // why the field stays open (gpud_ring_range_stats)
@@ -313,7 +312,7 @@ __global__ void __launch_bounds__(kSelThreads) k_range_finish(int F, int nw, int
       }
     }
     if (s.done) { s.nbits = 64; s.prefix = s.ans; }
-    s.pad = mode == 0 ? why : 0;
+    s.why = mode == 0 ? why : 0;
     st[f] = s;
     s_mode = mode;
     if (mode == 1) out[4 * F + f] = __longlong_as_double((long long)gpud_key_f64bits(s.ans));
@@ -478,95 +477,174 @@ __global__ void __launch_bounds__(256) k_sel_final(const SelState* __restrict__ 
 
 }  // namespace
 
+// Everything gpud_ring_reduce_range keeps between calls (gpud_ring::range).  Every buffer is grown on demand and kept.
+struct gpud_range_state {
+  double* d_win[5] = {};  size_t win_cap[5] = {};              // the pass, per window [F][nw]: min, max, mean, EMA, EMA partial sums
+  uint32_t* d_win_nover = nullptr;  size_t win_nover_cap = 0;  //   and n_over
+  uint4* d_cls = nullptr;  size_t cls_cap = 0;                  // sampled pass: per-window class counts [F][nw]
+  unsigned long long* d_lists = nullptr;  size_t lists_cap = 0; // sampled pass: the keys between the pivots [F][list_cap]
+  double* d_piv = nullptr;  size_t piv_cap = 0;                 // sampled pass: pivots [F][2] lo, hi
+  unsigned* d_fill = nullptr;  size_t fill_cap = 0;             // sampled pass: list fill counters [F]
+  double* d_out = nullptr;  size_t out_cap = 0;                 // the call's result [5][F]
+  uint32_t* d_nover = nullptr;  size_t nover_cap = 0;           //   and n_over [F]
+  SelState* d_st = nullptr;  size_t st_cap = 0;                 // radix select state [F]
+  unsigned* d_open = nullptr;  size_t open_cap = 0;             // [0] = number of fields left open by k_range_finish, [1..] = their ids
+  unsigned* d_hist = nullptr;  size_t hist_cap = 0;             // radix select: digit histograms [fields selected][kBins]
+  unsigned long long* d_cand = nullptr;  size_t cand_cap = 0;   // radix select: candidate lists [fields selected][kCollectMax]
+  cudaEvent_t ev[3] = {};         // before the pivots / after the pass and carry / after the finish
+  bool timed = false;             // the last call took the sampled single pass (and ran to the end)
+  int reasons[GPUD_RANGE_N_OPEN_REASONS] = {};   // its open fields by reason
+  int fields_open = 0;            // fields it handed to the radix select
+  int nw = 0;                     // windows of its pass (rows of d_cls per field)
+};
+
+void gpud_range_state_free(gpud_range_state* s) {
+  if (!s) return;
+  for (auto* p : s->d_win) cudaFree(p);
+  cudaFree(s->d_win_nover); cudaFree(s->d_cls); cudaFree(s->d_lists); cudaFree(s->d_piv); cudaFree(s->d_fill);
+  cudaFree(s->d_out); cudaFree(s->d_nover); cudaFree(s->d_st); cudaFree(s->d_open); cudaFree(s->d_hist); cudaFree(s->d_cand);
+  for (auto& ev : s->ev) if (ev) cudaEventDestroy(ev);
+  delete s;
+}
+
 extern "C" int32_t gpud_ring_reduce_range(gpud_ring* ring, int64_t last_n, double* out_f64, uint32_t* out_n_over) {
   if (!ring || !out_f64 || !out_n_over || last_n < 0) return GPUD_E_INVALID;
-  gpud_range_view v;
-  int64_t total = 0, count = 0, nwin = 0;
-  gpud_ring_counts(ring, &total, &count, &nwin);
+  const int64_t count = ring_count(ring);
   if (count == 0) return GPUD_E_STATE;
-  { int32_t rc = gpud_ring_range_prepare(ring, last_n, &v); if (rc) return rc; }
-  gpud_ctx* ctx = v.ctx;
-  double* d_out = nullptr;
-  uint32_t* d_nover = nullptr;
-  unsigned* d_hist = nullptr;          // histogram path scratch, allocated only when a field needs it
-  SelState* d_st = nullptr;
-  unsigned long long* d_lists = nullptr;
-  unsigned* d_open = nullptr;          // [0] = number of fields left open by k_range_finish, [1..] = their ids
+  gpud_ctx* ctx = ring->ctx;
+  const cudaStream_t stream = ring->stream;
+  const int F = ring->F;
+  const int64_t n = last_n == 0 || last_n > count ? count : last_n;
+  int64_t start = ring_start(ring) + (count - n);
+  if (start >= ring->cap) start -= ring->cap;
+  const int Wp = (int)std::min<int64_t>(GPUD_MAX_WINDOW, n);
+  const int nw = (int)((n + Wp - 1) / Wp);
+  const bool sampled = n >= kSampledMin;
+  const unsigned list_cap = (unsigned)std::min<int64_t>(kListCap, n);
+  const long long k_from_top = gpud_rank_from_top(n, ring->q_num, ring->q_den);
+
+  GPUD_CUDA(ctx, cudaSetDevice(ring->dev));
+  if (!ring->range) ring->range = new gpud_range_state();
+  gpud_range_state* s = ring->range;
+  s->timed = false;                    // until this call has run to the end: a failed grow may free the last call's scratch
+  const size_t per = (size_t)F * nw;
+  for (int i = 0; i < 5; ++i) GPUD_CUDA(ctx, gpud_grow(&s->d_win[i], &s->win_cap[i], per));
+  GPUD_CUDA(ctx, gpud_grow(&s->d_win_nover, &s->win_nover_cap, per));
+  if (sampled) {
+    GPUD_CUDA(ctx, gpud_grow(&s->d_cls, &s->cls_cap, per));
+    GPUD_CUDA(ctx, gpud_grow(&s->d_lists, &s->lists_cap, (size_t)F * list_cap));
+    GPUD_CUDA(ctx, gpud_grow(&s->d_piv, &s->piv_cap, 2 * (size_t)F));
+    GPUD_CUDA(ctx, gpud_grow(&s->d_fill, &s->fill_cap, (size_t)F));
+  }
+  GPUD_CUDA(ctx, gpud_grow(&s->d_out, &s->out_cap, 5 * (size_t)F));
+  GPUD_CUDA(ctx, gpud_grow(&s->d_nover, &s->nover_cap, (size_t)F));
+  GPUD_CUDA(ctx, gpud_grow(&s->d_st, &s->st_cap, (size_t)F));
+  GPUD_CUDA(ctx, gpud_grow(&s->d_open, &s->open_cap, 1 + (size_t)F));
+  for (auto& ev : s->ev) if (!ev) GPUD_CUDA(ctx, cudaEventCreate(&ev));
+  s->nw = nw;
+  std::fill(s->reasons, s->reasons + GPUD_RANGE_N_OPEN_REASONS, 0);
+  const double* piv = sampled ? s->d_piv : nullptr;
+  unsigned* fill = sampled ? s->d_fill : nullptr;
+  uint4* cls = sampled ? s->d_cls : nullptr;
+  unsigned long long* lists = sampled ? s->d_lists : nullptr;
+
   unsigned h_open = 0;
-  int reasons[GPUD_RANGE_N_OPEN_REASONS] = {0};
-  cudaError_t e = cudaMallocAsync(&d_out, 5 * v.F * sizeof(double), v.stream);
-  if (e == cudaSuccess) e = cudaMallocAsync(&d_nover, v.F * sizeof(uint32_t), v.stream);
-  if (e == cudaSuccess) e = cudaMallocAsync(&d_st, v.F * sizeof(SelState), v.stream);
-  if (e == cudaSuccess) e = cudaMallocAsync(&d_open, (1 + (size_t)v.F) * sizeof(unsigned), v.stream);
-  if (e == cudaSuccess) e = cudaMemsetAsync(d_open, 0, sizeof(unsigned), v.stream);
-  if (e == cudaSuccess) e = cudaEventRecord(v.ev[0], v.stream);
-  if (e == cudaSuccess && v.sampled) {
-    long long r = (long long)((v.n * v.q_num + v.q_den - 1) / v.q_den);
-    r = r < 1 ? 1 : (r > v.n ? v.n : r);
-    const int S = (int)std::min<int64_t>(kSampleMax, v.n / 8);
-    const int64_t stride = v.n / S;
-    const bool use_ring_sample = (v.n >> v.smp_shift) >= 2048 && v.smp_slots <= kSampleMax;   // else too few of the ring's sample slots fall into the range
-    e = cudaFuncSetAttribute(k_range_pivots, cudaFuncAttributeMaxDynamicSharedMemorySize, kSampleMax * (int)sizeof(unsigned long long));
-    if (e == cudaSuccess) k_range_pivots<<<v.F, kSelThreads, (size_t)kSampleMax * sizeof(unsigned long long), v.stream>>>(v.ring, v.cap, v.start, v.n, S, stride, v.n - r + 1, v.piv, v.fill,
-                                                                                                          use_ring_sample ? v.sample : nullptr, v.smp_shift, v.smp_slots);
+  cudaError_t e = cudaMemsetAsync(s->d_open, 0, sizeof(unsigned), stream);
+  if (e == cudaSuccess) e = cudaEventRecord(s->ev[0], stream);
+  if (e == cudaSuccess && sampled) {
+    const int S = (int)std::min<int64_t>(GPUD_RANGE_SAMPLE_MAX, n / 8);
+    const int64_t stride = n / S;
+    const bool use_ring_sample = (n >> ring->smp_shift) >= 2048;   // else too few of the ring's sample slots fall into the range
+    const size_t smem = (size_t)GPUD_RANGE_SAMPLE_MAX * sizeof(unsigned long long);
+    e = cudaFuncSetAttribute(k_range_pivots, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) k_range_pivots<<<F, kSelThreads, smem, stream>>>(ring->d_ring, ring->cap, start, n, S, stride, k_from_top, s->d_piv, s->d_fill,
+                                                                          use_ring_sample ? ring->d_sample : nullptr, ring->smp_shift, ring->smp_slots);
     if (e == cudaSuccess) e = cudaGetLastError();
   }
   if (e == cudaSuccess) {
-    int32_t rc = gpud_ring_range_pass(ring, &v);
-    if (rc) { cudaFreeAsync(d_out, v.stream); cudaFreeAsync(d_nover, v.stream); cudaFreeAsync(d_st, v.stream); cudaFreeAsync(d_open, v.stream); return rc; }
-    e = cudaEventRecord(v.ev[1], v.stream);
+    int32_t rc = gpud_ring_window_pass(ring, start, n, Wp, s->d_win, s->d_win_nover, piv, cls, lists, fill, list_cap);
+    if (rc) return rc;
+    e = cudaEventRecord(s->ev[1], stream);
   }
   if (e == cudaSuccess) {
-    k_range_finish<<<v.F, kSelThreads, 0, v.stream>>>(v.F, v.nw, v.Wp, v.n, v.w_min, v.w_max, v.w_mean, v.w_ema, v.w_nover, v.q_num, v.q_den, v.sampled, v.piv, v.fill,
-                                              v.w_cls, v.lists, v.list_cap, d_out, d_nover, d_st, d_open, reinterpret_cast<int*>(d_open + 1));
+    k_range_finish<<<F, kSelThreads, 0, stream>>>(F, nw, Wp, n, s->d_win[0], s->d_win[1], s->d_win[2], s->d_win[3], s->d_win_nover, ring->q_num, ring->q_den,
+                                                  sampled ? 1 : 0, piv, fill, cls, lists, list_cap, s->d_out, s->d_nover, s->d_st, s->d_open,
+                                                  reinterpret_cast<int*>(s->d_open + 1));
     e = cudaGetLastError();
   }
-  if (e == cudaSuccess) e = cudaEventRecord(v.ev[2], v.stream);
-  if (e == cudaSuccess && v.sampled) {   // a short range leaves every non-constant field to the radix select: no need to ask
-    e = cudaMemcpyAsync(&h_open, d_open, sizeof(unsigned), cudaMemcpyDeviceToHost, v.stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out_f64, d_out, 5 * v.F * sizeof(double), cudaMemcpyDeviceToHost, v.stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out_n_over, d_nover, v.F * sizeof(uint32_t), cudaMemcpyDeviceToHost, v.stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(v.stream);
+  if (e == cudaSuccess) e = cudaEventRecord(s->ev[2], stream);
+  if (e == cudaSuccess && sampled) {   // a short range leaves every non-constant field to the radix select: no need to ask
+    e = cudaMemcpyAsync(&h_open, s->d_open, sizeof(unsigned), cudaMemcpyDeviceToHost, stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(out_f64, s->d_out, 5 * F * sizeof(double), cudaMemcpyDeviceToHost, stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(out_n_over, s->d_nover, F * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
   }
-  if (e == cudaSuccess && (h_open > 0 || !v.sampled)) {
+  if (e == cudaSuccess && (h_open > 0 || !sampled)) {
     // radix select for the fields still open: every non-constant field of a short range, or the rare field the sampled pass
     // could not settle.  The grid covers only the open fields, with enough blocks each to fill the machine.
-    const int* ids = v.sampled ? reinterpret_cast<const int*>(d_open + 1) : nullptr;
-    const int n_sel = v.sampled ? (int)h_open : v.F;
-    if (v.sampled) {
-      std::vector<SelState> h_st(v.F);
-      e = cudaMemcpyAsync(h_st.data(), d_st, v.F * sizeof(SelState), cudaMemcpyDeviceToHost, v.stream);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(v.stream);
-      for (const SelState& q : h_st) if (q.pad > 0 && q.pad < GPUD_RANGE_N_OPEN_REASONS) ++reasons[q.pad];
+    const int* ids = sampled ? reinterpret_cast<const int*>(s->d_open + 1) : nullptr;
+    const int n_sel = sampled ? (int)h_open : F;
+    if (sampled) {
+      std::vector<SelState> h_st(F);
+      e = cudaMemcpyAsync(h_st.data(), s->d_st, F * sizeof(SelState), cudaMemcpyDeviceToHost, stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+      for (const SelState& q : h_st) if (q.why > 0 && q.why < GPUD_RANGE_N_OPEN_REASONS) ++s->reasons[q.why];
     }
-    if (e == cudaSuccess) e = cudaMallocAsync(&d_hist, (size_t)n_sel * kBins * sizeof(unsigned), v.stream);
-    if (e == cudaSuccess) e = cudaMallocAsync(&d_lists, (size_t)n_sel * kCollectMax * sizeof(unsigned long long), v.stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_hist, 0, (size_t)n_sel * kBins * sizeof(unsigned), v.stream);
+    if (e == cudaSuccess) e = gpud_grow(&s->d_hist, &s->hist_cap, (size_t)n_sel * kBins);
+    if (e == cudaSuccess) e = gpud_grow(&s->d_cand, &s->cand_cap, (size_t)n_sel * kCollectMax);
+    if (e == cudaSuccess) e = cudaMemsetAsync(s->d_hist, 0, (size_t)n_sel * kBins * sizeof(unsigned), stream);
     if (e == cudaSuccess) {
       // blocks per field: enough CTAs to fill the machine a few times over, each streaming >= 16 Ki keys
-      const int bpf = (int)std::max<int64_t>(1, std::min<int64_t>((v.n + 16383) / 16384, std::max(1, 8 * v.sm_count / n_sel + 1)));
-      if (v.n > kCollectMax) {
+      const int bpf = (int)std::max<int64_t>(1, std::min<int64_t>((n + 16383) / 16384, std::max(1, 8 * ring->sm_count / n_sel + 1)));
+      if (n > kCollectMax) {
         for (int pass = 0; pass < kMaxHistPasses; ++pass) {          // later passes exit at once for fields that are already narrow
-          k_sel_hist<<<dim3(bpf, n_sel), 256, 0, v.stream>>>(v.ring, v.cap, v.start, v.n, d_st, d_hist, ids);
-          k_sel_pick<<<n_sel, 256, 0, v.stream>>>(d_hist, d_st, ids);
+          k_sel_hist<<<dim3(bpf, n_sel), 256, 0, stream>>>(ring->d_ring, ring->cap, start, n, s->d_st, s->d_hist, ids);
+          k_sel_pick<<<n_sel, 256, 0, stream>>>(s->d_hist, s->d_st, ids);
         }
       }
-      k_sel_collect<<<dim3(bpf, n_sel), 256, 0, v.stream>>>(v.ring, v.cap, v.start, v.n, d_st, d_lists, ids);
-      k_sel_final<<<n_sel, 256, 0, v.stream>>>(d_st, d_lists, v.F, d_out, ids);
+      k_sel_collect<<<dim3(bpf, n_sel), 256, 0, stream>>>(ring->d_ring, ring->cap, start, n, s->d_st, s->d_cand, ids);
+      k_sel_final<<<n_sel, 256, 0, stream>>>(s->d_st, s->d_cand, F, s->d_out, ids);
       e = cudaGetLastError();
     }
-    if (e == cudaSuccess && !v.sampled) {
-      e = cudaMemcpyAsync(out_f64, d_out, 5 * v.F * sizeof(double), cudaMemcpyDeviceToHost, v.stream);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(out_n_over, d_nover, v.F * sizeof(uint32_t), cudaMemcpyDeviceToHost, v.stream);
+    if (e == cudaSuccess && !sampled) {
+      e = cudaMemcpyAsync(out_f64, s->d_out, 5 * F * sizeof(double), cudaMemcpyDeviceToHost, stream);
+      if (e == cudaSuccess) e = cudaMemcpyAsync(out_n_over, s->d_nover, F * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream);
     } else if (e == cudaSuccess) {
-      e = cudaMemcpyAsync(out_f64 + 4 * (size_t)v.F, d_out + 4 * (size_t)v.F, v.F * sizeof(double), cudaMemcpyDeviceToHost, v.stream);
+      e = cudaMemcpyAsync(out_f64 + 4 * (size_t)F, s->d_out + 4 * (size_t)F, F * sizeof(double), cudaMemcpyDeviceToHost, stream);
     }
-    if (d_hist) cudaFreeAsync(d_hist, v.stream);
-    if (d_lists) cudaFreeAsync(d_lists, v.stream);
   }
-  cudaFreeAsync(d_out, v.stream); cudaFreeAsync(d_nover, v.stream); cudaFreeAsync(d_st, v.stream); cudaFreeAsync(d_open, v.stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(v.stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
   if (e != cudaSuccess) return gpud_fail(ctx, GPUD_E_CUDA, "reduce_range: %s", cudaGetErrorString(e));
-  gpud_ring_range_note(ring, v.sampled != 0, h_open, reasons);
+  s->timed = sampled;
+  s->fields_open = (int)h_open;
+  return GPUD_OK;
+}
+
+extern "C" int32_t gpud_ring_range_stats(gpud_ring* r, float* pass_ms, float* total_ms, int32_t* fields_by_histogram, int32_t* reasons) {
+  if (!r || !pass_ms || !total_ms || !fields_by_histogram) return GPUD_E_INVALID;
+  const gpud_range_state* s = r->range;
+  if (!s || !s->timed) return gpud_fail(r->ctx, GPUD_E_STATE, "the last reduce_range (if any) did not take the sampled single pass");
+  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
+  GPUD_CUDA(r->ctx, cudaEventSynchronize(s->ev[2]));
+  GPUD_CUDA(r->ctx, cudaEventElapsedTime(pass_ms, s->ev[0], s->ev[1]));
+  GPUD_CUDA(r->ctx, cudaEventElapsedTime(total_ms, s->ev[0], s->ev[2]));
+  *fields_by_histogram = s->fields_open;
+  if (reasons) std::copy(s->reasons, s->reasons + GPUD_RANGE_N_OPEN_REASONS, reasons);
+  return GPUD_OK;
+}
+
+// Test hook (include/gpud_b200_hooks.h): what the last sampled reduce_range left in its scratch - each field's pivots {lo, hi},
+// its list fill counter (which may exceed the list's capacity) and, when cls is given, its per-window class counts.
+extern "C" int32_t gpudh_ring_range_scratch(gpud_ring* r, double* piv, uint32_t* fill, uint32_t* cls, int64_t* nw) {
+  if (!r || !piv || !fill || !nw) return GPUD_E_INVALID;
+  const gpud_range_state* s = r->range;
+  if (!s || !s->timed) return gpud_fail(r->ctx, GPUD_E_STATE, "the last reduce_range (if any) did not take the sampled single pass");
+  const size_t F = (size_t)r->F;
+  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
+  GPUD_CUDA(r->ctx, cudaMemcpyAsync(piv, s->d_piv, 2 * F * sizeof(double), cudaMemcpyDeviceToHost, r->stream));
+  GPUD_CUDA(r->ctx, cudaMemcpyAsync(fill, s->d_fill, F * sizeof(uint32_t), cudaMemcpyDeviceToHost, r->stream));
+  if (cls) GPUD_CUDA(r->ctx, cudaMemcpyAsync(cls, s->d_cls, F * s->nw * sizeof(uint4), cudaMemcpyDeviceToHost, r->stream));
+  GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));
+  *nw = s->nw;
   return GPUD_OK;
 }

@@ -12,9 +12,9 @@ from fractions import Fraction
 
 import numpy as np
 
-SAMPLED_MIN = 65536          # GPUD_RANGE_SAMPLED_MIN
-LIST_CAP = 65536             # GPUD_RANGE_LIST_CAP
-SAMPLE_MAX = 8192            # GPUD_RANGE_SAMPLE_MAX, kSampleMax
+SAMPLED_MIN = 65536          # kSampledMin (select.cu)
+LIST_CAP = 65536             # kListCap (select.cu)
+SAMPLE_MAX = 8192            # GPUD_RANGE_SAMPLE_MAX (internal.h)
 POS_NAN = np.array([0x7FFFFFFFFFFFFFFF], dtype=np.uint64).view(np.float64)[0]    # the largest totalOrder key
 NEG_NAN = np.array([0xFFFFFFFFFFFFFFFF], dtype=np.uint64).view(np.float64)[0]    # the smallest key (0)
 
@@ -29,7 +29,7 @@ def smp_shift(cap):
 
 
 def range_start(cap, pushed, n):
-    """physical column of the oldest sample of the newest n (gpud_ring_range_prepare)"""
+    """physical column of the oldest sample of the newest n (gpud_ring_reduce_range)"""
     count = min(pushed, cap)
     start = (0 if pushed <= cap else pushed % cap) + (count - n)
     return start - cap if start >= cap else start
