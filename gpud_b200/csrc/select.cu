@@ -8,8 +8,8 @@
 //   1. the bits on which the field's min and max keys agree are skipped (they are common to every key);
 //   2. one 11-bit histogram pass over the first varying digit usually leaves <= kCollectMax keys in the bin that holds the
 //      rank; further histogram passes run only for fields that still have more (heavy ties);
-//   3. one collect pass compacts the surviving keys of every field, and a final per-field kernel selects among them
-//      bit by bit in registers.
+//   3. one collect pass compacts the surviving keys of every field, and a final per-field kernel selects among them with
+//      the same 11-bit list select that k_range_finish runs on the sampled pass's list.
 // Typical cost: 3 reads of the range (window pass, histogram, collect) instead of the 7 of a plain 6-digit radix select.
 // Definitions: oracle/SPEC.md (parity unpinned: the reference has no such aggregate, SURVEY.md §0).
 #include <stdarg.h>
@@ -23,18 +23,16 @@ namespace {
 
 constexpr int kBins = 2048;
 constexpr int kDigit = 11;
-constexpr int kCollectMax = 8192;      // candidates the final kernel keeps in registers: 256 threads x 32 keys
+constexpr int kCollectMax = 8192;      // candidates the collect pass keeps per field for the final list select
 constexpr int kMaxHistPasses = 6;      // 64 bits / 11
 
-struct SelState {                      // one per field, device resident
-  unsigned long long prefix;           // the key bits fixed so far, right-aligned
-  unsigned long long kk;               // rank (1-based, from the top) among the keys that match the prefix
-  unsigned long long cnt;              // how many keys match the prefix
-  unsigned long long ans;              // valid when done
-  int nbits;                           // number of fixed bits, from the MSB
-  int done;
+struct SelState {                      // one per field, device resident; nbits first keeps k_sel_hist at 32 registers (CUDA 12.9)
+  int nbits;                           // number of fixed bits, from the MSB; 64: the field is finished
   unsigned collected;                  // fill counter of the candidate list
   int why;                             // GPUD_RANGE_OPEN_*: why k_range_finish left the field open (0: it did not)
+  unsigned long long prefix;           // the key bits fixed so far, right-aligned; the answer once nbits == 64
+  unsigned long long kk;               // rank (1-based, from the top) among the keys that match the prefix
+  unsigned long long cnt;              // how many keys match the prefix
 };
 
 __device__ __forceinline__ bool key_matches(unsigned long long key, const SelState& s) {
@@ -79,7 +77,7 @@ __device__ __forceinline__ void for_each_key(const double* __restrict__ base, in
 // answered by the histogram path below - results never depend on the sample.  S <= GPUD_RANGE_SAMPLE_MAX (internal.h).
 constexpr int64_t kSampledMin = 65536; // ranges at least this long take the sampled-pivot single pass
 constexpr unsigned kListCap = 65536;   // keys between the pivots kept per field
-constexpr int kSelThreads = 512;       // block size of k_range_pivots / k_range_finish: latency-bound, one block per field
+constexpr int kSelThreads = 512;       // block size of the one-block-per-field kernels (pivots, finish, pick, final): latency-bound
 
 // The kkA-th and kkB-th largest (1-based) of keys[0..cnt) in shared memory, both at once; kSelThreads threads.  MSB-first 8-bit digits
 // starting below the bits all keys share; a target whose chosen bin holds a single key is finished by one more sweep that
@@ -221,9 +219,66 @@ __global__ void __launch_bounds__(kSelThreads) k_range_pivots(const double* __re
   }
 }
 
+struct BinPick { int bin; unsigned above; };   // the chosen digit bin and the keys in the bins above it
+
+// The bin of hist[0..nb) (shared memory) that holds the kk-th largest (1-based) key; every thread of the block calls it and gets
+// the same result.  Thread t sums kBpt bins from the top, a block-wide exclusive scan of those sums finds the thread whose bins
+// reach kk, and that thread walks them.  Callers keep kk <= the histogram's total; were it larger, the lowest bin is chosen, so
+// every call fixes one more digit and no caller can loop without advancing.
+__device__ __forceinline__ BinPick pick_bin(const unsigned* hist, int nb, unsigned long long kk) {
+  constexpr int kBpt = kBins / kSelThreads;
+  __shared__ unsigned s_part[kSelThreads / 32];
+  __shared__ BinPick s_pick;
+  const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
+  const int top = nb - 1 - kBpt * t;                     // this thread's highest bin
+  unsigned loc = 0;
+#pragma unroll
+  for (int j = 0; j < kBpt; ++j) if (top - j >= 0) loc += hist[top - j];
+  unsigned incl = loc;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned u = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += u;
+  }
+  if (lane == 31) s_part[wid] = incl;
+  __syncthreads();
+  unsigned before = incl - loc;
+  for (int w = 0; w < wid; ++w) before += s_part[w];
+  if ((unsigned long long)before < kk && (kk <= (unsigned long long)before + loc || (top >= 0 && top < kBpt))) {
+    unsigned acc = before;
+    int b = top;
+    while (b > 0 && (unsigned long long)acc + hist[b] < kk) { acc += hist[b]; --b; }
+    s_pick = {b, acc};
+  }
+  __syncthreads();
+  return s_pick;                       // read before the next call's first barrier, after which the owner may rewrite it
+}
+
+// The kk-th largest (1-based) of the keys in list[0..cnt) (global memory) whose top nbits bits equal prefix, MSB-first in 11-bit
+// digits; kk must not exceed the number of such keys.  Every thread of the block calls it and gets the answer.
+__device__ __forceinline__ unsigned long long list_select(const unsigned long long* __restrict__ list, unsigned cnt, int nbits,
+                                                         unsigned long long prefix, unsigned long long kk) {
+  __shared__ unsigned s_hist[kBins];
+  while (nbits < 64) {
+    const int d = min(kDigit, 64 - nbits), shift = 64 - nbits - d, nb = 1 << d;
+    for (int i = threadIdx.x; i < kBins; i += kSelThreads) s_hist[i] = 0;
+    __syncthreads();
+    for (unsigned i = threadIdx.x; i < cnt; i += kSelThreads) {
+      const unsigned long long key = list[i];
+      if (nbits == 0 || (key >> (64 - nbits)) == prefix) atomicAdd(&s_hist[(unsigned)(key >> shift) & (unsigned)(nb - 1)], 1u);
+    }
+    __syncthreads();
+    const BinPick p = pick_bin(s_hist, nb, kk);
+    prefix = (prefix << d) | (unsigned long long)p.bin;
+    nbits += d;
+    kk -= p.above;
+  }
+  return prefix;
+}
+
 // One block per field after the window pass: fold the per-window partials into the field's min / max / mean / EMA / n_over,
 // initialise the histogram path's state, and - sampled mode - settle the order statistic from the class counts and the list.
-// Fields left open (done == 0) are counted in *n_open.
+// Fields left open (nbits < 64) are counted in *n_open.
 __global__ void __launch_bounds__(kSelThreads) k_range_finish(int F, int nw, int Wp, int64_t n, const double* __restrict__ w_min, const double* __restrict__ w_max,
                                                        const double* __restrict__ w_mean, const double* __restrict__ w_ema, const uint32_t* __restrict__ w_nover,
                                                        int q_num, int q_den, int sampled, const double* __restrict__ piv, const unsigned* __restrict__ fill,
@@ -232,10 +287,8 @@ __global__ void __launch_bounds__(kSelThreads) k_range_finish(int F, int nw, int
                                                        unsigned* __restrict__ n_open, int* __restrict__ open_ids) {
   __shared__ unsigned long long s_red[kSelThreads / 32][6];
   __shared__ double s_sum[kSelThreads / 32];
-  __shared__ unsigned s_hist[kBins];
   __shared__ unsigned long long s_prefix, s_kk;
   __shared__ int s_nbits, s_mode;
-  __shared__ unsigned s_part[kSelThreads / 32];
   const int f = blockIdx.x, t = threadIdx.x, lane = t & 31, wid = t >> 5;
   unsigned long long kmin = ~0ull, kmax = 0ull, c_abv = 0, c_eh = 0, c_el = 0, nov = 0;
   double sum = 0.0;
@@ -280,14 +333,12 @@ __global__ void __launch_bounds__(kSelThreads) k_range_finish(int F, int nw, int
     int mode = 0;                      // 0: left to the histogram path, 1: answered, 2: select from the list
     int why = GPUD_RANGE_OPEN_SHORT;   // why the field stays open (gpud_ring_range_stats)
     if (diff == 0ull) {                // a constant field: every key is the answer
-      s.prefix = kmax; s.nbits = 64; s.done = 1; s.ans = kmax;
+      s.prefix = kmax; s.nbits = 64;
       mode = 1;
     } else {
       const int cp = __clzll((long long)diff);   // leading bits common to all keys of the field
       s.nbits = cp;
       s.prefix = cp ? (kmax >> (64 - cp)) : 0ull;
-      s.done = 0;
-      s.ans = 0ull;
       if (sampled && kmax > gpud_f64_key(0x7ff0000000000000ull)) why = GPUD_RANGE_OPEN_NAN;   // a +NaN was classified as "below"
       if (sampled && kmax <= gpud_f64_key(0x7ff0000000000000ull)) {
         const unsigned long long lok = gpud_f64_key((unsigned long long)__double_as_longlong(piv[2 * f]));
@@ -296,7 +347,7 @@ __global__ void __launch_bounds__(kSelThreads) k_range_finish(int F, int nw, int
         const unsigned long long k = s.kk;
         why = !(lok <= hik) ? GPUD_RANGE_OPEN_PIVOTS : (k <= c_abv ? GPUD_RANGE_OPEN_ABOVE : GPUD_RANGE_OPEN_BELOW);
         if (lok <= hik && k > c_abv) {
-          if (k <= c_abv + c_eh) { s.done = 1; s.ans = hik; mode = 1; }
+          if (k <= c_abv + c_eh) { s.prefix = hik; s.nbits = 64; mode = 1; }
           else if (k <= c_abv + c_eh + inside) {
             why = GPUD_RANGE_OPEN_OVERFLOW;
             if (inside <= (unsigned long long)list_cap) {
@@ -307,64 +358,23 @@ __global__ void __launch_bounds__(kSelThreads) k_range_finish(int F, int nw, int
               s_prefix = cp2 ? (hik >> (64 - cp2)) : 0ull;
               s_kk = k - c_abv - c_eh;
             }
-          } else if (k <= c_abv + c_eh + inside + c_el) { s.done = 1; s.ans = lok; mode = 1; }
+          } else if (k <= c_abv + c_eh + inside + c_el) { s.prefix = lok; s.nbits = 64; mode = 1; }
         }
       }
     }
-    if (s.done) { s.nbits = 64; s.prefix = s.ans; }
     s.why = mode == 0 ? why : 0;
     st[f] = s;
     s_mode = mode;
-    if (mode == 1) out[4 * F + f] = __longlong_as_double((long long)gpud_key_f64bits(s.ans));
+    if (mode == 1) out[4 * F + f] = __longlong_as_double((long long)gpud_key_f64bits(s.prefix));
     if (mode == 0) open_ids[atomicAdd(n_open, 1u)] = f;
   }
   __syncthreads();
   if (s_mode != 2) return;
-  const unsigned cnt = fill[f];
-  const unsigned long long* __restrict__ list = lists + (int64_t)f * list_cap;
-  while (s_nbits < 64) {               // radix select over the L2-resident list, 11-bit digits
-    const int nbits = s_nbits;
-    const unsigned long long prefix = s_prefix;
-    const int d = min(kDigit, 64 - nbits), shift = 64 - nbits - d, nb = 1 << d;
-    for (int i = t; i < kBins; i += kSelThreads) s_hist[i] = 0;
-    __syncthreads();
-    for (unsigned i = t; i < cnt; i += kSelThreads) {
-      const unsigned long long key = list[i];
-      if (nbits == 0 || (key >> (64 - nbits)) == prefix) atomicAdd(&s_hist[(unsigned)(key >> shift) & (unsigned)(nb - 1)], 1u);
-    }
-    __syncthreads();
-    // thread t owns kBpt bins from the top (nb-1-kBpt t downwards); block-wide exclusive scan of the per-thread sums finds the owner
-    constexpr int kBpt = kBins / kSelThreads;
-    unsigned loc = 0;
-#pragma unroll
-    for (int j = 0; j < kBpt; ++j) { const int b = nb - 1 - kBpt * t - j; if (b >= 0) loc += s_hist[b]; }
-    unsigned incl = loc;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned u = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += u;
-    }
-    if (lane == 31) s_part[wid] = incl;
-    __syncthreads();
-    unsigned before = incl - loc;
-    for (int w = 0; w < wid; ++w) before += s_part[w];
-    const unsigned long long kk = s_kk;
-    __syncthreads();                                   // everyone has read s_kk / s_part before the owner rewrites them
-    if ((unsigned long long)before < kk && kk <= (unsigned long long)before + loc) {
-      unsigned acc = before;
-      int b = nb - 1 - kBpt * t;
-      while ((unsigned long long)acc + s_hist[b] < kk) { acc += s_hist[b]; --b; }
-      s_prefix = (nbits ? (prefix << d) : 0ull) | (unsigned long long)b;
-      s_nbits = nbits + d;
-      s_kk = kk - acc;
-    }
-    __syncthreads();
-  }
+  const unsigned long long ans = list_select(lists + (int64_t)f * list_cap, fill[f], s_nbits, s_prefix, s_kk);   // the L2-resident list
   if (t == 0) {
-    SelState s = st[f];
-    s.done = 1; s.ans = s_prefix; s.nbits = 64; s.prefix = s_prefix;
-    st[f] = s;
-    out[4 * F + f] = __longlong_as_double((long long)gpud_key_f64bits(s_prefix));
+    st[f].prefix = ans;
+    st[f].nbits = 64;
+    out[4 * F + f] = __longlong_as_double((long long)gpud_key_f64bits(ans));
   }
 }
 
@@ -374,7 +384,7 @@ __global__ void __launch_bounds__(256) k_sel_hist(const double* __restrict__ rin
   __shared__ unsigned s_hist[kBins];
   const int f = ids ? ids[blockIdx.y] : blockIdx.y;
   const SelState s = st[f];
-  if (s.done || s.cnt <= (unsigned long long)kCollectMax) return;   // block-uniform: nothing left to narrow for this field
+  if (s.nbits == 64 || s.cnt <= (unsigned long long)kCollectMax) return;   // block-uniform: nothing left to narrow for this field
   for (int i = threadIdx.x; i < kBins; i += blockDim.x) s_hist[i] = 0;
   __syncthreads();
   const int d = min(kDigit, 64 - s.nbits), shift = 64 - s.nbits - d;
@@ -390,32 +400,22 @@ __global__ void __launch_bounds__(256) k_sel_hist(const double* __restrict__ rin
     if (s_hist[i]) atomicAdd(&hist[(int64_t)blockIdx.y * kBins + i], s_hist[i]);
 }
 
-// one block per field: walk the digit histogram from the top, fix the next digit of the k-th largest key
-__global__ void __launch_bounds__(256) k_sel_pick(unsigned* __restrict__ hist, SelState* __restrict__ st, const int* __restrict__ ids) {
-  __shared__ unsigned s[kBins];
-  __shared__ unsigned s_sum[256];
-  const int f = ids ? ids[blockIdx.x] : blockIdx.x, t = threadIdx.x;
+// one block per field: fix the next digit of the k-th largest key from the digit histogram (and zero it for the next pass)
+__global__ void __launch_bounds__(kSelThreads) k_sel_pick(unsigned* __restrict__ hist, SelState* __restrict__ st, const int* __restrict__ ids) {
+  __shared__ unsigned s_hist[kBins];
+  const int f = ids ? ids[blockIdx.x] : blockIdx.x;
   SelState cur = st[f];
-  if (cur.done || cur.cnt <= (unsigned long long)kCollectMax) return;
-  const int d = min(kDigit, 64 - cur.nbits), nb = 1 << d;
-  for (int i = t; i < kBins; i += 256) { s[i] = i < nb ? hist[(int64_t)blockIdx.x * kBins + i] : 0; hist[(int64_t)blockIdx.x * kBins + i] = 0; }
+  if (cur.nbits == 64 || cur.cnt <= (unsigned long long)kCollectMax) return;
+  unsigned* __restrict__ h = hist + (int64_t)blockIdx.x * kBins;
+  for (int i = threadIdx.x; i < kBins; i += kSelThreads) { s_hist[i] = h[i]; h[i] = 0; }
   __syncthreads();
-  unsigned loc = 0;                    // thread t owns bins [8t, 8t+8) counted from the TOP
-  for (int j = 8 * t; j < 8 * t + 8; ++j) if (j < nb) loc += s[nb - 1 - j];
-  s_sum[t] = loc;
-  __syncthreads();
-  if (t == 0) {
-    unsigned long long acc = 0;
-    int g = 0;
-    while (g < 255 && acc + s_sum[g] < cur.kk) { acc += s_sum[g]; ++g; }
-    int j = 8 * g;
-    while (j < nb - 1 && acc + s[nb - 1 - j] < cur.kk) { acc += s[nb - 1 - j]; ++j; }
-    const unsigned bin = (unsigned)(nb - 1 - j);
-    cur.prefix = (cur.nbits ? (cur.prefix << d) : 0ull) | bin;
+  const int d = min(kDigit, 64 - cur.nbits);
+  const BinPick p = pick_bin(s_hist, 1 << d, cur.kk);
+  if (threadIdx.x == 0) {
+    cur.prefix = (cur.prefix << d) | (unsigned long long)p.bin;
     cur.nbits += d;
-    cur.kk -= acc;
-    cur.cnt = s[bin];
-    if (cur.nbits >= 64) { cur.done = 1; cur.ans = cur.prefix; }
+    cur.kk -= p.above;
+    cur.cnt = s_hist[p.bin];
     st[f] = cur;
   }
 }
@@ -425,7 +425,7 @@ __global__ void __launch_bounds__(256) k_sel_collect(const double* __restrict__ 
                                                       SelState* __restrict__ st, unsigned long long* __restrict__ lists, const int* __restrict__ ids) {
   const int f = ids ? ids[blockIdx.y] : blockIdx.y;
   const SelState s = st[f];
-  if (s.done) return;
+  if (s.nbits == 64) return;
   const int64_t per = (((n + gridDim.x - 1) / gridDim.x) + 1) & ~(int64_t)1;
   const int64_t b = min(n, (int64_t)blockIdx.x * per), e = min(n, b + per);
   const double* __restrict__ base = ring + (int64_t)f * cap;
@@ -439,40 +439,14 @@ __global__ void __launch_bounds__(256) k_sel_collect(const double* __restrict__ 
   });
 }
 
-// one block per field: k-th largest of the (<= kCollectMax) collected keys, remaining bits fixed one at a time;
-// every thread keeps its 32 keys in registers, the per-bit counts meet in shared memory
-__global__ void __launch_bounds__(256) k_sel_final(const SelState* __restrict__ st, const unsigned long long* __restrict__ lists, int F,
-                                                    double* __restrict__ out, const int* __restrict__ ids) {
-  __shared__ unsigned s_cnt[8];
-  const int f = ids ? ids[blockIdx.x] : blockIdx.x, t = threadIdx.x, lane = t & 31, wid = t >> 5;
+// one block per field: its answer, selected from its (<= kCollectMax) collected keys unless the histogram passes finished it
+__global__ void __launch_bounds__(kSelThreads) k_sel_final(const SelState* __restrict__ st, const unsigned long long* __restrict__ lists, int F,
+                                                           double* __restrict__ out, const int* __restrict__ ids) {
+  const int f = ids ? ids[blockIdx.x] : blockIdx.x;
   const SelState s = st[f];
-  unsigned long long ans = s.ans;
-  if (!s.done) {
-    const unsigned n = (unsigned)min((unsigned long long)kCollectMax, (unsigned long long)s.collected);
-    const unsigned long long* __restrict__ list = lists + (int64_t)blockIdx.x * kCollectMax;
-    unsigned long long key[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) { const unsigned idx = (unsigned)i * 256u + (unsigned)t; key[i] = idx < n ? list[idx] : 0ull; }   // 0 never matches a set bit
-    unsigned long long pref = s.nbits ? (s.prefix << (64 - s.nbits)) : 0ull;
-    unsigned long long kk = s.kk;
-    for (int b = 63 - s.nbits; b >= 0; --b) {
-      const unsigned long long trial = pref | (1ull << b);
-      const unsigned long long himask = ~((1ull << b) - 1ull);
-      unsigned c = 0;
-#pragma unroll
-      for (int i = 0; i < 32; ++i) c += ((key[i] & himask) == trial) ? 1u : 0u;
-      c = __reduce_add_sync(0xffffffffu, c);
-      if (lane == 0) s_cnt[wid] = c;
-      __syncthreads();
-      unsigned tot = 0;
-#pragma unroll
-      for (int w = 0; w < 8; ++w) tot += s_cnt[w];
-      __syncthreads();
-      if ((unsigned long long)tot >= kk) pref = trial; else kk -= tot;
-    }
-    ans = pref;
-  }
-  if (t == 0) out[4 * F + f] = __longlong_as_double((long long)gpud_key_f64bits(ans));
+  const unsigned n = min((unsigned)kCollectMax, s.collected);
+  const unsigned long long ans = list_select(lists + (int64_t)blockIdx.x * kCollectMax, n, s.nbits, s.prefix, s.kk);
+  if (threadIdx.x == 0) out[4 * F + f] = __longlong_as_double((long long)gpud_key_f64bits(ans));
 }
 
 }  // namespace
@@ -599,11 +573,11 @@ extern "C" int32_t gpud_ring_reduce_range(gpud_ring* ring, int64_t last_n, doubl
       if (n > kCollectMax) {
         for (int pass = 0; pass < kMaxHistPasses; ++pass) {          // later passes exit at once for fields that are already narrow
           k_sel_hist<<<dim3(bpf, n_sel), 256, 0, stream>>>(ring->d_ring, ring->cap, start, n, s->d_st, s->d_hist, ids);
-          k_sel_pick<<<n_sel, 256, 0, stream>>>(s->d_hist, s->d_st, ids);
+          k_sel_pick<<<n_sel, kSelThreads, 0, stream>>>(s->d_hist, s->d_st, ids);
         }
       }
       k_sel_collect<<<dim3(bpf, n_sel), 256, 0, stream>>>(ring->d_ring, ring->cap, start, n, s->d_st, s->d_cand, ids);
-      k_sel_final<<<n_sel, 256, 0, stream>>>(s->d_st, s->d_cand, F, s->d_out, ids);
+      k_sel_final<<<n_sel, kSelThreads, 0, stream>>>(s->d_st, s->d_cand, F, s->d_out, ids);
       e = cudaGetLastError();
     }
     if (e == cudaSuccess && !sampled) {

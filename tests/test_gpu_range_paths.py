@@ -111,8 +111,8 @@ def test_sampled_range_routes(env, case):
 
 @pytest.mark.parametrize("case", RC.short_cases(), ids=[c[0] for c in RC.short_cases()])
 def test_short_range_radix_select(env, case):
-    """ranges below 64 Ki: every non-constant field through k_sel_hist / k_sel_pick / k_sel_collect / k_sel_final; no sampled
-    pass, so range_stats and the scratch hook report GPUD_E_STATE"""
+    """ranges below 64 Ki: every non-constant field through k_sel_hist / k_sel_pick / k_sel_collect and the list select of
+    k_sel_final; no sampled pass, so range_stats and the scratch hook report GPUD_E_STATE"""
     name, cap, pushed, last_n, q_num, q_den, xs = case
     got, stats, reasons, scratch = _run(env, cap, pushed, last_n, q_num, q_den, xs)
     assert stats == E_STATE and scratch == E_STATE, (stats, scratch)

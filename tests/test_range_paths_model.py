@@ -7,8 +7,8 @@ the RANGE pass of k_window_reduce in ring.cu).  The model restates, per field:
     when lo and hi are equal and not a zero; per 1024-sample window, plus the list fill;
   - k_range_finish: the outcome (constant, hi, lo, select from the list) or the reason the field stays open;
   - the radix select the open fields (and every non-constant field of a short range) go through: the k_sel_hist / k_sel_pick
-    passes that do work, whether the field finishes in pick, how many keys k_sel_collect gathers, and which load path
-    for_each_key takes in each block's slice.
+    passes that do work, whether the field finishes in pick, how many keys k_sel_collect gathers for k_sel_final's list select
+    (the one k_range_finish runs on its list), and which load path for_each_key takes in each block's slice.
 The tests check that the model's answer equals a sort of the keys on every case, and that the cases of test_gpu_range_paths.py
 reach every route, both sample sources and every load path.  test_gpu_range_paths.py checks the device against the model."""
 import collections
