@@ -1642,32 +1642,46 @@ static int32_t scan_launch(gpud_ctx* ctx, gpud_scan_state* s, const uint8_t* d_b
   return GPUD_OK;
 }
 
-static int32_t scan_collect(gpud_ctx* ctx, gpud_scan_state* s, gpud_xid_hit* hits, int64_t cap, int64_t* n_hits, int64_t* n_units,
-                            cudaStream_t st) {
+// The scan, finished on the host.  The match kernel keeps whichever hits take the first hit_cap slots, in arrival order, so a
+// list that overflowed holds an arbitrary subset: scan once more with room for every hit (the buffer is still resident), so that
+// the first `cap` hits handed out are the buffer's first and the duplicates of the extra matchers are dropped from the count.
+static int32_t scan_run(gpud_ctx* ctx, gpud_scan_state* s, const uint8_t* d_buf, int64_t len, int32_t mode, int64_t cap, cudaStream_t st) {
+  int32_t rc = scan_launch(ctx, s, d_buf, len, mode, cap, st);
+  if (rc) return rc;
   GPUD_CUDA(ctx, cudaStreamSynchronize(st));
   const int64_t found = (int64_t)s->h_counters[1];
-  const int64_t have = std::min<int64_t>(found, (int64_t)s->hit_cap);
+  if (found <= (int64_t)s->hit_cap) return GPUD_OK;
+  rc = scan_launch(ctx, s, d_buf, len, mode, found, st);
+  if (rc) return rc;
+  GPUD_CUDA(ctx, cudaStreamSynchronize(st));
+  return GPUD_OK;
+}
+
+// after scan_run: the device list holds every hit
+static int32_t scan_collect(gpud_ctx* ctx, gpud_scan_state* s, gpud_xid_hit* hits, int64_t cap, int64_t* n_hits, int64_t* n_units,
+                            cudaStream_t st) {
+  const int64_t found = (int64_t)s->h_counters[1];
   if (n_hits) *n_hits = found;
   if (n_units) *n_units = (int64_t)s->h_counters[2] + 1;
   if (s->h_counters[0] > s->cand_cap) return gpud_fail(ctx, GPUD_E_CAPACITY, "candidate list overflow (%llu)", s->h_counters[0]);
   // hits land in a pinned host buffer; only 24-byte keys are sorted, each 288-byte record moves once
-  if ((size_t)have > s->h_hits_cap) {
+  if ((size_t)found > s->h_hits_cap) {
     if (s->h_hits) cudaFreeHost(s->h_hits);
     s->h_hits = nullptr;
     s->h_hits_cap = 0;
-    const size_t want = std::max<size_t>((size_t)have, 4096);
+    const size_t want = std::max<size_t>((size_t)found, 4096);
     GPUD_CUDA(ctx, cudaMallocHost(&s->h_hits, want * sizeof(gpud_xid_hit)));
     s->h_hits_cap = want;
   }
-  if (have) {
-    GPUD_CUDA(ctx, cudaMemcpyAsync(s->h_hits, s->d_hits, (size_t)have * sizeof(gpud_xid_hit), cudaMemcpyDeviceToHost, st));
+  if (found) {
+    GPUD_CUDA(ctx, cudaMemcpyAsync(s->h_hits, s->d_hits, (size_t)found * sizeof(gpud_xid_hit), cudaMemcpyDeviceToHost, st));
     GPUD_CUDA(ctx, cudaStreamSynchronize(st));
   }
   // device threads finish in arbitrary order: present hits in (unit, kind) order like the sequential reference loop.
   // Extra line matchers: several anchors of one unit may match the same pattern; the reference reports the leftmost.
   struct Key { int64_t unit; int64_t link; int32_t kind; int32_t idx; };
-  std::vector<Key> keys((size_t)have);
-  for (int64_t i = 0; i < have; ++i) {
+  std::vector<Key> keys((size_t)found);
+  for (int64_t i = 0; i < found; ++i) {
     const gpud_xid_hit& h = s->h_hits[i];
     keys[(size_t)i] = Key{h.unit_index, h.kind > GPUD_KIND_SXID ? h.link : 0, h.kind, (int32_t)i};
   }
@@ -1676,16 +1690,15 @@ static int32_t scan_collect(gpud_ctx* ctx, gpud_scan_state* s, gpud_xid_hit* hit
     if (a.kind != b.kind) return a.kind < b.kind;
     return a.link != b.link ? a.link < b.link : a.idx < b.idx;
   });
-  if (have == found)
-    keys.erase(std::unique(keys.begin(), keys.end(), [](const Key& a, const Key& b) {
-                 return a.kind > GPUD_KIND_SXID && a.unit == b.unit && a.kind == b.kind;
-               }), keys.end());
-  const int64_t found_u = have == found ? (int64_t)keys.size() : found;
+  keys.erase(std::unique(keys.begin(), keys.end(), [](const Key& a, const Key& b) {
+               return a.kind > GPUD_KIND_SXID && a.unit == b.unit && a.kind == b.kind;
+             }), keys.end());
+  const int64_t found_u = (int64_t)keys.size();
   if (n_hits) *n_hits = found_u;
-  const int64_t n_copy = std::min<int64_t>((int64_t)keys.size(), cap);
+  const int64_t n_copy = std::min<int64_t>(found_u, cap);
   if (hits)
     for (int64_t i = 0; i < n_copy; ++i) hits[i] = s->h_hits[keys[(size_t)i].idx];
-  if (found_u > cap || found > have) return gpud_fail(ctx, GPUD_E_CAPACITY, "%lld hits, caller capacity %lld", (long long)found_u, (long long)cap);
+  if (found_u > cap) return gpud_fail(ctx, GPUD_E_CAPACITY, "%lld hits, caller capacity %lld", (long long)found_u, (long long)cap);
   return GPUD_OK;
 }
 
@@ -1696,7 +1709,7 @@ extern "C" int32_t gpud_kmsg_scan_device(gpud_ctx* ctx, int32_t dev, const uint8
   int32_t rc = scan_state_get(ctx, dev, &s);
   if (rc) return rc;
   cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : s->stream;
-  rc = scan_launch(ctx, s, dev_buf, len, mode, cap, st);
+  rc = scan_run(ctx, s, dev_buf, len, mode, cap, st);
   if (rc) return rc;
   return scan_collect(ctx, s, hits, cap, n_hits, n_units, st);
 }
@@ -1733,7 +1746,7 @@ extern "C" int32_t gpud_kmsg_scan(gpud_ctx* ctx, int32_t dev, const uint8_t* buf
       }
     }
   }
-  rc = scan_launch(ctx, s, s->d_buf, len, mode, cap, s->stream);
+  rc = scan_run(ctx, s, s->d_buf, len, mode, cap, s->stream);
   if (rc) return rc;
   return scan_collect(ctx, s, hits, cap, n_hits, n_units, s->stream);
 }

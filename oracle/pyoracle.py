@@ -132,7 +132,8 @@ SXID_DETAILS = {d["sxid"]: d for d in CATALOG["sxid"]}
 
 
 def get_detail(code: int) -> Optional[Detail]:                      # xid.go:74-77
-    return XID_DETAILS.get(code)
+    d = XID_DETAILS.get(code)                                          # a copy, like Go's &e of the map value: callers
+    return None if d is None else d.copy()                             # (detailFromNVLinkInfo) edit what they get
 
 
 def event_type_from_severity(s: str) -> int:                         # xid.go:3263-3272
