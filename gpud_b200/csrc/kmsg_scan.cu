@@ -557,34 +557,64 @@ __device__ bool go_parse_hex32(const ScanBuf& b, int64_t s, int64_t e, uint32_t*
 }
 
 // ---------------------------------------------------------------------------------------------
+// literal searches, shared by the Xid / SXid automata, the match kernel's worker rule and the extra matchers
+// ---------------------------------------------------------------------------------------------
+__device__ int64_t find_lit(const ScanBuf& b, int64_t from, int64_t to, const char* lit, int n) {   // first start in [from, to - n], else -1
+  const unsigned c0 = (unsigned char)lit[0];
+  for (int64_t i = find_byte(b, from, to, c0); i + n <= to; i = find_byte(b, i + 1, to, c0)) {
+    bool ok = true;
+    for (int k = 1; k < n && ok; ++k) ok = __ldg(b.p + i + k) == (uint8_t)lit[k];
+    if (ok) return i;
+  }
+  return -1;
+}
+template <int N>
+__device__ __forceinline__ int64_t find_lit(const ScanBuf& b, int64_t from, int64_t to, const char (&s)[N]) { return find_lit(b, from, to, s, N - 1); }
+
+// last start in [from, to - n] of the n-byte literal, else -1
+__device__ int64_t rfind_lit(const ScanBuf& b, int64_t from, int64_t to, const char* lit, int n) {
+  const unsigned c0 = (unsigned char)lit[0];
+  for (int64_t i = rfind_byte(b, from, to - n + 1, c0); i >= from; i = rfind_byte(b, from, i, c0)) {
+    bool ok = true;
+    for (int k = 1; k < n && ok; ++k) ok = __ldg(b.p + i + k) == (uint8_t)lit[k];
+    if (ok) return i;
+  }
+  return -1;
+}
+template <int N>
+__device__ __forceinline__ int64_t rfind_lit(const ScanBuf& b, int64_t from, int64_t to, const char (&s)[N]) { return rfind_lit(b, from, to, s, N - 1); }
+__device__ __forceinline__ int64_t digits_end(const ScanBuf& b, int64_t p, int64_t e) { while (p < e && is_digit(ld8(b, p))) ++p; return p; }
+
+// ---------------------------------------------------------------------------------------------
 // the automata.  [s, e) is the unit's message span; every function returns the match for the leftmost anchor
 // at which the whole pattern succeeds (Go FindStringSubmatch: leftmost-first).
 // ---------------------------------------------------------------------------------------------
+// `.*?: (\d+),` from i (the tail of R1 and R5): `.*?` stops at the first ": " digits+ "," and cannot cross '\n'
+__device__ __forceinline__ bool lazy_code(const ScanBuf& b, int64_t i, int64_t e, int64_t* cs, int64_t* ce) {
+  for (; i < e; ++i) {
+    const int c = ld8(b, i);
+    if (c == '\n') break;
+    if (c == ':' && ld8(b, i + 1) == ' ' && is_digit(ld8(b, i + 2))) {
+      const int64_t j = digits_end(b, i + 2, e);
+      if (j < e && ld8(b, j) == ',') { *cs = i + 2; *ce = j; return true; }
+    }
+  }
+  return false;
+}
+
 struct R1Match { int64_t dev_s, dev_e, code_s, code_e; };
 // R1  NVRM: Xid \(((?:PCI:)?[0-9a-fA-F:]+)\).*?: (\d+),
 //  - "PCI:" is taken iff present ('P','I' are not in the class, so the no-prefix branch dies on it);
 //  - the class run is maximal and must be followed by ')' (a shorter run would be followed by a class byte);
 //  - `.*?` stops at the first ": " digits+ "," and cannot cross '\n'.
 __device__ bool match_r1(const ScanBuf& b, int64_t s, int64_t e, R1Match* m) {
-  for (int64_t a = find_byte(b, s, e, 'N'); a + 11 <= e; a = find_byte(b, a + 1, e, 'N')) {
-    if (ld8(b, a) != 'N' || !lit_at(b, a, e, "NVRM: Xid (")) continue;
+  for (int64_t a = find_lit(b, s, e, "NVRM: Xid ("); a >= 0; a = find_lit(b, a + 1, e, "NVRM: Xid (")) {
     int64_t p = a + 11, q = p;
     if (lit_at(b, q, e, "PCI:")) q += 4;
     int64_t r = q;
     while (r < e && (is_hex(ld8(b, r)) || ld8(b, r) == ':')) ++r;
     if (r == q || r >= e || ld8(b, r) != ')') continue;
-    for (int64_t i = r + 1; i < e; ++i) {
-      const int c = ld8(b, i);
-      if (c == '\n') break;
-      if (c == ':' && ld8(b, i + 1) == ' ' && is_digit(ld8(b, i + 2))) {
-        int64_t j = i + 2;
-        while (j < e && is_digit(ld8(b, j))) ++j;
-        if (j < e && ld8(b, j) == ',') {
-          m->dev_s = p; m->dev_e = r; m->code_s = i + 2; m->code_e = j;
-          return true;
-        }
-      }
-    }
+    if (lazy_code(b, r + 1, e, &m->code_s, &m->code_e)) { m->dev_s = p; m->dev_e = r; return true; }
   }
   return false;
 }
@@ -610,8 +640,7 @@ __device__ __forceinline__ bool take_hexword(const ScanBuf& b, int64_t& i, int64
 // R2 (kmsg.go:29).  Deterministic given the anchor: every greedy run is maximal and followed by a byte outside its class;
 // the optional ", pid=…, name=…" group is exclusive with the bare ", " continuation ('p' is not in [A-Z_]).
 __device__ bool match_r2(const ScanBuf& b, int64_t s, int64_t e, R2Match* m) {
-  for (int64_t a = find_byte(b, s, e, 'N'); a + 15 <= e; a = find_byte(b, a + 1, e, 'N')) {
-    if (ld8(b, a) != 'N' || !lit_at(b, a, e, "NVRM: Xid (PCI:")) continue;
+  for (int64_t a = find_lit(b, s, e, "NVRM: Xid (PCI:"); a >= 0; a = find_lit(b, a + 1, e, "NVRM: Xid (PCI:")) {
     int64_t i = a + 15;
     m->dev_s = i;
     while (i < e && (is_hex(ld8(b, i)) || ld8(b, i) == ':')) ++i;
@@ -702,16 +731,17 @@ __device__ bool take_bdf(const ScanBuf& b, int64_t i, int64_t e, int64_t* bs, in
   }
   return false;
 }
+// the head of R3 / R4, NVRM:\s+<lit>(BDF), at the "NVRM:" at a
+template <int N>
+__device__ __forceinline__ bool nvrm_bdf(const ScanBuf& b, int64_t a, int64_t e, const char (&lit)[N], int64_t* bs, int64_t* be) {
+  int64_t i = a + 5;
+  return skip_ws1(b, i, e) && lit_at(b, i, e, lit) && take_bdf(b, i + (N - 1), e, bs, be);
+}
 // R4  NVRM:\s+GPU (BDF)\.0:\s+GPU has fallen off the bus\.?
 __device__ bool match_r4(const ScanBuf& b, int64_t s, int64_t e, int64_t* bs, int64_t* be) {
-  for (int64_t a = find_byte(b, s, e, 'N'); a + 5 <= e; a = find_byte(b, a + 1, e, 'N')) {
-    if (ld8(b, a) != 'N' || !lit_at(b, a, e, "NVRM:")) continue;
-    int64_t i = a + 5;
-    if (!skip_ws1(b, i, e)) continue;
-    if (!lit_at(b, i, e, "GPU ")) continue;
-    i += 4;
-    if (!take_bdf(b, i, e, bs, be)) continue;
-    i = *be;
+  for (int64_t a = find_lit(b, s, e, "NVRM:"); a >= 0; a = find_lit(b, a + 1, e, "NVRM:")) {
+    if (!nvrm_bdf(b, a, e, "GPU ", bs, be)) continue;
+    int64_t i = *be;
     if (!lit_at(b, i, e, ".0:")) continue;
     i += 3;
     if (!skip_ws1(b, i, e)) continue;
@@ -722,41 +752,21 @@ __device__ bool match_r4(const ScanBuf& b, int64_t s, int64_t e, int64_t* bs, in
 }
 // R3  (?s)NVRM:\s+The NVIDIA GPU (BDF)\.0.*?fallen off the bus and is not responding to commands\.
 __device__ bool match_r3(const ScanBuf& b, int64_t s, int64_t e, int64_t* bs, int64_t* be) {
-  for (int64_t a = find_byte(b, s, e, 'N'); a + 5 <= e; a = find_byte(b, a + 1, e, 'N')) {
-    if (ld8(b, a) != 'N' || !lit_at(b, a, e, "NVRM:")) continue;
-    int64_t i = a + 5;
-    if (!skip_ws1(b, i, e)) continue;
-    if (!lit_at(b, i, e, "The NVIDIA GPU ")) continue;
-    i += 15;
-    if (!take_bdf(b, i, e, bs, be)) continue;
-    i = *be;
-    if (!lit_at(b, i, e, ".0")) continue;
-    i += 2;
-    for (int64_t k = i; k < e; ++k)
-      if (ld8(b, k) == 'f' && lit_at(b, k, e, "fallen off the bus and is not responding to commands.")) return true;
+  for (int64_t a = find_lit(b, s, e, "NVRM:"); a >= 0; a = find_lit(b, a + 1, e, "NVRM:")) {
+    if (!nvrm_bdf(b, a, e, "The NVIDIA GPU ", bs, be) || !lit_at(b, *be, e, ".0")) continue;
+    if (find_lit(b, *be + 2, e, "fallen off the bus and is not responding to commands.") >= 0) return true;
   }
   return false;
 }
 // R5  SXid.*?: (\d+),
 __device__ bool match_r5(const ScanBuf& b, int64_t s, int64_t e, int64_t* cs, int64_t* ce) {
-  for (int64_t a = find_byte(b, s, e, 'S'); a + 4 <= e; a = find_byte(b, a + 1, e, 'S')) {
-    if (ld8(b, a) != 'S' || !lit_at(b, a, e, "SXid")) continue;
-    for (int64_t i = a + 4; i < e; ++i) {
-      const int c = ld8(b, i);
-      if (c == '\n') break;
-      if (c == ':' && ld8(b, i + 1) == ' ' && is_digit(ld8(b, i + 2))) {
-        int64_t j = i + 2;
-        while (j < e && is_digit(ld8(b, j))) ++j;
-        if (j < e && ld8(b, j) == ',') { *cs = i + 2; *ce = j; return true; }
-      }
-    }
-  }
+  for (int64_t a = find_lit(b, s, e, "SXid"); a >= 0; a = find_lit(b, a + 1, e, "SXid"))
+    if (lazy_code(b, a + 4, e, cs, ce)) return true;
   return false;
 }
 // R6  SXid \((PCI:[0-9a-fA-F:\.]+)\)
 __device__ bool match_r6(const ScanBuf& b, int64_t s, int64_t e, int64_t* ds, int64_t* de) {
-  for (int64_t a = find_byte(b, s, e, 'S'); a + 10 <= e; a = find_byte(b, a + 1, e, 'S')) {
-    if (ld8(b, a) != 'S' || !lit_at(b, a, e, "SXid (PCI:")) continue;
+  for (int64_t a = find_lit(b, s, e, "SXid (PCI:"); a >= 0; a = find_lit(b, a + 1, e, "SXid (PCI:")) {
     int64_t i = a + 10;
     while (i < e && (is_hex(ld8(b, i)) || ld8(b, i) == ':' || ld8(b, i) == '.')) ++i;
     if (i == a + 10 || i >= e || ld8(b, i) != ')') continue;
@@ -895,49 +905,42 @@ __device__ void copy_span(const ScanBuf& b, int64_t s, int64_t e, char* dst, int
 __device__ bool xid_match_unit(const ScanBuf& g, int64_t s, int64_t e, const gpud_tables* T, gpud_xid_hit* h) {
   const ScanBuf b{g.p, e};      // every byte access of the automata is bounded by the unit end
   R2Match m2;
-  if (match_r2(b, s, e, &m2)) {                         // ExtractNVRMXidInfoExtended (kmsg.go:116-183)
-    long long code, link;
-    uint32_t intr, es;
-    if (go_atoi(b, m2.code_s, m2.code_e, &code) && go_parse_hex32(b, m2.hex_s[0], m2.hex_e[0], &intr) &&
-        go_parse_hex32(b, m2.hex_s[1], m2.hex_e[1], &es) && go_atoi(b, m2.link_s, m2.link_e, &link) && code > 0 && code < GPUD_T_MAX_XID) {
-      h->kind = GPUD_KIND_XID; h->code = (int32_t)code; h->flags = GPUD_HIT_EXTENDED;
-      h->intrinfo = intr; h->error_status = es; h->link = link; h->sub_code = (int32_t)((intr >> 20) & 0x3F);
-      h->severity_fatal = m2.fatal; h->xc = m2.xc;
-      h->n_extra = 0;
-      for (int k = 2; k < m2.n_hex; ++k) {
-        uint32_t v;
-        if (go_parse_hex32(b, m2.hex_s[k], m2.hex_e[k], &v)) h->extra[h->n_extra++] = v;
-      }
-      h->unit_name_off = m2.unit_s; h->unit_name_len = (int32_t)(m2.unit_e - m2.unit_s);
-      h->pid_off = m2.pid_s; h->pid_len = (int32_t)(m2.pid_e - m2.pid_s);
-      h->pname_off = m2.name_s; h->pname_len = (int32_t)(m2.name_e - m2.name_s);
-      h->inj_off = m2.inj_s; h->inj_len = (int32_t)(m2.inj_e - m2.inj_s);
-      copy_span(b, m2.unit_s, m2.unit_e, h->unit_name, 40, nullptr);
-      if (h->unit_name_len >= 40) h->flags |= GPUD_HIT_DEV_TRUNCATED;   // inline copy cut; no catalog alias is that long
-      if (h->code > 0 && h->code < GPUD_T_MAX_XID && T->xid[h->code].present) {   // detailFromNVLinkInfo needs only the base code to
-        h->event_type = kPendingExtended;                                            // exist; the table searches run warp-wide in k_scan_finish
-        h->dev_off = m2.dev_s; h->dev_len = (int32_t)(m2.dev_e - m2.dev_s);
-        copy_span(b, m2.dev_s, m2.dev_e, h->device, 40, "PCI:");      // kmsg.go:206-208
-        if (h->dev_len + 4 > 39) h->flags |= GPUD_HIT_DEV_TRUNCATED;
-        return true;
-      }
-      // base code unknown -> fall through to the combined regex, like Match does
-      h->flags = 0; h->n_extra = 0; h->sub_code = 0; h->intrinfo = h->error_status = 0; h->link = 0; h->unit_name[0] = 0;
-      h->unit_name_len = h->pid_len = h->pname_len = h->inj_len = 0; h->severity_fatal = h->xc = 0;
+  long long code, link;
+  uint32_t intr, es;
+  // ExtractNVRMXidInfoExtended (kmsg.go:116-183).  detailFromNVLinkInfo needs only the base code to exist (its table searches run
+  // warp-wide in k_scan_finish); an unknown base code falls through to the combined regex, like Match does
+  if (match_r2(b, s, e, &m2) && go_atoi(b, m2.code_s, m2.code_e, &code) && go_parse_hex32(b, m2.hex_s[0], m2.hex_e[0], &intr) &&
+      go_parse_hex32(b, m2.hex_s[1], m2.hex_e[1], &es) && go_atoi(b, m2.link_s, m2.link_e, &link) && code > 0 && code < GPUD_T_MAX_XID &&
+      T->xid[code].present) {
+    h->kind = GPUD_KIND_XID; h->code = (int32_t)code; h->flags = GPUD_HIT_EXTENDED;
+    h->intrinfo = intr; h->error_status = es; h->link = link; h->sub_code = (int32_t)((intr >> 20) & 0x3F);
+    h->severity_fatal = m2.fatal; h->xc = m2.xc;
+    h->n_extra = 0;
+    for (int k = 2; k < m2.n_hex; ++k) {
+      uint32_t v;
+      if (go_parse_hex32(b, m2.hex_s[k], m2.hex_e[k], &v)) h->extra[h->n_extra++] = v;
     }
+    h->unit_name_off = m2.unit_s; h->unit_name_len = (int32_t)(m2.unit_e - m2.unit_s);
+    h->pid_off = m2.pid_s; h->pid_len = (int32_t)(m2.pid_e - m2.pid_s);
+    h->pname_off = m2.name_s; h->pname_len = (int32_t)(m2.name_e - m2.name_s);
+    h->inj_off = m2.inj_s; h->inj_len = (int32_t)(m2.inj_e - m2.inj_s);
+    copy_span(b, m2.unit_s, m2.unit_e, h->unit_name, 40, nullptr);
+    if (h->unit_name_len >= 40) h->flags |= GPUD_HIT_DEV_TRUNCATED;   // inline copy cut; no catalog alias is that long
+    h->event_type = kPendingExtended;
+    h->dev_off = m2.dev_s; h->dev_len = (int32_t)(m2.dev_e - m2.dev_s);
+    copy_span(b, m2.dev_s, m2.dev_e, h->device, 40, "PCI:");      // kmsg.go:206-208
+    if (h->dev_len + 4 > 39) h->flags |= GPUD_HIT_DEV_TRUNCATED;
+    return true;
   }
   R1Match m1;
-  if (match_r1(b, s, e, &m1)) {                         // ExtractNVRMXidInfo (kmsg.go:73-80)
-    long long code;
-    if (go_atoi(b, m1.code_s, m1.code_e, &code) && code != 0) {
-      if (code < 0 || code >= GPUD_T_MAX_XID) return false;       // GetDetail miss => nil, no fall-through (kmsg.go:219-222)
-      h->kind = GPUD_KIND_XID; h->code = (int32_t)code; h->flags = 0;
-      if (!classify_plain_xid(T, h)) return false;
-      h->dev_off = m1.dev_s; h->dev_len = (int32_t)(m1.dev_e - m1.dev_s);
-      copy_span(b, m1.dev_s, m1.dev_e, h->device, 40, nullptr);
-      if (h->dev_len > 39) h->flags |= GPUD_HIT_DEV_TRUNCATED;
-      return true;
-    }
+  if (match_r1(b, s, e, &m1) && go_atoi(b, m1.code_s, m1.code_e, &code) && code != 0) {   // ExtractNVRMXidInfo (kmsg.go:73-80)
+    if (code < 0 || code >= GPUD_T_MAX_XID) return false;       // GetDetail miss => nil, no fall-through (kmsg.go:219-222)
+    h->kind = GPUD_KIND_XID; h->code = (int32_t)code; h->flags = 0;
+    if (!classify_plain_xid(T, h)) return false;
+    h->dev_off = m1.dev_s; h->dev_len = (int32_t)(m1.dev_e - m1.dev_s);
+    copy_span(b, m1.dev_s, m1.dev_e, h->device, 40, nullptr);
+    if (h->dev_len > 39) h->flags |= GPUD_HIT_DEV_TRUNCATED;
+    return true;
   }
   int64_t bs, be;
   if (match_r4(b, s, e, &bs, &be) || match_r3(b, s, e, &bs, &be)) {   // extractFallenOffBusXidInfo (kmsg.go:247-257)
@@ -973,34 +976,9 @@ __device__ bool sxid_match_unit(const ScanBuf& g, int64_t s, int64_t e, const gp
 // `.` never crosses '\n' (no (?s) in these patterns); negated classes do.  Returns the hit kind (0 = no match) and,
 // for the patterns with a capture the component puts in its message, the capture span.
 // ---------------------------------------------------------------------------------------------
-__device__ int64_t find_lit(const ScanBuf& b, int64_t from, int64_t to, const char* lit, int n) {   // first start in [from, to - n], else -1
-  const unsigned c0 = (unsigned char)lit[0];
-  for (int64_t i = find_byte(b, from, to, c0); i + n <= to; i = find_byte(b, i + 1, to, c0)) {
-    bool ok = true;
-    for (int k = 1; k < n && ok; ++k) ok = __ldg(b.p + i + k) == (uint8_t)lit[k];
-    if (ok) return i;
-  }
-  return -1;
-}
-template <int N>
-__device__ __forceinline__ int64_t find_lit(const ScanBuf& b, int64_t from, int64_t to, const char (&s)[N]) { return find_lit(b, from, to, s, N - 1); }
-__device__ __forceinline__ int64_t digits_end(const ScanBuf& b, int64_t p, int64_t e) { while (p < e && is_digit(ld8(b, p))) ++p; return p; }
 __device__ __forceinline__ bool is_word(int c) { return is_digit(c) || (c >= 'a' && c <= 'z') || (c >= 'A' && c <= 'Z') || c == '_'; }
 
-// last start in [from, to - n] of the n-byte literal, else -1
-__device__ int64_t rfind_lit(const ScanBuf& b, int64_t from, int64_t to, const char* lit, int n) {
-  const unsigned c0 = (unsigned char)lit[0];
-  for (int64_t i = rfind_byte(b, from, to - n + 1, c0); i >= from; i = rfind_byte(b, from, i, c0)) {
-    bool ok = true;
-    for (int k = 1; k < n && ok; ++k) ok = __ldg(b.p + i + k) == (uint8_t)lit[k];
-    if (ok) return i;
-  }
-  return -1;
-}
-template <int N>
-__device__ __forceinline__ int64_t rfind_lit(const ScanBuf& b, int64_t from, int64_t to, const char (&s)[N]) { return rfind_lit(b, from, to, s, N - 1); }
-
-// sp_off / sp_len: up to five capture spans in the hit's slot order (dev, unit_name, pid, pname, inj)
+// sp_off / sp_len: up to five capture spans in the hit's slot order (cap_slot)
 __device__ int ext_match_at(int fam, const ScanBuf& b, int64_t a, int64_t ms, int64_t ue, int64_t* sp_off, int32_t* sp_len) {
   int64_t* cap_off = sp_off;
   int32_t* cap_len = sp_len;
@@ -1154,6 +1132,18 @@ __device__ int ext_match_at(int fam, const ScanBuf& b, int64_t a, int64_t ms, in
 // ---------------------------------------------------------------------------------------------
 // K5c: one thread per candidate anchor
 // ---------------------------------------------------------------------------------------------
+// capture slot k of a hit (offset and length in the buffer): 0 dev, 1 unit_name, 2 pid, 3 pname, 4 inj
+struct CapSlot { int64_t& off; int32_t& len; };
+__host__ __device__ __forceinline__ CapSlot cap_slot(gpud_xid_hit& h, int k) {
+  switch (k) {
+    case 0: return {h.dev_off, h.dev_len};
+    case 1: return {h.unit_name_off, h.unit_name_len};
+    case 2: return {h.pid_off, h.pid_len};
+    case 3: return {h.pname_off, h.pname_len};
+    default: return {h.inj_off, h.inj_len};
+  }
+}
+
 __device__ __forceinline__ bool is_sep(const ScanBuf& b, int64_t i, int mode) {
   if (ld8(b, i) != '\n') return false;
   return mode == GPUD_SCAN_LINES || ld8(b, i + 1) != ' ';
@@ -1273,11 +1263,8 @@ __global__ void __launch_bounds__(128, GPUD_MATCH_BLOCKS) k_scan_match(ScanBuf b
       h.rule_index = -1;
       h.unit_offset = us;
       h.link = a;                                          // where the match is anchored (ties between candidates of one unit)
-      h.dev_off = sp_off[0]; h.dev_len = sp_len[0];
-      h.unit_name_off = sp_off[1]; h.unit_name_len = sp_len[1];
-      h.pid_off = sp_off[2]; h.pid_len = sp_len[2];
-      h.pname_off = sp_off[3]; h.pname_len = sp_len[3];
-      h.inj_off = sp_off[4]; h.inj_len = sp_len[4];
+#pragma unroll
+      for (int k = 0; k < 5; ++k) { const CapSlot c = cap_slot(h, k); c.off = sp_off[k]; c.len = sp_len[k]; }
       for (int i = 0; i < sp_len[0] && i < 39; ++i) h.device[i] = (char)ld8(b, sp_off[0] + i);
       for (int i = 0; i < sp_len[1] && i < 39; ++i) h.unit_name[i] = (char)ld8(b, sp_off[1] + i);
       if (sp_len[0] > 39) h.flags |= GPUD_HIT_DEV_TRUNCATED;
@@ -1291,31 +1278,23 @@ __global__ void __launch_bounds__(128, GPUD_MATCH_BLOCKS) k_scan_match(ScanBuf b
     // its kind, and it runs the whole decision procedure from the unit's first relevant "NVRM:" anchor.
     // The three scans of [unit start, a) below are skipped when the walk back saw none of their first bytes there - the usual case
     // (a timestamp, then the anchor): they were 3 of the ~5 passes a candidate makes over its line.
+    // An earlier literal starts in [ms, a) but may run on past a, up to the unit end: hence the search bounds min(a + n - 1, ue).
     const bool no_nf = !note.all && (note.nf & 0x80808080u) == 0u, no_s = !note.all && (note.s & 0x80808080u) == 0u;
-    bool first = true;
     int64_t a0 = a;
     if (fam == kFamS) {
-      if (!no_s)
-        for (int64_t i = find_byte(b, ms, a, 'S'); i < a && first; i = find_byte(b, i + 1, a, 'S'))
-          if (lit_at(b, i, ue, "SXid")) first = false;
+      if (!no_s && find_lit(b, ms, min(a + 3, ue), "SXid") >= 0) return false;
     } else {
       if (fam == kFamX && !lit_at(b, a, ue, "NVRM: Xid (")) return false;          // the filter judged it against the buffer end, not the unit end
       if (fam == kFamB && !lit_at(b, a, ue, "fallen off the bus")) return false;
-      if (!no_nf) {
-        for (int64_t i = find_byte(b, ms, a, 'N'); i < a && first; i = find_byte(b, i + 1, a, 'N'))
-          if (lit_at(b, i, ue, "NVRM: Xid (")) first = false;
-        for (int64_t i = find_byte(b, ms, a, 'f'); i < a && first; i = find_byte(b, i + 1, a, 'f'))
-          if (lit_at(b, i, ue, "fallen off the bus")) first = false;
-      }
-      if (!first) return false;
+      if (!no_nf && (find_lit(b, ms, min(a + 10, ue), "NVRM: Xid (") >= 0 || find_lit(b, ms, min(a + 17, ue), "fallen off the bus") >= 0))
+        return false;
       a0 = -1;                                                                   // the unit's first "NVRM:" an R1-R4 match can start at
       if (no_nf && fam == kFamX) a0 = a;                                         // no 'N' before a, and a is "NVRM: Xid ("
       else
-        for (int64_t i = find_byte(b, no_nf && a > ms ? a : ms, ue, 'N'); i < ue; i = find_byte(b, i + 1, ue, 'N'))
-          if (lit_at(b, i, ue, "NVRM:") && nvrm_family(b, i, ue)) { a0 = i; break; }
+        for (int64_t i = find_lit(b, no_nf && a > ms ? a : ms, ue, "NVRM:"); i >= 0; i = find_lit(b, i + 1, ue, "NVRM:"))
+          if (nvrm_family(b, i, ue)) { a0 = i; break; }
       if (a0 < 0) return false;
     }
-    if (!first) return false;
     memset(&h, 0, sizeof h);
     // every pattern starts with this family's anchor literal and `a` is the unit's first such anchor: start there
     const bool ok = (fam == kFamS) ? sxid_match_unit(b, a, ue, T, &h) : xid_match_unit(b, a0, ue, T, &h);
@@ -1426,6 +1405,15 @@ __global__ void k_classify(const gpud_tables* __restrict__ T, gpud_xid_hit* hits
 // =================================================================================================
 // host side
 // =================================================================================================
+// the scan's device counters, zeroed before every scan; the kernels take pointers to the members.  The host reads back the four
+// scalars (up to fam_cnt).
+struct ScanCounters {
+  unsigned long long n_cand, n_hits, n_sep;   // verified anchors (candidates), hits, unit separators
+  unsigned long long ticket;                  // k_scan_prefix_tiles: the last tile to finish scans the tile totals
+  unsigned long long fam_cnt[kSortBins];      // family histogram of the candidates (k_scan_filter)
+  unsigned long long fam_pos[kSortBins];      // per-family cursors of k_cand_scatter
+};
+
 struct gpud_scan_state {
   int dev = 0;
   gpud_tables* d_tables = nullptr;
@@ -1434,8 +1422,8 @@ struct gpud_scan_state {
   unsigned long long* d_cands = nullptr; size_t cand_cap = 0;
   unsigned long long* d_side = nullptr; size_t side_cap = 0;   // family-sorted copy of short candidate lists
   gpud_xid_hit* d_hits = nullptr; size_t hit_cap = 0;
-  unsigned long long* d_counters = nullptr;   // [0] n_cand [1] n_hits [2] n_sep
-  unsigned long long* h_counters = nullptr;   // pinned
+  ScanCounters* d_counters = nullptr;
+  ScanCounters* h_counters = nullptr;         // pinned
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};   // around filter / prefix / match of the last scan
   bool phase_timing = false;                                  // record ev[1], ev[2] too (and give up the overlapped launches, see launch_chain)
@@ -1467,8 +1455,8 @@ static int32_t scan_state_get(gpud_ctx* ctx, int dev, gpud_scan_state** out) {
     s->dev = dev;
     cudaError_t e = cudaMalloc(&s->d_tables, sizeof(gpud_tables));
     if (e == cudaSuccess) e = cudaMemcpy(s->d_tables, gpud_host_tables(), sizeof(gpud_tables), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMalloc(&s->d_counters, (4 + 2 * kSortBins) * sizeof(unsigned long long));   // + family histogram and cursors
-    if (e == cudaSuccess) e = cudaMallocHost(&s->h_counters, 4 * sizeof(unsigned long long));
+    if (e == cudaSuccess) e = cudaMalloc(&s->d_counters, sizeof(ScanCounters));
+    if (e == cudaSuccess) e = cudaMallocHost(&s->h_counters, sizeof(ScanCounters));
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
     for (auto& ev : s->ev) if (e == cudaSuccess) e = cudaEventCreate(&ev);
     if (e != cudaSuccess) {
@@ -1594,7 +1582,7 @@ static int32_t scan_launch(gpud_ctx* ctx, gpud_scan_state* s, const uint8_t* d_b
   GPUD_CUDA(ctx, gpud_grow(&s->d_tile_base, &s->tile_cap, (size_t)n_chunks / 1024 + 2));
   GPUD_CUDA(ctx, gpud_grow(&s->d_cands, &s->cand_cap, (size_t)(len / 4 + 1024)));
   GPUD_CUDA(ctx, gpud_grow(&s->d_hits, &s->hit_cap, (size_t)std::max<int64_t>(hit_cap_req, 1024)));
-  GPUD_CUDA(ctx, cudaMemsetAsync(s->d_counters, 0, (4 + 2 * kSortBins) * sizeof(unsigned long long), st));
+  GPUD_CUDA(ctx, cudaMemsetAsync(s->d_counters, 0, sizeof(ScanCounters), st));
   GPUD_CUDA(ctx, gpud_grow(&s->d_side, &s->side_cap, std::min<size_t>(s->cand_cap, (size_t)1 << 20)));
   if (len == 0) {
     GPUD_CUDA(ctx, cudaMemsetAsync(s->d_chunk_sep, 0, sizeof(uint32_t), st));
@@ -1606,39 +1594,36 @@ static int32_t scan_launch(gpud_ctx* ctx, gpud_scan_state* s, const uint8_t* d_b
   const bool ext = (mode & GPUD_SCAN_EXT_MATCHERS) != 0;
   mode &= kModeMask;
   const int grid = std::max(grid_f, 1);
-  const unsigned long long ccap = (unsigned long long)s->cand_cap;
-  if (mode == GPUD_SCAN_LINES && !ext) k_scan_filter<GPUD_SCAN_LINES, false><<<grid, 256, 0, st>>>(b, s->d_chunk_sep, s->d_cands, s->d_counters + 0, ccap, s->d_counters + 4, ext_tab());
-  else if (mode == GPUD_SCAN_LINES) k_scan_filter<GPUD_SCAN_LINES, true><<<grid, 256, 0, st>>>(b, s->d_chunk_sep, s->d_cands, s->d_counters + 0, ccap, s->d_counters + 4, ext_tab());
-  else if (!ext) k_scan_filter<GPUD_SCAN_RAW_KMSG, false><<<grid, 256, 0, st>>>(b, s->d_chunk_sep, s->d_cands, s->d_counters + 0, ccap, s->d_counters + 4, ext_tab());
-  else k_scan_filter<GPUD_SCAN_RAW_KMSG, true><<<grid, 256, 0, st>>>(b, s->d_chunk_sep, s->d_cands, s->d_counters + 0, ccap, s->d_counters + 4, ext_tab());
-  GPUD_CUDA(ctx, cudaGetLastError());
+  ScanCounters* const c = s->d_counters;
+  const auto filter = mode == GPUD_SCAN_LINES ? (ext ? k_scan_filter<GPUD_SCAN_LINES, true> : k_scan_filter<GPUD_SCAN_LINES, false>)
+                                              : (ext ? k_scan_filter<GPUD_SCAN_RAW_KMSG, true> : k_scan_filter<GPUD_SCAN_RAW_KMSG, false>);
+  GPUD_CUDA(ctx, launch_chain(false, filter, dim3(grid), dim3(256), st, b, s->d_chunk_sep, s->d_cands, &c->n_cand, (unsigned long long)s->cand_cap,
+                              c->fam_cnt, ext_tab()));
   // phase timing off (the default): no event between the kernels, so each launch may carry the programmatic-serialization attribute
   // (pdl_wait / pdl_release in the kernels); on: ev[1], ev[2] split the scan into filter / prefix / match and the launches are plain.
   const bool phased = s->phase_timing;
   s->last_phased = phased;
   if (phased) cudaEventRecord(s->ev[1], st);
   GPUD_CUDA(ctx, launch_chain(!phased, k_scan_prefix_tiles, dim3((unsigned)n_tiles), dim3(1024), st, (const uint32_t*)s->d_chunk_sep, s->d_chunk_local, n_chunks, s->d_tile_base,
-                              n_tiles, s->d_counters + 2, s->d_counters + 3));
+                              n_tiles, &c->n_sep, &c->ticket));
   if (phased) cudaEventRecord(s->ev[2], st);
   // candidates sorted by matcher family before the match step: faster on 100 MiB buffers, most with all 22 families switched on
   const unsigned long long side_cap = (unsigned long long)s->side_cap;
-  GPUD_CUDA(ctx, launch_chain(!phased, k_cand_scatter, dim3(64), dim3(256), st, (const unsigned long long*)s->d_cands, (const unsigned long long*)(s->d_counters + 0),
-                              (unsigned long long)s->cand_cap, (unsigned long long)s->side_cap, (const unsigned long long*)(s->d_counters + 4), s->d_counters + 4 + kSortBins,
-                              s->d_side));
+  GPUD_CUDA(ctx, launch_chain(!phased, k_cand_scatter, dim3(64), dim3(256), st, (const unsigned long long*)s->d_cands, &c->n_cand,
+                              (unsigned long long)s->cand_cap, (unsigned long long)s->side_cap, c->fam_cnt, c->fam_pos, s->d_side));
   static const int match_blocks = [] {
     int nb = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_scan_match, 128, 0) != cudaSuccess || nb < 1) nb = 4;
     return nb;
   }();
   GPUD_CUDA(ctx, launch_chain(!phased, k_scan_match, dim3((unsigned)(ctx->sm_count * match_blocks)), dim3(128), st, b, (int)mode,
-                              (const unsigned long long*)s->d_cands, (const unsigned long long*)s->d_side, side_cap, (const unsigned long long*)(s->d_counters + 0),
+                              (const unsigned long long*)s->d_cands, (const unsigned long long*)s->d_side, side_cap, &c->n_cand,
                               (unsigned long long)s->cand_cap, (const uint32_t*)s->d_chunk_local, (const unsigned long long*)s->d_tile_base, (const gpud_tables*)s->d_tables,
-                              s->d_hits, (unsigned long long)s->hit_cap, s->d_counters + 1));
+                              s->d_hits, (unsigned long long)s->hit_cap, &c->n_hits));
   GPUD_CUDA(ctx, launch_chain(!phased, k_scan_finish, dim3((unsigned)(ctx->sm_count * 16)), dim3(256), st, b, (int)mode, (const uint32_t*)s->d_chunk_local,
-                              (const unsigned long long*)s->d_tile_base, (const gpud_tables*)s->d_tables, s->d_hits, (const unsigned long long*)(s->d_counters + 1),
-                              (unsigned long long)s->hit_cap));
+                              (const unsigned long long*)s->d_tile_base, (const gpud_tables*)s->d_tables, s->d_hits, &c->n_hits, (unsigned long long)s->hit_cap));
   cudaEventRecord(s->ev[3], st);
-  GPUD_CUDA(ctx, cudaMemcpyAsync(s->h_counters, s->d_counters, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  GPUD_CUDA(ctx, cudaMemcpyAsync(s->h_counters, c, offsetof(ScanCounters, fam_cnt), cudaMemcpyDeviceToHost, st));
   return GPUD_OK;
 }
 
@@ -1649,7 +1634,7 @@ static int32_t scan_run(gpud_ctx* ctx, gpud_scan_state* s, const uint8_t* d_buf,
   int32_t rc = scan_launch(ctx, s, d_buf, len, mode, cap, st);
   if (rc) return rc;
   GPUD_CUDA(ctx, cudaStreamSynchronize(st));
-  const int64_t found = (int64_t)s->h_counters[1];
+  const int64_t found = (int64_t)s->h_counters->n_hits;
   if (found <= (int64_t)s->hit_cap) return GPUD_OK;
   rc = scan_launch(ctx, s, d_buf, len, mode, found, st);
   if (rc) return rc;
@@ -1660,10 +1645,11 @@ static int32_t scan_run(gpud_ctx* ctx, gpud_scan_state* s, const uint8_t* d_buf,
 // after scan_run: the device list holds every hit
 static int32_t scan_collect(gpud_ctx* ctx, gpud_scan_state* s, gpud_xid_hit* hits, int64_t cap, int64_t* n_hits, int64_t* n_units,
                             cudaStream_t st) {
-  const int64_t found = (int64_t)s->h_counters[1];
+  const ScanCounters& c = *s->h_counters;
+  const int64_t found = (int64_t)c.n_hits;
   if (n_hits) *n_hits = found;
-  if (n_units) *n_units = (int64_t)s->h_counters[2] + 1;
-  if (s->h_counters[0] > s->cand_cap) return gpud_fail(ctx, GPUD_E_CAPACITY, "candidate list overflow (%llu)", s->h_counters[0]);
+  if (n_units) *n_units = (int64_t)c.n_sep + 1;
+  if (c.n_cand > s->cand_cap) return gpud_fail(ctx, GPUD_E_CAPACITY, "candidate list overflow (%llu)", c.n_cand);
   // hits land in a pinned host buffer; only 24-byte keys are sorted, each 288-byte record moves once
   if ((size_t)found > s->h_hits_cap) {
     if (s->h_hits) cudaFreeHost(s->h_hits);
@@ -1861,8 +1847,8 @@ extern "C" int32_t gpud_kmsg_scan_stats(gpud_ctx* ctx, int32_t dev, int64_t* out
   gpud_scan_state* s;
   int32_t rc = scan_state_get(ctx, dev, &s);
   if (rc) return rc;
-  out3[0] = (int64_t)s->h_counters[0];   // verified anchors (candidates)
-  out3[1] = (int64_t)s->h_counters[1];   // hits
-  out3[2] = (int64_t)s->h_counters[2];   // separators
+  out3[0] = (int64_t)s->h_counters->n_cand;
+  out3[1] = (int64_t)s->h_counters->n_hits;
+  out3[2] = (int64_t)s->h_counters->n_sep;
   return GPUD_OK;
 }
