@@ -8,7 +8,7 @@ from typing import List, Optional, Sequence
 import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("GPUD_B200_LIB") or os.path.join(_HERE, "libgpud_b200.so")   # override: kernel-variant experiments only
+LIB_PATH = os.environ.get("GPUD_B200_LIB") or os.path.join(_HERE, "libgpud_b200.so")   # override: another build of the library, e.g. the ASan build of tools/build_asan.sh
 
 OPS = {"min": 0, "max": 1, "mean": 2, "ema": 3, "p99": 4, "n_over": 5}
 EVENT_NAMES = ["Unknown", "Info", "Warning", "Critical", "Fatal"]

@@ -41,17 +41,12 @@ constexpr int kPendingExtended = -77;         // event_type of an extended hit w
 constexpr int kFamShift = 58;               // candidate word = byte offset | family << 58
 constexpr int kExtFam0 = 4, kNumFam = 25;
 constexpr int kModeMask = 0xff;
-#ifndef GPUD_MATCH_BLOCKS
-#define GPUD_MATCH_BLOCKS 5                  // resident 128-thread blocks per SM the match kernel is compiled for (register budget)
-#endif
-#ifndef GPUD_FILTER_BLOCKS
-#define GPUD_FILTER_BLOCKS 3
-#endif
+constexpr int kMatchBlocks = 5;             // resident 128-thread blocks per SM the match kernel is compiled for (register budget)
 // Resident 256-thread blocks per SM of k_scan_filter (its launch bounds and grid).  H100 (sm_90a), 100 MiB buffer, whole scan / filter
 // alone: 4 blocks cap the filter at 64 registers and ptxas spills (36 B per thread, 148 B with the extra matchers): 0.186-0.189 / 0.089
 // ms, extra matchers 0.238-0.244 ms; 3 blocks (72 / 80 registers, no spill) 0.171-0.177 / 0.084-0.087, extra matchers 0.225; 2 blocks
 // 0.173-0.177, extra matchers 0.233-0.236.  Hits identical throughout.
-constexpr int kFilterBlocks = GPUD_FILTER_BLOCKS;
+constexpr int kFilterBlocks = 3;
 
 // Programmatic dependent launch (sm_90+): the five kernels of a scan run back to back on one stream, each short enough that the gap
 // between one grid draining and the next starting was a large share of the scan.  Every kernel lets its successor be
@@ -1187,7 +1182,7 @@ __global__ void __launch_bounds__(256) k_cand_scatter(const unsigned long long* 
   }
 }
 
-__global__ void __launch_bounds__(128, GPUD_MATCH_BLOCKS) k_scan_match(ScanBuf b, int mode, const unsigned long long* __restrict__ cands_in,
+__global__ void __launch_bounds__(128, kMatchBlocks) k_scan_match(ScanBuf b, int mode, const unsigned long long* __restrict__ cands_in,
                                                      const unsigned long long* __restrict__ side, unsigned long long side_cap,
                                                      const unsigned long long* __restrict__ n_cand, unsigned long long cand_cap,
                                                      const uint32_t* __restrict__ chunk_local, const unsigned long long* __restrict__ tile_base, const gpud_tables* __restrict__ T,

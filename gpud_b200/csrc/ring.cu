@@ -21,10 +21,7 @@
 
 namespace {
 
-#ifndef GPUD_WARPS_PER_BLOCK
-#define GPUD_WARPS_PER_BLOCK 8
-#endif
-constexpr int kWarpsPerBlock = GPUD_WARPS_PER_BLOCK;
+constexpr int kWarpsPerBlock = 8;
 constexpr int kCandMax = 64;
 constexpr unsigned kFull = 0xffffffffu;
 constexpr size_t kStageBytes = 32u << 20;   // pinned staging buffers (x2)
@@ -220,6 +217,7 @@ constexpr int kWarpSmemBytes = kCntOff + 16;
 constexpr int kBlockSmemBytes = kWarpsPerBlock * kWarpSmemBytes;
 
 __device__ __forceinline__ int elem_index(int row, int col) { return 64 * (col >> 1) + 2 * row + (col & 1); }   // chronological t
+__device__ __forceinline__ int elem_slot(int t) { return ((t & 63) >> 1) * kRowU64 + 2 * (t >> 6) + (t & 1); }   // its inverse: t's offset in the key rows
 
 // Append the entries of the flagged rows that pass the bound to cand[] (any order, RAW form).  HI_ONLY: keys whose high
 // word is >= Lh (the fast path's bound is (Lh, 0), inclusive), tested on the raw word: key_hi >= Lh  <=>
@@ -326,29 +324,77 @@ __device__ __forceinline__ double2 ld_stream(const double2* p) {
   asm volatile("ld.global.nc.L1::no_allocate.L2::256B.v2.f64 {%0, %1}, [%2];" : "=d"(r.x), "=d"(r.y) : "l"(p));
   return r;
 }
-#ifndef GPUD_PREFETCH_PAIRS
-#define GPUD_PREFETCH_PAIRS 8
-#endif
-constexpr int kPrefetchPairs = GPUD_PREFETCH_PAIRS;      // register pairs of the NEXT window loaded under the current post-processing
+constexpr int kPrefetchPairs = 8;                        // register pairs of the NEXT window loaded under the current post-processing
 // H100 SXM (400 W limit), survey stream, kernel ms for 4 GiB: 8 pairs + 2 CTAs/SM (112 registers, no spill) 1.53; 12 pairs + 2 CTAs
 // 1.53; 16 pairs + 2 CTAs 2.95 (the 128-register cap spills ~530 B per thread); 16 pairs + 1 CTA 1.62; 8 pairs + 3 CTAs (80-register
 // cap, spills) 1.85.  The rest of the window is loaded by fetch_rest() at the top of the trip that consumes it.
 constexpr int kCtasPerSM = 2;                            // k_window_reduce occupancy: its launch bounds and its persistent grid
 
-#ifdef GPUD_EXPERIMENT_FINISH
-// EXPERIMENT (`-DGPUD_EXPERIMENT_FINISH`, tools/exp_warp_finish.py): every warp of the hot instantiation records its %globaltimer at
-// entry and at exit and the number of windows it reduced, so the spread of warp finish times within one launch can be read back.
-constexpr int kExpMaxWarps = 4096;
-__device__ unsigned long long g_exp_finish[kExpMaxWarps][3];   // {start ns, end ns, windows}
-__device__ __forceinline__ unsigned long long global_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
+// Whole-range pass (RANGE): no per-window order statistic.  The exact maximum is found the way the minimum is, then the samples
+// pass 1 flagged (lo <= x <= hi as doubles) are classified exactly on their totalOrder keys: above hi (+0 over a -0 pivot), == hi,
+// == lo, below lo (-0 under a +0 pivot), and the rest - strictly inside - goes to the field's list.  Returns the window's
+// {keys above hi, keys == hi, keys == lo, keys strictly inside}.
+__device__ __forceinline__ uint4 classify_window(const WinParams& p, const unsigned long long* sk, int f, int m, bool lo_zero, unsigned mh,
+                                                 unsigned abv, unsigned inmask, double piv_lo, double piv_hi, int lane, K64& wmax) {
+  wmax.hi = __reduce_max_sync(kFull, mh);
+  if (lo_zero) {
+    wmax.lo = true_lo(wmax.hi, 0u);
+  } else {
+    wmax.lo = extreme_lo<true>(sk, mh, wmax.hi, m, lane);
+  }
+  unsigned n_eh = 0, n_el = 0, n_in = 0;
+  if (__any_sync(kFull, inmask != 0u)) {
+    const unsigned long long lok = gpud_f64_key((unsigned long long)__double_as_longlong(piv_lo));
+    const unsigned long long hik = gpud_f64_key((unsigned long long)__double_as_longlong(piv_hi));
+    // equal pivots that are not a zero: lo <= x <= hi as doubles already means key == hi (a tie-heavy gauge: every flagged
+    // sample is a copy of the pivot), no need to look at the keys
+    const bool all_equal = lok == hik && piv_hi != 0.0;
+    if (all_equal) { n_eh = (unsigned)__popc(inmask); inmask = 0u; }
+    unsigned mm = inmask;
+    while (mm) {
+      const int i = __ffs(mm) - 1;
+      mm &= mm - 1;
+      const unsigned long long key = true_key(sk[lane * kRowU64 + i]);
+      const bool inside = key > lok && key < hik;
+      abv += key > hik ? 1u : 0u;
+      n_eh += key == hik ? 1u : 0u;
+      n_el += (key == lok && lok != hik) ? 1u : 0u;
+      if (!inside) inmask ^= 1u << i;
+    }
+    const int c = __popc(inmask);
+    int incl = c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(kFull, incl, o);
+      if (lane >= o) incl += t;
+    }
+    n_in = (unsigned)__shfl_sync(kFull, incl, 31);
+    if (n_in) {
+      unsigned base = 0;
+      if (lane == 0) base = atomicAdd(p.fill + f, n_in);
+      base = __shfl_sync(kFull, base, 0);
+      unsigned pos = base + (unsigned)(incl - c);
+      unsigned long long* __restrict__ list = p.lists + (int64_t)f * p.list_cap;
+      mm = inmask;
+      while (mm) {
+        const int i = __ffs(mm) - 1;
+        mm &= mm - 1;
+        if (pos < p.list_cap) list[pos] = true_key(sk[lane * kRowU64 + i]);
+        ++pos;
+      }
+    }
+  }
+  uint4 cls;
+  cls.x = __reduce_add_sync(kFull, abv);
+  cls.y = __reduce_add_sync(kFull, n_eh);
+  cls.z = __reduce_add_sync(kFull, n_el);
+  cls.w = n_in;
+  return cls;
 }
-#endif
 
 // The warp loop of k_window_reduce: reduces the units it claims from the work cursor until the cursor runs out and returns how
 // many it reduced.  TAIL: the units are the w_skip[0..n_tail) windows of every field (claimed from cursor[1]).
+// Nothing reads the count.  It stays because without it ptxas (CUDA 12.9) emits pass 1's four accumulator zeroings in another order.
 template <bool ALIGNED, int JF, bool RANGE, bool TAIL>
 __device__ __forceinline__ int window_loop(const WinParams& p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -407,6 +453,17 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
       if (t0 + 1 < q.m) { int64_t a = q.p0 + t0 + 1; if (a >= p.cap) a -= p.cap; v[j].y = __ldcs(base + a); }
     }
   };
+  // register pairs [j0, j1) of an aligned window.  The loop walks all 16 pairs: starting it at j0 moves registers in <true, 15, false>.
+  auto load_pairs = [&](const WinUnit& q, int j0, int j1) {
+    const double2* __restrict__ b2 = reinterpret_cast<const double2*>(p.ring + (int64_t)q.f * p.cap + q.p0) + lane;
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      if (j < j0 || j >= j1) continue;
+      if (JF >= 0 && j < JF) { v[j] = ld_stream(b2 + 32 * j); continue; }
+      v[j] = make_double2(0.0, 0.0);
+      if (64 * j + 2 * lane < q.m) v[j] = ld_stream(b2 + 32 * j);   // element t0+1 == m is masked in pass 1 (the ring has slack)
+    }
+  };
   // fetch the next non-skipped unit of this warp (if any) and issue its first kPrefetchPairs loads.  Alternatives that were
   // slower: choosing the next unit BEFORE pass 1 (its address/threshold registers live through pass 1) and issuing each
   // pair's load inside pass 1 right after the pair is consumed.  TAIL loads nothing ahead: a warp reduces at most a few tail
@@ -424,35 +481,16 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
     q.m = JF >= 0 ? p.W : (int)min((int64_t)p.W, p.count - c0);
     q.p0 = p.start + c0;
     if (q.p0 >= p.cap) q.p0 -= p.cap;
-    const double* __restrict__ base = p.ring + (int64_t)q.f * p.cap;
     thr_next = __ldg(p.thr + q.f);
     if (RANGE) { lo_next = __ldg(p.piv + 2 * q.f); hi_next = __ldg(p.piv + 2 * q.f + 1); }
-    if (ALIGNED) {
-      const double2* __restrict__ b2 = reinterpret_cast<const double2*>(base + q.p0) + lane;
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        if (j >= PF) continue;                                     // the rest is loaded by fetch_rest() at the top of the next trip
-        if (JF >= 0 && j < JF) { v[j] = ld_stream(b2 + 32 * j); continue; }
-        v[j] = make_double2(0.0, 0.0);
-        if (64 * j + 2 * lane < q.m) v[j] = ld_stream(b2 + 32 * j);   // element t0+1 == m is masked in pass 1 (the ring has slack)
-      }
-    } else if (!TAIL) {
-      load_unaligned(q);
-    }
+    if (ALIGNED) load_pairs(q, 0, PF);   // the rest is loaded by fetch_rest() at the top of the next trip
+    else if (!TAIL) load_unaligned(q);
     return true;
   };
 
   auto fetch_rest = [&](const WinUnit& q) {
     if (TAIL) load_unaligned(q);
-    if (PF >= 16) return;
-    const double2* __restrict__ b2 = reinterpret_cast<const double2*>(p.ring + (int64_t)q.f * p.cap + q.p0) + lane;
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      if (j < PF) continue;
-      if (JF >= 0 && j < JF) { v[j] = ld_stream(b2 + 32 * j); continue; }
-      v[j] = make_double2(0.0, 0.0);
-      if (64 * j + 2 * lane < q.m) v[j] = ld_stream(b2 + 32 * j);
-    }
+    if (PF < 16) load_pairs(q, PF, 16);
   };
 
   WinUnit cur, nxt;
@@ -562,7 +600,7 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
     bool positional = false;
     if (!RANGE && !lo_zero && tied_nonneg && m == p.W && m > 960 && p.k_full >= 1 && p.k_full <= 32) {
       const int tk = m - p.k_full;
-      auto at = [&](int t) { return __longlong_as_double((long long)sk[((t & 63) >> 1) * kRowU64 + 2 * (t >> 6) + (t & 1)]); };
+      auto at = [&](int t) { return __longlong_as_double((long long)sk[elem_slot(t)]); };
       const double e0 = at(0), tv = at(tk), el = at(m - 1);
       bool ok = true;
       const int i_low = tk >= 960 ? 30 : 0;          // the usual case (k <= m - 960): entries 0..29 (t < 960) all lie before sample m - k
@@ -605,7 +643,7 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
       bool done = false;
       if (positional) {
         const int tk = m - k, tl = m - 1;
-        const unsigned long long ra = sk[((tk & 63) >> 1) * kRowU64 + 2 * (tk >> 6) + (tk & 1)], rl = sk[((tl & 63) >> 1) * kRowU64 + 2 * (tl >> 6) + (tl & 1)];
+        const unsigned long long ra = sk[elem_slot(tk)], rl = sk[elem_slot(tl)];
         ans.hi = key_hi_of((unsigned)(ra >> 32)); ans.lo = true_lo(ans.hi, (unsigned)ra);
         wmax.hi = key_hi_of((unsigned)(rl >> 32)); wmax.lo = true_lo(wmax.hi, (unsigned)rl);
         done = true;
@@ -673,61 +711,7 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
         }
       }
     } else {
-      // ---- whole-range pass: no per-window order statistic.  Exact maximum the way the minimum is found, then the samples
-      // flagged in pass 1 (lo <= x <= hi as doubles) are classified exactly on their totalOrder keys: above hi (+0 over a -0
-      // pivot), == hi, == lo, below lo (-0 under a +0 pivot), and the rest - strictly inside - goes to the field's list.
-      wmax.hi = __reduce_max_sync(kFull, mh);
-      if (lo_zero) {
-        wmax.lo = true_lo(wmax.hi, 0u);
-      } else {
-        wmax.lo = extreme_lo<true>(sk, mh, wmax.hi, m, lane);
-      }
-      unsigned n_eh = 0, n_el = 0, n_in = 0;
-      if (__any_sync(kFull, inmask != 0u)) {
-        const unsigned long long lok = gpud_f64_key((unsigned long long)__double_as_longlong(piv_lo));
-        const unsigned long long hik = gpud_f64_key((unsigned long long)__double_as_longlong(piv_hi));
-        // equal pivots that are not a zero: lo <= x <= hi as doubles already means key == hi (a tie-heavy gauge: every flagged
-        // sample is a copy of the pivot), no need to look at the keys
-        const bool all_equal = lok == hik && piv_hi != 0.0;
-        if (all_equal) { n_eh = (unsigned)__popc(inmask); inmask = 0u; }
-        unsigned mm = inmask;
-        while (mm) {
-          const int i = __ffs(mm) - 1;
-          mm &= mm - 1;
-          const unsigned long long key = true_key(sk[lane * kRowU64 + i]);
-          const bool inside = key > lok && key < hik;
-          abv += key > hik ? 1u : 0u;
-          n_eh += key == hik ? 1u : 0u;
-          n_el += (key == lok && lok != hik) ? 1u : 0u;
-          if (!inside) inmask ^= 1u << i;
-        }
-        const int c = __popc(inmask);
-        int incl = c;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const int t = __shfl_up_sync(kFull, incl, o);
-          if (lane >= o) incl += t;
-        }
-        n_in = (unsigned)__shfl_sync(kFull, incl, 31);
-        if (n_in) {
-          unsigned base = 0;
-          if (lane == 0) base = atomicAdd(p.fill + f, n_in);
-          base = __shfl_sync(kFull, base, 0);
-          unsigned pos = base + (unsigned)(incl - c);
-          unsigned long long* __restrict__ list = p.lists + (int64_t)f * p.list_cap;
-          mm = inmask;
-          while (mm) {
-            const int i = __ffs(mm) - 1;
-            mm &= mm - 1;
-            if (pos < p.list_cap) list[pos] = true_key(sk[lane * kRowU64 + i]);
-            ++pos;
-          }
-        }
-      }
-      cls.x = __reduce_add_sync(kFull, abv);
-      cls.y = __reduce_add_sync(kFull, n_eh);
-      cls.z = __reduce_add_sync(kFull, n_el);
-      cls.w = n_in;
+      cls = classify_window(p, sk, f, m, lo_zero, mh, abv, inmask, piv_lo, piv_hi, lane, wmax);
     }
     __syncwarp();                            // every lane is done with this window's rows before pass 1 of the next overwrites them
 
@@ -750,22 +734,10 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
 // launch reduces them itself once its cursor has run out (n_tail > 0), through the same loop instantiated for them.
 template <bool ALIGNED, int JF, bool RANGE>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, kCtasPerSM) k_window_reduce(const WinParams p) {
-#ifdef GPUD_EXPERIMENT_FINISH
-  const unsigned long long exp_t0 = global_ns();
-#endif
-  int n_done = window_loop<ALIGNED, JF, RANGE, false>(p);
+  window_loop<ALIGNED, JF, RANGE, false>(p);
   if constexpr (ALIGNED) {
-    if (p.n_tail > 0) n_done += window_loop<false, -1, RANGE, true>(p);
+    if (p.n_tail > 0) window_loop<false, -1, RANGE, true>(p);
   }
-#ifdef GPUD_EXPERIMENT_FINISH
-  const int exp_warp = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
-  if (ALIGNED && JF >= 0 && !RANGE && (threadIdx.x & 31) == 0 && exp_warp < kExpMaxWarps) {
-    g_exp_finish[exp_warp][0] = exp_t0;
-    g_exp_finish[exp_warp][1] = global_ns();
-    g_exp_finish[exp_warp][2] = (unsigned long long)n_done;
-  }
-#endif
-  (void)n_done;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1021,10 +993,7 @@ extern "C" int32_t gpud_ring_counts(gpud_ring* r, int64_t* total, int64_t* count
 // window shape when W >> 6 is 15 or 16, i.e. W in 960..1024); the window that wraps the physical end of the ring and a trailing
 // partial window go through the generic run-time code at the end of the same launch.  The generic instantiation on its own
 // serves rings in which some window starts on an odd element.
-#ifndef GPUD_RUN_WINDOWS
-#define GPUD_RUN_WINDOWS 8
-#endif
-constexpr int kRunWindows = GPUD_RUN_WINDOWS;   // windows per claim of the work cursor while the ring is far from done
+constexpr int kRunWindows = 8;   // windows per claim of the work cursor while the ring is far from done
 
 // Claims of kRunWindows units, then single units for the last warps x kRunWindows / 2: when the runs are gone the warps are on
 // average half a run from the end of theirs, and the single units fill that in.
@@ -1123,19 +1092,6 @@ extern "C" int32_t gpud_ring_kernel_ms(gpud_ring* r, float* reduce_ms, float* ca
   GPUD_CUDA(r->ctx, cudaEventElapsedTime(carry_ms, r->ev_k[1], r->ev_k[2]));
   return GPUD_OK;
 }
-
-#ifdef GPUD_EXPERIMENT_FINISH
-// Copies the per-warp {start ns, end ns, windows} records of the hot launches since the last call into out[n_warps][3] and clears them.
-extern "C" int32_t gpud_exp_warp_finish(gpud_ring* r, unsigned long long* out, int32_t n_warps) {
-  if (!r || !out || n_warps < 1 || n_warps > kExpMaxWarps) return GPUD_E_INVALID;
-  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
-  GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));
-  GPUD_CUDA(r->ctx, cudaMemcpyFromSymbol(out, g_exp_finish, (size_t)n_warps * 3 * sizeof(unsigned long long)));
-  static const unsigned long long zeros[kExpMaxWarps][3] = {};
-  GPUD_CUDA(r->ctx, cudaMemcpyToSymbol(g_exp_finish, zeros, sizeof(zeros)));
-  return GPUD_OK;
-}
-#endif
 
 extern "C" int32_t gpud_ring_sync(gpud_ring* r) {
   if (!r) return GPUD_E_INVALID;
