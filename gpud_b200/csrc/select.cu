@@ -527,6 +527,8 @@ struct gpud_range_state {
   int reasons[GPUD_RANGE_N_OPEN_REASONS] = {};   // its open fields by reason
   int fields_open = 0;            // fields it handed to the radix select
   int nw = 0;                     // windows of its pass (rows of d_cls per field)
+  int64_t n_segs = 0;             // segments of its select (d_piv / d_fill entries) and class-count rows of its pass (d_cls
+  int64_t n_rows = 0;             //   entries, all fields): gpudh_ring_segment_scratch
 };
 
 void gpud_range_state_free(gpud_range_state* s) {
@@ -626,6 +628,8 @@ static int32_t run_select(gpud_ring* ring, gpud_range_state* s, const SegJob& j,
   GPUD_CUDA(ctx, gpud_grow(&s->d_open, &s->open_cap, 1 + (size_t)n_segs));
   for (auto& ev : s->ev) if (!ev) GPUD_CUDA(ctx, cudaEventCreate(&ev));
   s->nw = nw;
+  s->n_segs = n_segs;
+  s->n_rows = (int64_t)per;
   std::fill(s->reasons, s->reasons + GPUD_RANGE_N_OPEN_REASONS, 0);
   const double* piv = sampled ? s->d_piv : nullptr;
   unsigned* fill = sampled ? s->d_fill : nullptr;
@@ -860,6 +864,7 @@ struct gpud_ranges_state {
   uint32_t* d_nover = nullptr;  size_t nover_cap = 0;           //   and n_over [F][n]
   cudaEvent_t ev[2] = {};
   bool timed = false;
+  bool seg_last = false;          // seg holds the last batch of the last call (that call had a long range)
   int64_t open = 0;
   int reasons[GPUD_RANGE_N_OPEN_REASONS] = {};
 };
@@ -908,6 +913,9 @@ static cudaError_t ranges_batch(gpud_ring* r, gpud_ranges_state* rs, const Range
   if (e == cudaSuccess) e = gpud_grow(&rs->d_geo, &rs->geo_cap, (size_t)n_long);
   if (e == cudaSuccess) e = gpud_grow(&rs->d_tile, &rs->tile_cap, (size_t)n_tiles);
   if (e != cudaSuccess) return e;
+  s->n_segs = n_segs;
+  s->n_rows = (int64_t)per;
+  rs->seg_last = true;
   std::vector<int32_t> tile(n_tiles);
   for (int64_t j = 0; j < n_long; ++j) {
     const gpud_range_geo& g = pl.geo[g0 + j];
@@ -965,6 +973,7 @@ extern "C" int32_t gpud_ring_reduce_ranges(gpud_ring* r, const int64_t* first, c
   gpud_ranges_state* rs = r->ranges;
   if (!rs->seg) rs->seg = new gpud_range_state();
   rs->timed = false;
+  rs->seg_last = false;
   rs->open = 0;
   std::fill(rs->reasons, rs->reasons + GPUD_RANGE_N_OPEN_REASONS, 0);
   const size_t plane = (size_t)r->F * n_ranges;
@@ -997,6 +1006,32 @@ extern "C" int32_t gpud_ring_ranges_stats(gpud_ring* r, float* device_ms, int64_
   GPUD_CUDA(r->ctx, cudaEventElapsedTime(device_ms, rs->ev[0], rs->ev[1]));
   if (segments_by_radix) *segments_by_radix = rs->open;
   if (reasons) std::copy(rs->reasons, rs->reasons + GPUD_RANGE_N_OPEN_REASONS, reasons);
+  return GPUD_OK;
+}
+
+// Test hook (include/gpud_b200_hooks.h): what the last segment select left in its scratch - the last batch of the last
+// gpud_ring_reduce_ranges (h NULL) or the last phase of handle h's last reduce - per segment its pivots {lo, hi} and list fill
+// counter, and the class counts of every row of its pass; each buffer may be NULL (all NULL: the sizes alone).
+extern "C" int32_t gpudh_ring_segment_scratch(gpud_ring* r, gpud_ring_windows* h, double* piv, uint32_t* fill, uint32_t* cls, int64_t* n_segs,
+                                              int64_t* n_rows) {
+  if (!r || !n_segs || !n_rows || (h && h->ring != r)) return GPUD_E_INVALID;
+  const gpud_range_state* s = nullptr;
+  if (h) {
+    if (h->L <= GPUD_MAX_WINDOW || !h->seg || !h->seg->timed)
+      return gpud_fail(r->ctx, GPUD_E_STATE, "no reduce of this handle has run the segment select to the end");
+    s = h->seg;
+  } else {
+    if (!r->ranges || !r->ranges->timed || !r->ranges->seg_last)
+      return gpud_fail(r->ctx, GPUD_E_STATE, "the last reduce_ranges (if any) had no long range");
+    s = r->ranges->seg;
+  }
+  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
+  if (piv) GPUD_CUDA(r->ctx, cudaMemcpyAsync(piv, s->d_piv, 2 * s->n_segs * sizeof(double), cudaMemcpyDeviceToHost, r->stream));
+  if (fill) GPUD_CUDA(r->ctx, cudaMemcpyAsync(fill, s->d_fill, s->n_segs * sizeof(uint32_t), cudaMemcpyDeviceToHost, r->stream));
+  if (cls) GPUD_CUDA(r->ctx, cudaMemcpyAsync(cls, s->d_cls, s->n_rows * sizeof(uint4), cudaMemcpyDeviceToHost, r->stream));
+  GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));
+  *n_segs = s->n_segs;
+  *n_rows = s->n_rows;
   return GPUD_OK;
 }
 

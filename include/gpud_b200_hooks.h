@@ -55,6 +55,14 @@ int32_t gpudh_store_event_sql(int32_t which, const char* table, char* out, int32
  * and, if cls is not NULL, the per-window class counts of the pass; *nw = that pass's number of 1024-sample windows */
 int32_t gpudh_ring_range_scratch(gpud_ring* r, double* piv /*[F][2] lo,hi*/, uint32_t* fill /*[F]*/,
                                  uint32_t* cls /*[F][nw][4] above, ==hi, ==lo, inside; may be NULL*/, int64_t* nw);
+/* what the last segment select left in its scratch: with h NULL the last batch of the last gpud_ring_reduce_ranges (segment
+ * f n_long + j = field f of that batch's long range j, in call order; rows [F][n_tiles] of 1024-sample tiles, the last tile of a
+ * range shorter), else handle h's last reduce that ran it (a hopping handle: its last phase; segment f n_new + j, rows [F][n_new L / Wp]).
+ * Per segment the pivots of k_range_pivots and its list fill counter (which may exceed the list's capacity), per row the class counts
+ * of the pass; any of piv / fill / cls may be NULL.  GPUD_E_STATE when the last reduce_ranges had no long range, or h has L <= 1024 or
+ * no such reduce yet. */
+int32_t gpudh_ring_segment_scratch(gpud_ring* r, gpud_ring_windows* h, double* piv /*[n_segs][2] lo,hi*/, uint32_t* fill /*[n_segs]*/,
+                                   uint32_t* cls /*[n_rows][4] above, ==hi, ==lo, inside*/, int64_t* n_segs, int64_t* n_rows);
 /* what ingest left in device memory, after synchronising the ring's stream: the physical ring [F][CAP] (column c = sample c of the
  * ring's storage, not rotated to chronological order) and its sample ring [F][smp_slots] (column c with c % 2^smp_shift ==
  * 2^smp_shift / 2 at slot c >> smp_shift).  Either buffer may be NULL; smp_shift / smp_slots may be NULL. */

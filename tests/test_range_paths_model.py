@@ -52,8 +52,9 @@ def pivots(x, pos, k):
     return lok, hik, rh, rl, S
 
 
-def classify(x, keys, lok, hik):
-    """the fused pass: per window [above, == hi, == lo, inside] (uint32 counts, as w_cls) and the flags it raised"""
+def classify(x, keys, lok, hik, wp=WP):
+    """the fused pass: per window of wp samples (the last one shorter) [above, == hi, == lo, inside] (uint32 counts, as w_cls)
+    and the flags it raised"""
     lo, hi = _f64(lok), _f64(hik)
     with np.errstate(invalid="ignore"):
         above_d = x > hi
@@ -67,7 +68,7 @@ def classify(x, keys, lok, hik):
         eh = flagged & (keys == hik_)
         el = flagged & (keys == lok_) & (lok != hik)
         ins = flagged & (keys > lok_) & (keys < hik_)
-    starts = np.arange(0, len(x), WP)
+    starts = np.arange(0, len(x), wp)
     cls = np.stack([np.add.reduceat(v.astype(np.int64), starts) for v in (a, eh, el, ins)], axis=1)
     return cls, ins
 
