@@ -833,7 +833,7 @@ def lib() -> C.CDLL:
         "gpud_ring_checkpoint_stats": (i32, [vp, C.POINTER(C.c_float), C.POINTER(C.c_float), vp]),
         "gpud_ring_checkpoint_delta_bound": (i32, [vp, C.POINTER(i64)]),
         "gpud_ring_checkpoint_delta": (i32, [vp, vp, i64, C.POINTER(i64)]), "gpud_ring_restore_delta": (i32, [vp, vp, i64]),
-        "gpudh_ring_windows_sub": (i32, [i32, i64]),
+        "gpudh_ring_windows_sub": (i32, [i32, i64]), "gpudh_ring_ckpt_grid": (i32, [vp, i32]),
         "gpud_kmsg_scan": (i32, [vp, i32, vp, i64, i32, C.POINTER(XidHit), i64, C.POINTER(i64), C.POINTER(i64)]),
         "gpud_kmsg_scan_sharded": (i32, [vp, vp, i64, i32, C.POINTER(XidHit), i64, C.POINTER(i64), C.POINTER(i64)]),
         "gpud_kmsg_scan_device": (i32, [vp, i32, vp, i64, i32, C.POINTER(XidHit), i64, C.POINTER(i64), C.POINTER(i64), vp]),

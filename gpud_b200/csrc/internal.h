@@ -70,6 +70,7 @@ struct gpud_ring {
   bool ck_timed = false;                               // gpud_ring_checkpoint_stats: a checkpoint or restore has run
   float ck_encode_ms = 0.f, ck_decode_ms = 0.f;        // ... device ms of the last checkpoint's encode and the last restore's decode
   int64_t ck_blocks[2] = {0, 0};                       // ... and the blocks of the last of either, by mode (RAW, INT)
+  int ck_grid_max = 0;                                 // > 0: at most this many CTAs per codec kernel (gpudh_ring_ckpt_grid); 0: the default
   int64_t handle_gen = 0;                              // stream / windows handles opened or closed so far
   // The chain marker (DESIGN.md §2 "Delta checkpoints"): the state of the last checkpoint this ring wrote or loaded, full or delta.
   // Each handle keeps its own `next` at the marker (gpud_ring_windows::ck_next).

@@ -288,7 +288,9 @@ struct CallScratch {
 };
 
 int ckpt_grid(const gpud_ring* r, int64_t units, int warps_per_cta) {
-  return (int)std::max<int64_t>(1, std::min<int64_t>((units + warps_per_cta - 1) / warps_per_cta, (int64_t)r->sm_count * 16));
+  int64_t most = (int64_t)r->sm_count * 16;
+  if (r->ck_grid_max > 0) most = std::min<int64_t>(most, r->ck_grid_max);
+  return (int)std::max<int64_t>(1, std::min<int64_t>((units + warps_per_cta - 1) / warps_per_cta, most));
 }
 
 // Samples [first, first + count) of the push order, first >= total - CAP.
@@ -914,6 +916,12 @@ extern "C" int32_t gpud_ring_restore_delta(gpud_ring* r, const void* in_v, int64
   std::vector<uint64_t> sums(F);
   memcpy(sums.data(), in + sum_off, 8 * F);
   set_marker(r, total, chain_link(prev_link, total, sums.data(), F, heads));
+  return GPUD_OK;
+}
+
+extern "C" int32_t gpudh_ring_ckpt_grid(gpud_ring* r, int32_t max_ctas) {
+  if (!r || max_ctas < 0) return GPUD_E_INVALID;
+  r->ck_grid_max = max_ctas;
   return GPUD_OK;
 }
 

@@ -75,6 +75,10 @@ int32_t gpudh_ring_stream_plan(int64_t total, int64_t cap, int32_t W, int64_t hi
 /* the window length the device pass of gpud_ring_windows_* runs on for windows of span x W samples: span x W itself up to 1024,
  * else the range pass's sub-window W g, g the largest divisor of span with W g <= 1024.  Pure arithmetic. */
 int32_t gpudh_ring_windows_sub(int32_t W, int64_t span);
+/* caps the grid of this ring's three checkpoint codec kernels (k_ckpt_size, k_ckpt_pack, k_ckpt_unpack) at max_ctas CTAs, so that
+ * each warp codes many blocks in turn; 0: the default (one warp per block, at most 16 CTAs per SM).  Checkpoint, restore, delta and
+ * delta apply on the ring all read it; the bytes and the restored ring do not depend on it. */
+int32_t gpudh_ring_ckpt_grid(gpud_ring* r, int32_t max_ctas);
 /* the host plan of one gpud_ring_windows_reduce of a handle of span x W samples every hop x W (P) on a ring of `total` pushed
  * samples and capacity cap, its history of at most `history` windows now holding [first, next), reseed = 1 when the handle re-seeds
  * its EMA at window next (opened, or restarted with nothing reduced since).  out[8] as gpudh_ring_stream_plan; ema[5] = {physical
