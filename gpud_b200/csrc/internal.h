@@ -179,45 +179,51 @@ int32_t gpud_ring_windows_new(gpud_ring* r, int64_t span, int64_t hop, int64_t h
 void gpud_ring_windows_free(gpud_ring_windows* s);
 
 // ring.cu: the window pass and the EMA carry over chronological samples [start, start + n) of the ring with window Wp, into the
-// caller's buffers w[0..4] = per-window min, max, mean, EMA, EMA partial sums and w_nover, each [F][ceil(n / Wp)].  With piv the
-// pass also classifies every sample against the field's pivots lo = piv[2f], hi = piv[2f + 1]: class counts {above hi, == hi,
+// caller's buffers w[0..4] = per-window min, max, mean, EMA, EMA partial sums and w_nover, each [F][nw], nw = ceil(n / Wp).  With piv
+// the pass also classifies every sample against the field's pivots lo = piv[2f], hi = piv[2f + 1]: class counts {above hi, == hi,
 // == lo, strictly inside} per window into w_cls, the keys strictly inside into lists [F][list_cap] behind the counters fill [F].
-// Segments: with seg_sub > 0 every seg_sub consecutive windows of a field form one segment, the classification uses segment
-// (f nw + w) / seg_sub's pivots, class counts and list; seg_sub = 0 is one segment per field.  w[3] == NULL: no EMA carry.
+// Segments: with seg_sub > 0 every seg_sub consecutive windows of a field form one segment, window w of field f uses segment
+// sg = f (nw / seg_sub) + w / seg_sub's pivots, fill counter and list [sg list_cap, (sg + 1) list_cap); seg_sub = 0 is one segment
+// per field.  These are the rows and lists of the segment select's table for n_geo = nw / seg_sub equal segments (gpud_range_geo
+// below: tile0 = j seg_sub, list0 = j list_cap).  w[3] == NULL: no EMA carry.
 int32_t gpud_ring_window_pass(gpud_ring* r, int64_t start, int64_t n, int Wp, double* const w[5], uint32_t* w_nover,
                               const double* piv, uint4* w_cls, unsigned long long* lists, unsigned* fill, unsigned list_cap, int seg_sub);
 
-// select.cu: exact aggregates of n_seg consecutive segments of seg_len samples of every field, from chronological ring column
-// `start` on: segment s = f n_seg + j is samples [start + j seg_len, start + (j + 1) seg_len) of field f.  The range pass runs in
-// sub-windows of Wp samples (Wp divides seg_len, Wp <= GPUD_MAX_WINDOW).  Synchronises the ring's stream once (the radix select's
-// grid is sized by the segments left open) and leaves the results on the device, valid until the next call on *st:
-// out [5][F n_seg] (MIN, MAX, MEAN, -, P99), nover [F n_seg], part [F][n_seg seg_len / Wp] the sub-windows' EMA partial sums.
+// select.cu: exact aggregates of n_seg consecutive segments of seg_len samples of every field, from physical ring column `start`
+// on: a segment select whose table entry j is samples [start + j seg_len, start + (j + 1) seg_len), for every field.  The window pass
+// runs in sub-windows of Wp samples (Wp divides seg_len, Wp <= GPUD_MAX_WINDOW).  Synchronises the ring's stream once (the radix
+// select's grid is sized by the segments left open) and leaves the results on the device, valid until the next call on *st:
+// out [5][F n_seg] (MIN, MAX, MEAN, -, P99: no EMA), nover [F n_seg], part [F][n_seg seg_len / Wp] the sub-windows' EMA partial sums.
 struct gpud_seg_out { const double* out; const uint32_t* nover; const double* part; int64_t open; const int* reasons; };
 int32_t gpud_ring_segments(gpud_ring* r, gpud_range_state** st, int64_t start, int64_t seg_len, int64_t n_seg, int Wp, gpud_seg_out* out);
 
 // gpud_ring_reduce_ranges (select.cu, DESIGN.md §2 "Ranges").  A short range (<= GPUD_MAX_WINDOW samples) is one warp's work:
 struct gpud_short_range { int64_t start; int32_t len; int32_t id; };   // physical column of its first sample, samples, index in the call
-// A long range is one segment per field of the segment select in its table geometry: segment s = f n_long + j is field f's samples of
-// long range j, read in tiles of GPUD_MAX_WINDOW samples (the last one shorter) that are rows tile0 .. of the [F][n_tiles] tile arrays.
+// The segment select (select.cu) of gpud_ring_reduce_range, of stream windows with L > GPUD_MAX_WINDOW and of the long ranges of
+// gpud_ring_reduce_ranges reads its segments from one table of n_geo entries: segment sg = f n_geo + j is entry j's samples of field f.
+// Its pass (the window pass, or the long route's tiles of GPUD_MAX_WINDOW samples, the last one shorter) writes segment sg's windows
+// to rows f n_rows + tile0 .. of the [F][n_rows] pass arrays and its keys between the pivots to [list0, list0 + lcap) of field f's
+// row of the lists.
 struct gpud_range_geo {
-  int64_t start, n;         // physical column of the range's first sample, its samples
+  int64_t start, n;         // physical column of the segment's first sample, its samples
   int64_t k;                // rank of the order statistic from the top
   int64_t stride;           // pivot sample: S strided reads, stride apart, unless smp (the ring's sample ring)
-  int64_t tile0;            // the range's first tile
-  int64_t list0;            // its segments' key lists: [list0, list0 + lcap) of each field's row of the lists
-  int64_t id;               // index in the call
-  double d_last;            // (1 - alpha)^(samples of the last tile)
+  int64_t tile0;            // the segment's first row
+  int64_t list0;            // its key lists: [list0, list0 + lcap) of each field's row of the lists
+  int64_t id;               // long ranges: index in the call
+  double d_last;            // long ranges: (1 - alpha)^(samples of the last tile)
   int32_t S, smp;
   uint32_t lcap;
   int32_t pad;
 };
 // ring.cu: the short route (one launch: every short range of every field, results into out [5][F][n_out] / nover [F][n_out] at
 // column id), the tile pass of the long route (per (field, tile): min, max, mean, EMA partial, n_over and the class counts against
-// segment (f, tile_range[t])'s pivots; keys strictly between them into the segment's list) and its EMA (seg_ema [F n_long]).
+// segment (f, tile_range[t])'s pivots; keys strictly between them into the segment's list) and its EMA (each segment's at its last
+// tile's row of ema [F][n_tiles]).
 cudaError_t gpud_ranges_short(gpud_ring* r, const gpud_short_range* rs, int n_short, int64_t n_out, double* out, uint32_t* nover);
 cudaError_t gpud_ranges_tiles(gpud_ring* r, const gpud_range_geo* geo, int64_t n_long, const int32_t* tile_range, int64_t n_tiles, const double* piv,
                               double* const w[5], uint32_t* w_nover, uint4* w_cls, unsigned long long* lists, int64_t list_row, unsigned* fill);
-cudaError_t gpud_ranges_ema(gpud_ring* r, const gpud_range_geo* geo, int64_t n_long, const double* part, int64_t n_tiles, double* seg_ema);
+cudaError_t gpud_ranges_ema(gpud_ring* r, const gpud_range_geo* geo, int64_t n_long, const double* part, int64_t n_tiles, double* ema);
 
 // kmsg_dedup.cu: the watcher's duplicate drop over the n_units units of the staged buffer d_buf, numbered by the scan that has just
 // run on `st` (its per-chunk and per-tile separator prefixes); dropped[n_units] is host memory.  _check: the cache belongs to

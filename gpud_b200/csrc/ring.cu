@@ -1047,10 +1047,11 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, kCtasPerSM) k_ranges_tile
   }
 }
 
-// Long route, the EMA: one 128-thread CTA per segment, the carry's scan over the segment's tiles from its first sample.
+// Long route, the EMA: one 128-thread CTA per segment, the carry's scan over the segment's tiles from its first sample, into its last
+// tile's row of ema [F][n_tiles].
 template <bool GUARD>
 __global__ void __launch_bounds__(128) k_ranges_ema(const double* __restrict__ part, int64_t n_tiles, const gpud_range_geo* __restrict__ geo, int64_t n_long,
-                                                     const double* __restrict__ ring, int64_t cap, double d_full, double* __restrict__ seg_ema) {
+                                                     const double* __restrict__ ring, int64_t cap, double d_full, double* __restrict__ ema) {
   __shared__ double s_warp[4];
   __shared__ double s_carry;
   const int64_t sg = blockIdx.x;
@@ -1059,7 +1060,7 @@ __global__ void __launch_bounds__(128) k_ranges_ema(const double* __restrict__ p
   const int nw = (int)((g.n + GPUD_MAX_WINDOW - 1) / GPUD_MAX_WINDOW);
   const double* __restrict__ P = part + (int64_t)f * n_tiles + g.tile0;
   decayed_scan<GUARD>(P, nw - 1, d_full, s_warp, s_carry, [&] { return ring[(int64_t)f * cap + g.start]; }, [](int, double) {});
-  if (threadIdx.x == 0) seg_ema[sg] = decay_fma<GUARD>(g.d_last, s_carry, __ldg(P + nw - 1));
+  if (threadIdx.x == 0) ema[(int64_t)f * n_tiles + g.tile0 + nw - 1] = decay_fma<GUARD>(g.d_last, s_carry, __ldg(P + nw - 1));
 }
 
 }  // namespace
@@ -1807,10 +1808,10 @@ cudaError_t gpud_ranges_tiles(gpud_ring* r, const gpud_range_geo* geo, int64_t n
 }
 
 // the guard choice of launch_ema_carry, for tiles of GPUD_MAX_WINDOW samples
-cudaError_t gpud_ranges_ema(gpud_ring* r, const gpud_range_geo* geo, int64_t n_long, const double* part, int64_t n_tiles, double* seg_ema) {
+cudaError_t gpud_ranges_ema(gpud_ring* r, const gpud_range_geo* geo, int64_t n_long, const double* part, int64_t n_tiles, double* ema) {
   const double d_full = pow(1.0 - r->alpha, (double)GPUD_MAX_WINDOW);
   const unsigned grid = (unsigned)((int64_t)r->F * n_long);
-  if (pow(d_full, 128.0) < 0x1p-900) k_ranges_ema<true><<<grid, 128, 0, r->stream>>>(part, n_tiles, geo, n_long, r->d_ring, r->cap, d_full, seg_ema);
-  else k_ranges_ema<false><<<grid, 128, 0, r->stream>>>(part, n_tiles, geo, n_long, r->d_ring, r->cap, d_full, seg_ema);
+  if (pow(d_full, 128.0) < 0x1p-900) k_ranges_ema<true><<<grid, 128, 0, r->stream>>>(part, n_tiles, geo, n_long, r->d_ring, r->cap, d_full, ema);
+  else k_ranges_ema<false><<<grid, 128, 0, r->stream>>>(part, n_tiles, geo, n_long, r->d_ring, r->cap, d_full, ema);
   return cudaGetLastError();
 }

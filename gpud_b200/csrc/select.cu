@@ -163,15 +163,19 @@ __device__ void block_select2_smem(const unsigned long long* keys, int cnt, int 
   *outB = z->ans[1];
 }
 
-// The sample comes from the ring's own sample ring when the range covers enough of its slots (the whole-ring case: 64 KB of contiguous
-// memory per field, kept current by the append kernel), else from S strided reads of the ring itself (one 32-byte sector each).
-// One block per segment: block b is segment j = b % n_seg of field b / n_seg, samples [start + j n, start + (j + 1) n), or (TABLE) the
-// samples of long range j of gpud_ring_reduce_ranges, whose start, length, rank and pivot sample come from geo[j].
-template <bool TABLE>
-__global__ void __launch_bounds__(kSelThreads) k_range_pivots(const double* __restrict__ ring, int64_t cap, int64_t start_all, int64_t n, int S, int64_t stride,
-                                                       int64_t k_from_top, double* __restrict__ piv, unsigned* __restrict__ fill,
-                                                       const double* __restrict__ sample, int smp_shift, int64_t smp_slots, int64_t n_seg,
-                                                       const gpud_range_geo* __restrict__ geo) {
+// Segment sg = f n_geo + j of a select is entry j of its table over field f (internal.h): its samples are field f's row of the ring from
+// physical column g.start on.
+__device__ __forceinline__ const gpud_range_geo& seg_geo(const gpud_range_geo* geo, int64_t n_geo, int64_t sg, int* f) {
+  *f = (int)(sg / n_geo);
+  return geo[sg - (int64_t)*f * n_geo];
+}
+
+// The sample comes from the ring's own sample ring when the segment covers enough of its slots (g.smp; the whole-ring case: 64 KB of
+// contiguous memory per field, kept current by the append kernel), else from g.S strided reads of the ring itself (one 32-byte sector
+// each).  One block per segment; 32 registers, so that four blocks fit an SM when the sample is small (a handle's many segments).
+__global__ void __launch_bounds__(kSelThreads, 4) k_range_pivots(const double* __restrict__ ring, int64_t cap, const gpud_range_geo* __restrict__ geo, int64_t n_geo,
+                                                       double* __restrict__ piv, unsigned* __restrict__ fill,
+                                                       const double* __restrict__ sample, int smp_shift, int64_t smp_slots) {
   extern __shared__ __align__(16) unsigned long long s_keys[];
   __shared__ unsigned s_hist[512];
   __shared__ unsigned long long s_red[2 * kSelThreads / 32];
@@ -179,17 +183,11 @@ __global__ void __launch_bounds__(kSelThreads) k_range_pivots(const double* __re
   __shared__ int s_cnt;
   const int t = threadIdx.x;
   const int64_t sg = blockIdx.x;
-  const int f = (int)(sg / n_seg);
-  int64_t start;
-  if constexpr (TABLE) {
-    const gpud_range_geo& g = geo[sg - (int64_t)f * n_seg];
-    start = g.start; n = g.n; S = g.S; stride = g.stride; k_from_top = g.k;
-    if (!g.smp) sample = nullptr;
-  } else {
-    start = start_all + (sg - (int64_t)f * n_seg) * n;
-    if (start >= cap) start -= cap;
-  }
-  if (sample) {
+  int f;
+  const gpud_range_geo& g = seg_geo(geo, n_geo, sg, &f);
+  const int64_t start = g.start, n = g.n, stride = g.stride;
+  int S = g.S;
+  if (g.smp) {
     if (t == 0) s_cnt = 0;
     __syncthreads();
     const double* __restrict__ sb = sample + (int64_t)f * smp_slots;
@@ -220,7 +218,7 @@ __global__ void __launch_bounds__(kSelThreads) k_range_pivots(const double* __re
     }
   }
   __syncthreads();
-  const double pr = (double)k_from_top / (double)n;
+  const double pr = (double)g.k / (double)n;
   const double r0 = pr * (double)S, d = 5.0 * sqrt((double)S * pr * (1.0 - pr)) + 2.0;
   const long long rh = (long long)floor(r0 - d), rl = (long long)ceil(r0 + d);
   unsigned long long hik, lok;
@@ -232,24 +230,6 @@ __global__ void __launch_bounds__(kSelThreads) k_range_pivots(const double* __re
     piv[2 * sg + 1] = __longlong_as_double((long long)gpud_key_f64bits(hik));
     fill[sg] = 0u;
   }
-}
-
-// Segment sg of the radix select: its field's row of the ring and the chronological column its samples start at.
-__device__ __forceinline__ const double* seg_base(const double* ring, int64_t cap, int64_t start_all, int64_t n, int64_t n_seg, int sg, int64_t* start) {
-  const int f = (int)(sg / n_seg);
-  int64_t s0 = start_all + (sg - (int64_t)f * n_seg) * n;
-  if (s0 >= cap) s0 -= cap;
-  *start = s0;
-  return ring + (int64_t)f * cap;
-}
-
-// ... in the table geometry: segment sg = f n_seg + j is long range j of field f (its length replaces *n).
-__device__ __forceinline__ const double* seg_table(const double* ring, int64_t cap, const gpud_range_geo* geo, int64_t n_seg, int sg, int64_t* start, int64_t* n) {
-  const int f = (int)(sg / n_seg);
-  const gpud_range_geo& g = geo[sg - (int64_t)f * n_seg];
-  *start = g.start;
-  *n = g.n;
-  return ring + (int64_t)f * cap;
 }
 
 struct BinPick { int bin; unsigned above; };   // the chosen digit bin and the keys in the bins above it
@@ -309,39 +289,31 @@ __device__ __forceinline__ unsigned long long list_select(const unsigned long lo
   return prefix;
 }
 
-// One block per field after the window pass: fold the per-window partials into the field's min / max / mean / EMA / n_over,
-// initialise the histogram path's state, and - sampled mode - settle the order statistic from the class counts and the list.
-// Fields left open (nbits < 64) are counted in *n_open.  TABLE: block f is segment f = field n_long + j of gpud_ring_reduce_ranges,
-// its windows are the tiles of long range j (rows geo[j].tile0 .. of the [F][n_tiles] tile arrays), its EMA comes from seg_ema and
-// its list is [list0, list0 + lcap) of the field's row of list_row keys.
-template <bool TABLE>
-__global__ void __launch_bounds__(kSelThreads) k_range_finish(int F, int nw, int Wp, int64_t n, const double* __restrict__ w_min, const double* __restrict__ w_max,
-                                                       const double* __restrict__ w_mean, const double* __restrict__ w_ema, const uint32_t* __restrict__ w_nover,
-                                                       int q_num, int q_den, int sampled, const double* __restrict__ piv, const unsigned* __restrict__ fill,
-                                                       const uint4* __restrict__ w_cls, const unsigned long long* __restrict__ lists, unsigned list_cap,
+// One block per segment after the pass: fold the per-window partials into the segment's min / max / mean / EMA / n_over, initialise
+// the histogram path's state, and - sampled mode - settle the order statistic from the class counts and the list.  Segments left open
+// (nbits < 64) are counted in *n_open.  Segment f = field fld's entry g of the table: its windows of Wp samples are rows g.tile0 .. of
+// the field's row of n_rows in the [F][n_rows] pass arrays, its EMA is w_ema at its last window's row (w_ema NULL: none), and its list is
+// [g.list0, g.list0 + g.lcap) of the field's row of list_row keys.
+__global__ void __launch_bounds__(kSelThreads) k_range_finish(int F, int Wp, const gpud_range_geo* __restrict__ geo, int64_t n_geo, int64_t n_rows, int64_t list_row,
+                                                       const double* __restrict__ w_min, const double* __restrict__ w_max, const double* __restrict__ w_mean,
+                                                       const double* __restrict__ w_ema, const uint32_t* __restrict__ w_nover,
+                                                       int sampled, const double* __restrict__ piv, const unsigned* __restrict__ fill,
+                                                       const uint4* __restrict__ w_cls, const unsigned long long* __restrict__ lists,
                                                        double* __restrict__ out /*[5][F]*/, uint32_t* __restrict__ out_nover, SelState* __restrict__ st,
-                                                       unsigned* __restrict__ n_open, int* __restrict__ open_ids,
-                                                       const gpud_range_geo* __restrict__ geo, int64_t n_long, int64_t n_tiles, int64_t list_row,
-                                                       const double* __restrict__ seg_ema) {
+                                                       unsigned* __restrict__ n_open, int* __restrict__ open_ids) {
   __shared__ unsigned long long s_red[kSelThreads / 32][6];
   __shared__ double s_sum[kSelThreads / 32];
   __shared__ unsigned long long s_prefix, s_kk;
   __shared__ int s_nbits, s_mode;
   const int f = blockIdx.x, t = threadIdx.x, lane = t & 31, wid = t >> 5;
-  int64_t row0 = 0, list0 = 0;
-  if constexpr (TABLE) {
-    const int fld = (int)(f / n_long);
-    const gpud_range_geo& g = geo[f - (int64_t)fld * n_long];
-    n = g.n;
-    nw = (int)((n + Wp - 1) / Wp);
-    row0 = (int64_t)fld * n_tiles + g.tile0;
-    list0 = (int64_t)fld * list_row + g.list0;
-    list_cap = g.lcap;
-  }
+  int fld;
+  const gpud_range_geo& g = seg_geo(geo, n_geo, f, &fld);
+  const int64_t n = g.n, row0 = (int64_t)fld * n_rows + g.tile0;
+  const int nw = (int)((n + Wp - 1) / Wp);
   unsigned long long kmin = ~0ull, kmax = 0ull, c_abv = 0, c_eh = 0, c_el = 0, nov = 0;
   double sum = 0.0;
   for (int w = t; w < nw; w += kSelThreads) {
-    const int64_t o = TABLE ? row0 + w : (int64_t)f * nw + w;
+    const int64_t o = row0 + w;
     const int m = (int)min((int64_t)Wp, n - (int64_t)w * Wp);
     kmin = min(kmin, gpud_f64_key((unsigned long long)__double_as_longlong(w_min[o])));
     kmax = max(kmax, gpud_f64_key((unsigned long long)__double_as_longlong(w_max[o])));
@@ -370,10 +342,10 @@ __global__ void __launch_bounds__(kSelThreads) k_range_finish(int F, int nw, int
     out[0 * F + f] = __longlong_as_double((long long)gpud_key_f64bits(kmin));
     out[1 * F + f] = __longlong_as_double((long long)gpud_key_f64bits(kmax));
     out[2 * F + f] = sum / (double)n;
-    out[3 * F + f] = TABLE ? seg_ema[f] : w_ema[(int64_t)f * nw + nw - 1];
+    if (w_ema) out[3 * F + f] = w_ema[row0 + nw - 1];
     out_nover[f] = (uint32_t)nov;
     SelState s;
-    s.kk = (unsigned long long)gpud_rank_from_top(n, q_num, q_den);
+    s.kk = (unsigned long long)g.k;
     s.cnt = (unsigned long long)n;
     s.collected = 0;
     s.why = 0;
@@ -398,7 +370,7 @@ __global__ void __launch_bounds__(kSelThreads) k_range_finish(int F, int nw, int
           if (k <= c_abv + c_eh) { s.prefix = hik; s.nbits = 64; mode = 1; }
           else if (k <= c_abv + c_eh + inside) {
             why = GPUD_RANGE_OPEN_OVERFLOW;
-            if (inside <= (unsigned long long)list_cap) {
+            if (inside <= (unsigned long long)g.lcap) {
               mode = 2;
               const unsigned long long d2 = lok ^ hik;     // every listed key lies between the pivots: skip their common bits
               const int cp2 = __clzll((long long)d2);
@@ -418,7 +390,7 @@ __global__ void __launch_bounds__(kSelThreads) k_range_finish(int F, int nw, int
   }
   __syncthreads();
   if (s_mode != 2) return;
-  const unsigned long long ans = list_select(lists + (TABLE ? list0 : (int64_t)f * list_cap), fill[f], s_nbits, s_prefix, s_kk);   // the L2-resident list
+  const unsigned long long ans = list_select(lists + (int64_t)fld * list_row + g.list0, fill[f], s_nbits, s_prefix, s_kk);   // the L2-resident list
   if (t == 0) {
     st[f].prefix = ans;
     st[f].nbits = 64;
@@ -426,12 +398,9 @@ __global__ void __launch_bounds__(kSelThreads) k_range_finish(int F, int nw, int
   }
 }
 
-// grid (blocks_per_segment, segments): histogram of the next digit over the keys that match the segment's prefix (TABLE: the segments
-// of gpud_ring_reduce_ranges, seg_table)
-template <bool TABLE>
-__global__ void __launch_bounds__(256) k_sel_hist(const double* __restrict__ ring, int64_t cap, int64_t start_all, int64_t n,
-                                                   const SelState* __restrict__ st, unsigned* __restrict__ hist, const int* __restrict__ ids, int64_t n_seg,
-                                                   const gpud_range_geo* __restrict__ geo) {
+// grid (blocks_per_segment, segments): histogram of the next digit over the keys that match the segment's prefix
+__global__ void __launch_bounds__(256) k_sel_hist(const double* __restrict__ ring, int64_t cap, const gpud_range_geo* __restrict__ geo, int64_t n_geo,
+                                                   const SelState* __restrict__ st, unsigned* __restrict__ hist, const int* __restrict__ ids) {
   __shared__ unsigned s_hist[kBins];
   const int f = ids ? ids[blockIdx.y] : blockIdx.y;   // the segment
   const SelState s = st[f];
@@ -440,12 +409,12 @@ __global__ void __launch_bounds__(256) k_sel_hist(const double* __restrict__ rin
   __syncthreads();
   const int d = min(kDigit, 64 - s.nbits), shift = 64 - s.nbits - d;
   const unsigned mask = (1u << d) - 1u;
-  int64_t start;
-  const double* __restrict__ tbase = TABLE ? seg_table(ring, cap, geo, n_seg, f, &start, &n) : nullptr;
+  int fld;
+  const gpud_range_geo& g = seg_geo(geo, n_geo, f, &fld);
+  const int64_t n = g.n;
   const int64_t per = (((n + gridDim.x - 1) / gridDim.x) + 1) & ~(int64_t)1;   // even, so aligned slices stay aligned
   const int64_t b = min(n, (int64_t)blockIdx.x * per), e = min(n, b + per);
-  const double* __restrict__ base = TABLE ? tbase : seg_base(ring, cap, start_all, n, n_seg, f, &start);
-  for_each_key(base, cap, start, b, e, [&](unsigned long long key) {
+  for_each_key(ring + (int64_t)fld * cap, cap, g.start, b, e, [&](unsigned long long key) {
     if (key_matches(key, s)) atomicAdd(&s_hist[(unsigned)(key >> shift) & mask], 1u);
   });
   __syncthreads();
@@ -474,21 +443,19 @@ __global__ void __launch_bounds__(kSelThreads) k_sel_pick(unsigned* __restrict__
 }
 
 // grid (blocks_per_segment, segments): compact the keys that still match into the segment's candidate list (<= kCollectMax of them)
-template <bool TABLE>
-__global__ void __launch_bounds__(256) k_sel_collect(const double* __restrict__ ring, int64_t cap, int64_t start_all, int64_t n,
-                                                      SelState* __restrict__ st, unsigned long long* __restrict__ lists, const int* __restrict__ ids, int64_t n_seg,
-                                                      const gpud_range_geo* __restrict__ geo) {
+__global__ void __launch_bounds__(256) k_sel_collect(const double* __restrict__ ring, int64_t cap, const gpud_range_geo* __restrict__ geo, int64_t n_geo,
+                                                      SelState* __restrict__ st, unsigned long long* __restrict__ lists, const int* __restrict__ ids) {
   const int f = ids ? ids[blockIdx.y] : blockIdx.y;   // the segment
   const SelState s = st[f];
   if (s.nbits == 64) return;
-  int64_t start;
-  const double* __restrict__ tbase = TABLE ? seg_table(ring, cap, geo, n_seg, f, &start, &n) : nullptr;
+  int fld;
+  const gpud_range_geo& g = seg_geo(geo, n_geo, f, &fld);
+  const int64_t n = g.n;
   const int64_t per = (((n + gridDim.x - 1) / gridDim.x) + 1) & ~(int64_t)1;
   const int64_t b = min(n, (int64_t)blockIdx.x * per), e = min(n, b + per);
-  const double* __restrict__ base = TABLE ? tbase : seg_base(ring, cap, start_all, n, n_seg, f, &start);
   unsigned long long* __restrict__ list = lists + (int64_t)blockIdx.y * kCollectMax;
   unsigned* fill = &st[f].collected;
-  for_each_key(base, cap, start, b, e, [&](unsigned long long key) {
+  for_each_key(ring + (int64_t)fld * cap, cap, g.start, b, e, [&](unsigned long long key) {
     if (key_matches(key, s)) {
       const unsigned pos = atomicAdd(fill, 1u);
       if (pos < (unsigned)kCollectMax) list[pos] = key;
@@ -508,68 +475,64 @@ __global__ void __launch_bounds__(kSelThreads) k_sel_final(const SelState* __res
 
 }  // namespace
 
-// Everything gpud_ring_reduce_range keeps between calls (gpud_ring::range).  Every buffer is grown on demand and kept.
+// Everything a segment select keeps between selects: gpud_ring_reduce_range's (gpud_ring::range), a handle's (gpud_ring_windows::seg)
+// and the long route's of gpud_ring_reduce_ranges (gpud_ranges_state::seg).  Every buffer is grown on demand and kept.
 struct gpud_range_state {
-  double* d_win[5] = {};  size_t win_cap[5] = {};              // the pass, per window [F][nw]: min, max, mean, EMA, EMA partial sums
+  gpud_range_geo* d_geo = nullptr;  size_t geo_cap = 0;         // the table of its segments [n_geo]
+  double* d_win[5] = {};  size_t win_cap[5] = {};              // the pass, per row [F][n_rows]: min, max, mean, EMA, EMA partial sums
   uint32_t* d_win_nover = nullptr;  size_t win_nover_cap = 0;  //   and n_over
-  uint4* d_cls = nullptr;  size_t cls_cap = 0;                  // sampled pass: per-window class counts [F][nw]
-  unsigned long long* d_lists = nullptr;  size_t lists_cap = 0; // sampled pass: the keys between the pivots [F][list_cap]
-  double* d_piv = nullptr;  size_t piv_cap = 0;                 // sampled pass: pivots [F][2] lo, hi
-  unsigned* d_fill = nullptr;  size_t fill_cap = 0;             // sampled pass: list fill counters [F]
-  double* d_out = nullptr;  size_t out_cap = 0;                 // the call's result [5][F]
-  uint32_t* d_nover = nullptr;  size_t nover_cap = 0;           //   and n_over [F]
-  SelState* d_st = nullptr;  size_t st_cap = 0;                 // radix select state [F]
-  unsigned* d_open = nullptr;  size_t open_cap = 0;             // [0] = number of fields left open by k_range_finish, [1..] = their ids
-  unsigned* d_hist = nullptr;  size_t hist_cap = 0;             // radix select: digit histograms [fields selected][kBins]
-  unsigned long long* d_cand = nullptr;  size_t cand_cap = 0;   // radix select: candidate lists [fields selected][kCollectMax]
+  uint4* d_cls = nullptr;  size_t cls_cap = 0;                  // sampled pass: per-row class counts [F][n_rows]
+  unsigned long long* d_lists = nullptr;  size_t lists_cap = 0; // sampled pass: the keys between the pivots [F][list_row]
+  double* d_piv = nullptr;  size_t piv_cap = 0;                 // sampled pass: pivots [segments][2] lo, hi
+  unsigned* d_fill = nullptr;  size_t fill_cap = 0;             // sampled pass: list fill counters [segments]
+  double* d_out = nullptr;  size_t out_cap = 0;                 // the select's result [5][segments]
+  uint32_t* d_nover = nullptr;  size_t nover_cap = 0;           //   and n_over [segments]
+  SelState* d_st = nullptr;  size_t st_cap = 0;                 // radix select state [segments]
+  unsigned* d_open = nullptr;  size_t open_cap = 0;             // [0] = number of segments left open by k_range_finish, [1..] = their ids
+  unsigned* d_hist = nullptr;  size_t hist_cap = 0;             // radix select: digit histograms [segments selected][kBins]
+  unsigned long long* d_cand = nullptr;  size_t cand_cap = 0;   // radix select: candidate lists [segments selected][kCollectMax]
   cudaEvent_t ev[3] = {};         // before the pivots / after the pass and carry / after the finish
-  bool timed = false;             // the last call took the sampled single pass (and ran to the end)
-  int reasons[GPUD_RANGE_N_OPEN_REASONS] = {};   // its open fields by reason
-  int fields_open = 0;            // fields it handed to the radix select
-  int nw = 0;                     // windows of its pass (rows of d_cls per field)
-  int64_t n_segs = 0;             // segments of its select (d_piv / d_fill entries) and class-count rows of its pass (d_cls
-  int64_t n_rows = 0;             //   entries, all fields): gpudh_ring_segment_scratch
+  bool timed = false;             // the last select was sampled (and ran to the end)
+  int reasons[GPUD_RANGE_N_OPEN_REASONS] = {};   // its open segments by reason
+  int fields_open = 0;            // segments it handed to the radix select
+  int64_t n_segs = 0;             // segments of its select (d_piv / d_fill entries) and rows of its pass (d_cls entries, all fields):
+  int64_t n_rows = 0;             //   gpudh_ring_range_scratch, gpudh_ring_segment_scratch
 };
 
 void gpud_range_state_free(gpud_range_state* s) {
   if (!s) return;
   for (auto* p : s->d_win) cudaFree(p);
-  cudaFree(s->d_win_nover); cudaFree(s->d_cls); cudaFree(s->d_lists); cudaFree(s->d_piv); cudaFree(s->d_fill);
+  cudaFree(s->d_geo); cudaFree(s->d_win_nover); cudaFree(s->d_cls); cudaFree(s->d_lists); cudaFree(s->d_piv); cudaFree(s->d_fill);
   cudaFree(s->d_out); cudaFree(s->d_nover); cudaFree(s->d_st); cudaFree(s->d_open); cudaFree(s->d_hist); cudaFree(s->d_cand);
   for (auto& ev : s->ev) if (ev) cudaEventDestroy(ev);
   delete s;
 }
 
-// One select over segments: n_seg segments of n samples per field from chronological column start (segment s = f n_seg + j,
-// internal.h).  gpud_ring_reduce_range is the case of one segment per field, gpud_ring_segments the stream windows of L > 1024.
-struct SegJob {
-  int64_t start, n, n_seg;
-  int Wp;              // window of the range pass; with n_seg > 1 it divides n
-  bool sampled;        // sampled pivots + classification fused into the pass (else every non-constant segment goes to the radix select)
-  bool carry;          // the EMA carry over each field's whole range (the range call's EMA; the stream commit runs its own)
-  int S;               // pivot sample: S strided reads, stride apart ...
-  int64_t stride;
-  bool ring_sample;    // ... or the ring's sample ring
-  size_t smem;         // k_range_pivots' dynamic shared memory
-  unsigned list_cap;   // keys between the pivots kept per segment
-};
 constexpr int kSelChunk = 4096;        // open segments per radix-select launch: its histograms and candidate lists are per segment
 
-// The keys per segment that the pivots of a sample of S keys out of n are expected to leave between them, twice over: the list
-// memory of a segment select scales with the segment, not with kListCap per segment (rank math of k_range_pivots).
-static unsigned seg_list_cap(int64_t n, int64_t S, long long k) {
-  const double pr = (double)k / (double)n, r0 = pr * (double)S, d = 5.0 * sqrt((double)S * pr * (1.0 - pr)) + 2.0;
+// The pivot sample and list of a segment of a handle with L > GPUD_MAX_WINDOW or of a long range, g->n samples of rank g->k: the ring's
+// sample ring when at least 2048 of its slots fall into the segment (the rule of the range call; windows of a quarter ring or more at
+// CAP = 1 Mi), else S = n / 32 strided reads (at least 64, at most GPUD_RANGE_SAMPLE_MAX), one 32-byte sector in every eight of the
+// segment: at L = 10 000 the sample ring holds only 78 slots, and the n / 8 stride of the range call would touch every other sector -
+// half a second read of the ring.  The list holds the keys the pivots of a sample of S are expected to leave between them, twice over:
+// the list memory of a segment select scales with the segment, not with kListCap per segment (rank math of k_range_pivots).
+static void seg_sample(gpud_range_geo* g, int smp_shift) {
+  const int64_t n = g->n;
+  g->smp = (n >> smp_shift) >= 2048;
+  if (!g->smp) {
+    g->S = (int)std::min<int64_t>(GPUD_RANGE_SAMPLE_MAX, std::max<int64_t>(64, n / 32));
+    g->stride = n / g->S;
+  }
+  const int64_t S = g->smp ? n >> smp_shift : g->S;
+  const double pr = (double)g->k / (double)n, r0 = pr * (double)S, d = 5.0 * sqrt((double)S * pr * (1.0 - pr)) + 2.0;
   const double ranks = std::min((double)S, ceil(r0 + d)) - std::max(0.0, floor(r0 - d)) + 1.0;
   const double want = 2.0 * ranks * (double)n / (double)S;
-  return (unsigned)std::min(std::min((double)n, (double)kListCap), std::max(256.0, ceil(want)));
+  g->lcap = (unsigned)std::min(std::min((double)n, (double)kListCap), std::max(256.0, ceil(want)));
 }
 
 // The radix select of the n_sel_all segments with ids (all n_segs when ids is NULL), kSelChunk at a time: digit histograms, then
-// the collect and the final list select, into s->d_out.  Segments of n samples from chronological column start (n_seg per field), or
-// (TABLE) the long ranges of gpud_ring_reduce_ranges, n their longest.
-template <bool TABLE>
-static cudaError_t radix_select(gpud_ring* ring, gpud_range_state* s, int64_t start, int64_t n, int64_t n_seg, int64_t n_segs, const int* ids, int n_sel_all,
-                                const gpud_range_geo* geo) {
+// the collect and the final list select, into s->d_out.  n: the longest segment of the table.
+static cudaError_t radix_select(gpud_ring* ring, gpud_range_state* s, int64_t n, int64_t n_geo, int64_t n_segs, const int* ids, int n_sel_all) {
   const cudaStream_t stream = ring->stream;
   cudaError_t e = cudaSuccess;
   const int chunk = ids ? kSelChunk : n_sel_all;
@@ -584,11 +547,11 @@ static cudaError_t radix_select(gpud_ring* ring, gpud_range_state* s, int64_t st
       const int bpf = (int)std::max<int64_t>(1, std::min<int64_t>((n + 16383) / 16384, std::max(1, 8 * ring->sm_count / n_sel + 1)));
       if (n > kCollectMax) {
         for (int pass = 0; pass < kMaxHistPasses; ++pass) {          // later passes exit at once for segments that are already narrow
-          k_sel_hist<TABLE><<<dim3(bpf, n_sel), 256, 0, stream>>>(ring->d_ring, ring->cap, start, n, s->d_st, s->d_hist, ids_c, n_seg, geo);
+          k_sel_hist<<<dim3(bpf, n_sel), 256, 0, stream>>>(ring->d_ring, ring->cap, s->d_geo, n_geo, s->d_st, s->d_hist, ids_c);
           k_sel_pick<<<n_sel, kSelThreads, 0, stream>>>(s->d_hist, s->d_st, ids_c);
         }
       }
-      k_sel_collect<TABLE><<<dim3(bpf, n_sel), 256, 0, stream>>>(ring->d_ring, ring->cap, start, n, s->d_st, s->d_cand, ids_c, n_seg, geo);
+      k_sel_collect<<<dim3(bpf, n_sel), 256, 0, stream>>>(ring->d_ring, ring->cap, s->d_geo, n_geo, s->d_st, s->d_cand, ids_c);
       k_sel_final<<<n_sel, kSelThreads, 0, stream>>>(s->d_st, s->d_cand, (int)n_segs, s->d_out, ids_c);
       e = cudaGetLastError();
     }
@@ -596,29 +559,37 @@ static cudaError_t radix_select(gpud_ring* ring, gpud_range_state* s, int64_t st
   return e;
 }
 
-// out_f64 / out_n_over: host results [5][F] / [F] (one segment per field), synchronous.  NULL: the results stay on the device in
-// s->d_out / s->d_nover and the call synchronises only to size the radix select.
-static int32_t run_select(gpud_ring* ring, gpud_range_state* s, const SegJob& j, double* out_f64, uint32_t* out_n_over) {
-  gpud_ctx* ctx = ring->ctx;
-  const cudaStream_t stream = ring->stream;
-  const int F = ring->F;
-  const int64_t start = j.start, n = j.n;
-  const int Wp = j.Wp;
-  const int64_t n_segs = (int64_t)F * j.n_seg;         // the per-field arrays of the finish and the radix select are per segment
-  const int nw = (int)((j.n_seg * n + Wp - 1) / Wp);  // windows of the pass per field
-  const int seg_sub = (int)(nw / j.n_seg);            // ... per segment
-  const bool sampled = j.sampled;
-  const unsigned list_cap = j.list_cap;
-  const long long k_from_top = gpud_rank_from_top(n, ring->q_num, ring->q_den);
+// One segment select over the table geo[0, n_geo) (internal.h), every field: the pivots (sampled), the pass, the finish, then the
+// radix select for the segments the finish left open.  The pass is the window pass in windows of Wp over the n_geo segments, which
+// follow one another from geo[0].start on, or (d_tile) the long route's tile pass over its tile list; with `ema` it leaves each
+// segment's EMA at the row of its last window of d_win[3] (the range call's carry, k_ranges_ema), which the finish reports.  Sampled,
+// the select synchronises once to size the radix select, and the range call's host results out_f64 [5][F] / out_n_over [F] are
+// copied in that synchronisation; unsampled, every segment that is not constant goes to the radix select without it.  The results
+// stay on the device in s->d_out / s->d_nover, valid until the next select on s.
+static int32_t run_select(gpud_ring* r, gpud_range_state* s, const gpud_range_geo* geo, int64_t n_geo, int Wp, bool sampled, bool ema,
+                          const int32_t* d_tile, double* out_f64, uint32_t* out_n_over) {
+  gpud_ctx* ctx = r->ctx;
+  const cudaStream_t stream = r->stream;
+  const int F = r->F;
+  const int64_t n_segs = (int64_t)F * n_geo;
+  const gpud_range_geo& last = geo[n_geo - 1];
+  const int64_t rows = last.tile0 + (last.n + Wp - 1) / Wp, list_row = last.list0 + last.lcap;   // per field
+  int64_t n_max = 0;
+  size_t smem = 0;                     // k_range_pivots: the largest sample of the table
+  for (int64_t j = 0; j < n_geo; ++j) {
+    n_max = std::max(n_max, geo[j].n);
+    smem = std::max(smem, (geo[j].smp ? (size_t)GPUD_RANGE_SAMPLE_MAX : (size_t)geo[j].S) * sizeof(unsigned long long));
+  }
 
-  GPUD_CUDA(ctx, cudaSetDevice(ring->dev));
-  s->timed = false;                    // until this call has run to the end: a failed grow may free the last call's scratch
-  const size_t per = (size_t)F * nw;
+  GPUD_CUDA(ctx, cudaSetDevice(r->dev));
+  s->timed = false;                    // until this select has run to the end: a failed grow may free the last one's scratch
+  const size_t per = (size_t)F * rows;
+  GPUD_CUDA(ctx, gpud_grow(&s->d_geo, &s->geo_cap, (size_t)n_geo));
   for (int i = 0; i < 5; ++i) GPUD_CUDA(ctx, gpud_grow(&s->d_win[i], &s->win_cap[i], per));
   GPUD_CUDA(ctx, gpud_grow(&s->d_win_nover, &s->win_nover_cap, per));
   if (sampled) {
     GPUD_CUDA(ctx, gpud_grow(&s->d_cls, &s->cls_cap, per));
-    GPUD_CUDA(ctx, gpud_grow(&s->d_lists, &s->lists_cap, (size_t)n_segs * list_cap));
+    GPUD_CUDA(ctx, gpud_grow(&s->d_lists, &s->lists_cap, (size_t)F * list_row));
     GPUD_CUDA(ctx, gpud_grow(&s->d_piv, &s->piv_cap, 2 * (size_t)n_segs));
     GPUD_CUDA(ctx, gpud_grow(&s->d_fill, &s->fill_cap, (size_t)n_segs));
   }
@@ -627,7 +598,6 @@ static int32_t run_select(gpud_ring* ring, gpud_range_state* s, const SegJob& j,
   GPUD_CUDA(ctx, gpud_grow(&s->d_st, &s->st_cap, (size_t)n_segs));
   GPUD_CUDA(ctx, gpud_grow(&s->d_open, &s->open_cap, 1 + (size_t)n_segs));
   for (auto& ev : s->ev) if (!ev) GPUD_CUDA(ctx, cudaEventCreate(&ev));
-  s->nw = nw;
   s->n_segs = n_segs;
   s->n_rows = (int64_t)per;
   std::fill(s->reasons, s->reasons + GPUD_RANGE_N_OPEN_REASONS, 0);
@@ -635,41 +605,43 @@ static int32_t run_select(gpud_ring* ring, gpud_range_state* s, const SegJob& j,
   unsigned* fill = sampled ? s->d_fill : nullptr;
   uint4* cls = sampled ? s->d_cls : nullptr;
   unsigned long long* lists = sampled ? s->d_lists : nullptr;
+  double* const w[5] = {s->d_win[0], s->d_win[1], s->d_win[2], ema ? s->d_win[3] : nullptr, s->d_win[4]};
 
   unsigned h_open = 0;
-  cudaError_t e = cudaMemsetAsync(s->d_open, 0, sizeof(unsigned), stream);
+  cudaError_t e = cudaMemcpyAsync(s->d_geo, geo, n_geo * sizeof(gpud_range_geo), cudaMemcpyHostToDevice, stream);
+  if (e == cudaSuccess) e = cudaMemsetAsync(s->d_open, 0, sizeof(unsigned), stream);
   if (e == cudaSuccess) e = cudaEventRecord(s->ev[0], stream);
   if (e == cudaSuccess && sampled) {
-    e = cudaFuncSetAttribute(k_range_pivots<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(GPUD_RANGE_SAMPLE_MAX * sizeof(unsigned long long)));
-    if (e == cudaSuccess) k_range_pivots<false><<<(unsigned)n_segs, kSelThreads, j.smem, stream>>>(ring->d_ring, ring->cap, start, n, j.S, j.stride, k_from_top, s->d_piv,
-                                                                                               s->d_fill, j.ring_sample ? ring->d_sample : nullptr, ring->smp_shift,
-                                                                                               ring->smp_slots, j.n_seg, nullptr);
+    e = cudaFuncSetAttribute(k_range_pivots, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(GPUD_RANGE_SAMPLE_MAX * sizeof(unsigned long long)));
+    if (e == cudaSuccess) k_range_pivots<<<(unsigned)n_segs, kSelThreads, smem, stream>>>(r->d_ring, r->cap, s->d_geo, n_geo, s->d_piv, s->d_fill, r->d_sample,
+                                                                                  r->smp_shift, r->smp_slots);
     if (e == cudaSuccess) e = cudaGetLastError();
   }
-  if (e == cudaSuccess) {
-    double* w[5] = {s->d_win[0], s->d_win[1], s->d_win[2], j.carry ? s->d_win[3] : nullptr, s->d_win[4]};
-    int32_t rc = gpud_ring_window_pass(ring, start, j.n_seg * n, Wp, w, s->d_win_nover, piv, cls, lists, fill, list_cap, seg_sub);
+  if (e == cudaSuccess && d_tile) {
+    e = gpud_ranges_tiles(r, s->d_geo, n_geo, d_tile, rows, piv, w, s->d_win_nover, cls, lists, list_row, fill);
+    if (e == cudaSuccess && ema) e = gpud_ranges_ema(r, s->d_geo, n_geo, w[4], rows, w[3]);
+  } else if (e == cudaSuccess) {
+    // segment j's windows are rows j rows / n_geo .. of its field's rows: the window kernel's seg_sub mapping
+    int32_t rc = gpud_ring_window_pass(r, geo[0].start, n_geo * geo[0].n, Wp, w, s->d_win_nover, piv, cls, lists, fill, geo[0].lcap, (int)(rows / n_geo));
     if (rc) return rc;
-    e = cudaEventRecord(s->ev[1], stream);
   }
+  if (e == cudaSuccess) e = cudaEventRecord(s->ev[1], stream);
   if (e == cudaSuccess) {
-    // the windows of segment s are rows s * seg_sub .. of the pass's [F][nw] output: the finish runs on them as on fields
-    k_range_finish<false><<<(unsigned)n_segs, kSelThreads, 0, stream>>>((int)n_segs, seg_sub, Wp, n, s->d_win[0], s->d_win[1], s->d_win[2],
-                                                                        j.carry ? s->d_win[3] : s->d_win[4], s->d_win_nover, ring->q_num, ring->q_den,
-                                                                        sampled ? 1 : 0, piv, fill, cls, lists, list_cap, s->d_out, s->d_nover, s->d_st, s->d_open,
-                                                                        reinterpret_cast<int*>(s->d_open + 1), nullptr, 0, 0, 0, nullptr);
+    k_range_finish<<<(unsigned)n_segs, kSelThreads, 0, stream>>>((int)n_segs, Wp, s->d_geo, n_geo, rows, list_row, w[0], w[1], w[2], w[3], s->d_win_nover,
+                                                            sampled ? 1 : 0, piv, fill, cls, lists, s->d_out, s->d_nover, s->d_st, s->d_open,
+                                                            reinterpret_cast<int*>(s->d_open + 1));
     e = cudaGetLastError();
   }
   if (e == cudaSuccess) e = cudaEventRecord(s->ev[2], stream);
-  if (e == cudaSuccess && sampled) {   // a short range leaves every non-constant field to the radix select: no need to ask
+  if (e == cudaSuccess && sampled) {   // unsampled, every non-constant segment goes to the radix select: no need to ask
     e = cudaMemcpyAsync(&h_open, s->d_open, sizeof(unsigned), cudaMemcpyDeviceToHost, stream);
     if (e == cudaSuccess && out_f64) e = cudaMemcpyAsync(out_f64, s->d_out, 5 * F * sizeof(double), cudaMemcpyDeviceToHost, stream);
     if (e == cudaSuccess && out_n_over) e = cudaMemcpyAsync(out_n_over, s->d_nover, F * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
   }
   if (e == cudaSuccess && (h_open > 0 || !sampled)) {
-    // radix select for the segments still open: every non-constant field of a short range, or the rare segment the sampled pass
-    // could not settle.  The grid covers only the open segments (kSelChunk at a time), with enough blocks each to fill the machine.
+    // radix select for the segments still open: every non-constant segment of an unsampled select, or the rare segment the sampled
+    // pass could not settle.  The grid covers only the open segments (kSelChunk at a time), with enough blocks each to fill the machine.
     const int* ids = sampled ? reinterpret_cast<const int*>(s->d_open + 1) : nullptr;
     const int n_sel_all = sampled ? (int)h_open : (int)n_segs;
     if (sampled) {
@@ -678,16 +650,9 @@ static int32_t run_select(gpud_ring* ring, gpud_range_state* s, const SegJob& j,
       if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
       for (const SelState& q : h_st) if (q.why > 0 && q.why < GPUD_RANGE_N_OPEN_REASONS) ++s->reasons[q.why];
     }
-    e = radix_select<false>(ring, s, start, n, j.n_seg, n_segs, ids, n_sel_all, nullptr);
-    if (e == cudaSuccess && out_f64 && !sampled) {
-      e = cudaMemcpyAsync(out_f64, s->d_out, 5 * F * sizeof(double), cudaMemcpyDeviceToHost, stream);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(out_n_over, s->d_nover, F * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream);
-    } else if (e == cudaSuccess && out_f64) {
-      e = cudaMemcpyAsync(out_f64 + 4 * (size_t)F, s->d_out + 4 * (size_t)F, F * sizeof(double), cudaMemcpyDeviceToHost, stream);
-    }
+    if (e == cudaSuccess) e = radix_select(r, s, n_max, n_geo, n_segs, ids, n_sel_all);
   }
-  if (e == cudaSuccess && out_f64) e = cudaStreamSynchronize(stream);
-  if (e != cudaSuccess) return gpud_fail(ctx, GPUD_E_CUDA, "%s: %s", out_f64 ? "reduce_range" : "windows_reduce", cudaGetErrorString(e));
+  if (e != cudaSuccess) return gpud_fail(ctx, GPUD_E_CUDA, "segment select: %s", cudaGetErrorString(e));
   s->timed = sampled;
   s->fields_open = (int)h_open;
   return GPUD_OK;
@@ -697,51 +662,50 @@ extern "C" int32_t gpud_ring_reduce_range(gpud_ring* ring, int64_t last_n, doubl
   if (!ring || !out_f64 || !out_n_over || last_n < 0) return GPUD_E_INVALID;
   const int64_t count = ring_count(ring);
   if (count == 0) return GPUD_E_STATE;
-  SegJob j{};
-  j.n = last_n == 0 || last_n > count ? count : last_n;
-  j.start = ring_start(ring) + (count - j.n);
-  if (j.start >= ring->cap) j.start -= ring->cap;
-  j.n_seg = 1;
-  j.Wp = (int)std::min<int64_t>(GPUD_MAX_WINDOW, j.n);
-  j.sampled = j.n >= kSampledMin;
-  j.carry = true;
-  j.S = (int)std::min<int64_t>(GPUD_RANGE_SAMPLE_MAX, j.n / 8);
-  j.stride = j.S ? j.n / j.S : 0;
-  j.ring_sample = (j.n >> ring->smp_shift) >= 2048;   // else too few of the ring's sample slots fall into the range
-  j.smem = (size_t)GPUD_RANGE_SAMPLE_MAX * sizeof(unsigned long long);
-  j.list_cap = (unsigned)std::min<int64_t>(kListCap, j.n);
+  // one segment per field, with the range call's own sample rule: S = n / 8 strided reads, or the sample ring when at least 2048 of
+  // its slots fall into the range (else too few of them do)
+  gpud_range_geo g{};
+  g.n = last_n == 0 || last_n > count ? count : last_n;
+  g.start = (ring_start(ring) + (count - g.n)) % ring->cap;
+  g.k = gpud_rank_from_top(g.n, ring->q_num, ring->q_den);
+  g.S = (int)std::min<int64_t>(GPUD_RANGE_SAMPLE_MAX, g.n / 8);
+  g.stride = g.S ? g.n / g.S : 0;
+  g.smp = (g.n >> ring->smp_shift) >= 2048;
+  g.lcap = (unsigned)std::min<int64_t>(kListCap, g.n);
+  const bool sampled = g.n >= kSampledMin;
   if (!ring->range) ring->range = new gpud_range_state();
-  return run_select(ring, ring->range, j, out_f64, out_n_over);
+  const gpud_range_state* s = ring->range;
+  { int32_t rc = run_select(ring, ring->range, &g, 1, (int)std::min<int64_t>(GPUD_MAX_WINDOW, g.n), sampled, true, nullptr, out_f64, out_n_over); if (rc) return rc; }
+  // what the select's synchronisation did not bring: every result of an unsampled call, the p99 of the fields the radix select took
+  const size_t F = (size_t)ring->F;
+  cudaError_t e = cudaSuccess;
+  if (!sampled) {
+    e = cudaMemcpyAsync(out_f64, s->d_out, 5 * F * sizeof(double), cudaMemcpyDeviceToHost, ring->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(out_n_over, s->d_nover, F * sizeof(uint32_t), cudaMemcpyDeviceToHost, ring->stream);
+  } else if (s->fields_open > 0) {
+    e = cudaMemcpyAsync(out_f64 + 4 * F, s->d_out + 4 * F, F * sizeof(double), cudaMemcpyDeviceToHost, ring->stream);
+  }
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ring->stream);
+  if (e != cudaSuccess) return gpud_fail(ring->ctx, GPUD_E_CUDA, "reduce_range: %s", cudaGetErrorString(e));
+  return GPUD_OK;
 }
 
-// Stream windows of L = seg_len > GPUD_MAX_WINDOW samples (internal.h).  Every segment takes the sampled single pass, whatever its
-// length.  The pivot sample of a segment: the ring's sample ring when at least 2048 of its slots fall into the segment (the rule of
-// the range call; windows of a quarter ring or more at CAP = 1 Mi), else S = seg_len / 32 strided reads (at least 64, at most
-// GPUD_RANGE_SAMPLE_MAX), one 32-byte sector in every eight of the segment: at L = 10 000 the sample ring holds only 78 slots, and
-// the n / 8 stride of the range call would touch every other sector - half a second read of the ring.  The list is sized from S.
+// Stream windows of L = seg_len > GPUD_MAX_WINDOW samples (internal.h): one sampled select over n_seg segments per field, each under
+// the rule of seg_sample, at the rows, lists, pivots and fill counters the window kernel's seg_sub mapping gives it.
 int32_t gpud_ring_segments(gpud_ring* r, gpud_range_state** st, int64_t start, int64_t seg_len, int64_t n_seg, int Wp, gpud_seg_out* out) {
-  SegJob j{};
-  j.start = start;
-  j.n = seg_len;
-  j.n_seg = n_seg;
-  j.Wp = Wp;
-  j.sampled = true;
-  j.carry = false;
-  j.ring_sample = (seg_len >> r->smp_shift) >= 2048;
-  int64_t s_est;
-  if (j.ring_sample) {
-    s_est = seg_len >> r->smp_shift;
-    j.smem = (size_t)GPUD_RANGE_SAMPLE_MAX * sizeof(unsigned long long);
-  } else {
-    j.S = (int)std::min<int64_t>(GPUD_RANGE_SAMPLE_MAX, std::max<int64_t>(64, seg_len / 32));
-    j.stride = seg_len / j.S;
-    s_est = j.S;
-    j.smem = (size_t)j.S * sizeof(unsigned long long);
+  gpud_range_geo g{};
+  g.n = seg_len;
+  g.k = gpud_rank_from_top(seg_len, r->q_num, r->q_den);
+  seg_sample(&g, r->smp_shift);
+  std::vector<gpud_range_geo> geo(n_seg, g);
+  for (int64_t j = 0; j < n_seg; ++j) {
+    geo[j].start = (start + j * seg_len) % r->cap;
+    geo[j].tile0 = j * (seg_len / Wp);
+    geo[j].list0 = j * (int64_t)g.lcap;
   }
-  j.list_cap = seg_list_cap(seg_len, s_est, gpud_rank_from_top(seg_len, r->q_num, r->q_den));
   if (!*st) *st = new gpud_range_state();
   gpud_range_state* s = *st;
-  { int32_t rc = run_select(r, s, j, nullptr, nullptr); if (rc) return rc; }
+  { int32_t rc = run_select(r, s, geo.data(), n_seg, Wp, true, false, nullptr, nullptr, nullptr); if (rc) return rc; }
   out->out = s->d_out;
   out->nover = s->d_nover;
   out->part = s->d_win[4];
@@ -773,9 +737,9 @@ extern "C" int32_t gpudh_ring_range_scratch(gpud_ring* r, double* piv, uint32_t*
   GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
   GPUD_CUDA(r->ctx, cudaMemcpyAsync(piv, s->d_piv, 2 * F * sizeof(double), cudaMemcpyDeviceToHost, r->stream));
   GPUD_CUDA(r->ctx, cudaMemcpyAsync(fill, s->d_fill, F * sizeof(uint32_t), cudaMemcpyDeviceToHost, r->stream));
-  if (cls) GPUD_CUDA(r->ctx, cudaMemcpyAsync(cls, s->d_cls, F * s->nw * sizeof(uint4), cudaMemcpyDeviceToHost, r->stream));
+  if (cls) GPUD_CUDA(r->ctx, cudaMemcpyAsync(cls, s->d_cls, s->n_rows * sizeof(uint4), cudaMemcpyDeviceToHost, r->stream));
   GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));
-  *nw = s->nw;
+  *nw = s->n_rows / r->F;
   return GPUD_OK;
 }
 
@@ -792,7 +756,7 @@ struct RangesPlan {
   std::vector<gpud_short_range> shorts;
   std::vector<gpud_range_geo> geo;            // the long ranges in call order, batch by batch; tile0 / list0 count from their batch's first
   std::vector<int64_t> batch0;                // batch b is geo[batch0[b], batch0[b + 1])
-  std::vector<int64_t> tiles0, lists0;        // ... its tiles and list keys before it (flat over the call)
+  std::vector<int64_t> tiles0;                // ... its tiles before it (flat over the call)
 };
 
 // Validation, the physical columns, the routes, the tile list and the batches.  Pure host arithmetic.
@@ -805,7 +769,6 @@ static int32_t ranges_plan(int64_t total, int64_t cap, int F, int q_num, int q_d
   pl->route.assign(n, 0);
   pl->batch0.assign(1, 0);
   pl->tiles0.assign(1, 0);
-  pl->lists0.assign(1, 0);
   int64_t bytes = 0, tiles = 0, keys = 0;
   for (int64_t i = 0; i < n; ++i) {
     pl->start[i] = first[i] % cap;             // column c holds every sample c + k CAP; sample first[i] is still in the ring
@@ -813,22 +776,12 @@ static int32_t ranges_plan(int64_t total, int64_t cap, int F, int q_num, int q_d
       pl->shorts.push_back({pl->start[i], (int32_t)len[i], (int32_t)i});
       continue;
     }
-    // the pivot sample: the rule of gpud_ring_segments
     gpud_range_geo g{};
     g.start = pl->start[i];
     g.n = len[i];
     g.k = gpud_rank_from_top(len[i], q_num, q_den);
     g.id = i;
-    g.smp = (len[i] >> smp_shift) >= 2048;
-    int64_t s_est;
-    if (g.smp) {
-      s_est = len[i] >> smp_shift;
-    } else {
-      g.S = (int)std::min<int64_t>(GPUD_RANGE_SAMPLE_MAX, std::max<int64_t>(64, len[i] / 32));
-      g.stride = len[i] / g.S;
-      s_est = g.S;
-    }
-    g.lcap = seg_list_cap(len[i], s_est, g.k);
+    seg_sample(&g, smp_shift);
     const int64_t nt = (len[i] + GPUD_MAX_WINDOW - 1) / GPUD_MAX_WINDOW;
     g.d_last = pow(1.0 - alpha, (double)(len[i] - (nt - 1) * GPUD_MAX_WINDOW));
     // per field: the tiles' min / max / mean / EMA partials / n_over / class counts, the key list, the segment's pivots, fill, result
@@ -837,7 +790,6 @@ static int32_t ranges_plan(int64_t total, int64_t cap, int F, int q_num, int q_d
     if ((int64_t)pl->geo.size() > pl->batch0.back() && bytes + b > kRangesBatchBytes) {
       pl->batch0.push_back((int64_t)pl->geo.size());
       pl->tiles0.push_back(pl->tiles0.back() + tiles);
-      pl->lists0.push_back(pl->lists0.back() + keys);
       bytes = tiles = keys = 0;
     }
     g.tile0 = tiles;
@@ -850,7 +802,6 @@ static int32_t ranges_plan(int64_t total, int64_t cap, int F, int q_num, int q_d
   }
   pl->batch0.push_back((int64_t)pl->geo.size());
   pl->tiles0.push_back(pl->tiles0.back() + tiles);
-  pl->lists0.push_back(pl->lists0.back() + keys);
   return GPUD_OK;
 }
 
@@ -858,8 +809,7 @@ static int32_t ranges_plan(int64_t total, int64_t cap, int F, int q_num, int q_d
 struct gpud_ranges_state {
   gpud_range_state* seg = nullptr;                              // the long route's segment select (apart from gpud_ring_reduce_range's)
   gpud_short_range* d_short = nullptr;  size_t short_cap = 0;
-  gpud_range_geo* d_geo = nullptr;  size_t geo_cap = 0;         // one batch's long ranges
-  int32_t* d_tile = nullptr;  size_t tile_cap = 0;              // ... and the long range of each of its tiles
+  int32_t* d_tile = nullptr;  size_t tile_cap = 0;              // the long range of each tile of one batch
   double* d_out = nullptr;  size_t out_cap = 0;                 // the call's result [5][F][n]
   uint32_t* d_nover = nullptr;  size_t nover_cap = 0;           //   and n_over [F][n]
   cudaEvent_t ev[2] = {};
@@ -872,7 +822,7 @@ struct gpud_ranges_state {
 void gpud_ranges_state_free(gpud_ranges_state* s) {
   if (!s) return;
   gpud_range_state_free(s->seg);
-  cudaFree(s->d_short); cudaFree(s->d_geo); cudaFree(s->d_tile); cudaFree(s->d_out); cudaFree(s->d_nover);
+  cudaFree(s->d_short); cudaFree(s->d_tile); cudaFree(s->d_out); cudaFree(s->d_nover);
   for (auto& ev : s->ev) if (ev) cudaEventDestroy(ev);
   delete s;
 }
@@ -889,73 +839,6 @@ __global__ void k_ranges_scatter(const double* __restrict__ seg_out, const uint3
   }
 }
 }  // namespace
-
-// One batch of the long route: pivots, tile pass, EMA, finish; one synchronisation; the radix select for the segments left open.
-static cudaError_t ranges_batch(gpud_ring* r, gpud_ranges_state* rs, const RangesPlan& pl, size_t b, int64_t n_out) {
-  gpud_range_state* s = rs->seg;
-  const cudaStream_t stream = r->stream;
-  const int F = r->F;
-  const int64_t g0 = pl.batch0[b], n_long = pl.batch0[b + 1] - g0;
-  const int64_t n_tiles = pl.tiles0[b + 1] - pl.tiles0[b], list_row = pl.lists0[b + 1] - pl.lists0[b];
-  const int64_t n_segs = (int64_t)F * n_long;
-  const size_t per = (size_t)F * n_tiles;
-  cudaError_t e = cudaSuccess;
-  for (int i = 0; i < 5 && e == cudaSuccess; ++i) e = gpud_grow(&s->d_win[i], &s->win_cap[i], per);
-  if (e == cudaSuccess) e = gpud_grow(&s->d_win_nover, &s->win_nover_cap, per);
-  if (e == cudaSuccess) e = gpud_grow(&s->d_cls, &s->cls_cap, per);
-  if (e == cudaSuccess) e = gpud_grow(&s->d_lists, &s->lists_cap, (size_t)F * list_row);
-  if (e == cudaSuccess) e = gpud_grow(&s->d_piv, &s->piv_cap, 2 * (size_t)n_segs);
-  if (e == cudaSuccess) e = gpud_grow(&s->d_fill, &s->fill_cap, (size_t)n_segs);
-  if (e == cudaSuccess) e = gpud_grow(&s->d_out, &s->out_cap, 5 * (size_t)n_segs);
-  if (e == cudaSuccess) e = gpud_grow(&s->d_nover, &s->nover_cap, (size_t)n_segs);
-  if (e == cudaSuccess) e = gpud_grow(&s->d_st, &s->st_cap, (size_t)n_segs);
-  if (e == cudaSuccess) e = gpud_grow(&s->d_open, &s->open_cap, 1 + (size_t)n_segs);
-  if (e == cudaSuccess) e = gpud_grow(&rs->d_geo, &rs->geo_cap, (size_t)n_long);
-  if (e == cudaSuccess) e = gpud_grow(&rs->d_tile, &rs->tile_cap, (size_t)n_tiles);
-  if (e != cudaSuccess) return e;
-  s->n_segs = n_segs;
-  s->n_rows = (int64_t)per;
-  rs->seg_last = true;
-  std::vector<int32_t> tile(n_tiles);
-  for (int64_t j = 0; j < n_long; ++j) {
-    const gpud_range_geo& g = pl.geo[g0 + j];
-    std::fill(tile.begin() + g.tile0, tile.begin() + g.tile0 + (g.n + GPUD_MAX_WINDOW - 1) / GPUD_MAX_WINDOW, (int32_t)j);
-  }
-  e = cudaMemcpyAsync(rs->d_geo, pl.geo.data() + g0, n_long * sizeof(gpud_range_geo), cudaMemcpyHostToDevice, stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(rs->d_tile, tile.data(), n_tiles * sizeof(int32_t), cudaMemcpyHostToDevice, stream);
-  if (e == cudaSuccess) e = cudaMemsetAsync(s->d_open, 0, sizeof(unsigned), stream);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(k_range_pivots<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(GPUD_RANGE_SAMPLE_MAX * sizeof(unsigned long long)));
-  if (e != cudaSuccess) return e;
-  k_range_pivots<true><<<(unsigned)n_segs, kSelThreads, GPUD_RANGE_SAMPLE_MAX * sizeof(unsigned long long), stream>>>(
-      r->d_ring, r->cap, 0, 0, 0, 0, 0, s->d_piv, s->d_fill, r->d_sample, r->smp_shift, r->smp_slots, n_long, rs->d_geo);
-  if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  double* const w[5] = {s->d_win[0], s->d_win[1], s->d_win[2], nullptr, s->d_win[4]};
-  if ((e = gpud_ranges_tiles(r, rs->d_geo, n_long, rs->d_tile, n_tiles, s->d_piv, w, s->d_win_nover, s->d_cls, s->d_lists, list_row, s->d_fill)) != cudaSuccess) return e;
-  double* seg_ema = s->d_win[3];                       // F n_tiles >= F n_long: a long range has two tiles or more
-  if ((e = gpud_ranges_ema(r, rs->d_geo, n_long, s->d_win[4], n_tiles, seg_ema)) != cudaSuccess) return e;
-  k_range_finish<true><<<(unsigned)n_segs, kSelThreads, 0, stream>>>((int)n_segs, 0, GPUD_MAX_WINDOW, 0, s->d_win[0], s->d_win[1], s->d_win[2], nullptr,
-                                                                     s->d_win_nover, r->q_num, r->q_den, 1, s->d_piv, s->d_fill, s->d_cls, s->d_lists, 0,
-                                                                     s->d_out, s->d_nover, s->d_st, s->d_open, reinterpret_cast<int*>(s->d_open + 1),
-                                                                     rs->d_geo, n_long, n_tiles, list_row, seg_ema);
-  if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  unsigned h_open = 0;
-  e = cudaMemcpyAsync(&h_open, s->d_open, sizeof(unsigned), cudaMemcpyDeviceToHost, stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-  if (e == cudaSuccess && h_open > 0) {
-    std::vector<SelState> h_st(n_segs);
-    e = cudaMemcpyAsync(h_st.data(), s->d_st, n_segs * sizeof(SelState), cudaMemcpyDeviceToHost, stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-    for (const SelState& q : h_st) if (q.why > 0 && q.why < GPUD_RANGE_N_OPEN_REASONS) ++rs->reasons[q.why];
-    int64_t n_max = 0;
-    for (int64_t j = 0; j < n_long; ++j) n_max = std::max(n_max, pl.geo[g0 + j].n);
-    if (e == cudaSuccess) e = radix_select<true>(r, s, 0, n_max, n_long, n_segs, reinterpret_cast<const int*>(s->d_open + 1), (int)h_open, rs->d_geo);
-    rs->open += h_open;
-  }
-  if (e != cudaSuccess) return e;
-  const int grid = (int)std::min<int64_t>((n_segs + 255) / 256, (int64_t)r->sm_count * 8);
-  k_ranges_scatter<<<grid, 256, 0, stream>>>(s->d_out, s->d_nover, rs->d_geo, n_long, F, n_out, rs->d_out, rs->d_nover);
-  return cudaGetLastError();
-}
 
 extern "C" int32_t gpud_ring_reduce_ranges(gpud_ring* r, const int64_t* first, const int64_t* len, int64_t n_ranges, double* out_f64, uint32_t* out_n_over) {
   if (!r || n_ranges < 0) return GPUD_E_INVALID;
@@ -981,14 +864,33 @@ extern "C" int32_t gpud_ring_reduce_ranges(gpud_ring* r, const int64_t* first, c
   GPUD_CUDA(r->ctx, gpud_grow(&rs->d_nover, &rs->nover_cap, plane));
   GPUD_CUDA(r->ctx, gpud_grow(&rs->d_short, &rs->short_cap, std::max<size_t>(1, pl.shorts.size())));
   for (auto& ev : rs->ev) if (!ev) GPUD_CUDA(r->ctx, cudaEventCreate(&ev));
-  cudaError_t e = cudaEventRecord(rs->ev[0], r->stream);
-  if (e == cudaSuccess && !pl.shorts.empty()) {
-    e = cudaMemcpyAsync(rs->d_short, pl.shorts.data(), pl.shorts.size() * sizeof(gpud_short_range), cudaMemcpyHostToDevice, r->stream);
-    if (e == cudaSuccess) e = gpud_ranges_short(r, rs->d_short, (int)pl.shorts.size(), n_ranges, rs->d_out, rs->d_nover);
+  GPUD_CUDA(r->ctx, cudaEventRecord(rs->ev[0], r->stream));
+  if (!pl.shorts.empty()) {
+    GPUD_CUDA(r->ctx, cudaMemcpyAsync(rs->d_short, pl.shorts.data(), pl.shorts.size() * sizeof(gpud_short_range), cudaMemcpyHostToDevice, r->stream));
+    GPUD_CUDA(r->ctx, gpud_ranges_short(r, rs->d_short, (int)pl.shorts.size(), n_ranges, rs->d_out, rs->d_nover));
   }
-  for (size_t b = 0; e == cudaSuccess && b + 1 < pl.batch0.size(); ++b)
-    if (pl.batch0[b + 1] > pl.batch0[b]) e = ranges_batch(r, rs, pl, b, n_ranges);
-  if (e == cudaSuccess) e = cudaEventRecord(rs->ev[1], r->stream);
+  for (size_t b = 0; b + 1 < pl.batch0.size(); ++b) {
+    // one batch of the long route: the segment select over its long ranges, read in tiles, then the scatter of its results
+    const int64_t g0 = pl.batch0[b], n_long = pl.batch0[b + 1] - g0, n_tiles = pl.tiles0[b + 1] - pl.tiles0[b];
+    if (n_long == 0) continue;
+    std::vector<int32_t> tile(n_tiles);
+    for (int64_t j = 0; j < n_long; ++j) {
+      const gpud_range_geo& g = pl.geo[g0 + j];
+      std::fill(tile.begin() + g.tile0, tile.begin() + g.tile0 + (g.n + GPUD_MAX_WINDOW - 1) / GPUD_MAX_WINDOW, (int32_t)j);
+    }
+    GPUD_CUDA(r->ctx, gpud_grow(&rs->d_tile, &rs->tile_cap, (size_t)n_tiles));
+    GPUD_CUDA(r->ctx, cudaMemcpyAsync(rs->d_tile, tile.data(), n_tiles * sizeof(int32_t), cudaMemcpyHostToDevice, r->stream));
+    gpud_range_state* s = rs->seg;
+    { int32_t rc = run_select(r, s, pl.geo.data() + g0, n_long, GPUD_MAX_WINDOW, true, true, rs->d_tile, nullptr, nullptr); if (rc) return rc; }
+    rs->seg_last = true;
+    rs->open += s->fields_open;
+    for (int i = 0; i < GPUD_RANGE_N_OPEN_REASONS; ++i) rs->reasons[i] += s->reasons[i];
+    const int64_t n_segs = (int64_t)r->F * n_long;
+    const int grid = (int)std::min<int64_t>((n_segs + 255) / 256, (int64_t)r->sm_count * 8);
+    k_ranges_scatter<<<grid, 256, 0, r->stream>>>(s->d_out, s->d_nover, s->d_geo, n_long, r->F, n_ranges, rs->d_out, rs->d_nover);
+    GPUD_CUDA(r->ctx, cudaGetLastError());
+  }
+  cudaError_t e = cudaEventRecord(rs->ev[1], r->stream);
   if (e == cudaSuccess) e = cudaMemcpyAsync(out_f64, rs->d_out, 5 * plane * sizeof(double), cudaMemcpyDeviceToHost, r->stream);
   if (e == cudaSuccess) e = cudaMemcpyAsync(out_n_over, rs->d_nover, plane * sizeof(uint32_t), cudaMemcpyDeviceToHost, r->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(r->stream);

@@ -32,7 +32,7 @@ def seg_sample(L):
 
 
 def seg_list_cap(n, S, k):
-    """select.cu seg_list_cap: twice the keys the pivots are expected to leave between them, in [256, min(n, 64 Ki)]"""
+    """the list capacity of select.cu seg_sample: twice the keys the pivots are expected to leave between them, in [256, min(n, 64 Ki)]"""
     pr = k / n
     r0 = pr * S
     d = 5.0 * math.sqrt(S * pr * (1.0 - pr)) + 2.0
