@@ -41,6 +41,7 @@ struct gpud_ring {
   double alpha = 0;
   int q_num = 99, q_den = 100;
   int64_t total = 0;
+  int64_t gen = 0;                 // pushes and restores so far: a box query started before one of them is refused (select.cu)
   double* d_ring = nullptr;
   double* d_thr = nullptr;
   double* d_pw = nullptr;

@@ -1255,6 +1255,7 @@ static int32_t launch_append(gpud_ring* r, const void* d_rows, int64_t n, int32_
   }
   GPUD_CUDA(r->ctx, cudaGetLastError());
   r->total += n;
+  ++r->gen;
   r->reduced_nw = -1;
   return GPUD_OK;
 }
@@ -1284,6 +1285,7 @@ extern "C" int32_t gpud_ring_push_raw(gpud_ring* r, const void* host_rows_v, int
   if (n > r->cap) {                      // rows that would be overwritten immediately never cross PCIe
     host_rows += (size_t)(n - r->cap) * r->F * esz;
     r->total += n - r->cap;
+    ++r->gen;
     n = r->cap;
   }
   // the staging pair is sized in bytes for stage_rows rows of doubles: narrower samples move more rows per piece

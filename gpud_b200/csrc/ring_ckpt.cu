@@ -725,6 +725,7 @@ extern "C" int32_t gpud_ring_restore(gpud_ring* r, const void* in_v, int64_t n_b
   }
   // ---- handles ----
   r->total = total;
+  ++r->gen;
   for (const CkHandle& h : recs) {
     gpud_ring_windows* s = nullptr;
     int32_t rc = gpud_ring_windows_new(r, h.span, h.hop, h.H, &s);
@@ -901,6 +902,7 @@ extern "C" int32_t gpud_ring_restore_delta(gpud_ring* r, const void* in_v, int64
   }
   // ---- state and handles ----
   r->total = total;
+  ++r->gen;
   for (size_t i = 0; i < recs.size(); ++i) {
     const CkHandle& h = recs[i];
     gpud_ring_windows* s = hs[i];

@@ -1,10 +1,13 @@
 """Host-side multi-GPU plumbing (one process per GPU, torch.distributed for rendezvous / collectives).
 
-Only two things on this path cross GPUs (SURVEY.md §8e):
+Only three things on this path cross GPUs (SURVEY.md §8e):
   * the whole-box NVLink/fabric view: one 128-byte record per GPU, all-gathered (NCCL over NVLink) and evaluated
     redundantly on every rank  — replaces the single-process loops of nvlink/component.go:164-311 and
     fabric-manager/fabric_state.go:67-113;
-  * an optional split of one large kmsg buffer across ranks at unit boundaries, hits concatenated in unit order.
+  * an optional split of one large kmsg buffer across ranks at unit boundaries, hits concatenated in unit order;
+  * box range sets (box_range_sets): a fixed header per rank, the results of the sets one rank's ring holds, and for a set spread over
+    several ranks only small objects: the samples of a short one, or for a long one its pivot sample, the per-rank class counts and
+    EMA partials, the keys between the pivots and, for the rare segment the pivots miss, digit histograms and the last candidates.
 Ring data is never exchanged: every GPU reduces its own counter stream.
 """
 from __future__ import annotations
@@ -66,3 +69,40 @@ def gather_fabric(ctx, raw, at_least: int = 0, group=None, device=None):
         v = ctx.fabric_verdict(table.data_ptr(), world, at_least, dev=dev.index, stream=side.cuda_stream)
     cur.wait_stream(side)
     return v
+
+
+class _DevBytes:
+    """a zero-copy uint8 view of library-owned device memory for torch.as_tensor"""
+
+    def __init__(self, ptr: int, n: int):
+        self.__cuda_array_interface__ = {"shape": (n,), "typestr": "|u1", "data": (ptr, False), "version": 3}
+
+
+def box_range_sets(ring, rank_of, first, length, set_off, group=None) -> dict:
+    """Range sets over the rings of every rank of the group, this process holding ring `rank` (gpud_box_query, DESIGN.md §2 "Box sets
+    across processes"): every rank calls this with the same arguments and gets the same {op: [F][n_sets]} result, identical to
+    capi.rings_reduce_range_sets over all the rings in one process.  NCCL all-gathers device buffers; any other backend (gloo) stages
+    through host memory."""
+    import torch
+    import torch.distributed as dist
+    from .capi import BoxQuery
+    rank, world = dist.get_rank(group), dist.get_world_size(group)
+    dev = torch.device("cuda", ring.dev)
+    nccl = dist.get_backend(group) == "nccl"
+    q = BoxQuery(ring, rank, world, rank_of, first, length, set_off)
+    try:
+        send_ptr, nb = q.step()
+        while nb:
+            send = torch.as_tensor(_DevBytes(send_ptr, nb), device=dev)
+            if nccl:
+                recv = torch.empty(world * nb, dtype=torch.uint8, device=dev)
+                dist.all_gather_into_tensor(recv, send, group=group)
+            else:
+                host = torch.empty(world * nb, dtype=torch.uint8)
+                dist.all_gather_into_tensor(host, send.cpu(), group=group)
+                recv = host.to(dev)
+            torch.cuda.synchronize(dev)          # the library reads recv on the ring's own stream
+            send_ptr, nb = q.step(recv.data_ptr())
+        return q.result()
+    finally:
+        q.close()

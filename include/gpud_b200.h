@@ -327,6 +327,36 @@ int32_t gpud_ring_reduce_range_sets(gpud_ring* ring, const int64_t* first, const
 int32_t gpud_rings_reduce_range_sets(gpud_ring* const* rings, int32_t n_rings, const int32_t* ring_of, const int64_t* first,
                                      const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets,
                                      double* out_f64 /*[5][F][n_sets]*/, uint32_t* out_n_over /*[F][n_sets]*/);
+/* Box sets across processes (DESIGN.md §2 "Box sets across processes"): the range sets of gpud_rings_reduce_range_sets when each ring
+ * belongs to its own process, rank r of a group of n_ranks owning ring r.  Every rank creates the query with the same arguments
+ * (rank_of[i]: the rank whose ring holds range i; first / len in that ring's own push order; set_off) and passes only its own ring.
+ * The caller drives it with its own all-gather (NCCL, gloo, any transport); the library never calls a collective:
+ *   step(dev_recv = NULL) -> (*dev_send, *send_bytes); all-gather every rank's send into [n_ranks][send_bytes] in rank order, on this
+ *   ring's device and complete; step(that buffer) -> the next round, until *send_bytes == 0.  send_bytes is the same on every rank at
+ *   every step, and *dev_send is complete when step returns (the ring's stream synchronised).
+ * Every rank ends with the whole result, identical on all ranks: gpud_box_query_result gives [5][F][n_sets] f64 and [F][n_sets] u32,
+ * what gpud_rings_reduce_range_sets gives over the same rings in one process: min / max / p99 / n_over bit for bit, every radix-select
+ * reason and pivot equal, and mean / EMA bit for bit too except for sets of more than 1024 samples spread over several ranks (within
+ * oracle/SPEC.md's tolerance there).  Only small objects are exchanged: results of sets one rank holds, samples of short spread sets,
+ * and for long ones pivot samples, per-rank counts and EMA partials, key lists and digit histograms (DESIGN.md §2).
+ * Refusals are collective: the verdict comes from the gathered headers, so every rank returns the same code and message from the same
+ * step.  GPUD_E_INVALID: what gpud_rings_reduce_range_sets refuses on its ranges and sets (each range against its own rank's ring),
+ * rank_of[i] outside [0, n_ranks), n_ranks outside [1, 32768], a rank duplicated, missing or out of order in the gather, arguments that
+ * differ between ranks, a config that differs from rank 0's (naming the field); on every rank at the next step, the code of a rank
+ * whose ring was pushed into or restored after create (GPUD_E_STATE) or whose round failed.  create itself refuses only NULL pointers,
+ * negative counts, n_sets < 1 and n_ranks outside [1, 32768].  The query owns its scratch: nothing the rings report
+ * (gpud_ring_reduce results, gpud_ring_ranges_stats, handles) changes.  The ring must outlive the query. */
+typedef struct gpud_box_query gpud_box_query;
+int32_t gpud_box_query_create(gpud_ring* ring, int32_t rank, int32_t n_ranks, const int32_t* rank_of, const int64_t* first,
+                              const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets, gpud_box_query** out);
+int32_t gpud_box_query_step(gpud_box_query* q, const void* dev_recv, const void** dev_send, int64_t* send_bytes);
+int32_t gpud_box_query_result(gpud_box_query* q, double* out_f64 /*[5][F][n_sets]*/, uint32_t* out_n_over /*[F][n_sets]*/);
+/* After the last step: this rank's device ms (each step's own work, summed; not the caller's gathers), the exchanges it took part in
+ * and the bytes it sent, and the segments that went to the radix select, by reason (reasons[GPUD_RANGE_OPEN_*], may be NULL): those of
+ * the spread sets, the same on every rank, plus those of the local sets this rank reduced.  GPUD_E_STATE before the end. */
+int32_t gpud_box_query_stats(gpud_box_query* q, float* device_ms, int32_t* rounds, int64_t* bytes_sent, int64_t* segments_by_radix,
+                             int32_t* reasons);
+void gpud_box_query_destroy(gpud_box_query* q);
 /* The last gpud_ring_reduce_ranges, gpud_ring_reduce_range_sets, or gpud_rings_reduce_range_sets homed on this ring (rings[0]; the
  * other rings of that call are not touched): device time from its first launch to its last kernel, how many
  * (field, range or set) segments went to the radix select, and why (reasons[GPUD_RANGE_OPEN_*], may be NULL).  GPUD_E_STATE before

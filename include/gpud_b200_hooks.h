@@ -117,6 +117,21 @@ int32_t gpudh_rings_range_sets_plan(const int64_t* totals, int32_t n_rings, int6
                                     int64_t n_sets, int32_t* route, int64_t* pieces, int64_t* tiles, int64_t tiles_cap, int64_t* n_tiles,
                                     int32_t* piv_n, int64_t* piv_cols, int32_t* piv_rings);
 
+/* The plan of one gpud_box_query over n_ranks rings of one config (alpha 0.5, zero thresholds) with totals[r] pushed samples: the
+ * consistent gathered headers [n_ranks][16] int64 into hdr_out (may be NULL) - words 0 magic, 1 rank, 2 n_ranks, 3 F, 4 W, 5 capacity,
+ * 6 alpha bits, 7 q_num, 8 q_den, 9 threshold hash, 10 total, 11 argument hash, 12 status, 13 status detail - and the verdict every
+ * rank reaches from hdr_in (NULL: those headers) as the return code with its message in msg.  When it is 0: each set's route (0: in one
+ * rank's ring, owner[s] that rank; 1: spread over several ranks, at most 1024 samples; 2: spread and longer, owner -1), send_bytes[3]
+ * of the header, samples(0) and summaries(0) rounds (0: no long spread set), equal on every rank, and per long spread set s its pivot
+ * reads piv_n[s] and the rank that reads each, piv_owner[s x 8192 + j].  Any output may be NULL. */
+int32_t gpudh_box_query_plan(int32_t n_ranks, const int64_t* totals, int64_t cap, int32_t n_fields, int32_t q_num, int32_t q_den,
+                             const int32_t* rank_of, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off,
+                             int64_t n_sets, int64_t* hdr_out, const int64_t* hdr_in, int32_t* route, int32_t* owner, int64_t* send_bytes,
+                             int32_t* piv_n, int32_t* piv_owner, char* msg, int32_t msg_cap);
+/* The pivots {lo, hi} of the last batch of long spread sets a finished box query reduced, [F][n_long] in the order of the sets: *n
+ * = F x n_long.  GPUD_E_STATE when it reduced none, GPUD_E_CAPACITY when *n > cap. */
+int32_t gpudh_box_query_pivots(gpud_box_query* q, double* piv, int64_t cap, int64_t* n);
+
 #ifdef __cplusplus
 }
 #endif
