@@ -761,7 +761,8 @@ SYMBOLS = ["gpud_abi_version", "gpud_sizeof", "gpud_ctx_create", "gpud_ctx_destr
            "gpud_fabric_issues", "gpud_fabric_suggest_reboot", "gpud_set_nvml_error_string", "gpud_nvml_error_strings_from_driver", "gpud_fabric_reason", "gpud_fabric_report_reason", "gpud_fabric_pack", "gpud_fabric_verdict_device", "gpud_comm_unique_id", "gpud_comm_init", "gpud_fabric_gather",
            "gpud_fabric_gather_p2p", "gpud_fm_log_syncer_create", "gpud_fm_log_syncer_destroy", "gpud_fm_log_syncer_feed",
            "gpud_fm_nothing_to_do_from_store", "gpud_ring_checkpoint_bound", "gpud_ring_checkpoint", "gpud_ring_restore",
-           "gpud_ring_checkpoint_stats", "gpud_ring_checkpoint_delta_bound", "gpud_ring_checkpoint_delta", "gpud_ring_restore_delta"]
+           "gpud_ring_checkpoint_stats", "gpud_ring_checkpoint_delta_bound", "gpud_ring_checkpoint_delta", "gpud_ring_restore_delta",
+           "gpud_ring_tier_open", "gpud_ring_tier_counts", "gpud_ring_tier_stats"]
 
 _lib = None
 
@@ -842,6 +843,12 @@ def lib() -> C.CDLL:
         "gpud_ring_checkpoint_delta_bound": (i32, [vp, C.POINTER(i64)]),
         "gpud_ring_checkpoint_delta": (i32, [vp, vp, i64, C.POINTER(i64)]), "gpud_ring_restore_delta": (i32, [vp, vp, i64]),
         "gpudh_ring_windows_sub": (i32, [i32, i64]), "gpudh_ring_ckpt_grid": (i32, [vp, i32]),
+        "gpud_ring_tier_open": (i32, [vp, i64]),
+        "gpud_ring_tier_counts": (i32, [vp, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64), C.POINTER(i64)]),
+        "gpud_ring_tier_stats": (i32, [vp, C.POINTER(C.c_float), C.POINTER(C.c_float), vp]),
+        "gpudh_ring_tier_plan": (i32, [i64, i32, i64, i64, vp, i64, vp, i64, vp, vp]),
+        "gpudh_ring_tier_split": (i32, [i64, i64, i32, i64, i64, vp, vp, i64, vp, i64, vp, vp, vp, i64, C.POINTER(i64), C.POINTER(i64)]),
+        "gpudh_ring_tier_row": (i32, [vp, i64, vp, i64, C.POINTER(i64)]), "gpudh_ring_tier_group": (i32, [vp, i32]),
         "gpud_kmsg_scan": (i32, [vp, i32, vp, i64, i32, C.POINTER(XidHit), i64, C.POINTER(i64), C.POINTER(i64)]),
         "gpud_kmsg_scan_sharded": (i32, [vp, vp, i64, i32, C.POINTER(XidHit), i64, C.POINTER(i64), C.POINTER(i64)]),
         "gpud_kmsg_scan_device": (i32, [vp, i32, vp, i64, i32, C.POINTER(XidHit), i64, C.POINTER(i64), C.POINTER(i64), vp]),
@@ -1402,6 +1409,38 @@ class Ring:
         blocks = (C.c_int64 * 2)()
         self.ctx._check(self._L.gpud_ring_checkpoint_stats(self._h, C.byref(enc), C.byref(dec), blocks))
         return float(enc.value), float(dec.value), {"raw": int(blocks[0]), "int": int(blocks[1])}
+
+    # ---- the tier: older samples kept delta-coded on the device, reached by reduce_ranges / reduce_range_sets ----
+    def tier_open(self, tier_bytes: int):
+        """gpud_ring_tier_open: keep block rows of 1024 samples, coded as checkpoint blocks, in tier_bytes of device memory"""
+        self.ctx._check(self._L.gpud_ring_tier_open(self._h, tier_bytes))
+
+    def tier_counts(self):
+        """-> (first_sample, next_sample, bytes_used, rows_lost_total): the tier holds samples [first_sample, next_sample)"""
+        v = [C.c_int64() for _ in range(4)]
+        self.ctx._check(self._L.gpud_ring_tier_counts(self._h, *[C.byref(x) for x in v]))
+        return tuple(x.value for x in v)
+
+    def tier_stats(self):
+        """-> (device ms of the last encode, device ms of the last range call's decode, {"raw": blocks, "int": blocks} of that encode)"""
+        enc, dec = C.c_float(), C.c_float()
+        blocks = (C.c_int64 * 2)()
+        self.ctx._check(self._L.gpud_ring_tier_stats(self._h, C.byref(enc), C.byref(dec), blocks))
+        return float(enc.value), float(dec.value), {"raw": int(blocks[0]), "int": int(blocks[1])}
+
+    def tier_row(self, row: int) -> bytes:
+        """test hook gpudh_ring_tier_row: block row `row` as it lies in the tier (record, then the blocks)"""
+        n = C.c_int64()
+        rc = self._L.gpudh_ring_tier_row(self._h, row, None, 0, C.byref(n))
+        if rc not in (0, -4):
+            self.ctx._check(rc)
+        buf = np.empty(n.value, dtype=np.uint8)
+        self.ctx._check(self._L.gpudh_ring_tier_row(self._h, row, C.c_void_p(buf.ctypes.data), n.value, C.byref(n)))
+        return buf.tobytes()
+
+    def tier_group(self, max_fields: int):
+        """test hook gpudh_ring_tier_group: at most max_fields fields per decoded group (0: the default)"""
+        self.ctx._check(self._L.gpudh_ring_tier_group(self._h, max_fields))
 
 
 def checkpoint_handles(blob) -> List[tuple]:

@@ -17,6 +17,7 @@ struct gpud_comm_state;   // fabric.cu
 struct gpud_range_state;  // select.cu
 struct gpud_ranges_state; // select.cu
 struct gpud_ring_windows; // below
+struct gpud_tier;         // below
 
 struct gpud_ctx {
   std::vector<int> devs;
@@ -79,7 +80,70 @@ struct gpud_ring {
   bool ck_marked = false;
   int64_t ck_total = 0, ck_gen = 0;                    // ... total and handle_gen at the marker
   uint64_t ck_link = 0;                                // ... and that blob's chain link
+  gpud_tier* tier = nullptr;                           // gpud_ring_tier_open: the delta-coded tier of older samples (ring_ckpt.cu)
 };
+
+// The tier of a ring (ring_ckpt.cu, DESIGN.md §2 "Tier"): block rows k = samples [1024 k, 1024 (k + 1)) of every field, each coded as
+// the checkpoint codes a block, kept in a byte ring of whole rows.  Placement and eviction run on the device (only it knows the coded
+// sizes): the control word below, the slot table {byte offset, bytes} of row k at slot k % slots and the row records live there.  The
+// host knows which rows were encoded (next) and lost; a query reads the control word to learn the rows still held.
+#define GPUD_TIER_ROW 1024
+struct gpud_tier_ctl { int64_t first, next, head, tail, used, n_int, n_units, pad; };   // rows [first, next); bytes [head, tail) wrap
+struct gpud_tier {
+  int64_t bytes = 0;               // B: the byte ring (8-byte multiple)
+  int64_t rec_bytes = 0;           // a row record: first sample, byte offset, directory bytes [F] (padded), block word offsets u32 [F] (padded)
+  int64_t slots = 0;               // rows the byte ring can hold at most (+ 1)
+  int64_t next = 0, lost = 0;      // host: rows [.., next) have been encoded; rows lost since open
+  unsigned long long* d_buf = nullptr;   // the byte ring [B], then a sink of one row coded at 64 bits for rows evicted by their own push
+  int64_t* d_slot = nullptr;             // [slots][2]
+  gpud_tier_ctl* d_ctl = nullptr;
+  uint8_t* d_dir = nullptr;              // encode scratch for the rows one push completes, [F][rows]
+  unsigned long long *d_words = nullptr, *d_offs = nullptr, *d_csum = nullptr;
+  int64_t* d_rowsz = nullptr;
+  int64_t units_cap = 0;
+  cudaEvent_t ev_enc[2] = {nullptr, nullptr}, ev_dec[2] = {nullptr, nullptr};
+  bool enc_timed = false;
+  float dec_ms = 0.f;              // the last query's decode, all its field groups
+  int group_max = 0;               // > 0: at most this many fields per decoded group (gpudh_ring_tier_group)
+  // query scratch, grown on demand: the virtual ring, its sample ring, the rows to decode and their directory
+  double* d_vring = nullptr;  size_t vring_cap = 0;
+  double* d_vsmp = nullptr;  size_t vsmp_cap = 0;
+  int64_t* d_rows = nullptr;  size_t rows_cap = 0;
+  uint8_t* d_vdir = nullptr;  size_t vdir_cap = 0;
+  unsigned long long* d_voffs = nullptr;  size_t voffs_cap = 0;
+};
+// ring_ckpt.cu: after every push into a tiered ring, on its stream: the loss rule, then the encode of every row the push completed.
+int32_t gpud_tier_push(gpud_ring* r);
+void gpud_tier_free(gpud_tier* t);
+// ring_ckpt.cu: synchronise the ring's stream and read the rows the tier holds, [*first, *next).
+int32_t gpud_tier_span(gpud_ring* r, int64_t* first, int64_t* next);
+// ring_ckpt.cu: fields [f0, f0 + G) of rows[0, n_rows) (each held by the tier, ascending) into virtual rows 0 .. n_rows - 1 of a ring
+// of G fields and capacity vcap, then the first tail_n samples of row rows_tail (not yet coded) from the ring itself into virtual row
+// n_rows; the sample ring by k_ring_append's rule.  The virtual ring and its sample ring are the tier's scratch (*vring, *vsmp).
+int32_t gpud_tier_decode(gpud_ring* r, const std::vector<int64_t>& rows, int64_t rows_tail, int64_t tail_n, int f0, int G, int64_t vcap,
+                         int smp_shift, int64_t smp_slots, double** vring, double** vsmp);
+// The placement of one row of s bytes (host plan and device encode): the oldest rows go until [off, off + s) overlaps none held.
+__host__ __device__ inline int64_t gpud_tier_place(gpud_tier_ctl& c, int64_t* slot, int64_t R, int64_t B, int64_t s) {
+  for (;;) {
+    const bool empty = c.first == c.next;
+    const int64_t off = c.tail + s <= B ? c.tail : 0;
+    // held bytes: [head, tail) unwrapped, or [head, end of the last row before the wrap) and [0, tail)
+    const bool clash = empty ? false : c.head < c.tail ? (off == 0 && c.head < s) : (off == 0 || off + s > c.head);
+    if (!clash) {
+      const int64_t k = c.next % R;
+      slot[2 * k] = off;
+      slot[2 * k + 1] = s;
+      if (empty) c.head = off;
+      ++c.next;
+      c.tail = off + s;
+      c.used += s;
+      return off;
+    }
+    c.used -= slot[2 * (c.first % R) + 1];
+    ++c.first;
+    if (c.first < c.next) c.head = slot[2 * (c.first % R)];
+  }
+}
 
 // Stream windows of a ring (ring.cu, DESIGN.md §2): the aggregates of windows [first, next) of the sample stream, window k =
 // samples [kP, kP + L) with L = span * W and P = hop * W (hop = span: tumbling windows), in history slot k % H.

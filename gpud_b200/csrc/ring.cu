@@ -1194,6 +1194,7 @@ extern "C" int32_t gpud_ring_destroy(gpud_ring* r) {
   for (auto& p : r->d_res) cudaFree(p);
   gpud_range_state_free(r->range);
   gpud_ranges_state_free(r->ranges);
+  gpud_tier_free(r->tier);
   windows_free(r->swin);
   for (gpud_ring_windows* w : r->handles) windows_free(w);
   for (int i = 0; i < 2; ++i) {
@@ -1264,7 +1265,8 @@ extern "C" int32_t gpud_ring_push_device(gpud_ring* r, const double* dev_rows, i
   if (!r || (!dev_rows && n) || n < 0) return GPUD_E_INVALID;
   if (n == 0) return GPUD_OK;
   GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
-  return launch_append(r, dev_rows, n, GPUD_DT_F64);
+  const int32_t rc = launch_append(r, dev_rows, n, GPUD_DT_F64);
+  return rc || !r->tier ? rc : gpud_tier_push(r);
 }
 
 extern "C" int32_t gpud_ring_push_raw(gpud_ring* r, const void* host_rows_v, int64_t n, int32_t dt) {
@@ -1314,6 +1316,7 @@ extern "C" int32_t gpud_ring_push_raw(gpud_ring* r, const void* host_rows_v, int
     done += rows;
     buf ^= 1;
   }
+  if (r->tier) { const int32_t rc = gpud_tier_push(r); if (rc) return rc; }
   if (pinned) GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));   // caller may reuse its buffer on return
   return GPUD_OK;
 }

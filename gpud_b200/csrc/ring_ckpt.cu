@@ -656,6 +656,7 @@ extern "C" int32_t gpud_ring_restore(gpud_ring* r, const void* in_v, int64_t n_b
   // ---- the target ----
   if (r->total != 0) return gpud_fail(ctx, GPUD_E_STATE, "restore: the ring has been pushed into");
   if (r->swin || !r->handles.empty()) return gpud_fail(ctx, GPUD_E_STATE, "restore: the ring has a stream or windows handle open");
+  if (r->tier) return gpud_fail(ctx, GPUD_E_STATE, "restore: the ring has a tier (a restored ring has none)");
   // ---- sections ----
   const int64_t total = get<int64_t>(in, 48), count = get<int64_t>(in, 56), dir_bytes = get<int64_t>(in, 72), pay_bytes = get<int64_t>(in, 80),
                 sum_bytes = get<int64_t>(in, 88), hnd_bytes = get<int64_t>(in, 96);
@@ -918,7 +919,7 @@ extern "C" int32_t gpud_ring_restore_delta(gpud_ring* r, const void* in_v, int64
   std::vector<uint64_t> sums(F);
   memcpy(sums.data(), in + sum_off, 8 * F);
   set_marker(r, total, chain_link(prev_link, total, sums.data(), F, heads));
-  return GPUD_OK;
+  return r->tier ? gpud_tier_push(r) : GPUD_OK;   // the delta's samples reach the tier as a push's would
 }
 
 extern "C" int32_t gpudh_ring_ckpt_grid(gpud_ring* r, int32_t max_ctas) {
@@ -933,5 +934,345 @@ extern "C" int32_t gpud_ring_checkpoint_stats(gpud_ring* r, float* encode_ms, fl
   if (encode_ms) *encode_ms = r->ck_encode_ms;
   if (decode_ms) *decode_ms = r->ck_decode_ms;
   if (blocks_by_mode) std::copy(r->ck_blocks, r->ck_blocks + 2, blocks_by_mode);
+  return GPUD_OK;
+}
+
+// ---- the tier (DESIGN.md §2 "Tier") ------------------------------------------------------------------------------------------------
+// Block row k is samples [1024 k, 1024 (k + 1)) of every field; field f's block is coded exactly as a checkpoint block (k_ckpt_size
+// decides its mode and width, k_ckpt_pack writes it).  A row is its record - first sample, byte offset, the F directory bytes and the
+// F block word offsets from the end of the record - then the blocks in field order.  k_tier_place lays the rows one push completed
+// into the byte ring (gpud_tier_place), writes their records and each block's word offset for k_ckpt_pack.  A decode gathers the
+// directory and offsets of the rows it wants from their records (k_tier_gather) and runs k_ckpt_unpack<true> into a virtual ring.
+namespace {
+
+constexpr int kPlaceThreads = 256;
+constexpr int64_t kTierRecHead = 16;               // first sample, byte offset
+__host__ __device__ __forceinline__ int64_t tier_pad8(int64_t x) { return (x + 7) & ~(int64_t)7; }
+
+int64_t tier_rec_bytes(int64_t F) { return kTierRecHead + tier_pad8(F) + tier_pad8(4 * F); }
+
+// One CTA.  Row sizes, then thread 0 places every row in push order (a row may evict rows of the same push), then the records of the
+// rows that are still held and each block's word offset: the byte ring, or the sink past it for a row this push placed and evicted,
+// so that k_ckpt_pack never writes over a row that is kept.
+__global__ void __launch_bounds__(kPlaceThreads) k_tier_place(const uint8_t* __restrict__ dir, const unsigned long long* __restrict__ words,
+                                                              int64_t nb, int F, int64_t row0, int clear, int64_t B, int64_t R, int64_t rec_bytes,
+                                                              unsigned long long* __restrict__ buf, int64_t* __restrict__ slot, gpud_tier_ctl* __restrict__ ctl,
+                                                              int64_t* __restrict__ rowsz, unsigned long long* __restrict__ offs) {
+  __shared__ unsigned long long s_part[kPlaceThreads];
+  __shared__ int64_t s_first;
+  const int tid = threadIdx.x;
+  for (int64_t j = 0; j < nb; ++j) {               // row j's payload words
+    unsigned long long w = 0;
+    for (int f = tid; f < F; f += kPlaceThreads) w += words[(int64_t)f * nb + j];
+    s_part[tid] = w;
+    __syncthreads();
+    for (int o = kPlaceThreads / 2; o > 0; o >>= 1) {
+      if (tid < o) s_part[tid] += s_part[tid + o];
+      __syncthreads();
+    }
+    if (tid == 0) rowsz[j] = rec_bytes + 8 * (int64_t)s_part[0];
+    __syncthreads();
+  }
+  if (tid == 0) {
+    gpud_tier_ctl c = *ctl;
+    if (clear) c = gpud_tier_ctl{row0, row0, 0, 0, 0, c.n_int, c.n_units, 0};
+    for (int64_t j = 0; j < nb; ++j) gpud_tier_place(c, slot, R, B, rowsz[j]);
+    if (nb > 0) {
+      int64_t n_int = 0;
+      for (int64_t u = 0; u < (int64_t)F * nb; ++u) n_int += dir[u] >> 7;
+      c.n_int = n_int;
+      c.n_units = (int64_t)F * nb;
+    }
+    *ctl = c;
+    s_first = c.first;
+  }
+  __syncthreads();
+  const int64_t dir_off = kTierRecHead, woff_off = kTierRecHead + tier_pad8(F);
+  for (int64_t j = 0; j < nb; ++j) {
+    const int64_t row = row0 + j;
+    const bool kept = row >= s_first;
+    const int64_t off = kept ? slot[2 * (row % R)] : B;   // the sink: past the byte ring
+    uint8_t* rec = reinterpret_cast<uint8_t*>(buf) + off;
+    // exclusive prefix of the blocks' words over the fields, 256 fields at a time
+    unsigned long long base = 0;
+    for (int f0 = 0; f0 < F; f0 += kPlaceThreads) {
+      const int f = f0 + tid;
+      const unsigned long long w = f < F ? words[(int64_t)f * nb + j] : 0ull;
+      s_part[tid] = w;
+      __syncthreads();
+      for (int o = 1; o < kPlaceThreads; o <<= 1) {    // Hillis-Steele inclusive scan
+        const unsigned long long y = tid >= o ? s_part[tid - o] : 0ull;
+        __syncthreads();
+        s_part[tid] += y;
+        __syncthreads();
+      }
+      if (f < F) {
+        const unsigned long long wo = base + s_part[tid] - w;
+        offs[(int64_t)f * nb + j] = (unsigned long long)((off + rec_bytes) / 8) + wo;
+        if (kept) {
+          rec[dir_off + f] = dir[(int64_t)f * nb + j];
+          reinterpret_cast<uint32_t*>(rec + woff_off)[f] = (uint32_t)wo;
+        }
+      }
+      base += s_part[kPlaceThreads - 1];
+      __syncthreads();
+    }
+    if (kept) {
+      if (tid == 0) {
+        reinterpret_cast<int64_t*>(rec)[0] = row * GPUD_TIER_ROW;
+        reinterpret_cast<int64_t*>(rec)[1] = off;
+      }
+      for (int64_t i = F + tid; i < tier_pad8(F); i += kPlaceThreads) rec[dir_off + i] = 0;
+      if ((F & 1) && tid == 0) reinterpret_cast<uint32_t*>(rec + woff_off)[F] = 0;
+    }
+    __syncthreads();
+  }
+}
+
+// Decode inputs of fields [f0, f0 + G) of rows[0, n): unit u = f n + j (k_ckpt_unpack's numbering) from row rows[j]'s record.
+__global__ void __launch_bounds__(256) k_tier_gather(const int64_t* __restrict__ rows, int64_t n, int f0, int G, int F, const unsigned long long* __restrict__ buf,
+                                                     const int64_t* __restrict__ slot, int64_t R, int64_t rec_bytes, uint8_t* __restrict__ dir,
+                                                     unsigned long long* __restrict__ offs) {
+  const int64_t units = (int64_t)G * n;
+  for (int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; u < units; u += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t f = u / n, j = u - f * n;
+    const int64_t off = slot[2 * (rows[j] % R)];
+    const uint8_t* rec = reinterpret_cast<const uint8_t*>(buf) + off;
+    dir[u] = rec[kTierRecHead + f0 + f];
+    offs[u] = (unsigned long long)((off + rec_bytes) / 8) + reinterpret_cast<const uint32_t*>(rec + kTierRecHead + tier_pad8(F))[f0 + f];
+  }
+}
+
+// The tail of the virtual ring: samples [first, first + n) of fields [f0, f0 + G) from the ring to virtual columns vcol0.., with the
+// sample ring kept as k_ring_append keeps it.
+__global__ void __launch_bounds__(256) k_tier_tail(const double* __restrict__ ring, int64_t cap, int64_t first, int64_t n, int f0, int G, double* __restrict__ vring,
+                                                   int64_t vcap, int64_t vcol0, double* __restrict__ vsmp, int smp_shift, int64_t smp_half, int64_t smp_slots) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < (int64_t)G * n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t f = i / n, t = i - f * n, c = vcol0 + t;
+    const double x = ring[(f0 + f) * cap + (first + t) % cap];
+    vring[f * vcap + c] = x;
+    if ((c & ((1ll << smp_shift) - 1)) == smp_half) vsmp[f * smp_slots + (c >> smp_shift)] = x;
+  }
+}
+
+}  // namespace
+
+void gpud_tier_free(gpud_tier* t) {
+  if (!t) return;
+  cudaFree(t->d_buf); cudaFree(t->d_slot); cudaFree(t->d_ctl); cudaFree(t->d_dir); cudaFree(t->d_words); cudaFree(t->d_offs); cudaFree(t->d_csum);
+  cudaFree(t->d_rowsz); cudaFree(t->d_vring); cudaFree(t->d_vsmp); cudaFree(t->d_rows); cudaFree(t->d_vdir); cudaFree(t->d_voffs);
+  for (auto& e : t->ev_enc) if (e) cudaEventDestroy(e);
+  for (auto& e : t->ev_dec) if (e) cudaEventDestroy(e);
+  delete t;
+}
+
+// The rows the tier can hold at most: every row at least its record and F anchors.
+static int64_t tier_slots(int64_t B, int64_t F) { return B / (tier_rec_bytes(F) + 8 * F) + 1; }
+
+// The encode of rows [row0, row0 + nb) (wholly in the ring), asynchronous on the ring's stream; clear: the tier restarts at row0.
+static int32_t tier_encode(gpud_ring* r, gpud_tier* t, int64_t row0, int64_t nb, bool clear) {
+  CkGeo g = ckpt_geo(r, row0 * kBlock, nb * kBlock);
+  const int64_t units = (int64_t)r->F * nb;
+  if (nb > 0) {
+    GPUD_CUDA(r->ctx, cudaEventRecord(t->ev_enc[0], r->stream));
+    k_ckpt_size<<<ckpt_grid(r, units, kCkThreads / 32), kCkThreads, 0, r->stream>>>(g, t->d_dir, t->d_words, t->d_csum);
+    GPUD_CUDA(r->ctx, cudaGetLastError());
+  }
+  k_tier_place<<<1, kPlaceThreads, 0, r->stream>>>(t->d_dir, t->d_words, nb, r->F, row0, clear ? 1 : 0, t->bytes, t->slots, t->rec_bytes, t->d_buf,
+                                                   t->d_slot, t->d_ctl, t->d_rowsz, t->d_offs);
+  GPUD_CUDA(r->ctx, cudaGetLastError());
+  if (nb > 0) {
+    k_ckpt_pack<<<ckpt_grid(r, units, kPackWarps), kPackWarps * 32, 0, r->stream>>>(g, t->d_dir, t->d_offs, t->d_buf);
+    GPUD_CUDA(r->ctx, cudaGetLastError());
+    GPUD_CUDA(r->ctx, cudaEventRecord(t->ev_enc[1], r->stream));
+    t->enc_timed = true;
+  }
+  return GPUD_OK;
+}
+
+int32_t gpud_tier_push(gpud_ring* r) {
+  gpud_tier* t = r->tier;
+  // rows wholly in the ring start at `whole`; a row before it that was never encoded is lost, and the tier restarts there
+  const int64_t whole = (r->total - ring_count(r) + kBlock - 1) / kBlock, done = r->total / kBlock;
+  bool clear = false;
+  if (t->next < whole) {
+    t->lost += whole - t->next;
+    t->next = whole;
+    clear = true;
+  }
+  if (done == t->next && !clear) return GPUD_OK;
+  const int64_t row0 = t->next;
+  t->next = done;
+  return tier_encode(r, t, row0, done - row0, clear);
+}
+
+int32_t gpud_tier_span(gpud_ring* r, int64_t* first, int64_t* next) {
+  gpud_tier_ctl c;
+  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
+  GPUD_CUDA(r->ctx, cudaMemcpyAsync(&c, r->tier->d_ctl, sizeof c, cudaMemcpyDeviceToHost, r->stream));
+  GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));
+  *first = c.first;
+  *next = c.next;
+  return GPUD_OK;
+}
+
+int32_t gpud_tier_decode(gpud_ring* r, const std::vector<int64_t>& rows, int64_t rows_tail, int64_t tail_n, int f0, int G, int64_t vcap,
+                         int smp_shift, int64_t smp_slots, double** vring, double** vsmp) {
+  gpud_tier* t = r->tier;
+  const int64_t n = (int64_t)rows.size(), units = (int64_t)G * n;
+  GPUD_CUDA(r->ctx, gpud_grow(&t->d_vring, &t->vring_cap, (size_t)G * vcap));
+  GPUD_CUDA(r->ctx, gpud_grow(&t->d_vsmp, &t->vsmp_cap, (size_t)G * smp_slots));
+  GPUD_CUDA(r->ctx, gpud_grow(&t->d_rows, &t->rows_cap, std::max<size_t>(1, n)));
+  GPUD_CUDA(r->ctx, gpud_grow(&t->d_vdir, &t->vdir_cap, std::max<size_t>(1, units)));
+  GPUD_CUDA(r->ctx, gpud_grow(&t->d_voffs, &t->voffs_cap, std::max<size_t>(1, units)));
+  for (auto& e : t->ev_dec) if (!e) GPUD_CUDA(r->ctx, cudaEventCreate(&e));
+  *vring = t->d_vring;
+  *vsmp = t->d_vsmp;
+  const int64_t half = (1ll << smp_shift) >> 1;
+  GPUD_CUDA(r->ctx, cudaEventRecord(t->ev_dec[0], r->stream));
+  if (n > 0) {
+    GPUD_CUDA(r->ctx, cudaMemcpyAsync(t->d_rows, rows.data(), n * sizeof(int64_t), cudaMemcpyHostToDevice, r->stream));
+    const int grid = (int)std::min<int64_t>((units + 255) / 256, (int64_t)r->sm_count * 8);
+    k_tier_gather<<<grid, 256, 0, r->stream>>>(t->d_rows, n, f0, G, r->F, t->d_buf, t->d_slot, t->slots, t->rec_bytes, t->d_vdir, t->d_voffs);
+    GPUD_CUDA(r->ctx, cudaGetLastError());
+    CkGeo g{};
+    g.ring = t->d_vring; g.sample = t->d_vsmp;
+    g.cap = vcap; g.start = 0; g.count = n * kBlock; g.nb = n;
+    g.smp_half = half; g.smp_slots = smp_slots; g.F = G; g.smp_shift = smp_shift;
+    // the field sums k_ckpt_unpack re-forms land in the encode's scratch, which no one reads
+    k_ckpt_unpack<true><<<ckpt_grid(r, units, kCkThreads / 32), kCkThreads, 0, r->stream>>>(g, t->d_vdir, t->d_voffs, t->d_buf, t->d_csum);
+    GPUD_CUDA(r->ctx, cudaGetLastError());
+  }
+  if (tail_n > 0) {
+    const int grid = (int)std::min<int64_t>(((int64_t)G * tail_n + 255) / 256, (int64_t)r->sm_count * 8);
+    k_tier_tail<<<grid, 256, 0, r->stream>>>(r->d_ring, r->cap, rows_tail * kBlock, tail_n, f0, G, t->d_vring, vcap, n * kBlock, t->d_vsmp, smp_shift, half,
+                                             smp_slots);
+    GPUD_CUDA(r->ctx, cudaGetLastError());
+  }
+  GPUD_CUDA(r->ctx, cudaEventRecord(t->ev_dec[1], r->stream));
+  return GPUD_OK;
+}
+
+extern "C" int32_t gpud_ring_tier_open(gpud_ring* r, int64_t tier_bytes) {
+  if (!r) return GPUD_E_INVALID;
+  if (r->tier) return gpud_fail(r->ctx, GPUD_E_STATE, "tier_open: the ring already has a tier");
+  const int64_t F = r->F, B = tier_bytes & ~(int64_t)7, rec = tier_rec_bytes(F), row_max = rec + 8 * F * kBlock;
+  if (r->cap < 2 * kBlock) return gpud_fail(r->ctx, GPUD_E_INVALID, "tier_open: capacity %lld is below %d", (long long)r->cap, 2 * kBlock);
+  if (tier_bytes < row_max)
+    return gpud_fail(r->ctx, GPUD_E_INVALID, "tier_open: %lld bytes do not hold one row coded at 64 bits (%lld bytes)", (long long)tier_bytes, (long long)row_max);
+  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
+  gpud_tier* t = new gpud_tier();
+  t->bytes = B;
+  t->rec_bytes = rec;
+  t->slots = tier_slots(B, F);
+  t->units_cap = F * (r->cap / kBlock + 1);
+  cudaError_t e = cudaMalloc(&t->d_buf, (size_t)(B + row_max));
+  if (e == cudaSuccess) e = cudaMalloc(&t->d_slot, (size_t)t->slots * 2 * sizeof(int64_t));
+  if (e == cudaSuccess) e = cudaMalloc(&t->d_ctl, sizeof(gpud_tier_ctl));
+  if (e == cudaSuccess) e = cudaMalloc(&t->d_dir, (size_t)t->units_cap);
+  if (e == cudaSuccess) e = cudaMalloc(&t->d_words, (size_t)t->units_cap * 8);
+  if (e == cudaSuccess) e = cudaMalloc(&t->d_offs, (size_t)t->units_cap * 8);
+  if (e == cudaSuccess) e = cudaMalloc(&t->d_csum, (size_t)F * 8);
+  if (e == cudaSuccess) e = cudaMalloc(&t->d_rowsz, (size_t)(r->cap / kBlock + 1) * 8);
+  for (int i = 0; i < 2 && e == cudaSuccess; ++i) e = cudaEventCreate(&t->ev_enc[i]);
+  // the tier starts at the first row wholly in the ring: the rows the ring already completed are encoded now, as a push would
+  const int64_t whole = (r->total - ring_count(r) + kBlock - 1) / kBlock;
+  const gpud_tier_ctl c0{whole, whole, 0, 0, 0, 0, 0, 0};
+  if (e == cudaSuccess) e = cudaMemcpyAsync(t->d_ctl, &c0, sizeof c0, cudaMemcpyHostToDevice, r->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(r->stream);
+  if (e != cudaSuccess) {
+    gpud_tier_free(t);
+    cudaGetLastError();
+    return gpud_fail(r->ctx, e == cudaErrorMemoryAllocation ? GPUD_E_NOMEM : GPUD_E_CUDA, "tier_open: %s", cudaGetErrorString(e));
+  }
+  t->next = whole;
+  r->tier = t;
+  return gpud_tier_push(r);
+}
+
+extern "C" int32_t gpud_ring_tier_counts(gpud_ring* r, int64_t* first_sample, int64_t* next_sample, int64_t* bytes_used, int64_t* rows_lost_total) {
+  if (!r) return GPUD_E_INVALID;
+  if (!r->tier) return gpud_fail(r->ctx, GPUD_E_STATE, "tier_counts: the ring has no tier");
+  gpud_tier_ctl c;
+  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
+  GPUD_CUDA(r->ctx, cudaMemcpyAsync(&c, r->tier->d_ctl, sizeof c, cudaMemcpyDeviceToHost, r->stream));
+  GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));
+  if (first_sample) *first_sample = c.first * kBlock;
+  if (next_sample) *next_sample = c.next * kBlock;
+  if (bytes_used) *bytes_used = c.used;
+  if (rows_lost_total) *rows_lost_total = r->tier->lost;
+  return GPUD_OK;
+}
+
+extern "C" int32_t gpud_ring_tier_stats(gpud_ring* r, float* encode_ms, float* decode_ms, int64_t* blocks_by_mode) {
+  if (!r) return GPUD_E_INVALID;
+  gpud_tier* t = r->tier;
+  if (!t) return gpud_fail(r->ctx, GPUD_E_STATE, "tier_stats: the ring has no tier");
+  gpud_tier_ctl c;
+  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
+  GPUD_CUDA(r->ctx, cudaMemcpyAsync(&c, t->d_ctl, sizeof c, cudaMemcpyDeviceToHost, r->stream));
+  GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));
+  float enc = 0.f;
+  if (t->enc_timed) GPUD_CUDA(r->ctx, cudaEventElapsedTime(&enc, t->ev_enc[0], t->ev_enc[1]));
+  if (encode_ms) *encode_ms = enc;
+  if (decode_ms) *decode_ms = t->dec_ms;
+  if (blocks_by_mode) { blocks_by_mode[0] = c.n_units - c.n_int; blocks_by_mode[1] = c.n_int; }
+  return GPUD_OK;
+}
+
+// Test hooks (include/gpud_b200_hooks.h).
+extern "C" int32_t gpudh_ring_tier_row(gpud_ring* r, int64_t row, void* out, int64_t cap, int64_t* n_bytes) {
+  if (!r || !n_bytes || cap < 0 || (cap > 0 && !out)) return GPUD_E_INVALID;
+  gpud_tier* t = r->tier;
+  if (!t) return gpud_fail(r->ctx, GPUD_E_STATE, "the ring has no tier");
+  int64_t first = 0, next = 0;
+  { const int32_t rc = gpud_tier_span(r, &first, &next); if (rc) return rc; }
+  if (row < first || row >= next) return gpud_fail(r->ctx, GPUD_E_INVALID, "row %lld is not in the tier's [%lld, %lld)", (long long)row, (long long)first, (long long)next);
+  int64_t s[2];
+  GPUD_CUDA(r->ctx, cudaMemcpy(s, t->d_slot + 2 * (row % t->slots), sizeof s, cudaMemcpyDeviceToHost));
+  *n_bytes = s[1];
+  if (cap < s[1]) return GPUD_E_CAPACITY;
+  GPUD_CUDA(r->ctx, cudaMemcpy(out, reinterpret_cast<const uint8_t*>(t->d_buf) + s[0], s[1], cudaMemcpyDeviceToHost));
+  return GPUD_OK;
+}
+
+extern "C" int32_t gpudh_ring_tier_group(gpud_ring* r, int32_t max_fields) {
+  if (!r || !r->tier || max_fields < 0) return GPUD_E_INVALID;
+  r->tier->group_max = max_fields;
+  return GPUD_OK;
+}
+
+// The tier's placement over a sequence of pushes, on the host: a ring of capacity cap and F fields with total0 samples pushed when the
+// tier of tier_bytes opened, then pushes of push_n[i] samples; row k codes to row_bytes[k] bytes (record included).  After push i (and
+// after the open, at i = -1 -> state[0]): state[6 (i + 1) ..] = {first row, next row, bytes in use, rows lost, head, tail}; row_off[k]
+// the byte offset row k was placed at (-1: never).
+extern "C" int32_t gpudh_ring_tier_plan(int64_t cap, int32_t F, int64_t tier_bytes, int64_t total0, const int64_t* push_n, int64_t n_push,
+                                        const int64_t* row_bytes, int64_t n_rows, int64_t* state, int64_t* row_off) {
+  if (cap < 2 * kBlock || F < 1 || total0 < 0 || n_push < 0 || !state || !row_off || (n_push && !push_n) || (n_rows && !row_bytes)) return GPUD_E_INVALID;
+  const int64_t B = tier_bytes & ~(int64_t)7, R = tier_slots(B, F);
+  if (tier_bytes < tier_rec_bytes(F) + 8 * (int64_t)F * kBlock) return GPUD_E_INVALID;
+  std::vector<int64_t> slot(2 * R);
+  std::fill(row_off, row_off + n_rows, -1);
+  int64_t total = total0, next = 0, lost = 0;
+  gpud_tier_ctl c{};
+  for (int64_t i = -1; i < n_push; ++i) {
+    if (i >= 0) {
+      if (push_n[i] < 0) return GPUD_E_INVALID;
+      total += push_n[i];
+    }
+    const int64_t count = std::min(total, cap), whole = (total - count + kBlock - 1) / kBlock, done = total / kBlock;
+    if (i < 0 || next < whole) {
+      if (i >= 0) lost += whole - next;
+      next = whole;
+      c = gpud_tier_ctl{whole, whole, 0, 0, 0, 0, 0, 0};
+    }
+    for (; next < done; ++next) {
+      if (next >= n_rows) return GPUD_E_CAPACITY;
+      if (row_bytes[next] <= 0 || (row_bytes[next] & 7) || row_bytes[next] > B) return GPUD_E_INVALID;
+      row_off[next] = gpud_tier_place(c, slot.data(), R, B, row_bytes[next]);
+    }
+    int64_t* o = state + 6 * (i + 1);
+    o[0] = c.first; o[1] = c.next; o[2] = c.used; o[3] = lost; o[4] = c.head; o[5] = c.tail;
+  }
   return GPUD_OK;
 }

@@ -1057,12 +1057,186 @@ static int32_t reduce_sets(gpud_ring* const* rings, int n_rings, const int32_t* 
   return GPUD_OK;
 }
 
+// ---- ranges that reach into the tier (DESIGN.md §2 "Tier") -------------------------------------------------------------------
+// A tiered ring holds samples [lo, total) with lo = min(total - count, 1024 tier_first).  The sets whose ranges all lie in the ring go
+// through reduce_sets untouched.  Each other set's ranges cover block rows; those rows, merged and ascending, are decoded into a
+// virtual ring (row j at columns [1024 j, 1024 (j + 1)); the newest row, not yet coded, copied from the ring), and reduce_sets runs
+// on that buffer as on a ring of its own capacity with the ring's alpha, quantile and thresholds - in groups of fields, each as large
+// as kTierGroupBytes of decoded samples allow.
+constexpr int64_t kTierGroupBytes = (int64_t)1 << 30;
+
+struct TierSplit {
+  std::vector<int32_t> route;        // per set: 0 the ring, 1 the tier
+  std::vector<int64_t> rows;         // the block rows the tier sets read, ascending
+  std::vector<int64_t> vfirst;       // per range of a tier set: its first sample in the virtual ring (-1: a ring set's range)
+  int64_t vtotal = 0;                // samples of the virtual ring
+};
+
+static int ring_smp_shift(int64_t cap);
+
+// Validation (every refusal of ranges_plan, against samples [lo, total)) and the split.  Pure host arithmetic.
+static int32_t tier_split(gpud_ctx* ctx, int64_t total, int64_t cap, int F, int64_t t_first, int64_t t_next, const int64_t* first, const int64_t* len,
+                          int64_t n, const int64_t* set_off, int64_t n_sets, TierSplit* sp) {
+  const int64_t count = std::min(total, cap), lo = std::min(total - count, t_first * GPUD_TIER_ROW);
+  {
+    // ranges_plan's checks with a capacity that holds [lo, total): the same refusals, against the tier's reach
+    RangesPlan pl;
+    int32_t rc = ranges_plan(ctx, &total, 1, nullptr, std::max<int64_t>(1, total - lo), F, 99, 100, 0.5, 0, first, len, n, set_off, n_sets, &pl);
+    if (rc) return rc;
+  }
+  sp->route.assign(n_sets, 0);
+  sp->vfirst.assign(n, -1);
+  std::vector<std::pair<int64_t, int64_t>> iv;
+  for (int64_t s = 0; s < n_sets; ++s) {
+    const int64_t a = set_off ? set_off[s] : s, e = set_off ? set_off[s + 1] : s + 1;
+    for (int64_t i = a; i < e; ++i) sp->route[s] |= first[i] < total - count;
+    if (!sp->route[s]) continue;
+    for (int64_t i = a; i < e; ++i) iv.push_back({first[i] / GPUD_TIER_ROW, (first[i] + len[i] + GPUD_TIER_ROW - 1) / GPUD_TIER_ROW});
+  }
+  std::sort(iv.begin(), iv.end());
+  sp->rows.clear();
+  for (const auto& v : iv)
+    for (int64_t k = std::max(v.first, sp->rows.empty() ? v.first : sp->rows.back() + 1); k < v.second; ++k) sp->rows.push_back(k);
+  for (int64_t s = 0; s < n_sets; ++s) {
+    if (!sp->route[s]) continue;
+    const int64_t a = set_off ? set_off[s] : s, e = set_off ? set_off[s + 1] : s + 1;
+    for (int64_t i = a; i < e; ++i) {
+      const int64_t j = std::lower_bound(sp->rows.begin(), sp->rows.end(), first[i] / GPUD_TIER_ROW) - sp->rows.begin();
+      sp->vfirst[i] = j * GPUD_TIER_ROW + first[i] % GPUD_TIER_ROW;
+    }
+  }
+  const int64_t nr = (int64_t)sp->rows.size();
+  sp->vtotal = nr * GPUD_TIER_ROW;
+  if (nr && sp->rows.back() == t_next) sp->vtotal -= GPUD_TIER_ROW - (total - t_next * GPUD_TIER_ROW);   // the newest row is partial
+  return GPUD_OK;
+}
+
+// results [5][G][n_sub] / [G][n_sub] of sets ids[] and fields [f0, f0 + G) into the caller's [5][F][n_sets] / [F][n_sets]
+static void tier_scatter(const std::vector<double>& f64, const std::vector<uint32_t>& nov, const std::vector<int64_t>& ids, int f0, int G, int F,
+                         int64_t n_sets, double* out_f64, uint32_t* out_n_over) {
+  const int64_t m = (int64_t)ids.size();
+  for (int op = 0; op < 5; ++op)
+    for (int f = 0; f < G; ++f)
+      for (int64_t j = 0; j < m; ++j) out_f64[((int64_t)op * F + f0 + f) * n_sets + ids[j]] = f64[((int64_t)op * G + f) * m + j];
+  for (int f = 0; f < G; ++f)
+    for (int64_t j = 0; j < m; ++j) out_n_over[(int64_t)(f0 + f) * n_sets + ids[j]] = nov[(int64_t)f * m + j];
+}
+
+// The sets ids[] of the call as a call of their own: their ranges (first[i] or, with vfirst, vfirst[i]) and set offsets.
+static void tier_subcall(const std::vector<int64_t>& ids, const int64_t* first, const int64_t* len, const int64_t* set_off, const std::vector<int64_t>* vfirst,
+                         std::vector<int64_t>& sf, std::vector<int64_t>& sl, std::vector<int64_t>& so) {
+  so.assign(1, 0);
+  for (int64_t s : ids) {
+    const int64_t a = set_off ? set_off[s] : s, e = set_off ? set_off[s + 1] : s + 1;
+    for (int64_t i = a; i < e; ++i) { sf.push_back(vfirst ? (*vfirst)[i] : first[i]); sl.push_back(len[i]); }
+    so.push_back((int64_t)sf.size());
+  }
+}
+
+static int32_t reduce_sets_tier(gpud_ring* r, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets,
+                                double* out_f64, uint32_t* out_n_over) {
+  gpud_tier* t = r->tier;
+  int64_t t_first = 0, t_next = 0;
+  { int32_t rc = gpud_tier_span(r, &t_first, &t_next); if (rc) return rc; }
+  TierSplit sp;
+  { int32_t rc = tier_split(r->ctx, r->total, r->cap, r->F, t_first, t_next, first, len, n_ranges, set_off, n_sets, &sp); if (rc) return rc; }
+  if (sp.rows.empty()) return reduce_sets(&r, 1, nullptr, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over, &r->ranges);
+  std::vector<int64_t> ids[2];
+  for (int64_t s = 0; s < n_sets; ++s) ids[sp.route[s]].push_back(s);
+  const int F = r->F;
+  cudaEvent_t ev[2] = {};
+  for (auto& e : ev) GPUD_CUDA(r->ctx, cudaEventCreate(&e));
+  struct EvFree { cudaEvent_t* e; ~EvFree() { for (int i = 0; i < 2; ++i) if (e[i]) cudaEventDestroy(e[i]); } } ev_free{ev};
+  GPUD_CUDA(r->ctx, cudaEventRecord(ev[0], r->stream));
+  int64_t open = 0;
+  int reasons[GPUD_RANGE_N_OPEN_REASONS] = {};
+  auto tally = [&]() {
+    open += r->ranges->open;
+    for (int i = 0; i < GPUD_RANGE_N_OPEN_REASONS; ++i) reasons[i] += r->ranges->reasons[i];
+  };
+  if (!ids[0].empty()) {
+    std::vector<int64_t> sf, sl, so;
+    tier_subcall(ids[0], first, len, set_off, nullptr, sf, sl, so);
+    const int64_t m = (int64_t)ids[0].size();
+    std::vector<double> f64(5 * (size_t)F * m);
+    std::vector<uint32_t> nov((size_t)F * m);
+    int32_t rc = reduce_sets(&r, 1, nullptr, sf.data(), sl.data(), (int64_t)sf.size(), so.data(), m, f64.data(), nov.data(), &r->ranges);
+    if (rc) return rc;
+    tier_scatter(f64, nov, ids[0], 0, F, F, n_sets, out_f64, out_n_over);
+    tally();
+  }
+  // the virtual ring: rows held by the tier are decoded, the newest one (partial) is copied from the ring
+  std::vector<int64_t> dec(sp.rows);
+  int64_t tail_n = 0;
+  if (dec.back() == t_next) {
+    tail_n = r->total - t_next * GPUD_TIER_ROW;
+    dec.pop_back();
+  }
+  const int64_t vcap = (int64_t)sp.rows.size() * GPUD_TIER_ROW;
+  const int smp_shift = ring_smp_shift(vcap);
+  const int64_t smp_slots = (vcap + (1ll << smp_shift) - 1) >> smp_shift, per_field = 8 * (vcap + smp_slots);
+  int G = (int)std::max<int64_t>(1, std::min<int64_t>(F, kTierGroupBytes / per_field));
+  if (t->group_max > 0) G = std::min(G, t->group_max);
+  std::vector<int64_t> sf, sl, so;
+  tier_subcall(ids[1], first, len, set_off, &sp.vfirst, sf, sl, so);
+  const int64_t m = (int64_t)ids[1].size();
+  t->dec_ms = 0.f;
+  for (int f0 = 0; f0 < F; f0 += G) {
+    const int g = std::min(G, F - f0);
+    gpud_ring v = *r;                  // the virtual ring: a view for reduce_sets, which owns nothing
+    v.F = g;
+    v.cap = vcap;
+    v.total = sp.vtotal;
+    v.d_thr = r->d_thr + f0;
+    v.smp_shift = smp_shift;
+    v.smp_slots = smp_slots;
+    { int32_t rc = gpud_tier_decode(r, dec, t_next, tail_n, f0, g, vcap, smp_shift, smp_slots, &v.d_ring, &v.d_sample); if (rc) return rc; }
+    std::vector<double> f64(5 * (size_t)g * m);
+    std::vector<uint32_t> nov((size_t)g * m);
+    gpud_ring* vp = &v;
+    int32_t rc = reduce_sets(&vp, 1, nullptr, sf.data(), sl.data(), (int64_t)sf.size(), so.data(), m, f64.data(), nov.data(), &r->ranges);
+    if (rc) return rc;
+    float ms = 0.f;
+    GPUD_CUDA(r->ctx, cudaEventElapsedTime(&ms, t->ev_dec[0], t->ev_dec[1]));
+    t->dec_ms += ms;
+    tier_scatter(f64, nov, ids[1], f0, g, F, n_sets, out_f64, out_n_over);
+    tally();
+  }
+  // gpud_ring_ranges_stats reports the whole call: its events now bracket everything above
+  gpud_ranges_state* rs = r->ranges;
+  GPUD_CUDA(r->ctx, cudaEventRecord(ev[1], r->stream));
+  GPUD_CUDA(r->ctx, cudaEventSynchronize(ev[1]));
+  std::swap(rs->ev[0], ev[0]);
+  std::swap(rs->ev[1], ev[1]);
+  rs->open = open;
+  std::copy(reasons, reasons + GPUD_RANGE_N_OPEN_REASONS, rs->reasons);
+  return GPUD_OK;
+}
+
+// Test hook (include/gpud_b200_hooks.h): the split of one call on a tiered ring that holds rows [tier_first, tier_next).
+extern "C" int32_t gpudh_ring_tier_split(int64_t total, int64_t cap, int32_t n_fields, int64_t tier_first, int64_t tier_next, const int64_t* first,
+                                         const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets, int32_t* route, int64_t* vfirst,
+                                         int64_t* rows, int64_t rows_cap, int64_t* n_rows, int64_t* vtotal) {
+  if (total < 0 || cap < 2 || n_fields < 1 || n_ranges < 0 || n_sets < 1 || !first || !len || !route || !vfirst || !n_rows || !vtotal) return GPUD_E_INVALID;
+  if (!set_off && n_sets != n_ranges) return GPUD_E_INVALID;
+  TierSplit sp;
+  if (tier_split(nullptr, total, cap, n_fields, tier_first, tier_next, first, len, n_ranges, set_off, n_sets, &sp)) return GPUD_E_INVALID;
+  std::copy(sp.route.begin(), sp.route.end(), route);
+  std::copy(sp.vfirst.begin(), sp.vfirst.end(), vfirst);
+  *n_rows = (int64_t)sp.rows.size();
+  *vtotal = sp.vtotal;
+  if (*n_rows > rows_cap || (*n_rows && !rows)) return GPUD_E_CAPACITY;
+  std::copy(sp.rows.begin(), sp.rows.end(), rows);
+  return GPUD_OK;
+}
+
 extern "C" int32_t gpud_ring_reduce_ranges(gpud_ring* r, const int64_t* first, const int64_t* len, int64_t n_ranges, double* out_f64, uint32_t* out_n_over) {
   if (!r || n_ranges < 0) return GPUD_E_INVALID;
   if (n_ranges == 0) return GPUD_OK;
   if (!first || !len || !out_f64 || !out_n_over) return GPUD_E_INVALID;
   if (n_ranges > GPUD_RANGES_MAX_SEGMENTS / r->F)
     return gpud_fail(r->ctx, GPUD_E_INVALID, "%d fields x %lld ranges exceed GPUD_RANGES_MAX_SEGMENTS", r->F, (long long)n_ranges);
+  if (r->tier) return reduce_sets_tier(r, first, len, n_ranges, nullptr, n_ranges, out_f64, out_n_over);
   return reduce_sets(&r, 1, nullptr, first, len, n_ranges, nullptr, n_ranges, out_f64, out_n_over, &r->ranges);
 }
 
@@ -1099,6 +1273,12 @@ extern "C" int32_t gpud_rings_reduce_range_sets(gpud_ring* const* rings, int32_t
 
 extern "C" int32_t gpud_ring_reduce_range_sets(gpud_ring* r, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets,
                                                double* out_f64, uint32_t* out_n_over) {
+  if (r && r->tier && n_sets > 0 && n_ranges >= 0) {
+    if (!first || !len || !set_off || !out_f64 || !out_n_over) return GPUD_E_INVALID;
+    if (n_sets > GPUD_RANGES_MAX_SEGMENTS / r->F)
+      return gpud_fail(r->ctx, GPUD_E_INVALID, "%d fields x %lld sets exceed GPUD_RANGES_MAX_SEGMENTS", r->F, (long long)n_sets);
+    return reduce_sets_tier(r, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over);
+  }
   return gpud_rings_reduce_range_sets(&r, 1, nullptr, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over);
 }
 

@@ -410,6 +410,30 @@ int32_t gpud_ring_restore_delta(gpud_ring* ring, const void* in, int64_t n_bytes
  * blocks coded by mode ([2]: RAW, INT) of the last of the four calls.  Any pointer may be NULL; GPUD_E_STATE before the first. */
 int32_t gpud_ring_checkpoint_stats(gpud_ring* ring, float* encode_ms, float* decode_ms, int64_t* blocks_by_mode);
 
+/* The tier (DESIGN.md §2 "Tier"): an opt-in, delta-coded copy of the ring's older samples on its device, so that the range calls reach
+ * back many times further than CAP for the same HBM.  Block row k is samples [1024 k, 1024 (k + 1)) of every field in push order;
+ * each field's block is coded exactly as a checkpoint block (DESIGN.md "Ring checkpoint format").  Every push entry point (push,
+ * _push_device, _push_raw, the poller, and gpud_ring_restore_delta's samples) encodes each row it completes, after its append, on the
+ * ring's stream, with no host synchronisation.  The tier is a byte ring of whole rows: placement and eviction run on the device, a row
+ * that does not fit before the end of the buffer goes to its start, and the oldest rows go until the new one fits.  A row overwritten in
+ * the ring before it was encoded (one push of more than about CAP - 1024 rows) is lost and counted, and the tier restarts at the first
+ * row wholly in the ring, so the tier and the ring always hold one contiguous run of the push order.
+ * On a tiered ring gpud_ring_reduce_ranges and gpud_ring_reduce_range_sets take any range with len >= 1, first + len <= total and
+ * first >= min(total - count, first_sample) (gpud_ring_tier_counts), with the same definitions and every other refusal unchanged;
+ * min / max / p99 / n_over equal bit for bit what a ring of a CAP that holds all those samples gives.  gpud_rings_reduce_range_sets,
+ * gpud_box_query, checkpoints and deltas ignore the tier (a restored ring has none; restore into a tiered ring -> GPUD_E_STATE).
+ * Open: once per ring (again -> GPUD_E_STATE); allocates tier_bytes (rounded down to 8) for the rows, plus 8 KiB per field and 16 B
+ * per row it could hold, on the ring's device until gpud_ring_destroy.  CAP < 2048, or tier_bytes below one row coded at 64 bits and
+ * its record (8192 F + 16 + pad8(F) + pad8(4 F)) -> GPUD_E_INVALID; a failed allocation -> GPUD_E_NOMEM / GPUD_E_CUDA with the ring
+ * unchanged.  A ring that already holds samples starts its tier at the first row wholly in it, encoded by the open. */
+int32_t gpud_ring_tier_open(gpud_ring* ring, int64_t tier_bytes);
+/* Synchronise the ring's stream: the tier holds samples [*first_sample, *next_sample) (multiples of 1024), in *bytes_used bytes,
+ * and *rows_lost_total rows were lost since the open.  Any pointer may be NULL; GPUD_E_STATE without a tier. */
+int32_t gpud_ring_tier_counts(gpud_ring* ring, int64_t* first_sample, int64_t* next_sample, int64_t* bytes_used, int64_t* rows_lost_total);
+/* Synchronise the ring's stream: device ms of the last encode (the last push that completed a row; 0 before one), of the last range
+ * call's decode (0 if none touched the tier), and the blocks of that encode by mode ([2]: RAW, INT).  GPUD_E_STATE without a tier. */
+int32_t gpud_ring_tier_stats(gpud_ring* ring, float* encode_ms, float* decode_ms, int64_t* blocks_by_mode);
+
 /* ------------------------------------------------------------------------------------------------
  * components.Component (components/types.go:20-66) for the three paths this library replaces, as objects: what a Go file that
  * implements the interface forwards to, method by method.

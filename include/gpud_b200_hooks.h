@@ -79,6 +79,25 @@ int32_t gpudh_ring_windows_sub(int32_t W, int64_t span);
  * each warp codes many blocks in turn; 0: the default (one warp per block, at most 16 CTAs per SM).  Checkpoint, restore, delta and
  * delta apply on the ring all read it; the bytes and the restored ring do not depend on it. */
 int32_t gpudh_ring_ckpt_grid(gpud_ring* r, int32_t max_ctas);
+/* The tier's placement on the host (gpud_ring_tier_open): a ring of capacity cap and n_fields fields with total0 samples when a tier
+ * of tier_bytes opens, then pushes of push_n[i] samples; row k codes to row_bytes[k] bytes, its record included (n_rows of them given,
+ * GPUD_E_CAPACITY if a push completes a row beyond).  state[6 (i + 1) .. + 6] after push i (state[0..6]: after the open) = {first row,
+ * next row, bytes in use, rows lost, head, tail} (head: byte offset of the oldest row, tail: end of the newest); row_off[k] = the byte
+ * offset row k was placed at, -1 if it never was. */
+int32_t gpudh_ring_tier_plan(int64_t cap, int32_t n_fields, int64_t tier_bytes, int64_t total0, const int64_t* push_n, int64_t n_push,
+                             const int64_t* row_bytes, int64_t n_rows, int64_t* state, int64_t* row_off);
+/* The split of one gpud_ring_reduce_range_sets (set_off NULL: gpud_ring_reduce_ranges, n_sets = n_ranges) on a tiered ring of `total`
+ * pushed samples, capacity cap, whose tier holds rows [tier_first, tier_next): route[s] = 0 (the ring, today's driver) or 1 (the
+ * virtual ring); the rows the virtual ring decodes (or copies: row tier_next), ascending; vfirst[i] the first sample of range i of a
+ * tier set in the virtual ring (-1 otherwise); *vtotal its samples.  GPUD_E_INVALID for what the call refuses. */
+int32_t gpudh_ring_tier_split(int64_t total, int64_t cap, int32_t n_fields, int64_t tier_first, int64_t tier_next, const int64_t* first,
+                              const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets, int32_t* route, int64_t* vfirst,
+                              int64_t* rows, int64_t rows_cap, int64_t* n_rows, int64_t* vtotal);
+/* Row `row` of the tier as it lies in its byte ring: the record, then the blocks (*n_bytes; GPUD_E_CAPACITY if cap is smaller, a row
+ * the tier does not hold -> GPUD_E_INVALID).  Synchronises. */
+int32_t gpudh_ring_tier_row(gpud_ring* r, int64_t row, void* out, int64_t cap, int64_t* n_bytes);
+/* At most max_fields fields per decoded group of a range call that reaches the tier (0: as many as 1 GiB of decoded rows allows). */
+int32_t gpudh_ring_tier_group(gpud_ring* r, int32_t max_fields);
 /* the host plan of one gpud_ring_windows_reduce of a handle of span x W samples every hop x W (P) on a ring of `total` pushed
  * samples and capacity cap, its history of at most `history` windows now holding [first, next), reseed = 1 when the handle re-seeds
  * its EMA at window next (opened, or restarted with nothing reduced since).  out[8] as gpudh_ring_stream_plan; ema[5] = {physical
