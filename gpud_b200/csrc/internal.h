@@ -14,8 +14,8 @@
 
 struct gpud_scan_state;   // kmsg_scan.cu
 struct gpud_comm_state;   // fabric.cu
-struct gpud_range_state;  // select.cu
-struct gpud_ranges_state; // select.cu
+struct gpud_range_state;  // segsel.h
+struct gpud_ranges_state; // segsel.h
 struct gpud_ring_windows; // below
 struct gpud_tier;         // below
 
@@ -42,7 +42,7 @@ struct gpud_ring {
   double alpha = 0;
   int q_num = 99, q_den = 100;
   int64_t total = 0;
-  int64_t gen = 0;                 // pushes and restores so far: a box query started before one of them is refused (select.cu)
+  int64_t gen = 0;                 // pushes and restores so far: a box query started before one of them is refused (box_query.cu)
   double* d_ring = nullptr;
   double* d_thr = nullptr;
   double* d_pw = nullptr;
@@ -175,6 +175,18 @@ struct gpud_ring_windows {
   int seg_reasons[GPUD_RANGE_N_OPEN_REASONS] = {};   // ... and why, by GPUD_RANGE_OPEN_*
 };
 
+// What the range launchers (ring.cu, select.cu, ranges.cu, box_query.cu) read of a ring; owns nothing.  gpud_view gives a real ring's;
+// the tier's decoded virtual ring and the box query's dense and pivot buffers are views of their own, with the ring's config.
+struct gpud_ring_view {
+  gpud_ctx* ctx; int dev; cudaStream_t stream; int sm_count;                         // where the launches run
+  int F; int64_t cap; double alpha; int q_num, q_den;                                // the ring's config
+  const double *d_ring, *d_thr, *d_pw, *d_sample; int smp_shift; int64_t smp_slots;  // samples [F][cap], thresholds, EMA powers, sample ring
+};
+inline gpud_ring_view gpud_view(const gpud_ring* r) {
+  return {r->ctx, r->dev, r->stream, r->sm_count, r->F, r->cap, r->alpha, r->q_num, r->q_den, r->d_ring, r->d_thr, r->d_pw, r->d_sample, r->smp_shift,
+          r->smp_slots};
+}
+
 inline int64_t ring_count(const gpud_ring* r) { return r->total < r->cap ? r->total : r->cap; }
 inline int64_t ring_start(const gpud_ring* r) { return r->total <= r->cap ? 0 : r->total % r->cap; }
 
@@ -263,7 +275,7 @@ int32_t gpud_ring_window_pass(gpud_ring* r, int64_t start, int64_t n, int Wp, do
 struct gpud_seg_out { const double* out; const uint32_t* nover; const double* part; int64_t open; const int* reasons; };
 int32_t gpud_ring_segments(gpud_ring* r, gpud_range_state** st, int64_t start, int64_t seg_len, int64_t n_seg, int Wp, gpud_seg_out* out);
 
-// gpud_ring_reduce_ranges and gpud_rings_reduce_range_sets (select.cu, DESIGN.md §2 "Ranges", "Range sets", "Box sets").  A set of
+// gpud_ring_reduce_ranges and gpud_rings_reduce_range_sets (ranges.cu, DESIGN.md §2 "Ranges", "Range sets", "Box sets").  A set of
 // several ranges, or of one range in a ring other than the home ring, reads its samples through the call's piece table: piece i of a
 // set is its i-th range, in ring slot gpud_piece_ring of the call's ring table at physical column gpud_piece_start, and its samples are
 // the set's concatenated samples [off, next piece's off) (the last piece: up to the set's length).  A set of one range in the home
@@ -326,12 +338,12 @@ struct gpud_range_geo {
 // A set with pieces reads through `pieces`: a short one from its p0, long set j from seg_p0[j]; its tile t's first sample is in its
 // piece tile_piece[t] (only read for such sets).  srcs (the call's ring table) is given only for a call whose pieces name a ring other
 // than the home ring; the kernels of a call of one ring never read a ring slot.  The EMA of a set starts at its first piece's ring.
-cudaError_t gpud_ranges_short(gpud_ring* r, const gpud_short_range* rs, int n_short, const gpud_piece* pieces, const gpud_ring_src* srcs, int64_t n_out,
+cudaError_t gpud_ranges_short(const gpud_ring_view& v, const gpud_short_range* rs, int n_short, const gpud_piece* pieces, const gpud_ring_src* srcs, int64_t n_out,
                               double* out, uint32_t* nover);
-cudaError_t gpud_ranges_tiles(gpud_ring* r, const gpud_range_geo* geo, int64_t n_long, const int32_t* tile_range, int64_t n_tiles, const double* piv,
+cudaError_t gpud_ranges_tiles(const gpud_ring_view& v, const gpud_range_geo* geo, int64_t n_long, const int32_t* tile_range, int64_t n_tiles, const double* piv,
                               double* const w[5], uint32_t* w_nover, uint4* w_cls, unsigned long long* lists, int64_t list_row, unsigned* fill,
                               const gpud_piece* pieces, const int64_t* seg_p0, const int64_t* tile_piece, const gpud_ring_src* srcs);
-cudaError_t gpud_ranges_ema(gpud_ring* r, const gpud_range_geo* geo, int64_t n_long, const double* part, int64_t n_tiles, double* ema,
+cudaError_t gpud_ranges_ema(const gpud_ring_view& v, const gpud_range_geo* geo, int64_t n_long, const double* part, int64_t n_tiles, double* ema,
                             const gpud_piece* pieces, const int64_t* seg_p0, const gpud_ring_src* srcs);
 
 // Let kernels on device dev read (and write) memory of device peer through the peer mapping, enabled once per ordered pair of a ctx

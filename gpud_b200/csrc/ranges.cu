@@ -1,0 +1,593 @@
+// ranges.cu — sets of sample ranges of one ring or of several: gpud_ring_reduce_ranges, gpud_ring_reduce_range_sets and
+// gpud_rings_reduce_range_sets, their plan, their driver over the segment select (segsel.h), and the ranges that reach into the tier.
+#include <algorithm>
+
+#include "segsel.h"
+
+// ---- gpud_ring_reduce_ranges and gpud_ring_reduce_range_sets (DESIGN.md §2 "Ranges", "Range sets") ----------------------------
+// Both calls reduce sets of ranges; gpud_ring_reduce_ranges is the one whose every set is a single range.  A set's samples are its
+// ranges' samples concatenated, one segment of m samples: up to GPUD_MAX_WINDOW it is one warp's work, else the long route cuts its
+// concatenation into tiles of GPUD_MAX_WINDOW (the last one shorter), so the finish and the EMA see exactly one range of m samples.
+// The long route works in batches of long sets whose scratch (tile arrays, key lists, per-segment state) fits kRangesBatchBytes, so
+// that a call over many long sets does not need memory in proportion to all of them at once; each batch is one run of the segment
+// select (four launches, one synchronisation, then the radix select for the segments it left open).  A set is never split: one that
+// needs more on its own is a batch by itself.
+constexpr int64_t kRangesBatchBytes = (int64_t)1 << 30;
+
+// Validation, the physical columns, the pieces, the routes, the tile list and the batches.  Pure host arithmetic.  Range i lies in ring
+// slot ring_of[i] of n_rings (ring_of NULL: all in slot 0, the home ring), which has pushed totals[ring_of[i]] samples; every ring has
+// capacity cap.  set_off NULL: every range is a set of its own (n_sets = n).  A refusal names the range or the set in ctx's last error
+// (ctx may be NULL).
+int32_t ranges_plan(gpud_ctx* ctx, const int64_t* totals, int n_rings, const int32_t* ring_of, int64_t cap, int F, int q_num, int q_den, double alpha,
+                    int smp_shift, const int64_t* first, const int64_t* len, int64_t n, const int64_t* set_off, int64_t n_sets, RangesPlan* pl) {
+  for (int64_t i = 0; i < n; ++i) {
+    const int32_t k = ring_of ? ring_of[i] : 0;
+    if (k < 0 || k >= n_rings) return gpud_fail(ctx, GPUD_E_INVALID, "range %lld: ring_of is %d, not a ring of the call's %d", (long long)i, k, n_rings);
+    const int64_t total = totals[k], count = total < cap ? total : cap;
+    if (len[i] < 1 || first[i] < total - count || first[i] > total - len[i])
+      return gpud_fail(ctx, GPUD_E_INVALID, "range %lld: samples [%lld, +%lld) are not all in ring %d (pushed %lld, held %lld)", (long long)i,
+                       (long long)first[i], (long long)len[i], k, (long long)total, (long long)count);
+  }
+  if (set_off) {
+    if (set_off[0] != 0) return gpud_fail(ctx, GPUD_E_INVALID, "set 0: set_off[0] is %lld, not 0", (long long)set_off[0]);
+    if (set_off[n_sets] != n)
+      return gpud_fail(ctx, GPUD_E_INVALID, "set %lld: set_off[%lld] is %lld, not n_ranges %lld", (long long)(n_sets - 1), (long long)n_sets,
+                       (long long)set_off[n_sets], (long long)n);
+    for (int64_t s = 0; s < n_sets; ++s)
+      if (set_off[s + 1] <= set_off[s])
+        return gpud_fail(ctx, GPUD_E_INVALID, "set %lld is empty: set_off[%lld] = %lld is not above set_off[%lld] = %lld", (long long)s, (long long)(s + 1),
+                         (long long)set_off[s + 1], (long long)s, (long long)set_off[s]);
+    for (int64_t s = 0; s < n_sets; ++s) {
+      int64_t m = 0;
+      for (int64_t i = set_off[s]; i < set_off[s + 1] && m <= (int64_t)UINT32_MAX; ++i) m += len[i];
+      if (m > (int64_t)UINT32_MAX) return gpud_fail(ctx, GPUD_E_INVALID, "set %lld: more than UINT32_MAX samples (its n_over is 32-bit)", (long long)s);
+    }
+  }
+  pl->start.resize(n);
+  pl->route.assign(n_sets, 0);
+  pl->batch0.assign(1, 0);
+  pl->tiles0.assign(1, 0);
+  for (int64_t i = 0; i < n; ++i) pl->start[i] = first[i] % cap;   // column c holds every sample c + k CAP; sample first[i] is still in the ring
+  int64_t bytes = 0, tiles = 0, keys = 0;
+  for (int64_t s = 0; s < n_sets; ++s) {
+    const int64_t a = set_off ? set_off[s] : s, e = set_off ? set_off[s + 1] : s + 1;
+    int64_t m = 0, p0 = 0;
+    const bool has_pieces = e - a > 1 || (ring_of && ring_of[a] != 0);   // several ranges, or one outside the home ring
+    if (has_pieces) {
+      p0 = (int64_t)pl->pieces.size();
+      for (int64_t i = a; i < e; ++i) { pl->pieces.push_back(gpud_piece_make(pl->start[i], m, ring_of ? ring_of[i] : 0)); m += len[i]; }
+    } else {
+      m = len[a];
+    }
+    const uint32_t np = has_pieces ? (uint32_t)(e - a) : 0u;   // at most m <= UINT32_MAX
+    if (m <= GPUD_MAX_WINDOW) {
+      pl->shorts.push_back({pl->start[a], (int32_t)m, (int32_t)s, p0, np, 0});
+      continue;
+    }
+    gpud_range_geo g{};
+    g.start = pl->start[a];
+    g.n = m;
+    g.k = gpud_rank_from_top(m, q_num, q_den);
+    g.id = s;
+    g.np = np;
+    seg_sample(&g, smp_shift);
+    const int64_t nt = (m + GPUD_MAX_WINDOW - 1) / GPUD_MAX_WINDOW;
+    g.d_last = pow(1.0 - alpha, (double)(m - (nt - 1) * GPUD_MAX_WINDOW));
+    // per field: the tiles' min / max / mean / EMA partials / n_over / class counts, the key list, the segment's pivots, fill, result
+    // and select state; per tile of a set with pieces its first piece
+    const int64_t b = (int64_t)F * (nt * (4 * 8 + 4 + 16) + (int64_t)g.lcap * 8 + 16 + 4 + 5 * 8 + 4 + (int64_t)sizeof(SelState) + 4 + 8) + (np ? nt * 8 : 0);
+    if ((int64_t)pl->geo.size() > pl->batch0.back() && bytes + b > kRangesBatchBytes) {
+      pl->batch0.push_back((int64_t)pl->geo.size());
+      pl->tiles0.push_back(pl->tiles0.back() + tiles);
+      bytes = tiles = keys = 0;
+    }
+    g.tile0 = tiles;
+    g.list0 = keys;
+    bytes += b;
+    tiles += nt;
+    keys += g.lcap;
+    pl->route[s] = (int32_t)pl->batch0.size();
+    pl->geo.push_back(g);
+    pl->p0.push_back(p0);
+  }
+  pl->batch0.push_back((int64_t)pl->geo.size());
+  pl->tiles0.push_back(pl->tiles0.back() + tiles);
+  return GPUD_OK;
+}
+
+// The piece of long set g (with pieces p) that holds the first sample of each of its tiles, counted from its first piece.
+static void tile_pieces(const gpud_range_geo& g, const gpud_piece* p, int64_t* tp) {
+  int64_t i = 0;
+  for (int64_t t = 0; t * GPUD_MAX_WINDOW < g.n; ++t) {
+    while (i + 1 < g.np && p[i + 1].off <= t * GPUD_MAX_WINDOW) ++i;
+    tp[t] = i;
+  }
+}
+
+void gpud_ranges_state_free(gpud_ranges_state* s) {
+  if (!s) return;
+  gpud_range_state_free(s->seg);
+  cudaFree(s->d_short); cudaFree(s->d_pieces); cudaFree(s->d_srcs); cudaFree(s->d_tile); cudaFree(s->d_tile_piece); cudaFree(s->d_out); cudaFree(s->d_nover);
+  for (auto& ev : s->ev) if (ev) cudaEventDestroy(ev);
+  delete s;
+}
+
+namespace {
+// one batch's long results [5][F n_long] / [F n_long] (segment f n_long + j) into the call's [5][F][n_out] / [F][n_out], column geo[j].id
+__global__ void k_ranges_scatter(const double* __restrict__ seg_out, const uint32_t* __restrict__ seg_nover, const gpud_range_geo* __restrict__ geo, int64_t n_long,
+                                 int F, int64_t n_out, double* __restrict__ out, uint32_t* __restrict__ nover) {
+  const int64_t n_segs = (int64_t)F * n_long, plane = (int64_t)F * n_out;
+  for (int64_t sg = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; sg < n_segs; sg += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t f = sg / n_long, o = f * n_out + geo[sg - f * n_long].id;
+    for (int op = 0; op < 5; ++op) out[op * plane + o] = seg_out[op * n_segs + sg];
+    nover[o] = seg_nover[sg];
+  }
+}
+}  // namespace
+
+cudaError_t ranges_scatter(const gpud_ring_view& v, const gpud_range_state* s, int64_t n_long, int64_t n_out, double* out, uint32_t* nover) {
+  const int64_t n_segs = (int64_t)v.F * n_long;
+  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n_segs + 255) / 256, (int64_t)v.sm_count * 8));
+  k_ranges_scatter<<<grid, 256, 0, v.stream>>>(s->d_out, s->d_nover, s->d_geo, n_long, v.F, n_out, out, nover);
+  return cudaGetLastError();
+}
+
+// The call behind both entry points, after their argument checks (and, for several rings, rings_check): every refusal comes from
+// ranges_plan, or the peer check after it, before any launch.  The kernels run on the home ring's device and stream, read through the
+// view v (the ring itself, or a buffer laid out as one: the tier's virtual ring), with the scratch *state (created on first use): the
+// home ring's own, or a box query's (gpud_box_query), which must leave the ring's untouched.  rings[1, n_rings) are the call's other rings.
+int32_t reduce_sets(const gpud_ring_view& v, int64_t home_total, gpud_ring* const* rings, int n_rings, const int32_t* ring_of, const int64_t* first,
+                    const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over,
+                    gpud_ranges_state** state) {
+  std::vector<int64_t> totals(n_rings, home_total);
+  std::vector<gpud_ring_src> src(n_rings, gpud_ring_src{v.d_ring, v.d_sample});
+  for (int i = 1; i < n_rings; ++i) {
+    totals[i] = rings[i]->total;
+    src[i] = {rings[i]->d_ring, rings[i]->d_sample};
+  }
+  RangesPlan pl;
+  { int32_t rc = ranges_plan(v.ctx, totals.data(), n_rings, ring_of, v.cap, v.F, v.q_num, v.q_den, v.alpha, v.smp_shift, first, len, n_ranges, set_off,
+                             n_sets, &pl); if (rc) return rc; }
+  // the last refusal: a ring whose device the home device cannot map.  Peer access is enabled only for a call that runs.
+  for (int i = 1; i < n_rings; ++i) {
+    if (rings[i]->dev == v.dev) continue;
+    const cudaError_t e = gpud_peer_enable(v.ctx, v.dev, rings[i]->dev);
+    if (e == cudaErrorPeerAccessUnsupported)
+      return gpud_fail(v.ctx, GPUD_E_UNSUPPORTED, "ring %d: device %d cannot map device %d's memory as a peer", i, v.dev, rings[i]->dev);
+    GPUD_CUDA(v.ctx, e);
+  }
+  // a piece in a ring other than the home ring makes the call MULTI (internal.h); a call of one ring reads no ring table
+  bool multi = false;
+  for (const gpud_piece& q : pl.pieces) multi |= gpud_piece_ring(q) != 0;
+  // the other rings' pushes are complete before the first launch: the home stream waits for each one's stream
+  for (int i = 1; i < n_rings; ++i) {
+    gpud_ring* o = rings[i];
+    if (o->stream == v.stream) continue;
+    cudaEvent_t ev = nullptr;
+    GPUD_CUDA(v.ctx, cudaSetDevice(o->dev));
+    GPUD_CUDA(v.ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    cudaError_t e = cudaEventRecord(ev, o->stream);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(v.stream, ev, 0);
+    cudaEventDestroy(ev);              // released once the wait has been satisfied
+    if (e != cudaSuccess) return gpud_fail(v.ctx, GPUD_E_CUDA, "ring %d: waiting for its stream: %s", i, cudaGetErrorString(e));
+  }
+  GPUD_CUDA(v.ctx, cudaSetDevice(v.dev));
+  if (!*state) *state = new gpud_ranges_state();
+  gpud_ranges_state* rs = *state;
+  if (!rs->seg) rs->seg = new gpud_range_state();
+  rs->timed = false;
+  rs->seg_last = false;
+  rs->open = 0;
+  std::fill(rs->reasons, rs->reasons + GPUD_RANGE_N_OPEN_REASONS, 0);
+  const size_t plane = (size_t)v.F * n_sets;
+  GPUD_CUDA(v.ctx, gpud_grow(&rs->d_out, &rs->out_cap, 5 * plane));
+  GPUD_CUDA(v.ctx, gpud_grow(&rs->d_nover, &rs->nover_cap, plane));
+  GPUD_CUDA(v.ctx, gpud_grow(&rs->d_short, &rs->short_cap, std::max<size_t>(1, pl.shorts.size())));
+  const gpud_piece* d_pieces = nullptr;
+  if (!pl.pieces.empty()) {
+    GPUD_CUDA(v.ctx, gpud_grow(&rs->d_pieces, &rs->pieces_cap, pl.pieces.size()));
+    if (multi) GPUD_CUDA(v.ctx, gpud_grow(&rs->d_srcs, &rs->srcs_cap, (size_t)n_rings));
+    d_pieces = rs->d_pieces;
+  }
+  for (auto& ev : rs->ev) if (!ev) GPUD_CUDA(v.ctx, cudaEventCreate(&ev));
+  GPUD_CUDA(v.ctx, cudaEventRecord(rs->ev[0], v.stream));
+  if (d_pieces) {
+    GPUD_CUDA(v.ctx, cudaMemcpyAsync(rs->d_pieces, pl.pieces.data(), pl.pieces.size() * sizeof(gpud_piece), cudaMemcpyHostToDevice, v.stream));
+    if (multi) GPUD_CUDA(v.ctx, cudaMemcpyAsync(rs->d_srcs, src.data(), n_rings * sizeof(gpud_ring_src), cudaMemcpyHostToDevice, v.stream));
+  }
+  const gpud_ring_src* d_srcs = multi ? rs->d_srcs : nullptr;
+  if (!pl.shorts.empty()) {
+    GPUD_CUDA(v.ctx, cudaMemcpyAsync(rs->d_short, pl.shorts.data(), pl.shorts.size() * sizeof(gpud_short_range), cudaMemcpyHostToDevice, v.stream));
+    GPUD_CUDA(v.ctx, gpud_ranges_short(v, rs->d_short, (int)pl.shorts.size(), d_pieces, d_srcs, n_sets, rs->d_out, rs->d_nover));
+  }
+  for (size_t b = 0; b + 1 < pl.batch0.size(); ++b) {
+    // one batch of the long route: the segment select over its long sets, read in tiles, then the scatter of its results
+    const int64_t g0 = pl.batch0[b], n_long = pl.batch0[b + 1] - g0, n_tiles = pl.tiles0[b + 1] - pl.tiles0[b];
+    if (n_long == 0) continue;
+    std::vector<int32_t> tile(n_tiles);
+    std::vector<int64_t> tile_piece;
+    for (int64_t j = 0; j < n_long; ++j) {
+      const gpud_range_geo& g = pl.geo[g0 + j];
+      std::fill(tile.begin() + g.tile0, tile.begin() + g.tile0 + (g.n + GPUD_MAX_WINDOW - 1) / GPUD_MAX_WINDOW, (int32_t)j);
+      if (g.np) {
+        tile_piece.resize(n_tiles);
+        tile_pieces(g, pl.pieces.data() + pl.p0[g0 + j], tile_piece.data() + g.tile0);
+      }
+    }
+    GPUD_CUDA(v.ctx, gpud_grow(&rs->d_tile, &rs->tile_cap, (size_t)n_tiles));
+    GPUD_CUDA(v.ctx, cudaMemcpyAsync(rs->d_tile, tile.data(), n_tiles * sizeof(int32_t), cudaMemcpyHostToDevice, v.stream));
+    if (!tile_piece.empty()) {
+      GPUD_CUDA(v.ctx, gpud_grow(&rs->d_tile_piece, &rs->tile_piece_cap, (size_t)n_tiles));
+      GPUD_CUDA(v.ctx, cudaMemcpyAsync(rs->d_tile_piece, tile_piece.data(), n_tiles * sizeof(int64_t), cudaMemcpyHostToDevice, v.stream));
+    }
+    gpud_range_state* s = rs->seg;
+    const bool pieces = !tile_piece.empty();   // a set with pieces in this batch
+    { int32_t rc = run_select(v, nullptr, s, pl.geo.data() + g0, n_long, GPUD_MAX_WINDOW, true, true, rs->d_tile, nullptr, nullptr, pieces ? d_pieces : nullptr,
+                              pl.p0.data() + g0, pieces ? rs->d_tile_piece : nullptr, pieces ? d_srcs : nullptr); if (rc) return rc; }
+    rs->seg_last = true;
+    rs->open += s->fields_open;
+    for (int i = 0; i < GPUD_RANGE_N_OPEN_REASONS; ++i) rs->reasons[i] += s->reasons[i];
+    GPUD_CUDA(v.ctx, ranges_scatter(v, s, n_long, n_sets, rs->d_out, rs->d_nover));
+  }
+  cudaError_t e = cudaEventRecord(rs->ev[1], v.stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(out_f64, rs->d_out, 5 * plane * sizeof(double), cudaMemcpyDeviceToHost, v.stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(out_n_over, rs->d_nover, plane * sizeof(uint32_t), cudaMemcpyDeviceToHost, v.stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(v.stream);
+  if (e != cudaSuccess) return gpud_fail(v.ctx, GPUD_E_CUDA, "reduce_ranges: %s", cudaGetErrorString(e));
+  rs->timed = true;
+  return GPUD_OK;
+}
+
+// ---- ranges that reach into the tier (DESIGN.md §2 "Tier") -------------------------------------------------------------------
+// A tiered ring holds samples [lo, total) with lo = min(total - count, 1024 tier_first).  The sets whose ranges all lie in the ring go
+// through reduce_sets untouched.  Each other set's ranges cover block rows; those rows, merged and ascending, are decoded into a
+// virtual ring (row j at columns [1024 j, 1024 (j + 1)); the newest row, not yet coded, copied from the ring), and reduce_sets runs
+// on that buffer as on a ring of its own capacity with the ring's alpha, quantile and thresholds - in groups of fields, each as large
+// as kTierGroupBytes of decoded samples allow.
+constexpr int64_t kTierGroupBytes = (int64_t)1 << 30;
+
+struct TierSplit {
+  std::vector<int32_t> route;        // per set: 0 the ring, 1 the tier
+  std::vector<int64_t> rows;         // the block rows the tier sets read, ascending
+  std::vector<int64_t> vfirst;       // per range of a tier set: its first sample in the virtual ring (-1: a ring set's range)
+  int64_t vtotal = 0;                // samples of the virtual ring
+};
+
+// Validation (every refusal of ranges_plan, against samples [lo, total)) and the split.  Pure host arithmetic.
+static int32_t tier_split(gpud_ctx* ctx, int64_t total, int64_t cap, int F, int64_t t_first, int64_t t_next, const int64_t* first, const int64_t* len,
+                          int64_t n, const int64_t* set_off, int64_t n_sets, TierSplit* sp) {
+  const int64_t count = std::min(total, cap), lo = std::min(total - count, t_first * GPUD_TIER_ROW);
+  {
+    // ranges_plan's checks with a capacity that holds [lo, total): the same refusals, against the tier's reach
+    RangesPlan pl;
+    int32_t rc = ranges_plan(ctx, &total, 1, nullptr, std::max<int64_t>(1, total - lo), F, 99, 100, 0.5, 0, first, len, n, set_off, n_sets, &pl);
+    if (rc) return rc;
+  }
+  sp->route.assign(n_sets, 0);
+  sp->vfirst.assign(n, -1);
+  std::vector<std::pair<int64_t, int64_t>> iv;
+  for (int64_t s = 0; s < n_sets; ++s) {
+    const int64_t a = set_off ? set_off[s] : s, e = set_off ? set_off[s + 1] : s + 1;
+    for (int64_t i = a; i < e; ++i) sp->route[s] |= first[i] < total - count;
+    if (!sp->route[s]) continue;
+    for (int64_t i = a; i < e; ++i) iv.push_back({first[i] / GPUD_TIER_ROW, (first[i] + len[i] + GPUD_TIER_ROW - 1) / GPUD_TIER_ROW});
+  }
+  std::sort(iv.begin(), iv.end());
+  sp->rows.clear();
+  for (const auto& v : iv)
+    for (int64_t k = std::max(v.first, sp->rows.empty() ? v.first : sp->rows.back() + 1); k < v.second; ++k) sp->rows.push_back(k);
+  for (int64_t s = 0; s < n_sets; ++s) {
+    if (!sp->route[s]) continue;
+    const int64_t a = set_off ? set_off[s] : s, e = set_off ? set_off[s + 1] : s + 1;
+    for (int64_t i = a; i < e; ++i) {
+      const int64_t j = std::lower_bound(sp->rows.begin(), sp->rows.end(), first[i] / GPUD_TIER_ROW) - sp->rows.begin();
+      sp->vfirst[i] = j * GPUD_TIER_ROW + first[i] % GPUD_TIER_ROW;
+    }
+  }
+  const int64_t nr = (int64_t)sp->rows.size();
+  sp->vtotal = nr * GPUD_TIER_ROW;
+  if (nr && sp->rows.back() == t_next) sp->vtotal -= GPUD_TIER_ROW - (total - t_next * GPUD_TIER_ROW);   // the newest row is partial
+  return GPUD_OK;
+}
+
+// results [5][G][n_sub] / [G][n_sub] of sets ids[] and fields [f0, f0 + G) into the caller's [5][F][n_sets] / [F][n_sets]
+static void tier_scatter(const std::vector<double>& f64, const std::vector<uint32_t>& nov, const std::vector<int64_t>& ids, int f0, int G, int F,
+                         int64_t n_sets, double* out_f64, uint32_t* out_n_over) {
+  const int64_t m = (int64_t)ids.size();
+  for (int op = 0; op < 5; ++op)
+    for (int f = 0; f < G; ++f)
+      for (int64_t j = 0; j < m; ++j) out_f64[((int64_t)op * F + f0 + f) * n_sets + ids[j]] = f64[((int64_t)op * G + f) * m + j];
+  for (int f = 0; f < G; ++f)
+    for (int64_t j = 0; j < m; ++j) out_n_over[(int64_t)(f0 + f) * n_sets + ids[j]] = nov[(int64_t)f * m + j];
+}
+
+int32_t reduce_subset(const gpud_ring_view& v, int64_t home_total, const std::vector<int64_t>& ids, const int64_t* first, const int64_t* len,
+                      const int64_t* set_off, const std::vector<int64_t>* vfirst, gpud_ranges_state** state, std::vector<double>& f64,
+                      std::vector<uint32_t>& nov) {
+  std::vector<int64_t> sf, sl, so(1, 0);
+  for (int64_t s : ids) {
+    const int64_t a = set_off ? set_off[s] : s, e = set_off ? set_off[s + 1] : s + 1;
+    for (int64_t i = a; i < e; ++i) { sf.push_back(vfirst ? (*vfirst)[i] : first[i]); sl.push_back(len[i]); }
+    so.push_back((int64_t)sf.size());
+  }
+  const int64_t m = (int64_t)ids.size();
+  f64.assign(5 * (size_t)v.F * m, 0.0);
+  nov.assign((size_t)v.F * m, 0u);
+  return reduce_sets(v, home_total, nullptr, 1, nullptr, sf.data(), sl.data(), (int64_t)sf.size(), so.data(), m, f64.data(), nov.data(), state);
+}
+
+static int32_t reduce_sets_tier(gpud_ring* r, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets,
+                                double* out_f64, uint32_t* out_n_over) {
+  gpud_tier* t = r->tier;
+  int64_t t_first = 0, t_next = 0;
+  { int32_t rc = gpud_tier_span(r, &t_first, &t_next); if (rc) return rc; }
+  TierSplit sp;
+  { int32_t rc = tier_split(r->ctx, r->total, r->cap, r->F, t_first, t_next, first, len, n_ranges, set_off, n_sets, &sp); if (rc) return rc; }
+  if (sp.rows.empty()) return reduce_sets(gpud_view(r), r->total, nullptr, 1, nullptr, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over, &r->ranges);
+  std::vector<int64_t> ids[2];
+  for (int64_t s = 0; s < n_sets; ++s) ids[sp.route[s]].push_back(s);
+  const int F = r->F;
+  cudaEvent_t ev[2] = {};
+  for (auto& e : ev) GPUD_CUDA(r->ctx, cudaEventCreate(&e));
+  struct EvFree { cudaEvent_t* e; ~EvFree() { for (int i = 0; i < 2; ++i) if (e[i]) cudaEventDestroy(e[i]); } } ev_free{ev};
+  GPUD_CUDA(r->ctx, cudaEventRecord(ev[0], r->stream));
+  int64_t open = 0;
+  int reasons[GPUD_RANGE_N_OPEN_REASONS] = {};
+  auto tally = [&]() {
+    open += r->ranges->open;
+    for (int i = 0; i < GPUD_RANGE_N_OPEN_REASONS; ++i) reasons[i] += r->ranges->reasons[i];
+  };
+  std::vector<double> f64;
+  std::vector<uint32_t> nov;
+  if (!ids[0].empty()) {
+    int32_t rc = reduce_subset(gpud_view(r), r->total, ids[0], first, len, set_off, nullptr, &r->ranges, f64, nov);
+    if (rc) return rc;
+    tier_scatter(f64, nov, ids[0], 0, F, F, n_sets, out_f64, out_n_over);
+    tally();
+  }
+  // the virtual ring: rows held by the tier are decoded, the newest one (partial) is copied from the ring
+  std::vector<int64_t> dec(sp.rows);
+  int64_t tail_n = 0;
+  if (dec.back() == t_next) {
+    tail_n = r->total - t_next * GPUD_TIER_ROW;
+    dec.pop_back();
+  }
+  const int64_t vcap = (int64_t)sp.rows.size() * GPUD_TIER_ROW;
+  const int smp_shift = ring_smp_shift(vcap);
+  const int64_t smp_slots = (vcap + (1ll << smp_shift) - 1) >> smp_shift, per_field = 8 * (vcap + smp_slots);
+  int G = (int)std::max<int64_t>(1, std::min<int64_t>(F, kTierGroupBytes / per_field));
+  if (t->group_max > 0) G = std::min(G, t->group_max);
+  t->dec_ms = 0.f;
+  for (int f0 = 0; f0 < F; f0 += G) {
+    const int g = std::min(G, F - f0);
+    double *vring = nullptr, *vsmp = nullptr;
+    { int32_t rc = gpud_tier_decode(r, dec, t_next, tail_n, f0, g, vcap, smp_shift, smp_slots, &vring, &vsmp); if (rc) return rc; }
+    gpud_ring_view v = gpud_view(r);   // the virtual ring: fields [f0, f0 + g) of the decoded rows
+    v.F = g;
+    v.cap = vcap;
+    v.d_ring = vring;
+    v.d_thr = r->d_thr + f0;
+    v.d_sample = vsmp;
+    v.smp_shift = smp_shift;
+    v.smp_slots = smp_slots;
+    int32_t rc = reduce_subset(v, sp.vtotal, ids[1], first, len, set_off, &sp.vfirst, &r->ranges, f64, nov);
+    if (rc) return rc;
+    float ms = 0.f;
+    GPUD_CUDA(r->ctx, cudaEventElapsedTime(&ms, t->ev_dec[0], t->ev_dec[1]));
+    t->dec_ms += ms;
+    tier_scatter(f64, nov, ids[1], f0, g, F, n_sets, out_f64, out_n_over);
+    tally();
+  }
+  // gpud_ring_ranges_stats reports the whole call: its events now bracket everything above
+  gpud_ranges_state* rs = r->ranges;
+  GPUD_CUDA(r->ctx, cudaEventRecord(ev[1], r->stream));
+  GPUD_CUDA(r->ctx, cudaEventSynchronize(ev[1]));
+  std::swap(rs->ev[0], ev[0]);
+  std::swap(rs->ev[1], ev[1]);
+  rs->open = open;
+  std::copy(reasons, reasons + GPUD_RANGE_N_OPEN_REASONS, rs->reasons);
+  return GPUD_OK;
+}
+
+// Test hook (include/gpud_b200_hooks.h): the split of one call on a tiered ring that holds rows [tier_first, tier_next).
+extern "C" int32_t gpudh_ring_tier_split(int64_t total, int64_t cap, int32_t n_fields, int64_t tier_first, int64_t tier_next, const int64_t* first,
+                                         const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets, int32_t* route, int64_t* vfirst,
+                                         int64_t* rows, int64_t rows_cap, int64_t* n_rows, int64_t* vtotal) {
+  if (total < 0 || cap < 2 || n_fields < 1 || n_ranges < 0 || n_sets < 1 || !first || !len || !route || !vfirst || !n_rows || !vtotal) return GPUD_E_INVALID;
+  if (!set_off && n_sets != n_ranges) return GPUD_E_INVALID;
+  TierSplit sp;
+  if (tier_split(nullptr, total, cap, n_fields, tier_first, tier_next, first, len, n_ranges, set_off, n_sets, &sp)) return GPUD_E_INVALID;
+  std::copy(sp.route.begin(), sp.route.end(), route);
+  std::copy(sp.vfirst.begin(), sp.vfirst.end(), vfirst);
+  *n_rows = (int64_t)sp.rows.size();
+  *vtotal = sp.vtotal;
+  if (*n_rows > rows_cap || (*n_rows && !rows)) return GPUD_E_CAPACITY;
+  std::copy(sp.rows.begin(), sp.rows.end(), rows);
+  return GPUD_OK;
+}
+
+extern "C" int32_t gpud_ring_reduce_ranges(gpud_ring* r, const int64_t* first, const int64_t* len, int64_t n_ranges, double* out_f64, uint32_t* out_n_over) {
+  if (!r || n_ranges < 0) return GPUD_E_INVALID;
+  if (n_ranges == 0) return GPUD_OK;
+  if (!first || !len || !out_f64 || !out_n_over) return GPUD_E_INVALID;
+  if (n_ranges > GPUD_RANGES_MAX_SEGMENTS / r->F)
+    return gpud_fail(r->ctx, GPUD_E_INVALID, "%d fields x %lld ranges exceed GPUD_RANGES_MAX_SEGMENTS", r->F, (long long)n_ranges);
+  if (r->tier) return reduce_sets_tier(r, first, len, n_ranges, nullptr, n_ranges, out_f64, out_n_over);
+  return reduce_sets(gpud_view(r), r->total, nullptr, 1, nullptr, first, len, n_ranges, nullptr, n_ranges, out_f64, out_n_over, &r->ranges);
+}
+
+// The refusals of a call over several rings beyond those of one ring (DESIGN.md §2 "Box sets"): one ctx and the home ring's config bit
+// for bit (gpud_ring_restore's comparison).  Whether the home device can map the others' memory is asked after the plan (reduce_sets).
+static int32_t rings_check(gpud_ring* const* rings, int n_rings) {
+  gpud_ring* h = rings[0];
+  gpud_ctx* ctx = h->ctx;
+  auto bits = [](double x) { uint64_t b; memcpy(&b, &x, 8); return b; };
+  for (int i = 1; i < n_rings; ++i) {
+    const gpud_ring* o = rings[i];
+    if (!o) return gpud_fail(ctx, GPUD_E_INVALID, "ring %d is NULL", i);
+    if (o->ctx != ctx) return gpud_fail(ctx, GPUD_E_INVALID, "ring %d belongs to another ctx than the home ring", i);
+    const char* field = o->F != h->F ? "n_fields" : o->W != h->W ? "window" : o->cap != h->cap ? "capacity" : bits(o->alpha) != bits(h->alpha) ? "ema_alpha"
+                      : o->q_num != h->q_num || o->q_den != h->q_den ? "quantile" : nullptr;
+    for (int f = 0; !field && f < h->F; ++f)
+      if (bits(o->thr[f]) != bits(h->thr[f])) field = "thresholds";
+    if (field) return gpud_fail(ctx, GPUD_E_INVALID, "ring %d: config field %s differs from the home ring's", i, field);
+  }
+  return GPUD_OK;
+}
+
+extern "C" int32_t gpud_rings_reduce_range_sets(gpud_ring* const* rings, int32_t n_rings, const int32_t* ring_of, const int64_t* first, const int64_t* len,
+                                                int64_t n_ranges, const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over) {
+  if (!rings || n_rings < 1 || n_rings > GPUD_PIECE_RINGS || !rings[0] || n_ranges < 0 || n_sets < 0) return GPUD_E_INVALID;
+  gpud_ring* r = rings[0];
+  if (n_sets == 0) return GPUD_OK;
+  if (!first || !len || !set_off || !out_f64 || !out_n_over || (n_rings > 1 && !ring_of)) return GPUD_E_INVALID;
+  if (n_sets > GPUD_RANGES_MAX_SEGMENTS / r->F)
+    return gpud_fail(r->ctx, GPUD_E_INVALID, "%d fields x %lld sets exceed GPUD_RANGES_MAX_SEGMENTS", r->F, (long long)n_sets);
+  { int32_t rc = rings_check(rings, n_rings); if (rc) return rc; }
+  return reduce_sets(gpud_view(r), r->total, rings, n_rings, ring_of, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over, &r->ranges);
+}
+
+extern "C" int32_t gpud_ring_reduce_range_sets(gpud_ring* r, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets,
+                                               double* out_f64, uint32_t* out_n_over) {
+  if (r && r->tier && n_sets > 0 && n_ranges >= 0) {
+    if (!first || !len || !set_off || !out_f64 || !out_n_over) return GPUD_E_INVALID;
+    if (n_sets > GPUD_RANGES_MAX_SEGMENTS / r->F)
+      return gpud_fail(r->ctx, GPUD_E_INVALID, "%d fields x %lld sets exceed GPUD_RANGES_MAX_SEGMENTS", r->F, (long long)n_sets);
+    return reduce_sets_tier(r, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over);
+  }
+  return gpud_rings_reduce_range_sets(&r, 1, nullptr, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over);
+}
+
+extern "C" int32_t gpud_ring_ranges_stats(gpud_ring* r, float* device_ms, int64_t* segments_by_radix, int32_t* reasons) {
+  if (!r || !device_ms) return GPUD_E_INVALID;
+  const gpud_ranges_state* rs = r->ranges;
+  if (!rs || !rs->timed) return gpud_fail(r->ctx, GPUD_E_STATE, "no gpud_ring_reduce_ranges has run to the end on this ring");
+  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
+  GPUD_CUDA(r->ctx, cudaEventSynchronize(rs->ev[1]));
+  GPUD_CUDA(r->ctx, cudaEventElapsedTime(device_ms, rs->ev[0], rs->ev[1]));
+  if (segments_by_radix) *segments_by_radix = rs->open;
+  if (reasons) std::copy(rs->reasons, rs->reasons + GPUD_RANGE_N_OPEN_REASONS, reasons);
+  return GPUD_OK;
+}
+
+// Test hook (include/gpud_b200_hooks.h): what the last segment select left in its scratch - the last batch of the last
+// gpud_ring_reduce_ranges (h NULL) or the last phase of handle h's last reduce - per segment its pivots {lo, hi} and list fill
+// counter, and the class counts of every row of its pass; each buffer may be NULL (all NULL: the sizes alone).
+extern "C" int32_t gpudh_ring_segment_scratch(gpud_ring* r, gpud_ring_windows* h, double* piv, uint32_t* fill, uint32_t* cls, int64_t* n_segs,
+                                              int64_t* n_rows) {
+  if (!r || !n_segs || !n_rows || (h && h->ring != r)) return GPUD_E_INVALID;
+  const gpud_range_state* s = nullptr;
+  if (h) {
+    if (h->L <= GPUD_MAX_WINDOW || !h->seg || !h->seg->timed)
+      return gpud_fail(r->ctx, GPUD_E_STATE, "no reduce of this handle has run the segment select to the end");
+    s = h->seg;
+  } else {
+    if (!r->ranges || !r->ranges->timed || !r->ranges->seg_last)
+      return gpud_fail(r->ctx, GPUD_E_STATE, "the last reduce_ranges (if any) had no long range");
+    s = r->ranges->seg;
+  }
+  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
+  if (piv) GPUD_CUDA(r->ctx, cudaMemcpyAsync(piv, s->d_piv, 2 * s->n_segs * sizeof(double), cudaMemcpyDeviceToHost, r->stream));
+  if (fill) GPUD_CUDA(r->ctx, cudaMemcpyAsync(fill, s->d_fill, s->n_segs * sizeof(uint32_t), cudaMemcpyDeviceToHost, r->stream));
+  if (cls) GPUD_CUDA(r->ctx, cudaMemcpyAsync(cls, s->d_cls, s->n_rows * sizeof(uint4), cudaMemcpyDeviceToHost, r->stream));
+  GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));
+  *n_segs = s->n_segs;
+  *n_rows = s->n_rows;
+  return GPUD_OK;
+}
+
+int ring_smp_shift(int64_t cap) {
+  int smp_shift = 0;
+  while (((cap + (1ll << smp_shift) - 1) >> smp_shift) > GPUD_RANGE_SAMPLE_MAX) ++smp_shift;
+  return smp_shift;
+}
+
+// Test hook (include/gpud_b200_hooks.h): the host plan of one gpud_ring_reduce_ranges.
+extern "C" int32_t gpudh_ring_ranges_plan(int64_t total, int64_t cap, int32_t n_fields, int32_t q_num, int32_t q_den, const int64_t* first, const int64_t* len,
+                                          int64_t n_ranges, int64_t* start, int32_t* route, int64_t* tiles, int64_t tiles_cap, int64_t* n_tiles) {
+  if (n_ranges < 0 || cap < 2 || (cap & 1) || total < 0 || n_fields < 1 || q_den <= 0 || q_num < 0 || q_num > q_den || !n_tiles) return GPUD_E_INVALID;
+  if (n_ranges == 0) { *n_tiles = 0; return GPUD_OK; }
+  if (!first || !len || !start || !route || n_ranges > GPUD_RANGES_MAX_SEGMENTS / n_fields) return GPUD_E_INVALID;
+  RangesPlan pl;
+  if (ranges_plan(nullptr, &total, 1, nullptr, cap, n_fields, q_num, q_den, 0.5, ring_smp_shift(cap), first, len, n_ranges, nullptr, n_ranges, &pl))
+    return GPUD_E_INVALID;
+  std::copy(pl.start.begin(), pl.start.end(), start);
+  std::copy(pl.route.begin(), pl.route.end(), route);
+  *n_tiles = pl.tiles0.back();
+  if (*n_tiles > tiles_cap || (*n_tiles && !tiles)) return GPUD_E_CAPACITY;
+  for (size_t b = 0; b + 1 < pl.batch0.size(); ++b)
+    for (int64_t j = pl.batch0[b]; j < pl.batch0[b + 1]; ++j) {
+      const gpud_range_geo& g = pl.geo[j];
+      for (int64_t t = 0; t * GPUD_MAX_WINDOW < g.n; ++t) {
+        int64_t* o = tiles + 3 * (pl.tiles0[b] + g.tile0 + t);
+        o[0] = g.id;
+        o[1] = (g.start + t * GPUD_MAX_WINDOW) % cap;
+        o[2] = std::min<int64_t>(GPUD_MAX_WINDOW, g.n - t * GPUD_MAX_WINDOW);
+      }
+    }
+  return GPUD_OK;
+}
+
+// Test hooks (include/gpud_b200_hooks.h): the host plan of one gpud_rings_reduce_range_sets over n_rings rings of totals[] pushed samples,
+// and the ring and column of each piece and of each pivot read.  gpudh_ring_range_sets_plan is the one-ring case without those.
+extern "C" int32_t gpudh_rings_range_sets_plan(const int64_t* totals, int32_t n_rings, int64_t cap, int32_t n_fields, int32_t q_num, int32_t q_den,
+                                               const int32_t* ring_of, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off,
+                                               int64_t n_sets, int32_t* route, int64_t* pieces, int64_t* tiles, int64_t tiles_cap, int64_t* n_tiles,
+                                               int32_t* piv_n, int64_t* piv_cols, int32_t* piv_rings) {
+  if (!totals || n_rings < 1 || n_rings > GPUD_PIECE_RINGS || n_ranges < 0 || n_sets < 0 || cap < 2 || (cap & 1) || n_fields < 1 || q_den <= 0 || q_num < 0 || q_num > q_den || !n_tiles)
+    return GPUD_E_INVALID;
+  for (int i = 0; i < n_rings; ++i) if (totals[i] < 0) return GPUD_E_INVALID;
+  if (n_sets == 0) { *n_tiles = 0; return GPUD_OK; }
+  if (!first || !len || !set_off || !route || n_sets > GPUD_RANGES_MAX_SEGMENTS / n_fields || (n_rings > 1 && !ring_of)) return GPUD_E_INVALID;
+  RangesPlan pl;
+  if (ranges_plan(nullptr, totals, n_rings, ring_of, cap, n_fields, q_num, q_den, 0.5, ring_smp_shift(cap), first, len, n_ranges, set_off, n_sets, &pl))
+    return GPUD_E_INVALID;
+  std::copy(pl.route.begin(), pl.route.end(), route);
+  *n_tiles = pl.tiles0.back();
+  if (*n_tiles > tiles_cap || (*n_tiles && !tiles)) return GPUD_E_CAPACITY;
+  if (pieces) {                        // per range {ring, column, offset in its set}: a set without pieces is one run of the home ring
+    for (int64_t i = 0; i < n_ranges; ++i) { pieces[3 * i] = 0; pieces[3 * i + 1] = pl.start[i]; pieces[3 * i + 2] = 0; }
+    for (int64_t s = 0, q = 0; s < n_sets; ++s) {
+      const int64_t a = set_off[s], e = set_off[s + 1];
+      const bool has = e - a > 1 || (ring_of && ring_of[a] != 0);
+      for (int64_t i = a; has && i < e; ++i, ++q) { pieces[3 * i] = gpud_piece_ring(pl.pieces[q]); pieces[3 * i + 1] = gpud_piece_start(pl.pieces[q]); pieces[3 * i + 2] = pl.pieces[q].off; }
+    }
+  }
+  if (piv_n) std::fill(piv_n, piv_n + n_sets, 0);
+  for (size_t b = 0; b + 1 < pl.batch0.size(); ++b)
+    for (int64_t j = pl.batch0[b]; j < pl.batch0[b + 1]; ++j) {
+      const gpud_range_geo& g = pl.geo[j];
+      const gpud_piece* p = g.np ? pl.pieces.data() + pl.p0[j] : nullptr;
+      const int64_t nt = (g.n + GPUD_MAX_WINDOW - 1) / GPUD_MAX_WINDOW, np = g.np ? (int64_t)g.np : 1;
+      std::vector<int64_t> tp(nt, 0);
+      if (p) tile_pieces(g, p, tp.data());
+      for (int64_t t = 0; t < nt; ++t) {
+        const int64_t off = t * GPUD_MAX_WINDOW, m = std::min<int64_t>(GPUD_MAX_WINDOW, g.n - off);
+        int64_t i = tp[t];
+        while (p && i < np && p[i].off < off + m) ++i;
+        int64_t* o = tiles + 5 * (pl.tiles0[b] + g.tile0 + t);
+        o[0] = g.id;
+        o[1] = off;
+        o[2] = m;
+        o[3] = set_off[g.id] + tp[t];
+        o[4] = p ? i - tp[t] : 1;
+      }
+      if (piv_n && !g.smp) {
+        piv_n[g.id] = g.S;
+        for (int64_t k = 0; (piv_cols || piv_rings) && k < g.S; ++k) {
+          const int64_t c = k * g.stride + (g.stride >> 1), o = g.id * GPUD_RANGE_SAMPLE_MAX + k;
+          const gpud_piece* q = p ? &p[gpud_piece_at(p, 0, np, c)] : nullptr;
+          if (piv_cols) piv_cols[o] = q ? gpud_piece_col(*q, c, cap) : (g.start + c) % cap;
+          if (piv_rings) piv_rings[o] = q ? gpud_piece_ring(*q) : 0;
+        }
+      }
+    }
+  return GPUD_OK;
+}
+
+extern "C" int32_t gpudh_ring_range_sets_plan(int64_t total, int64_t cap, int32_t n_fields, int32_t q_num, int32_t q_den, const int64_t* first,
+                                              const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets, int32_t* route, int64_t* tiles,
+                                              int64_t tiles_cap, int64_t* n_tiles, int32_t* piv_n, int64_t* piv_cols) {
+  return gpudh_rings_range_sets_plan(&total, 1, cap, n_fields, q_num, q_den, nullptr, first, len, n_ranges, set_off, n_sets, route, nullptr, tiles, tiles_cap,
+                                     n_tiles, piv_n, piv_cols, nullptr);
+}

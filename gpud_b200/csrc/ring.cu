@@ -1839,41 +1839,41 @@ int32_t gpud_ring_window_pass(gpud_ring* r, int64_t start, int64_t n, int Wp, do
   return GPUD_OK;
 }
 
-// ---- gpud_ring_reduce_ranges: the launches of its routes (select.cu plans them; internal.h says what goes in and out) ----
+// ---- gpud_ring_reduce_ranges: the launches of its routes (ranges.cu plans them; internal.h says what goes in and out) ----
 // Both warp kernels take a grid of kCtasPerSM CTAs per SM at most and walk their units grid-strided.
-static int ranges_grid(const gpud_ring* r, int64_t units) {
-  return (int)std::max<int64_t>(1, std::min<int64_t>((units + kWarpsPerBlock - 1) / kWarpsPerBlock, (int64_t)r->sm_count * kCtasPerSM));
+static int ranges_grid(const gpud_ring_view& v, int64_t units) {
+  return (int)std::max<int64_t>(1, std::min<int64_t>((units + kWarpsPerBlock - 1) / kWarpsPerBlock, (int64_t)v.sm_count * kCtasPerSM));
 }
 
-cudaError_t gpud_ranges_short(gpud_ring* r, const gpud_short_range* rs, int n_short, const gpud_piece* pieces, const gpud_ring_src* srcs, int64_t n_out,
-                              double* out, uint32_t* nover) {
+cudaError_t gpud_ranges_short(const gpud_ring_view& v, const gpud_short_range* rs, int n_short, const gpud_piece* pieces, const gpud_ring_src* srcs,
+                              int64_t n_out, double* out, uint32_t* nover) {
   const auto k = srcs ? k_ranges_short<true> : k_ranges_short<false>;
   const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kBlockSmemBytes);
   if (e != cudaSuccess) return e;
-  k<<<ranges_grid(r, (int64_t)r->F * n_short), kWarpsPerBlock * 32, kBlockSmemBytes, r->stream>>>(
-      r->d_ring, r->cap, r->F, rs, n_short, pieces, n_out, r->d_thr, r->d_pw, pow(1.0 - r->alpha, 64.0), r->alpha, r->q_num, r->q_den, out, nover, srcs);
+  k<<<ranges_grid(v, (int64_t)v.F * n_short), kWarpsPerBlock * 32, kBlockSmemBytes, v.stream>>>(
+      v.d_ring, v.cap, v.F, rs, n_short, pieces, n_out, v.d_thr, v.d_pw, pow(1.0 - v.alpha, 64.0), v.alpha, v.q_num, v.q_den, out, nover, srcs);
   return cudaGetLastError();
 }
 
-cudaError_t gpud_ranges_tiles(gpud_ring* r, const gpud_range_geo* geo, int64_t n_long, const int32_t* tile_range, int64_t n_tiles, const double* piv,
+cudaError_t gpud_ranges_tiles(const gpud_ring_view& v, const gpud_range_geo* geo, int64_t n_long, const int32_t* tile_range, int64_t n_tiles, const double* piv,
                               double* const w[5], uint32_t* w_nover, uint4* w_cls, unsigned long long* lists, int64_t list_row, unsigned* fill,
                               const gpud_piece* pieces, const int64_t* seg_p0, const int64_t* tile_piece, const gpud_ring_src* srcs) {
   const auto k = srcs ? k_ranges_tiles<true> : k_ranges_tiles<false>;
   const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kBlockSmemBytes);
   if (e != cudaSuccess) return e;
-  k<<<ranges_grid(r, (int64_t)r->F * n_tiles), kWarpsPerBlock * 32, kBlockSmemBytes, r->stream>>>(
-      r->d_ring, r->cap, r->F, geo, n_long, tile_range, n_tiles, r->d_thr, r->d_pw, pow(1.0 - r->alpha, 64.0), r->alpha, piv, w[0], w[1], w[2], w[4],
+  k<<<ranges_grid(v, (int64_t)v.F * n_tiles), kWarpsPerBlock * 32, kBlockSmemBytes, v.stream>>>(
+      v.d_ring, v.cap, v.F, geo, n_long, tile_range, n_tiles, v.d_thr, v.d_pw, pow(1.0 - v.alpha, 64.0), v.alpha, piv, w[0], w[1], w[2], w[4],
       w_nover, w_cls, lists, list_row, fill, pieces, seg_p0, tile_piece, srcs);
   return cudaGetLastError();
 }
 
 // the guard choice of launch_ema_carry, for tiles of GPUD_MAX_WINDOW samples
-cudaError_t gpud_ranges_ema(gpud_ring* r, const gpud_range_geo* geo, int64_t n_long, const double* part, int64_t n_tiles, double* ema,
+cudaError_t gpud_ranges_ema(const gpud_ring_view& v, const gpud_range_geo* geo, int64_t n_long, const double* part, int64_t n_tiles, double* ema,
                             const gpud_piece* pieces, const int64_t* seg_p0, const gpud_ring_src* srcs) {
-  const double d_full = pow(1.0 - r->alpha, (double)GPUD_MAX_WINDOW);
-  const unsigned grid = (unsigned)((int64_t)r->F * n_long);
+  const double d_full = pow(1.0 - v.alpha, (double)GPUD_MAX_WINDOW);
+  const unsigned grid = (unsigned)((int64_t)v.F * n_long);
   const bool guard = pow(d_full, 128.0) < 0x1p-900;
   const auto k = srcs ? (guard ? k_ranges_ema<true, true> : k_ranges_ema<false, true>) : (guard ? k_ranges_ema<true, false> : k_ranges_ema<false, false>);
-  k<<<grid, 128, 0, r->stream>>>(part, n_tiles, geo, n_long, r->d_ring, r->cap, d_full, ema, pieces, seg_p0, srcs);
+  k<<<grid, 128, 0, v.stream>>>(part, n_tiles, geo, n_long, v.d_ring, v.cap, d_full, ema, pieces, seg_p0, srcs);
   return cudaGetLastError();
 }
