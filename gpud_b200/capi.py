@@ -1348,26 +1348,29 @@ class Ring:
         self.ctx._check(self._L.gpud_ring_checkpoint_bound(self._h, C.byref(n)))
         return n.value
 
-    def checkpoint(self, out=None):
-        """gpud_ring_checkpoint.  out None: -> the checkpoint as bytes.  Otherwise a writable buffer (bytearray, numpy array, pinned
-        memory as a ctypes array) that receives it: -> its length in bytes."""
+    def _write_blob(self, write, bound, out):
+        """one checkpoint call, full or delta: out None -> the bytes, sized by bound(); otherwise into out -> their length"""
         n = C.c_int64()
         if out is None:
-            buf = bytearray(self.checkpoint_bound())
-            cbuf = (C.c_char * len(buf)).from_buffer(buf)
-            self.ctx._check(self._L.gpud_ring_checkpoint(self._h, C.cast(cbuf, C.c_void_p), len(buf), C.byref(n)))
+            buf = bytearray(bound())
+            cbuf = (C.c_char * max(1, len(buf))).from_buffer(buf)
+            self.ctx._check(write(self._h, C.cast(cbuf, C.c_void_p), len(buf), C.byref(n)))
             del cbuf
             return bytes(memoryview(buf)[:n.value])
         mv = memoryview(out).cast("B")
         cbuf = (C.c_char * len(mv)).from_buffer(mv)
-        self.ctx._check(self._L.gpud_ring_checkpoint(self._h, C.cast(cbuf, C.c_void_p), len(mv), C.byref(n)))
+        self.ctx._check(write(self._h, C.cast(cbuf, C.c_void_p), len(mv), C.byref(n)))
         return n.value
+
+    def checkpoint(self, out=None):
+        """gpud_ring_checkpoint.  out None: -> the checkpoint as bytes.  Otherwise a writable buffer (bytearray, numpy array, pinned
+        memory as a ctypes array) that receives it: -> its length in bytes."""
+        return self._write_blob(self._L.gpud_ring_checkpoint, self.checkpoint_bound, out)
 
     def restore(self, blob) -> List["RingWindows"]:
         """gpud_ring_restore into this ring (just created with the checkpoint's config, never pushed into, no handle open): -> the
         windows handles in the order they had been opened.  The stream handle, if there was one, is open again on the ring."""
-        mv = memoryview(blob).cast("B")
-        src = C.c_void_p(np.frombuffer(mv, dtype=np.uint8).ctypes.data) if len(mv) else None
+        mv, src = _blob_ptr(blob)
         recs = checkpoint_handles(mv)
         cap = sum(1 for kind, _, _ in recs if kind == 1)
         hs = (C.c_void_p * max(1, cap))()
@@ -1385,22 +1388,11 @@ class Ring:
     def checkpoint_delta(self, out=None):
         """gpud_ring_checkpoint_delta: everything since the ring's chain marker, which then moves to this delta.  out None: -> the
         delta as bytes.  Otherwise a writable buffer (bytearray, numpy array, pinned memory as a ctypes array): -> its length."""
-        n = C.c_int64()
-        if out is None:
-            buf = bytearray(self.checkpoint_delta_bound())
-            cbuf = (C.c_char * max(1, len(buf))).from_buffer(buf)
-            self.ctx._check(self._L.gpud_ring_checkpoint_delta(self._h, C.cast(cbuf, C.c_void_p), len(buf), C.byref(n)))
-            del cbuf
-            return bytes(memoryview(buf)[:n.value])
-        mv = memoryview(out).cast("B")
-        cbuf = (C.c_char * len(mv)).from_buffer(mv)
-        self.ctx._check(self._L.gpud_ring_checkpoint_delta(self._h, C.cast(cbuf, C.c_void_p), len(mv), C.byref(n)))
-        return n.value
+        return self._write_blob(self._L.gpud_ring_checkpoint_delta, self.checkpoint_delta_bound, out)
 
     def restore_delta(self, blob) -> None:
         """gpud_ring_restore_delta: apply the next delta of the chain onto this ring (a base restored, the deltas before it applied)"""
-        mv = memoryview(blob).cast("B")
-        src = C.c_void_p(np.frombuffer(mv, dtype=np.uint8).ctypes.data) if len(mv) else None
+        mv, src = _blob_ptr(blob)
         self.ctx._check(self._L.gpud_ring_restore_delta(self._h, src, len(mv)))
 
     def checkpoint_stats(self):
@@ -1441,6 +1433,12 @@ class Ring:
     def tier_group(self, max_fields: int):
         """test hook gpudh_ring_tier_group: at most max_fields fields per decoded group (0: the default)"""
         self.ctx._check(self._L.gpudh_ring_tier_group(self._h, max_fields))
+
+
+def _blob_ptr(blob):
+    """a checkpoint's bytes as a byte view and the pointer the restore calls take (None for no bytes)"""
+    mv = memoryview(blob).cast("B")
+    return mv, C.c_void_p(np.frombuffer(mv, dtype=np.uint8).ctypes.data) if len(mv) else None
 
 
 def checkpoint_handles(blob) -> List[tuple]:

@@ -11,6 +11,12 @@
 // and width and adds the field checksums, an exclusive scan of the block sizes places the blocks, k_ckpt_pack re-reads the ring and
 // writes each block at its offset.  Decode: k_ckpt_unpack writes the ring and its sample ring from offsets the host computed out of
 // the validated directory, so no address comes from payload bits.  A delta runs the same kernels on the run of samples it holds.
+// The tier launches them too; launch_size, launch_pack and launch_unpack own their grids.
+//
+// Both kinds of blob share one frame, and one host path each way handles both: write_blob writes either; read_frame checks either
+// against the ring in one order, load_samples decodes its samples and finish_restore sets the ring's marker and stats.  What tells
+// the kinds apart is data wherever it can be: the magic, the four header words at 32, the thresholds section, the head words of a
+// handle record, where its body starts and the link's predecessor.
 #include <math.h>
 #include <string.h>
 
@@ -26,10 +32,9 @@ constexpr int kBlock = 1024;                        // samples per coded block
 constexpr int kCkThreads = 256;                     // k_ckpt_size / k_ckpt_unpack: 8 warps, one block each at a time
 constexpr int kPackWarps = 4;                       // k_ckpt_pack: 8 KB of residuals per warp in shared memory
 constexpr uint64_t kGolden = 0x9E3779B97F4A7C15ull;
-constexpr char kMagic[8] = {'G', 'P', 'U', 'D', 'R', 'C', 'K', '1'};
-constexpr char kDeltaMagic[8] = {'G', 'P', 'U', 'D', 'R', 'C', 'D', '1'};
+constexpr char kMagic[2][8] = {{'G', 'P', 'U', 'D', 'R', 'C', 'K', '1'}, {'G', 'P', 'U', 'D', 'R', 'C', 'D', '1'}};   // [delta]
 constexpr uint32_t kVersion = 1;                    // of both formats
-constexpr int64_t kHeaderBytes = 128, kHandleHeadBytes = 64, kDeltaHeadBytes = 80;
+constexpr int64_t kHeaderBytes = 128;
 enum { kKindStream = 0, kKindWindows = 1 };
 
 __host__ __device__ __forceinline__ uint64_t mix64(uint64_t z) {   // the splitmix64 finalizer
@@ -217,7 +222,7 @@ __global__ void __launch_bounds__(kCkThreads) k_ckpt_unpack(const CkGeo g, const
 }
 
 // ---- host ----
-int64_t pad8(int64_t x) { return (x + 7) & ~(int64_t)7; }
+__host__ __device__ __forceinline__ int64_t pad8(int64_t x) { return (x + 7) & ~(int64_t)7; }
 // one handle's record after its head: [5][F][n] f64 history, [F][n] u32 n_over (padded to 8 bytes), [F] f64 EMA state
 int64_t handle_body_bytes(int64_t F, int64_t n) { return 40 * F * n + pad8(4 * F * n) + 8 * F; }
 
@@ -229,20 +234,20 @@ std::vector<gpud_ring_windows*> ckpt_handles(const gpud_ring* r) {
   return v;
 }
 
-int64_t handles_bytes(const gpud_ring* r) {
-  int64_t n = 0;
-  for (const gpud_ring_windows* s : ckpt_handles(r)) n += kHandleHeadBytes + handle_body_bytes(r->F, s->next - s->first);
-  return n;
-}
+// What sets a delta's frame apart from a full checkpoint's: five sections or four (no thresholds), and eight head words per handle
+// record or ten (prev_next, from).
+int n_sections(bool delta) { return delta ? 4 : 5; }
+int head_words(bool delta) { return delta ? 10 : 8; }
 
-// A delta's samples start at its first_d = max(marker total, total - CAP), and each handle's record holds windows [from, next) with
-// from = max(first, next at the marker).
-int64_t delta_first(const gpud_ring* r) { return std::max(r->ck_total, r->total - r->cap); }
-int64_t delta_from(const gpud_ring_windows* s) { return std::max(s->first, s->ck_next); }
+// A blob's samples are [first, total): a full checkpoint holds the ring's, a delta those since its marker, first_d = max(marker total,
+// total - CAP).  Each handle's record holds windows [from, next): all of them in a full checkpoint, from = max(first, next at the
+// marker) in a delta.
+int64_t blob_first(const gpud_ring* r, bool delta) { return std::max(delta ? r->ck_total : 0, r->total - r->cap); }
+int64_t body_from(const gpud_ring_windows* s, bool delta) { return delta ? std::max(s->first, s->ck_next) : s->first; }
 
-int64_t delta_handles_bytes(const gpud_ring* r) {
+int64_t handles_bytes(const gpud_ring* r, bool delta) {
   int64_t n = 0;
-  for (const gpud_ring_windows* s : ckpt_handles(r)) n += kDeltaHeadBytes + handle_body_bytes(r->F, s->next - delta_from(s));
+  for (const gpud_ring_windows* s : ckpt_handles(r)) n += 8 * head_words(delta) + handle_body_bytes(r->F, s->next - body_from(s, delta));
   return n;
 }
 
@@ -291,6 +296,24 @@ int ckpt_grid(const gpud_ring* r, int64_t units, int warps_per_cta) {
   int64_t most = (int64_t)r->sm_count * 16;
   if (r->ck_grid_max > 0) most = std::min<int64_t>(most, r->ck_grid_max);
   return (int)std::max<int64_t>(1, std::min<int64_t>((units + warps_per_cta - 1) / warps_per_cta, most));
+}
+
+// The codec kernels' launches on the ring's stream, for checkpoints and the tier alike: each sizes its grid by the blocks of g.
+cudaError_t launch_size(const gpud_ring* r, const CkGeo& g, uint8_t* dir, unsigned long long* words, unsigned long long* csum) {
+  k_ckpt_size<<<ckpt_grid(r, (int64_t)g.F * g.nb, kCkThreads / 32), kCkThreads, 0, r->stream>>>(g, dir, words, csum);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_pack(const gpud_ring* r, const CkGeo& g, const uint8_t* dir, const unsigned long long* offs, unsigned long long* payload) {
+  k_ckpt_pack<<<ckpt_grid(r, (int64_t)g.F * g.nb, kPackWarps), kPackWarps * 32, 0, r->stream>>>(g, dir, offs, payload);
+  return cudaGetLastError();
+}
+
+template <bool kStore>
+cudaError_t launch_unpack(const gpud_ring* r, const CkGeo& g, const uint8_t* dir, const unsigned long long* offs, const unsigned long long* payload,
+                          unsigned long long* csum) {
+  k_ckpt_unpack<kStore><<<ckpt_grid(r, (int64_t)g.F * g.nb, kCkThreads / 32), kCkThreads, 0, r->stream>>>(g, dir, offs, payload, csum);
+  return cudaGetLastError();
 }
 
 // Samples [first, first + count) of the push order, first >= total - CAP.
@@ -456,8 +479,7 @@ struct Encoder {
       return gpud_fail(r->ctx, e == cudaErrorMemoryAllocation ? GPUD_E_NOMEM : GPUD_E_CUDA, "%s: %s", what, cudaGetErrorString(e));
     GPUD_CUDA(r->ctx, cudaMemsetAsync(d_csum, 0, F * sizeof(unsigned long long), r->stream));
     GPUD_CUDA(r->ctx, cudaEventRecord(ev[0], r->stream));
-    k_ckpt_size<<<ckpt_grid(r, units, kCkThreads / 32), kCkThreads, 0, r->stream>>>(g, d_dir, d_words, d_csum);
-    GPUD_CUDA(r->ctx, cudaGetLastError());
+    GPUD_CUDA(r->ctx, launch_size(r, g, d_dir, d_words, d_csum));
     GPUD_CUDA(r->ctx, cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_words, d_offs, (int)units, r->stream));
     GPUD_CUDA(r->ctx, cudaEventRecord(ev[1], r->stream));
     unsigned long long last[2];
@@ -474,8 +496,7 @@ struct Encoder {
     if (e != cudaSuccess)
       return gpud_fail(r->ctx, e == cudaErrorMemoryAllocation ? GPUD_E_NOMEM : GPUD_E_CUDA, "%s: %s", what, cudaGetErrorString(e));
     GPUD_CUDA(r->ctx, cudaEventRecord(ev[2], r->stream));
-    k_ckpt_pack<<<ckpt_grid(r, units, kPackWarps), kPackWarps * 32, 0, r->stream>>>(g, d_dir, d_offs, d_payload);
-    GPUD_CUDA(r->ctx, cudaGetLastError());
+    GPUD_CUDA(r->ctx, launch_pack(r, g, d_dir, d_offs, d_payload));
     GPUD_CUDA(r->ctx, cudaEventRecord(ev[3], r->stream));
     GPUD_CUDA(r->ctx, cudaMemcpyAsync(dir.data(), d_dir, units, cudaMemcpyDeviceToHost, r->stream));
     GPUD_CUDA(r->ctx, cudaMemcpyAsync(csum.data(), d_csum, r->F * 8, cudaMemcpyDeviceToHost, r->stream));
@@ -547,10 +568,8 @@ struct Decoder {
   // one decode pass between events ev[e0] and ev[e0 + 1]; -> the re-formed field checksums
   template <bool kStore>
   int32_t run(gpud_ring* r, const CkGeo& g, int e0, std::vector<uint64_t>& csum) {
-    const int64_t units = (int64_t)g.F * g.nb;
     GPUD_CUDA(r->ctx, cudaEventRecord(ev[e0], r->stream));
-    k_ckpt_unpack<kStore><<<ckpt_grid(r, units, kCkThreads / 32), kCkThreads, 0, r->stream>>>(g, d_dir, d_offs, d_payload, d_csum);
-    GPUD_CUDA(r->ctx, cudaGetLastError());
+    GPUD_CUDA(r->ctx, launch_unpack<kStore>(r, g, d_dir, d_offs, d_payload, d_csum));
     GPUD_CUDA(r->ctx, cudaEventRecord(ev[e0 + 1], r->stream));
     csum.resize(g.F);
     GPUD_CUDA(r->ctx, cudaMemcpyAsync(csum.data(), d_csum, g.F * 8, cudaMemcpyDeviceToHost, r->stream));
@@ -565,85 +584,91 @@ struct Decoder {
   }
 };
 
-struct CkHandle { int64_t kind, span, hop, H, first, next, lost, reseed, prev_next, from, off; };
-
-}  // namespace
-
-extern "C" int32_t gpud_ring_checkpoint_bound(gpud_ring* r, int64_t* bytes) {
-  if (!r || !bytes) return GPUD_E_INVALID;
-  const int64_t F = r->F, count = ring_count(r), nb = (count + kBlock - 1) / kBlock;
-  *bytes = kHeaderBytes + 8 * F + pad8(F * nb) + 8 * F * count + 8 * F + handles_bytes(r);
-  return GPUD_OK;
-}
-
-extern "C" int32_t gpud_ring_checkpoint(gpud_ring* r, void* out_v, int64_t cap, int64_t* n_bytes) {
+// Both kinds of checkpoint.  A delta follows the ring's chain marker and needs the handles the marker saw.
+int32_t write_blob(gpud_ring* r, bool delta, void* out_v, int64_t cap, int64_t* n_bytes) {
   if (!r || !n_bytes || cap < 0 || (cap > 0 && !out_v)) return GPUD_E_INVALID;
   uint8_t* out = (uint8_t*)out_v;
+  const char* what = delta ? "checkpoint_delta" : "checkpoint";
+  if (delta && !r->ck_marked) return gpud_fail(r->ctx, GPUD_E_STATE, "checkpoint_delta: no checkpoint written or restored on this ring yet");
+  if (delta && r->handle_gen != r->ck_gen)
+    return gpud_fail(r->ctx, GPUD_E_STATE, "checkpoint_delta: a handle was opened or closed since the last checkpoint: write a full one");
   GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
   GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));
-  const int64_t F = r->F, count = ring_count(r);
+  const int64_t F = r->F, first = blob_first(r, delta), count = r->total - first;
   Encoder en;
-  { const int32_t rc = en.size(r, r->total - count, count, "checkpoint"); if (rc) return rc; }
-  const int64_t units = en.units, dir_bytes = pad8(units), pay_bytes = 8 * en.words, hnd_bytes = handles_bytes(r);
-  const int64_t thr_off = kHeaderBytes, dir_off = thr_off + 8 * F, pay_off = dir_off + dir_bytes, sum_off = pay_off + pay_bytes,
-                hnd_off = sum_off + 8 * F, size = hnd_off + hnd_bytes;
+  { const int32_t rc = en.size(r, first, count, what); if (rc) return rc; }
+  // the sections in blob order; a delta has no thresholds section
+  const int64_t sec[5] = {delta ? 0 : 8 * F, pad8(en.units), 8 * en.words, 8 * F, handles_bytes(r, delta)};
+  const int64_t dir_off = kHeaderBytes + sec[0], pay_off = dir_off + sec[1], sum_off = pay_off + sec[2], hnd_off = sum_off + sec[3],
+                size = hnd_off + sec[4];
   *n_bytes = size;
-  if (cap < size) return gpud_fail(r->ctx, GPUD_E_CAPACITY, "checkpoint needs %lld bytes", (long long)size);
+  if (cap < size) return gpud_fail(r->ctx, GPUD_E_CAPACITY, "%s needs %lld bytes", what, (long long)size);
   bool pinned = false;
   { const int32_t rc = host_pinned(r, out, &pinned); if (rc) return rc; }
-  { const int32_t rc = en.pack(r, out + pay_off, pinned, "checkpoint"); if (rc) return rc; }
+  { const int32_t rc = en.pack(r, out + pay_off, pinned, what); if (rc) return rc; }
   const std::vector<gpud_ring_windows*> hs = ckpt_handles(r);
-  // header
+  // header: the kind's four words at 32 are α's bits, q_num and q_den (i32 each), total and count in a full checkpoint, and
+  // prev_total, total, first_d and prev_link in a delta
+  const int64_t kind_words[2][4] = {{get<int64_t>((const uint8_t*)&r->alpha, 0), (int64_t)((uint32_t)r->q_num | (uint64_t)(uint32_t)r->q_den << 32), r->total, count},
+                                    {r->ck_total, r->total, first, (int64_t)r->ck_link}};
   memset(out, 0, kHeaderBytes);
-  memcpy(out, kMagic, 8);
+  memcpy(out, kMagic[delta], 8);
   put<uint32_t>(out, 8, kVersion);
   put<uint32_t>(out, 12, (uint32_t)F);
   put<uint32_t>(out, 16, (uint32_t)r->W);
   put<uint32_t>(out, 20, (uint32_t)hs.size());
   put<int64_t>(out, 24, r->cap);
-  put<double>(out, 32, r->alpha);
-  put<int32_t>(out, 40, r->q_num);
-  put<int32_t>(out, 44, r->q_den);
-  put<int64_t>(out, 48, r->total);
-  put<int64_t>(out, 56, count);
-  put<int64_t>(out, 64, 8 * F);
-  put<int64_t>(out, 72, dir_bytes);
-  put<int64_t>(out, 80, pay_bytes);
-  put<int64_t>(out, 88, 8 * F);
-  put<int64_t>(out, 96, hnd_bytes);
-  memcpy(out + thr_off, r->thr.data(), 8 * F);
-  memset(out + dir_off, 0, dir_bytes);
-  memcpy(out + dir_off, en.dir.data(), units);
+  memcpy(out + 32, kind_words[delta], 32);
+  const int ns = n_sections(delta);
+  for (int i = 0; i < ns; ++i) put<int64_t>(out, 64 + 8 * i, sec[5 - ns + i]);
+  memcpy(out + kHeaderBytes, r->thr.data(), sec[0]);
+  memset(out + dir_off, 0, sec[1]);
+  memcpy(out + dir_off, en.dir.data(), en.units);
   memcpy(out + sum_off, en.csum.data(), 8 * F);
   // handles
+  const int nh = head_words(delta);
   int64_t off = hnd_off;
   std::vector<int64_t> heads;
   for (gpud_ring_windows* s : hs) {
-    const int64_t head[8] = {s == r->swin ? kKindStream : kKindWindows, s->span, s->hop, s->H, s->first, s->next, s->lost, s->reseed ? 1 : 0};
-    memcpy(out + off, head, sizeof head);
-    heads.insert(heads.end(), head, head + 8);
-    { const int32_t rc = write_handle_body(r, s, s->first, out + off + kHandleHeadBytes); if (rc) return rc; }
-    off += kHandleHeadBytes + handle_body_bytes(F, s->next - s->first);
+    const int64_t from = body_from(s, delta);
+    const int64_t head[10] = {s == r->swin ? kKindStream : kKindWindows, s->span, s->hop, s->H, s->first, s->next, s->lost, s->reseed ? 1 : 0,
+                              s->ck_next, from};
+    memcpy(out + off, head, 8 * nh);
+    heads.insert(heads.end(), head, head + nh);
+    { const int32_t rc = write_handle_body(r, s, from, out + off + 8 * nh); if (rc) return rc; }
+    off += 8 * nh + handle_body_bytes(F, s->next - from);
   }
   en.stats(r);
-  set_marker(r, r->total, chain_link(0, r->total, en.csum.data(), F, heads));
+  set_marker(r, r->total, chain_link(delta ? r->ck_link : 0, r->total, en.csum.data(), F, heads));
   return GPUD_OK;
 }
 
-extern "C" int32_t gpud_ring_restore(gpud_ring* r, const void* in_v, int64_t n_bytes, gpud_ring_windows** handles, int32_t cap_handles,
-                                     int32_t* n_handles) {
-  if (!r || (!in_v && n_bytes) || n_bytes < 0 || cap_handles < 0 || (cap_handles > 0 && !handles)) return GPUD_E_INVALID;
-  const uint8_t* in = (const uint8_t*)in_v;
+// Every block coded at 64 bits (a block of n samples takes n words), and the other sections.
+int32_t blob_bound(gpud_ring* r, bool delta, int64_t* bytes) {
+  if (!r || !bytes) return GPUD_E_INVALID;
+  const int64_t F = r->F, count = r->total - blob_first(r, delta), nb = (count + kBlock - 1) / kBlock;
+  *bytes = kHeaderBytes + (delta ? 0 : 8 * F) + pad8(F * nb) + 8 * F * count + 8 * F + handles_bytes(r, delta);
+  return GPUD_OK;
+}
+
+struct CkHandle { int64_t kind, span, hop, H, first, next, lost, reseed, prev_next, from, off; };
+
+// A blob whose frame checked out against the ring it goes into: its samples [first, total), where its sections are, and its handle
+// records, each with its head words for the chain link.
+struct Frame {
+  int64_t total = 0, first = 0, count = 0, units = 0, n_int = 0, pay_bytes = 0;
+  uint64_t prev_link = 0;                       // the link the blob follows: 0 for a full checkpoint
+  const uint8_t *dir = nullptr, *payload = nullptr, *sums = nullptr;
+  std::vector<unsigned long long> offs;         // each block's offset in words, from the directory
+  std::vector<gpud_ring_windows*> hs;           // the ring's handles, in checkpoint order: a delta's records follow them
+  std::vector<CkHandle> recs;
+  std::vector<int64_t> heads;
+};
+
+// A full checkpoint goes into a ring created with its config (α, q and every threshold, bit for bit) and not used since.
+int32_t full_target_ok(gpud_ring* r, const uint8_t* in, int64_t n_bytes) {
   gpud_ctx* ctx = r->ctx;
-  // ---- header and config ----
-  if (n_bytes < kHeaderBytes || memcmp(in, kMagic, 8) != 0) return gpud_fail(ctx, GPUD_E_INVALID, "restore: not a ring checkpoint");
-  if (get<uint32_t>(in, 8) != kVersion) return gpud_fail(ctx, GPUD_E_INVALID, "restore: checkpoint version %u, this library reads %u", get<uint32_t>(in, 8), kVersion);
-  for (int i = 104; i < kHeaderBytes; ++i)
-    if (in[i]) return gpud_fail(ctx, GPUD_E_INVALID, "restore: header byte %d is not zero", i);
   const int64_t F = r->F;
-  if (get<uint32_t>(in, 12) != (uint32_t)F) return gpud_fail(ctx, GPUD_E_INVALID, "restore: n_fields %u, the ring has %lld", get<uint32_t>(in, 12), (long long)F);
-  if (get<uint32_t>(in, 16) != (uint32_t)r->W) return gpud_fail(ctx, GPUD_E_INVALID, "restore: window %u, the ring has %d", get<uint32_t>(in, 16), r->W);
-  if (get<int64_t>(in, 24) != r->cap) return gpud_fail(ctx, GPUD_E_INVALID, "restore: capacity %lld, the ring has %lld", (long long)get<int64_t>(in, 24), (long long)r->cap);
   if (get<uint64_t>(in, 32) != get<uint64_t>((const uint8_t*)&r->alpha, 0))
     return gpud_fail(ctx, GPUD_E_INVALID, "restore: ema_alpha %.17g, the ring has %.17g", get<double>(in, 32), r->alpha);
   if (get<int32_t>(in, 40) != r->q_num) return gpud_fail(ctx, GPUD_E_INVALID, "restore: q_num %d, the ring has %d", get<int32_t>(in, 40), r->q_num);
@@ -653,81 +678,194 @@ extern "C" int32_t gpud_ring_restore(gpud_ring* r, const void* in_v, int64_t n_b
   for (int64_t f = 0; f < F; ++f)
     if (get<uint64_t>(in, kHeaderBytes + 8 * f) != get<uint64_t>((const uint8_t*)(r->thr.data() + f), 0))
       return gpud_fail(ctx, GPUD_E_INVALID, "restore: thresholds[%lld] %.17g, the ring has %.17g", (long long)f, get<double>(in, kHeaderBytes + 8 * f), r->thr[f]);
-  // ---- the target ----
   if (r->total != 0) return gpud_fail(ctx, GPUD_E_STATE, "restore: the ring has been pushed into");
   if (r->swin || !r->handles.empty()) return gpud_fail(ctx, GPUD_E_STATE, "restore: the ring has a stream or windows handle open");
   if (r->tier) return gpud_fail(ctx, GPUD_E_STATE, "restore: the ring has a tier (a restored ring has none)");
-  // ---- sections ----
-  const int64_t total = get<int64_t>(in, 48), count = get<int64_t>(in, 56), dir_bytes = get<int64_t>(in, 72), pay_bytes = get<int64_t>(in, 80),
-                sum_bytes = get<int64_t>(in, 88), hnd_bytes = get<int64_t>(in, 96);
-  const uint32_t n_rec = get<uint32_t>(in, 20);
-  if (total < 0 || count != std::min(total, r->cap)) return gpud_fail(ctx, GPUD_E_INVALID, "restore: total %lld and count %lld disagree", (long long)total, (long long)count);
-  const int64_t nb = (count + kBlock - 1) / kBlock, units = F * nb;
-  if (dir_bytes != pad8(units) || sum_bytes != 8 * F || pay_bytes < 0 || (pay_bytes & 7) || hnd_bytes < 0 || pay_bytes > n_bytes || hnd_bytes > n_bytes ||
-      kHeaderBytes + thr_bytes + dir_bytes + pay_bytes + sum_bytes + hnd_bytes != n_bytes)
-    return gpud_fail(ctx, GPUD_E_INVALID, "restore: section lengths do not add up to the %lld bytes given", (long long)n_bytes);
-  const int64_t dir_off = kHeaderBytes + thr_bytes, pay_off = dir_off + dir_bytes, sum_off = pay_off + pay_bytes, hnd_off = sum_off + sum_bytes;
-  std::vector<unsigned long long> offs;
-  int64_t n_int = 0;
-  { const int32_t rc = read_directory(ctx, in + dir_off, units, nb, count, dir_bytes, pay_bytes, offs, &n_int, "restore"); if (rc) return rc; }
-  std::vector<CkHandle> recs;
-  std::vector<int64_t> heads;
-  int64_t off = hnd_off, n_win = 0;
-  for (uint32_t i = 0; i < n_rec; ++i) {
-    if (off + kHandleHeadBytes > n_bytes) return gpud_fail(ctx, GPUD_E_INVALID, "restore: truncated handle %u", i);
-    CkHandle h;
-    int64_t v[8];
-    memcpy(v, in + off, sizeof v);
-    heads.insert(heads.end(), v, v + 8);
-    h.kind = v[0]; h.span = v[1]; h.hop = v[2]; h.H = v[3]; h.first = v[4]; h.next = v[5]; h.lost = v[6]; h.reseed = v[7];
-    h.off = off + kHandleHeadBytes;
-    const bool kind_ok = h.kind == kKindWindows || (h.kind == kKindStream && i == 0 && h.span == 1 && h.hop == 1);
-    const bool shape_ok = h.span >= 1 && h.span <= r->cap / r->W && h.hop >= 1 && h.hop <= h.span && h.span % h.hop == 0;
-    const int64_t L = h.span * r->W, P = h.hop * r->W, complete = total < L ? 0 : (total - L) / P + 1;
-    const bool hist_ok = h.H >= 1 && h.H <= ((int64_t)1 << 40) / F && h.first >= 0 && h.first <= h.next && h.next - h.first <= h.H &&
-                         h.next <= complete && h.lost >= 0 && (h.reseed == 0 || h.reseed == 1);
-    if (!kind_ok || !shape_ok || !hist_ok)
-      return gpud_fail(ctx, GPUD_E_INVALID, "restore: handle %u (kind %lld, span %lld, hop %lld, history %lld, windows [%lld, %lld)) is not one this ring can hold",
-                       i, (long long)h.kind, (long long)h.span, (long long)h.hop, (long long)h.H, (long long)h.first, (long long)h.next);
-    const int64_t body = handle_body_bytes(F, h.next - h.first);
-    if (h.off + body > hnd_off + hnd_bytes) return gpud_fail(ctx, GPUD_E_INVALID, "restore: truncated handle %u", i);
-    off = h.off + body;
-    n_win += h.kind == kKindWindows;
-    recs.push_back(h);
+  return GPUD_OK;
+}
+
+// A delta goes onto a ring at the chain marker of the blob it follows, with the marker's handles, neither pushed into nor committed
+// since.
+int32_t delta_target_ok(gpud_ring* r, const uint8_t* in, const std::vector<gpud_ring_windows*>& hs) {
+  gpud_ctx* ctx = r->ctx;
+  if (!r->ck_marked) return gpud_fail(ctx, GPUD_E_STATE, "restore_delta: no checkpoint written or restored on this ring yet");
+  const uint64_t prev_link = get<uint64_t>(in, 56);
+  if (prev_link != r->ck_link)
+    return gpud_fail(ctx, GPUD_E_INVALID, "restore_delta: the delta follows link %016llx, the ring is at %016llx (out of order, applied twice, or another chain)",
+                     (unsigned long long)prev_link, (unsigned long long)r->ck_link);
+  if (r->handle_gen != r->ck_gen) return gpud_fail(ctx, GPUD_E_STATE, "restore_delta: a handle was opened or closed since the ring's last checkpoint");
+  if (r->total != r->ck_total) return gpud_fail(ctx, GPUD_E_STATE, "restore_delta: the ring has been pushed into since its last checkpoint");
+  for (const gpud_ring_windows* s : hs)
+    if (s->next != s->ck_next) return gpud_fail(ctx, GPUD_E_STATE, "restore_delta: a handle has committed windows since the ring's last checkpoint");
+  return GPUD_OK;
+}
+
+// A full checkpoint's record i: a handle this ring can hold, the stream handle only first.
+int32_t full_record_ok(gpud_ring* r, const CkHandle& h, uint32_t i, int64_t total) {
+  const bool kind_ok = h.kind == kKindWindows || (h.kind == kKindStream && i == 0 && h.span == 1 && h.hop == 1);
+  const bool shape_ok = h.span >= 1 && h.span <= r->cap / r->W && h.hop >= 1 && h.hop <= h.span && h.span % h.hop == 0;
+  const int64_t L = h.span * r->W, P = h.hop * r->W, complete = total < L ? 0 : (total - L) / P + 1;
+  const bool hist_ok = h.H >= 1 && h.H <= ((int64_t)1 << 40) / r->F && h.first >= 0 && h.first <= h.next && h.next - h.first <= h.H &&
+                       h.next <= complete && h.lost >= 0 && (h.reseed == 0 || h.reseed == 1);
+  if (!kind_ok || !shape_ok || !hist_ok)
+    return gpud_fail(r->ctx, GPUD_E_INVALID, "restore: handle %u (kind %lld, span %lld, hop %lld, history %lld, windows [%lld, %lld)) is not one this ring can hold",
+                     i, (long long)h.kind, (long long)h.span, (long long)h.hop, (long long)h.H, (long long)h.first, (long long)h.next);
+  return GPUD_OK;
+}
+
+// A delta's record i: the successor of the ring's handle s.
+int32_t delta_record_ok(gpud_ring* r, const gpud_ring_windows* s, const CkHandle& h, uint32_t i, int64_t total) {
+  const bool same = h.kind == (s == r->swin ? kKindStream : kKindWindows) && h.span == s->span && h.hop == s->hop && h.H == s->H;
+  const int64_t complete = total < s->L ? 0 : (total - s->L) / s->P + 1;
+  const bool hist_ok = h.prev_next == s->ck_next && h.first >= s->first && h.first <= h.next && h.next - h.first <= h.H && h.next >= h.prev_next &&
+                       h.from == std::max(h.first, h.prev_next) && h.next <= complete && h.lost >= 0 && (h.reseed == 0 || h.reseed == 1);
+  if (!same || !hist_ok)
+    return gpud_fail(r->ctx, GPUD_E_INVALID, "restore_delta: handle %u (kind %lld, span %lld, hop %lld, history %lld, windows [%lld, %lld) from %lld) is not this ring's handle's successor",
+                     i, (long long)h.kind, (long long)h.span, (long long)h.hop, (long long)h.H, (long long)h.first, (long long)h.next, (long long)h.from);
+  return GPUD_OK;
+}
+
+// The frame of a blob of either kind, checked against the ring in a fixed order: magic, version and header padding; F, W and CAP;
+// the kind's target (the config of a fresh ring, or the chain); the totals; the section lengths; the directory; the handle records.
+// Nothing is launched.
+int32_t read_frame(gpud_ring* r, const uint8_t* in, int64_t n_bytes, bool delta, Frame* fr) {
+  gpud_ctx* ctx = r->ctx;
+  const char *what = delta ? "restore_delta" : "restore", *noun = delta ? "delta" : "checkpoint";
+  const int ns = n_sections(delta), nh = head_words(delta);
+  if (n_bytes < kHeaderBytes || memcmp(in, kMagic[delta], 8) != 0)
+    return gpud_fail(ctx, GPUD_E_INVALID, "%s: not a ring %s", what, delta ? "delta checkpoint" : "checkpoint");
+  if (get<uint32_t>(in, 8) != kVersion)
+    return gpud_fail(ctx, GPUD_E_INVALID, "%s: %s version %u, this library reads %u", what, noun, get<uint32_t>(in, 8), kVersion);
+  for (int i = 64 + 8 * ns; i < kHeaderBytes; ++i)
+    if (in[i]) return gpud_fail(ctx, GPUD_E_INVALID, "%s: header byte %d is not zero", what, i);
+  const int64_t F = r->F;
+  if (get<uint32_t>(in, 12) != (uint32_t)F) return gpud_fail(ctx, GPUD_E_INVALID, "%s: n_fields %u, the ring has %lld", what, get<uint32_t>(in, 12), (long long)F);
+  if (get<uint32_t>(in, 16) != (uint32_t)r->W) return gpud_fail(ctx, GPUD_E_INVALID, "%s: window %u, the ring has %d", what, get<uint32_t>(in, 16), r->W);
+  if (get<int64_t>(in, 24) != r->cap) return gpud_fail(ctx, GPUD_E_INVALID, "%s: capacity %lld, the ring has %lld", what, (long long)get<int64_t>(in, 24), (long long)r->cap);
+  fr->hs = ckpt_handles(r);
+  { const int32_t rc = delta ? delta_target_ok(r, in, fr->hs) : full_target_ok(r, in, n_bytes); if (rc) return rc; }
+  if (delta) {
+    const int64_t prev_total = get<int64_t>(in, 32), total = get<int64_t>(in, 40), first_d = get<int64_t>(in, 48);
+    if (prev_total != r->ck_total || total < prev_total || first_d != std::max(prev_total, total - r->cap))
+      return gpud_fail(ctx, GPUD_E_INVALID, "%s: totals %lld -> %lld and first sample %lld disagree", what, (long long)prev_total, (long long)total, (long long)first_d);
+    fr->total = total;
+    fr->first = first_d;
+    fr->prev_link = get<uint64_t>(in, 56);
+  } else {
+    const int64_t total = get<int64_t>(in, 48), count = get<int64_t>(in, 56);
+    if (total < 0 || count != std::min(total, r->cap)) return gpud_fail(ctx, GPUD_E_INVALID, "%s: total %lld and count %lld disagree", what, (long long)total, (long long)count);
+    fr->total = total;
+    fr->first = total - count;
   }
-  if (off != hnd_off + hnd_bytes) return gpud_fail(ctx, GPUD_E_INVALID, "restore: the handle section has %lld bytes after its last handle", (long long)(hnd_off + hnd_bytes - off));
-  if (n_handles) *n_handles = (int32_t)n_win;
-  if (n_win > cap_handles) return gpud_fail(ctx, GPUD_E_CAPACITY, "restore: %lld windows handles, room for %d", (long long)n_win, cap_handles);
-  // ---- decode ----
+  // the section lengths: thresholds (none in a delta), directory, payload, checksums, handles
+  int64_t sec[5] = {0, 0, 0, 0, 0};
+  for (int i = 0; i < ns; ++i) sec[5 - ns + i] = get<int64_t>(in, 64 + 8 * i);
+  const int64_t thr_bytes = sec[0], dir_bytes = sec[1], pay_bytes = sec[2], sum_bytes = sec[3], hnd_bytes = sec[4];
+  fr->count = fr->total - fr->first;
+  const int64_t nb = (fr->count + kBlock - 1) / kBlock;
+  fr->units = F * nb;
+  if (dir_bytes != pad8(fr->units) || sum_bytes != 8 * F || pay_bytes < 0 || (pay_bytes & 7) || hnd_bytes < 0 || pay_bytes > n_bytes || hnd_bytes > n_bytes ||
+      kHeaderBytes + thr_bytes + dir_bytes + pay_bytes + sum_bytes + hnd_bytes != n_bytes)
+    return gpud_fail(ctx, GPUD_E_INVALID, "%s: section lengths do not add up to the %lld bytes given", what, (long long)n_bytes);
+  const int64_t dir_off = kHeaderBytes + thr_bytes, pay_off = dir_off + dir_bytes, sum_off = pay_off + pay_bytes, hnd_off = sum_off + sum_bytes,
+                hnd_end = hnd_off + hnd_bytes;
+  fr->dir = in + dir_off;
+  fr->payload = in + pay_off;
+  fr->sums = in + sum_off;
+  fr->pay_bytes = pay_bytes;
+  { const int32_t rc = read_directory(ctx, fr->dir, fr->units, nb, fr->count, dir_bytes, pay_bytes, fr->offs, &fr->n_int, what); if (rc) return rc; }
+  // the handle records
+  const uint32_t n_rec = get<uint32_t>(in, 20);
+  if (delta && n_rec != fr->hs.size()) return gpud_fail(ctx, GPUD_E_INVALID, "%s: %u handle records, the ring has %zu handles", what, n_rec, fr->hs.size());
+  int64_t off = hnd_off;
+  for (uint32_t i = 0; i < n_rec; ++i) {
+    if (off + 8 * nh > n_bytes) return gpud_fail(ctx, GPUD_E_INVALID, "%s: truncated handle %u", what, i);
+    int64_t v[10] = {};
+    memcpy(v, in + off, 8 * nh);
+    fr->heads.insert(fr->heads.end(), v, v + nh);
+    const CkHandle h{v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7], v[8], delta ? v[9] : v[4], off + 8 * nh};
+    { const int32_t rc = delta ? delta_record_ok(r, fr->hs[i], h, i, fr->total) : full_record_ok(r, h, i, fr->total); if (rc) return rc; }
+    const int64_t body = handle_body_bytes(F, h.next - h.from);
+    if (h.off + body > hnd_end) return gpud_fail(ctx, GPUD_E_INVALID, "%s: truncated handle %u", what, i);
+    off = h.off + body;
+    fr->recs.push_back(h);
+  }
+  if (off != hnd_end) return gpud_fail(ctx, GPUD_E_INVALID, "%s: the handle section has %lld bytes after its last handle", what, (long long)(hnd_end - off));
+  return GPUD_OK;
+}
+
+// The ring and its sample ring back to zero, as created.
+void zero_ring(gpud_ring* r) {
+  cudaMemsetAsync(r->d_ring, 0, (size_t)r->F * r->cap * sizeof(double) + 64, r->stream);
+  cudaMemsetAsync(r->d_sample, 0, (size_t)r->F * r->smp_slots * sizeof(double), r->stream);
+  cudaStreamSynchronize(r->stream);
+}
+
+// The blob's samples into the ring, then its total and a new generation.  A full checkpoint goes into a ring as created and is decoded
+// once; on a checksum mismatch the ring is zeroed again.  A delta is decoded twice: a check pass that writes nothing, then the write
+// pass.
+int32_t load_samples(gpud_ring* r, const Frame& fr, bool delta, float* ms) {
+  gpud_ctx* ctx = r->ctx;
+  const char* what = delta ? "restore_delta" : "restore";
   GPUD_CUDA(ctx, cudaSetDevice(r->dev));
   GPUD_CUDA(ctx, cudaStreamSynchronize(r->stream));
-  const size_t ring_bytes = (size_t)F * r->cap * sizeof(double) + 64, smp_bytes = (size_t)F * r->smp_slots * sizeof(double);
-  // back to the state of a new ring (zeroed ring and sample ring, no handle), for a decode or handle re-creation that fails
-  auto unwind = [&](std::vector<gpud_ring_windows*>& made) {
-    for (gpud_ring_windows* s : made) gpud_ring_windows_free(s);
-    made.clear();
-    cudaMemsetAsync(r->d_ring, 0, ring_bytes, r->stream);
-    cudaMemsetAsync(r->d_sample, 0, smp_bytes, r->stream);
-    cudaStreamSynchronize(r->stream);
-  };
-  std::vector<gpud_ring_windows*> made;
-  float ms_dec = 0.f;
-  if (units > 0) {
+  *ms = 0.f;
+  if (fr.units > 0) {
     Decoder de;
-    { const int32_t rc = de.stage(r, in + dir_off, offs, in + pay_off, pay_bytes, "restore"); if (rc) return rc; }
+    { const int32_t rc = de.stage(r, fr.dir, fr.offs, fr.payload, fr.pay_bytes, what); if (rc) return rc; }
+    const CkGeo g = ckpt_geo(r, fr.first, fr.count);
     std::vector<uint64_t> csum;
-    { const int32_t rc = de.run<true>(r, ckpt_geo(r, total - count, count), 0, csum); if (rc) return rc; }
-    ms_dec = de.ms(0);
-    for (int64_t f = 0; f < F; ++f)
-      if (csum[f] != get<uint64_t>(in, sum_off + 8 * f)) {
-        unwind(made);
-        return gpud_fail(ctx, GPUD_E_INVALID, "restore: checksum mismatch in field %lld: the checkpoint is corrupt", (long long)f);
+    { const int32_t rc = delta ? de.run<false>(r, g, 0, csum) : de.run<true>(r, g, 0, csum); if (rc) return rc; }
+    for (int64_t f = 0; f < r->F; ++f)
+      if (csum[f] != get<uint64_t>(fr.sums, 8 * f)) {
+        if (!delta) zero_ring(r);
+        return gpud_fail(ctx, GPUD_E_INVALID, "%s: checksum mismatch in field %lld: the %s", what, (long long)f,
+                         delta ? "delta is corrupt; nothing was written" : "checkpoint is corrupt");
       }
+    // the write pass re-forms the same sums into d_csum on top of the first; they are not read again
+    if (delta) { const int32_t rc = de.run<true>(r, g, 2, csum); if (rc) return rc; }
+    *ms = delta ? de.ms(0) + de.ms(2) : de.ms(0);
   }
-  // ---- handles ----
-  r->total = total;
+  r->total = fr.total;
   ++r->gen;
-  for (const CkHandle& h : recs) {
+  return GPUD_OK;
+}
+
+// After the records were applied: no reduce to read yet, the decode's stats, and the ring at the blob's point of the chain.  A delta's
+// samples reach a tiered ring's tier as a push's would; a full restore refuses a tiered ring.
+int32_t finish_restore(gpud_ring* r, const Frame& fr, float ms) {
+  r->reduced_nw = -1;
+  r->ck_timed = true;
+  r->ck_decode_ms = ms;
+  r->ck_blocks[0] = fr.units - fr.n_int;
+  r->ck_blocks[1] = fr.n_int;
+  std::vector<uint64_t> sums(r->F);
+  memcpy(sums.data(), fr.sums, 8 * r->F);
+  set_marker(r, fr.total, chain_link(fr.prev_link, fr.total, sums.data(), r->F, fr.heads));
+  return r->tier ? gpud_tier_push(r) : GPUD_OK;
+}
+
+}  // namespace
+
+extern "C" int32_t gpud_ring_checkpoint_bound(gpud_ring* r, int64_t* bytes) { return blob_bound(r, false, bytes); }
+extern "C" int32_t gpud_ring_checkpoint_delta_bound(gpud_ring* r, int64_t* bytes) { return blob_bound(r, true, bytes); }
+extern "C" int32_t gpud_ring_checkpoint(gpud_ring* r, void* out, int64_t cap, int64_t* n_bytes) { return write_blob(r, false, out, cap, n_bytes); }
+extern "C" int32_t gpud_ring_checkpoint_delta(gpud_ring* r, void* out, int64_t cap, int64_t* n_bytes) { return write_blob(r, true, out, cap, n_bytes); }
+
+extern "C" int32_t gpud_ring_restore(gpud_ring* r, const void* in_v, int64_t n_bytes, gpud_ring_windows** handles, int32_t cap_handles,
+                                     int32_t* n_handles) {
+  if (!r || (!in_v && n_bytes) || n_bytes < 0 || cap_handles < 0 || (cap_handles > 0 && !handles)) return GPUD_E_INVALID;
+  const uint8_t* in = (const uint8_t*)in_v;
+  Frame fr;
+  { const int32_t rc = read_frame(r, in, n_bytes, false, &fr); if (rc) return rc; }
+  const int64_t n_win = std::count_if(fr.recs.begin(), fr.recs.end(), [](const CkHandle& h) { return h.kind == kKindWindows; });
+  if (n_handles) *n_handles = (int32_t)n_win;
+  if (n_win > cap_handles) return gpud_fail(r->ctx, GPUD_E_CAPACITY, "restore: %lld windows handles, room for %d", (long long)n_win, cap_handles);
+  float ms = 0.f;
+  { const int32_t rc = load_samples(r, fr, false, &ms); if (rc) return rc; }
+  // the handles, re-created; a failure leaves the ring as created
+  std::vector<gpud_ring_windows*> made;
+  for (const CkHandle& h : fr.recs) {
     gpud_ring_windows* s = nullptr;
     int32_t rc = gpud_ring_windows_new(r, h.span, h.hop, h.H, &s);
     if (rc == GPUD_OK) {
@@ -736,190 +874,39 @@ extern "C" int32_t gpud_ring_restore(gpud_ring* r, const void* in_v, int64_t n_b
       rc = read_handle_body(r, s, h.first, in + h.off, "restore");
     }
     if (rc) {
+      for (gpud_ring_windows* x : made) gpud_ring_windows_free(x);
       r->total = 0;
-      unwind(made);
+      zero_ring(r);
       return rc;
     }
   }
   int32_t k = 0;
-  for (size_t i = 0; i < recs.size(); ++i) {
-    if (recs[i].kind == kKindStream) {
+  for (size_t i = 0; i < fr.recs.size(); ++i) {
+    if (fr.recs[i].kind == kKindStream) {
       r->swin = made[i];
     } else {
       r->handles.push_back(made[i]);
       handles[k++] = made[i];
     }
   }
-  r->reduced_nw = -1;
-  r->ck_timed = true;
-  r->ck_decode_ms = ms_dec;
-  r->ck_blocks[0] = units - n_int;
-  r->ck_blocks[1] = n_int;
-  std::vector<uint64_t> sums(F);
-  memcpy(sums.data(), in + sum_off, 8 * F);
-  set_marker(r, total, chain_link(0, total, sums.data(), F, heads));
-  return GPUD_OK;
-}
-
-extern "C" int32_t gpud_ring_checkpoint_delta_bound(gpud_ring* r, int64_t* bytes) {
-  if (!r || !bytes) return GPUD_E_INVALID;
-  const int64_t F = r->F, count = r->total - delta_first(r), nb = (count + kBlock - 1) / kBlock;
-  *bytes = kHeaderBytes + pad8(F * nb) + 8 * F * count + 8 * F + delta_handles_bytes(r);
-  return GPUD_OK;
-}
-
-extern "C" int32_t gpud_ring_checkpoint_delta(gpud_ring* r, void* out_v, int64_t cap, int64_t* n_bytes) {
-  if (!r || !n_bytes || cap < 0 || (cap > 0 && !out_v)) return GPUD_E_INVALID;
-  uint8_t* out = (uint8_t*)out_v;
-  if (!r->ck_marked) return gpud_fail(r->ctx, GPUD_E_STATE, "checkpoint_delta: no checkpoint written or restored on this ring yet");
-  if (r->handle_gen != r->ck_gen)
-    return gpud_fail(r->ctx, GPUD_E_STATE, "checkpoint_delta: a handle was opened or closed since the last checkpoint: write a full one");
-  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
-  GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));
-  const int64_t F = r->F, first_d = delta_first(r), count = r->total - first_d;
-  Encoder en;
-  { const int32_t rc = en.size(r, first_d, count, "checkpoint_delta"); if (rc) return rc; }
-  const std::vector<gpud_ring_windows*> hs = ckpt_handles(r);
-  const int64_t units = en.units, dir_bytes = pad8(units), pay_bytes = 8 * en.words, hnd_bytes = delta_handles_bytes(r);
-  const int64_t dir_off = kHeaderBytes, pay_off = dir_off + dir_bytes, sum_off = pay_off + pay_bytes, hnd_off = sum_off + 8 * F,
-                size = hnd_off + hnd_bytes;
-  *n_bytes = size;
-  if (cap < size) return gpud_fail(r->ctx, GPUD_E_CAPACITY, "checkpoint_delta needs %lld bytes", (long long)size);
-  bool pinned = false;
-  { const int32_t rc = host_pinned(r, out, &pinned); if (rc) return rc; }
-  { const int32_t rc = en.pack(r, out + pay_off, pinned, "checkpoint_delta"); if (rc) return rc; }
-  memset(out, 0, kHeaderBytes);
-  memcpy(out, kDeltaMagic, 8);
-  put<uint32_t>(out, 8, kVersion);
-  put<uint32_t>(out, 12, (uint32_t)F);
-  put<uint32_t>(out, 16, (uint32_t)r->W);
-  put<uint32_t>(out, 20, (uint32_t)hs.size());
-  put<int64_t>(out, 24, r->cap);
-  put<int64_t>(out, 32, r->ck_total);
-  put<int64_t>(out, 40, r->total);
-  put<int64_t>(out, 48, first_d);
-  put<uint64_t>(out, 56, r->ck_link);
-  put<int64_t>(out, 64, dir_bytes);
-  put<int64_t>(out, 72, pay_bytes);
-  put<int64_t>(out, 80, 8 * F);
-  put<int64_t>(out, 88, hnd_bytes);
-  memset(out + dir_off, 0, dir_bytes);
-  memcpy(out + dir_off, en.dir.data(), units);
-  memcpy(out + sum_off, en.csum.data(), 8 * F);
-  int64_t off = hnd_off;
-  std::vector<int64_t> heads;
-  for (gpud_ring_windows* s : hs) {
-    const int64_t from = delta_from(s);
-    const int64_t head[10] = {s == r->swin ? kKindStream : kKindWindows, s->span, s->hop, s->H, s->first, s->next, s->lost, s->reseed ? 1 : 0,
-                              s->ck_next, from};
-    memcpy(out + off, head, sizeof head);
-    heads.insert(heads.end(), head, head + 10);
-    { const int32_t rc = write_handle_body(r, s, from, out + off + kDeltaHeadBytes); if (rc) return rc; }
-    off += kDeltaHeadBytes + handle_body_bytes(F, s->next - from);
-  }
-  en.stats(r);
-  set_marker(r, r->total, chain_link(r->ck_link, r->total, en.csum.data(), F, heads));
-  return GPUD_OK;
+  return finish_restore(r, fr, ms);
 }
 
 extern "C" int32_t gpud_ring_restore_delta(gpud_ring* r, const void* in_v, int64_t n_bytes) {
   if (!r || (!in_v && n_bytes) || n_bytes < 0) return GPUD_E_INVALID;
   const uint8_t* in = (const uint8_t*)in_v;
-  gpud_ctx* ctx = r->ctx;
-  const char* what = "restore_delta";
-  // ---- header, config and the chain ----
-  if (n_bytes < kHeaderBytes || memcmp(in, kDeltaMagic, 8) != 0) return gpud_fail(ctx, GPUD_E_INVALID, "%s: not a ring delta checkpoint", what);
-  if (get<uint32_t>(in, 8) != kVersion) return gpud_fail(ctx, GPUD_E_INVALID, "%s: delta version %u, this library reads %u", what, get<uint32_t>(in, 8), kVersion);
-  for (int i = 96; i < kHeaderBytes; ++i)
-    if (in[i]) return gpud_fail(ctx, GPUD_E_INVALID, "%s: header byte %d is not zero", what, i);
-  const int64_t F = r->F;
-  if (get<uint32_t>(in, 12) != (uint32_t)F) return gpud_fail(ctx, GPUD_E_INVALID, "%s: n_fields %u, the ring has %lld", what, get<uint32_t>(in, 12), (long long)F);
-  if (get<uint32_t>(in, 16) != (uint32_t)r->W) return gpud_fail(ctx, GPUD_E_INVALID, "%s: window %u, the ring has %d", what, get<uint32_t>(in, 16), r->W);
-  if (get<int64_t>(in, 24) != r->cap) return gpud_fail(ctx, GPUD_E_INVALID, "%s: capacity %lld, the ring has %lld", what, (long long)get<int64_t>(in, 24), (long long)r->cap);
-  if (!r->ck_marked) return gpud_fail(ctx, GPUD_E_STATE, "%s: no checkpoint written or restored on this ring yet", what);
-  const uint64_t prev_link = get<uint64_t>(in, 56);
-  if (prev_link != r->ck_link)
-    return gpud_fail(ctx, GPUD_E_INVALID, "%s: the delta follows link %016llx, the ring is at %016llx (out of order, applied twice, or another chain)", what,
-                     (unsigned long long)prev_link, (unsigned long long)r->ck_link);
-  const std::vector<gpud_ring_windows*> hs = ckpt_handles(r);
-  if (r->handle_gen != r->ck_gen) return gpud_fail(ctx, GPUD_E_STATE, "%s: a handle was opened or closed since the ring's last checkpoint", what);
-  if (r->total != r->ck_total) return gpud_fail(ctx, GPUD_E_STATE, "%s: the ring has been pushed into since its last checkpoint", what);
-  for (const gpud_ring_windows* s : hs)
-    if (s->next != s->ck_next) return gpud_fail(ctx, GPUD_E_STATE, "%s: a handle has committed windows since the ring's last checkpoint", what);
-  // ---- sections ----
-  const int64_t prev_total = get<int64_t>(in, 32), total = get<int64_t>(in, 40), first_d = get<int64_t>(in, 48), dir_bytes = get<int64_t>(in, 64),
-                pay_bytes = get<int64_t>(in, 72), sum_bytes = get<int64_t>(in, 80), hnd_bytes = get<int64_t>(in, 88);
-  const uint32_t n_rec = get<uint32_t>(in, 20);
-  if (prev_total != r->ck_total || total < prev_total || first_d != std::max(prev_total, total - r->cap))
-    return gpud_fail(ctx, GPUD_E_INVALID, "%s: totals %lld -> %lld and first sample %lld disagree", what, (long long)prev_total, (long long)total, (long long)first_d);
-  const int64_t count = total - first_d, nb = (count + kBlock - 1) / kBlock, units = F * nb;
-  if (dir_bytes != pad8(units) || sum_bytes != 8 * F || pay_bytes < 0 || (pay_bytes & 7) || hnd_bytes < 0 || pay_bytes > n_bytes || hnd_bytes > n_bytes ||
-      kHeaderBytes + dir_bytes + pay_bytes + sum_bytes + hnd_bytes != n_bytes)
-    return gpud_fail(ctx, GPUD_E_INVALID, "%s: section lengths do not add up to the %lld bytes given", what, (long long)n_bytes);
-  const int64_t dir_off = kHeaderBytes, pay_off = dir_off + dir_bytes, sum_off = pay_off + pay_bytes, hnd_off = sum_off + sum_bytes;
-  std::vector<unsigned long long> offs;
-  int64_t n_int = 0;
-  { const int32_t rc = read_directory(ctx, in + dir_off, units, nb, count, dir_bytes, pay_bytes, offs, &n_int, what); if (rc) return rc; }
-  if (n_rec != hs.size()) return gpud_fail(ctx, GPUD_E_INVALID, "%s: %u handle records, the ring has %zu handles", what, n_rec, hs.size());
-  std::vector<CkHandle> recs;
-  std::vector<int64_t> heads;
-  int64_t off = hnd_off;
-  for (uint32_t i = 0; i < n_rec; ++i) {
-    const gpud_ring_windows* s = hs[i];
-    if (off + kDeltaHeadBytes > n_bytes) return gpud_fail(ctx, GPUD_E_INVALID, "%s: truncated handle %u", what, i);
-    int64_t v[10];
-    memcpy(v, in + off, sizeof v);
-    heads.insert(heads.end(), v, v + 10);
-    const CkHandle h{v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7], v[8], v[9], off + kDeltaHeadBytes};
-    const bool same = h.kind == (s == r->swin ? kKindStream : kKindWindows) && h.span == s->span && h.hop == s->hop && h.H == s->H;
-    const int64_t complete = total < s->L ? 0 : (total - s->L) / s->P + 1;
-    const bool hist_ok = h.prev_next == s->ck_next && h.first >= s->first && h.first <= h.next && h.next - h.first <= h.H && h.next >= h.prev_next &&
-                         h.from == std::max(h.first, h.prev_next) && h.next <= complete && h.lost >= 0 && (h.reseed == 0 || h.reseed == 1);
-    if (!same || !hist_ok)
-      return gpud_fail(ctx, GPUD_E_INVALID, "%s: handle %u (kind %lld, span %lld, hop %lld, history %lld, windows [%lld, %lld) from %lld) is not this ring's handle's successor",
-                       what, i, (long long)h.kind, (long long)h.span, (long long)h.hop, (long long)h.H, (long long)h.first, (long long)h.next, (long long)h.from);
-    const int64_t body = handle_body_bytes(F, h.next - h.from);
-    if (h.off + body > hnd_off + hnd_bytes) return gpud_fail(ctx, GPUD_E_INVALID, "%s: truncated handle %u", what, i);
-    off = h.off + body;
-    recs.push_back(h);
-  }
-  if (off != hnd_off + hnd_bytes) return gpud_fail(ctx, GPUD_E_INVALID, "%s: the handle section has %lld bytes after its last handle", what, (long long)(hnd_off + hnd_bytes - off));
-  // ---- decode: a check pass that writes nothing, then the write pass ----
-  GPUD_CUDA(ctx, cudaSetDevice(r->dev));
-  GPUD_CUDA(ctx, cudaStreamSynchronize(r->stream));
-  float ms_dec = 0.f;
-  if (units > 0) {
-    Decoder de;
-    { const int32_t rc = de.stage(r, in + dir_off, offs, in + pay_off, pay_bytes, what); if (rc) return rc; }
-    const CkGeo g = ckpt_geo(r, first_d, count);
-    std::vector<uint64_t> csum;
-    { const int32_t rc = de.run<false>(r, g, 0, csum); if (rc) return rc; }
-    for (int64_t f = 0; f < F; ++f)
-      if (csum[f] != get<uint64_t>(in, sum_off + 8 * f))
-        return gpud_fail(ctx, GPUD_E_INVALID, "%s: checksum mismatch in field %lld: the delta is corrupt; nothing was written", what, (long long)f);
-    // the write pass re-forms the same sums into d_csum on top of the first; they are not read again
-    { const int32_t rc = de.run<true>(r, g, 2, csum); if (rc) return rc; }
-    ms_dec = de.ms(0) + de.ms(2);
-  }
-  // ---- state and handles ----
-  r->total = total;
-  ++r->gen;
-  for (size_t i = 0; i < recs.size(); ++i) {
-    const CkHandle& h = recs[i];
-    gpud_ring_windows* s = hs[i];
+  Frame fr;
+  { const int32_t rc = read_frame(r, in, n_bytes, true, &fr); if (rc) return rc; }
+  float ms = 0.f;
+  { const int32_t rc = load_samples(r, fr, true, &ms); if (rc) return rc; }
+  for (size_t i = 0; i < fr.recs.size(); ++i) {
+    const CkHandle& h = fr.recs[i];
+    gpud_ring_windows* s = fr.hs[i];
     s->first = h.first; s->next = h.next; s->lost = h.lost; s->reseed = h.reseed != 0; s->timed = false;
-    const int32_t rc = read_handle_body(r, s, h.from, in + h.off, what);
+    const int32_t rc = read_handle_body(r, s, h.from, in + h.off, "restore_delta");
     if (rc) return rc;
   }
-  r->reduced_nw = -1;
-  r->ck_timed = true;
-  r->ck_decode_ms = ms_dec;
-  r->ck_blocks[0] = units - n_int;
-  r->ck_blocks[1] = n_int;
-  std::vector<uint64_t> sums(F);
-  memcpy(sums.data(), in + sum_off, 8 * F);
-  set_marker(r, total, chain_link(prev_link, total, sums.data(), F, heads));
-  return r->tier ? gpud_tier_push(r) : GPUD_OK;   // the delta's samples reach the tier as a push's would
+  return finish_restore(r, fr, ms);
 }
 
 extern "C" int32_t gpudh_ring_ckpt_grid(gpud_ring* r, int32_t max_ctas) {
@@ -947,9 +934,8 @@ namespace {
 
 constexpr int kPlaceThreads = 256;
 constexpr int64_t kTierRecHead = 16;               // first sample, byte offset
-__host__ __device__ __forceinline__ int64_t tier_pad8(int64_t x) { return (x + 7) & ~(int64_t)7; }
 
-int64_t tier_rec_bytes(int64_t F) { return kTierRecHead + tier_pad8(F) + tier_pad8(4 * F); }
+int64_t tier_rec_bytes(int64_t F) { return kTierRecHead + pad8(F) + pad8(4 * F); }
 
 // One CTA.  Row sizes, then thread 0 places every row in push order (a row may evict rows of the same push), then the records of the
 // rows that are still held and each block's word offset: the byte ring, or the sink past it for a row this push placed and evicted,
@@ -987,7 +973,7 @@ __global__ void __launch_bounds__(kPlaceThreads) k_tier_place(const uint8_t* __r
     s_first = c.first;
   }
   __syncthreads();
-  const int64_t dir_off = kTierRecHead, woff_off = kTierRecHead + tier_pad8(F);
+  const int64_t dir_off = kTierRecHead, woff_off = kTierRecHead + pad8(F);
   for (int64_t j = 0; j < nb; ++j) {
     const int64_t row = row0 + j;
     const bool kept = row >= s_first;
@@ -1022,7 +1008,7 @@ __global__ void __launch_bounds__(kPlaceThreads) k_tier_place(const uint8_t* __r
         reinterpret_cast<int64_t*>(rec)[0] = row * GPUD_TIER_ROW;
         reinterpret_cast<int64_t*>(rec)[1] = off;
       }
-      for (int64_t i = F + tid; i < tier_pad8(F); i += kPlaceThreads) rec[dir_off + i] = 0;
+      for (int64_t i = F + tid; i < pad8(F); i += kPlaceThreads) rec[dir_off + i] = 0;
       if ((F & 1) && tid == 0) reinterpret_cast<uint32_t*>(rec + woff_off)[F] = 0;
     }
     __syncthreads();
@@ -1039,7 +1025,7 @@ __global__ void __launch_bounds__(256) k_tier_gather(const int64_t* __restrict__
     const int64_t off = slot[2 * (rows[j] % R)];
     const uint8_t* rec = reinterpret_cast<const uint8_t*>(buf) + off;
     dir[u] = rec[kTierRecHead + f0 + f];
-    offs[u] = (unsigned long long)((off + rec_bytes) / 8) + reinterpret_cast<const uint32_t*>(rec + kTierRecHead + tier_pad8(F))[f0 + f];
+    offs[u] = (unsigned long long)((off + rec_bytes) / 8) + reinterpret_cast<const uint32_t*>(rec + kTierRecHead + pad8(F))[f0 + f];
   }
 }
 
@@ -1071,19 +1057,16 @@ static int64_t tier_slots(int64_t B, int64_t F) { return B / (tier_rec_bytes(F) 
 
 // The encode of rows [row0, row0 + nb) (wholly in the ring), asynchronous on the ring's stream; clear: the tier restarts at row0.
 static int32_t tier_encode(gpud_ring* r, gpud_tier* t, int64_t row0, int64_t nb, bool clear) {
-  CkGeo g = ckpt_geo(r, row0 * kBlock, nb * kBlock);
-  const int64_t units = (int64_t)r->F * nb;
+  const CkGeo g = ckpt_geo(r, row0 * kBlock, nb * kBlock);
   if (nb > 0) {
     GPUD_CUDA(r->ctx, cudaEventRecord(t->ev_enc[0], r->stream));
-    k_ckpt_size<<<ckpt_grid(r, units, kCkThreads / 32), kCkThreads, 0, r->stream>>>(g, t->d_dir, t->d_words, t->d_csum);
-    GPUD_CUDA(r->ctx, cudaGetLastError());
+    GPUD_CUDA(r->ctx, launch_size(r, g, t->d_dir, t->d_words, t->d_csum));
   }
   k_tier_place<<<1, kPlaceThreads, 0, r->stream>>>(t->d_dir, t->d_words, nb, r->F, row0, clear ? 1 : 0, t->bytes, t->slots, t->rec_bytes, t->d_buf,
                                                    t->d_slot, t->d_ctl, t->d_rowsz, t->d_offs);
   GPUD_CUDA(r->ctx, cudaGetLastError());
   if (nb > 0) {
-    k_ckpt_pack<<<ckpt_grid(r, units, kPackWarps), kPackWarps * 32, 0, r->stream>>>(g, t->d_dir, t->d_offs, t->d_buf);
-    GPUD_CUDA(r->ctx, cudaGetLastError());
+    GPUD_CUDA(r->ctx, launch_pack(r, g, t->d_dir, t->d_offs, t->d_buf));
     GPUD_CUDA(r->ctx, cudaEventRecord(t->ev_enc[1], r->stream));
     t->enc_timed = true;
   }
@@ -1140,8 +1123,7 @@ int32_t gpud_tier_decode(gpud_ring* r, const std::vector<int64_t>& rows, int64_t
     g.cap = vcap; g.start = 0; g.count = n * kBlock; g.nb = n;
     g.smp_half = half; g.smp_slots = smp_slots; g.F = G; g.smp_shift = smp_shift;
     // the field sums k_ckpt_unpack re-forms land in the encode's scratch, which no one reads
-    k_ckpt_unpack<true><<<ckpt_grid(r, units, kCkThreads / 32), kCkThreads, 0, r->stream>>>(g, t->d_vdir, t->d_voffs, t->d_buf, t->d_csum);
-    GPUD_CUDA(r->ctx, cudaGetLastError());
+    GPUD_CUDA(r->ctx, launch_unpack<true>(r, g, t->d_vdir, t->d_voffs, t->d_buf, t->d_csum));
   }
   if (tail_n > 0) {
     const int grid = (int)std::min<int64_t>(((int64_t)G * tail_n + 255) / 256, (int64_t)r->sm_count * 8);

@@ -350,36 +350,41 @@ def test_refusals(env):
     hd = RC.header(blob)
     lay = RC.layout(F, hd["count"], hd["payload_bytes"] // 8, hd["handle_bytes"])
 
-    # every config field
-    for bad, word in ((Cfg(F + 1, cap, W, 0.3, (9, 10), np.append(thr, 1.0)), "n_fields"), (Cfg(F, cap, W + 1, 0.3, (9, 10), thr), "window"),
-                      (Cfg(F, cap + 2, W, 0.3, (9, 10), thr), "capacity"), (Cfg(F, cap, W, 0.3000000001, (9, 10), thr), "ema_alpha"),
-                      (Cfg(F, cap, W, 0.3, (8, 10), thr), "q_num"), (Cfg(F, cap, W, 0.3, (9, 11), thr), "q_den"),
-                      (Cfg(F, cap, W, 0.3, (9, 10), np.array([50.0, -0.0 + 60.000000000001, 70.0])), "thresholds[1]")):
+    # every config field, each with the whole message
+    for bad, msg in ((Cfg(F + 1, cap, W, 0.3, (9, 10), np.append(thr, 1.0)), "restore: n_fields 3, the ring has 4"),
+                     (Cfg(F, cap, W + 1, 0.3, (9, 10), thr), "restore: window 10, the ring has 11"),
+                     (Cfg(F, cap + 2, W, 0.3, (9, 10), thr), "restore: capacity 6000, the ring has 6002"),
+                     (Cfg(F, cap, W, 0.3000000001, (9, 10), thr), "restore: ema_alpha %.17g, the ring has %.17g" % (0.3, 0.3000000001)),
+                     (Cfg(F, cap, W, 0.3, (8, 10), thr), "restore: q_num 9, the ring has 8"),
+                     (Cfg(F, cap, W, 0.3, (9, 11), thr), "restore: q_den 10, the ring has 11"),
+                     (Cfg(F, cap, W, 0.3, (9, 10), np.array([50.0, -0.0 + 60.000000000001, 70.0])),
+                      "restore: thresholds[1] %.17g, the ring has %.17g" % (60.0, 60.000000000001)),
+                     (Cfg(F, cap, W, 0.3, (9, 10), np.array([50.0, 60.0, -70.0])), "restore: thresholds[2] 70, the ring has -70")):
         r = bad.ring(g, ctx)
-        assert raw_restore(L, r, blob)[0] == E_INVALID, word
-        assert word in last_error(g, ctx), (word, last_error(g, ctx))
+        assert raw_restore(L, r, blob)[0] == E_INVALID, msg
+        assert last_error(g, ctx) == msg
         untouched(L, r)
         r.close()
-    r = Cfg(F, cap, W, 0.3, (9, 10), np.array([50.0, 60.0, -70.0])).ring(g, ctx)
-    assert raw_restore(L, r, blob)[0] == E_INVALID and "thresholds[2]" in last_error(g, ctx)
-    r.close()
 
     # a target that is not as created
     r = cfg.ring(g, ctx)
     r.push(rows[:1])
     assert raw_restore(L, r, blob)[0] == E_STATE
+    assert last_error(g, ctx) == "restore: the ring has been pushed into"
     assert r.counts()[0] == 1
     r.close()
     for opener in (lambda r: r.stream_open(0), lambda r: r.windows(2)):
         r = cfg.ring(g, ctx)
         opener(r)
         assert raw_restore(L, r, blob)[0] == E_STATE
+        assert last_error(g, ctx) == "restore: the ring has a stream or windows handle open"
         untouched(L, r)
         r.close()
 
     # cap_handles too small
     r = cfg.ring(g, ctx)
     assert raw_restore(L, r, blob, cap_handles=0) == (E_CAPACITY, 1)
+    assert last_error(g, ctx) == "restore: 1 windows handles, room for 0"
     untouched(L, r)
 
     # malformed bytes
@@ -388,27 +393,46 @@ def test_refusals(env):
         import struct
         struct.pack_into(fmt, b, off, value)
         return bytes(b)
+    hs = RC.decode(blob)["handles"]
+
+    def bad_handle(i, **edits):
+        h = dict(hs[i], **edits)
+        return "restore: handle %d (kind %d, span %d, hop %d, history %d, windows [%d, %d)) is not one this ring can hold" % (
+            i, h["kind"], h["span"], h["hop"], h["H"], h["first"], h["next"])
+    n, pay = len(blob), hd["payload_bytes"]
     malformed = {
-        "truncated by 8": blob[:-8], "header only": blob[:128], "short header": blob[:100], "empty": b"",
-        "magic": b"GPUDRCK0" + blob[8:], "version": edit(8, "<I", 2), "header padding": edit(120, "<Q", 1),
-        "width 65": edit(lay["dir"] + 1, "<B", 65), "width 127 INT": edit(lay["dir"], "<B", 0xFF),
-        "directory padding": edit(lay["dir"] + F * lay["nb"], "<B", 1),
-        "payload length": edit(80, "<q", hd["payload_bytes"] + 8)[:lay["payload"]] + bytes(8) + blob[lay["payload"]:],
-        "count": edit(56, "<q", hd["count"] - 1), "total": edit(48, "<q", -1),
-        "n_handles": edit(20, "<I", 3), "handle span": edit(lay["handles"] + 8, "<q", cap), "handle history": edit(lay["handles"] + 24, "<q", 0),
-        "handle next": edit(lay["handles"] + 40, "<q", 10 ** 6), "handle first > next": edit(lay["handles"] + 32, "<q", 10 ** 6),
-        "two stream handles": edit(lay["handles"] + 64 + RC.handle_body_bytes(F, RC.decode(blob)["handles"][0]["next"] - RC.decode(blob)["handles"][0]["first"]), "<q", 0),
-        "handle reseed 2": edit(lay["handles"] + 56, "<q", 2), "trailing byte": blob + b"\0",
+        "truncated by 8": (blob[:-8], "restore: section lengths do not add up to the %d bytes given" % (n - 8)),
+        "header only": (blob[:128], "restore: truncated thresholds section"),
+        "short header": (blob[:100], "restore: not a ring checkpoint"), "empty": (b"", "restore: not a ring checkpoint"),
+        "magic": (b"GPUDRCK0" + blob[8:], "restore: not a ring checkpoint"),
+        "version": (edit(8, "<I", 2), "restore: checkpoint version 2, this library reads 1"),
+        "header padding": (edit(120, "<Q", 1), "restore: header byte 120 is not zero"),
+        "width 65": (edit(lay["dir"] + 1, "<B", 65), "restore: block 1 has width 65"),
+        "width 127 INT": (edit(lay["dir"], "<B", 0xFF), "restore: block 0 has width 127"),
+        "directory padding": (edit(lay["dir"] + F * lay["nb"], "<B", 1), "restore: directory padding is not zero"),
+        "payload length": (edit(80, "<q", pay + 8)[:lay["payload"]] + bytes(8) + blob[lay["payload"]:],
+                           "restore: the directory codes %d payload bytes, the section has %d" % (pay, pay + 8)),
+        "count": (edit(56, "<q", hd["count"] - 1), "restore: total %d and count %d disagree" % (hd["total"], hd["count"] - 1)),
+        "total": (edit(48, "<q", -1), "restore: total -1 and count %d disagree" % hd["count"]),
+        "n_handles": (edit(20, "<I", 3), "restore: truncated handle 2"),
+        "handle span": (edit(lay["handles"] + 8, "<q", cap), bad_handle(0, span=cap)),
+        "handle history": (edit(lay["handles"] + 24, "<q", 0), bad_handle(0, H=0)),
+        "handle next": (edit(lay["handles"] + 40, "<q", 10 ** 6), bad_handle(0, next=10 ** 6)),
+        "handle first > next": (edit(lay["handles"] + 32, "<q", 10 ** 6), bad_handle(0, first=10 ** 6)),
+        "two stream handles": (edit(lay["handles"] + 64 + RC.handle_body_bytes(F, hs[0]["next"] - hs[0]["first"]), "<q", 0), bad_handle(1, kind=0)),
+        "handle reseed 2": (edit(lay["handles"] + 56, "<q", 2), bad_handle(0)),
+        "trailing byte": (blob + b"\0", "restore: section lengths do not add up to the %d bytes given" % (n + 1)),
     }
-    for what, b in malformed.items():
+    for what, (b, msg) in malformed.items():
         assert raw_restore(L, r, b)[0] == E_INVALID, what
+        assert last_error(g, ctx) == msg, what
         untouched(L, r)
 
     # a flipped payload bit: the checksum catches it after the decode, and the ring is as created again
     b = bytearray(blob)
     b[lay["payload"] + 40] ^= 0x04
     assert raw_restore(L, r, bytes(b))[0] == E_INVALID
-    assert "checksum" in last_error(g, ctx)
+    assert last_error(g, ctx) == "restore: checksum mismatch in field 0: the checkpoint is corrupt"
     untouched(L, r)
     fresh = cfg.ring(g, ctx)
     for x in (r, fresh):

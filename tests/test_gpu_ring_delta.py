@@ -198,7 +198,7 @@ def test_write_refusals(env):
     r = cfg.ring(g, ctx)
     r.push(rows[:1000])
     assert raw_delta(L, r, 1 << 20)[0] == E_STATE            # no marker yet
-    assert "no checkpoint" in last_error(g, ctx)
+    assert last_error(g, ctx) == "checkpoint_delta: no checkpoint written or restored on this ring yet"
     r.checkpoint()
     for change in (lambda r: r.stream_open(0), lambda r: r.windows(3), lambda r: r.windows(3).close()):
         x = cfg.ring(g, ctx)
@@ -206,7 +206,7 @@ def test_write_refusals(env):
         x.checkpoint()
         change(x)
         assert raw_delta(L, x, 1 << 20)[0] == E_STATE
-        assert "full one" in last_error(g, ctx)
+        assert last_error(g, ctx) == "checkpoint_delta: a handle was opened or closed since the last checkpoint: write a full one"
         x.checkpoint()                                       # a full checkpoint starts a new chain
         assert RD.decode(x.checkpoint_delta())["total"] == 1000
         x.close()
@@ -219,7 +219,9 @@ def test_write_refusals(env):
     want = twin.checkpoint_delta()
     rc, n, got = raw_delta(L, r, len(want) - 1)
     assert rc == E_CAPACITY and n == len(want) and got == bytes(len(want) - 1)
+    assert last_error(g, ctx) == "checkpoint_delta needs %d bytes" % len(want)
     assert raw_delta(L, r, 0)[:2] == (E_CAPACITY, len(want))
+    assert last_error(g, ctx) == "checkpoint_delta needs %d bytes" % len(want)
     assert r.checkpoint_delta() == want
     r.close()
     twin.close()
@@ -256,8 +258,9 @@ def test_apply_refusals(env):
         hs = r.restore(base)
         return r, hs, snapshot(L, r)
 
-    def unchanged(r, snap, code, blob, what):
+    def unchanged(r, snap, code, blob, what, msg):
         assert raw_apply(L, r, blob) == code, (what, last_error(g, ctx))
+        assert last_error(g, ctx) == msg, what
         x = snapshot(L, r)
         same(x[0], snap[0], what)
         same(x[1], snap[1], what)
@@ -265,14 +268,19 @@ def test_apply_refusals(env):
         r.restore_delta(d1)                                  # and the right delta still applies
         r.close()
 
+    def bad_link(blob, ring_link):
+        return ("restore_delta: the delta follows link %016x, the ring is at %016x (out of order, applied twice, or another chain)" %
+                (RD.header(blob)["prev_link"], ring_link))
+
     # the chain
     for what, blob in (("out of order", d2), ("another chain", d_other)):
         r, _, snap = target()
-        unchanged(r, snap, E_INVALID, blob, what)
+        unchanged(r, snap, E_INVALID, blob, what, bad_link(blob, RD.full_link(base)))
     r, _, _ = target()
     r.restore_delta(d1)
     snap = snapshot(L, r)
     assert raw_apply(L, r, d1) == E_INVALID                  # applied twice
+    assert last_error(g, ctx) == bad_link(d1, RD.decode(d1)["link"])
     same(snapshot(L, r)[0], snap[0], "twice")
     r.restore_delta(d2)
     r.close()
@@ -280,20 +288,24 @@ def test_apply_refusals(env):
     r, _, snap = target()
     r.push(rows[:1])
     assert raw_apply(L, r, d1) == E_STATE and r.counts()[0] == 7778
+    assert last_error(g, ctx) == "restore_delta: the ring has been pushed into since its last checkpoint"
     r.close()
     for change in (lambda r, hs: hs[0].close(), lambda r, hs: r.windows(2)):
         r, hs, snap = target()
         change(r, hs)
         assert raw_apply(L, r, d1) == E_STATE
+        assert last_error(g, ctx) == "restore_delta: a handle was opened or closed since the ring's last checkpoint"
         same(snapshot(L, r)[0], snap[0], "handles changed")
         r.close()
     # a handle that committed windows since the marker, with nothing pushed: the base's windows handle had never been reduced
     r, hs, snap = target()
     n_new, _ = hs[0].reduce()
     assert n_new > 0 and raw_apply(L, r, d1) == E_STATE
+    assert last_error(g, ctx) == "restore_delta: a handle has committed windows since the ring's last checkpoint"
     r.close()
     r = cfg.ring(g, ctx)
     assert raw_apply(L, r, d1) == E_STATE                    # no marker
+    assert last_error(g, ctx) == "restore_delta: no checkpoint written or restored on this ring yet"
     r.close()
 
     # malformed bytes
@@ -304,32 +316,56 @@ def test_apply_refusals(env):
         b = bytearray(b)
         struct.pack_into(fmt, b, off, value)
         return bytes(b)
+    hs = RD.decode(d1)["handles"]
     h0 = lay["handles"]
-    h1 = h0 + 80 + RC.handle_body_bytes(F, RD.decode(d1)["handles"][0]["next"] - RD.decode(d1)["handles"][0]["from"])
+    h1 = h0 + 80 + RC.handle_body_bytes(F, hs[0]["next"] - hs[0]["from"])
+
+    def bad_handle(i, **edits):
+        h = dict(hs[i], **edits)
+        return ("restore_delta: handle %d (kind %d, span %d, hop %d, history %d, windows [%d, %d) from %d) is not this ring's handle's successor" %
+                (i, h["kind"], h["span"], h["hop"], h["H"], h["first"], h["next"], h["from"]))
+    n, pay = len(d1), hd["payload_bytes"]
+    sections = "restore_delta: section lengths do not add up to the %d bytes given"
+    totals = "restore_delta: totals %d -> %d and first sample %d disagree"
     malformed = {
-        "empty": b"", "short header": d1[:100], "header only": d1[:128], "truncated by 8": d1[:-8], "trailing byte": d1 + b"\0",
-        "magic": b"GPUDRCK1" + d1[8:], "version": edit(8, "<I", 2), "header padding": edit(120, "<Q", 1),
-        "F": edit(12, "<I", F + 1), "W": edit(16, "<I", W + 1), "CAP": edit(24, "<q", cap + 1), "prev_total": edit(32, "<q", 7776),
-        "total": edit(40, "<q", 9001), "first_d": edit(48, "<q", 7778),
-        "width 65": edit(lay["dir"], "<B", 65), "directory padding": edit(lay["dir"] + F * lay["nb"], "<B", 1),
-        "payload length": edit(72, "<q", hd["payload_bytes"] + 8)[:lay["payload"]] + bytes(8) + d1[lay["payload"]:],
-        "n_handles": edit(20, "<I", 1), "kind": edit(h0, "<q", 1), "span": edit(h1 + 8, "<q", 5), "hop": edit(h1 + 16, "<q", 2),
-        "H": edit(h1 + 24, "<q", 99), "first > from": edit(h0 + 32, "<q", 10 ** 6), "next": edit(h0 + 40, "<q", 10 ** 6),
-        "prev_next": edit(h0 + 64, "<q", 1), "from": edit(h0 + 72, "<q", 0), "reseed 2": edit(h0 + 56, "<q", 2),
+        "empty": (b"", "restore_delta: not a ring delta checkpoint"), "short header": (d1[:100], "restore_delta: not a ring delta checkpoint"),
+        "header only": (d1[:128], sections % 128), "truncated by 8": (d1[:-8], sections % (n - 8)), "trailing byte": (d1 + b"\0", sections % (n + 1)),
+        "magic": (b"GPUDRCK1" + d1[8:], "restore_delta: not a ring delta checkpoint"),
+        "version": (edit(8, "<I", 2), "restore_delta: delta version 2, this library reads 1"),
+        "header padding": (edit(120, "<Q", 1), "restore_delta: header byte 120 is not zero"),
+        "F": (edit(12, "<I", F + 1), "restore_delta: n_fields 4, the ring has 3"), "W": (edit(16, "<I", W + 1), "restore_delta: window 11, the ring has 10"),
+        "CAP": (edit(24, "<q", cap + 1), "restore_delta: capacity 6001, the ring has 6000"),
+        "prev_total": (edit(32, "<q", 7776), totals % (7776, 9000, 7777)),
+        # a consistent total one sample on: field 1's last block (width 10) codes one payload word more than the section holds
+        "total": (edit(40, "<q", 9001), "restore_delta: the directory codes %d payload bytes, the section has %d" % (pay + 8, pay)),
+        "first_d": (edit(48, "<q", 7778), totals % (7777, 9000, 7778)),
+        "width 65": (edit(lay["dir"], "<B", 65), "restore_delta: block 0 has width 65"),
+        "directory padding": (edit(lay["dir"] + F * lay["nb"], "<B", 1), "restore_delta: directory padding is not zero"),
+        "payload length": (edit(72, "<q", pay + 8)[:lay["payload"]] + bytes(8) + d1[lay["payload"]:],
+                           "restore_delta: the directory codes %d payload bytes, the section has %d" % (pay, pay + 8)),
+        "n_handles": (edit(20, "<I", 1), "restore_delta: 1 handle records, the ring has 2 handles"),
+        "kind": (edit(h0, "<q", 1), bad_handle(0, kind=1)), "span": (edit(h1 + 8, "<q", 5), bad_handle(1, span=5)),
+        "hop": (edit(h1 + 16, "<q", 2), bad_handle(1, hop=2)), "H": (edit(h1 + 24, "<q", 99), bad_handle(1, H=99)),
+        "first > from": (edit(h0 + 32, "<q", 10 ** 6), bad_handle(0, first=10 ** 6)), "next": (edit(h0 + 40, "<q", 10 ** 6), bad_handle(0, next=10 ** 6)),
+        "prev_next": (edit(h0 + 64, "<q", 1), bad_handle(0)), "from": (edit(h0 + 72, "<q", 0), bad_handle(0, **{"from": 0})),
+        "reseed 2": (edit(h0 + 56, "<q", 2), bad_handle(0)),
     }
-    for what, blob in malformed.items():
+    for what, (blob, msg) in malformed.items():
         r, _, snap = target()
-        unchanged(r, snap, E_INVALID, blob, what)
-    for bad in (Cfg(F + 1, cap, W, 0.3, thr=np.array([50.0, 60.0, 70.0, 1.0])), Cfg(F, cap, W + 1, 0.3, thr=np.array([50.0, 60.0, 70.0]))):
+        unchanged(r, snap, E_INVALID, blob, what, msg)
+    for bad, msg in ((Cfg(F + 1, cap, W, 0.3, thr=np.array([50.0, 60.0, 70.0, 1.0])), "restore_delta: n_fields 3, the ring has 4"),
+                     (Cfg(F, cap, W + 1, 0.3, thr=np.array([50.0, 60.0, 70.0])), "restore_delta: window 10, the ring has 11")):
         r = bad.ring(g, ctx)
         assert raw_apply(L, r, d1) == E_INVALID
+        assert last_error(g, ctx) == msg
         r.close()
 
     # a flipped payload bit: the check pass catches it and nothing is written; the right delta applies afterwards
     b = bytearray(d1)
     b[lay["payload"] + 40] ^= 0x04
     r, _, snap = target()
-    assert raw_apply(L, r, bytes(b)) == E_INVALID and "checksum" in last_error(g, ctx)
+    assert raw_apply(L, r, bytes(b)) == E_INVALID
+    assert last_error(g, ctx) == "restore_delta: checksum mismatch in field 0: the delta is corrupt; nothing was written"
     x = snapshot(L, r)
     same(x[0], snap[0], "flip")
     same(x[1], snap[1], "flip")
