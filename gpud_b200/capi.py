@@ -762,7 +762,8 @@ SYMBOLS = ["gpud_abi_version", "gpud_sizeof", "gpud_ctx_create", "gpud_ctx_destr
            "gpud_fabric_gather_p2p", "gpud_fm_log_syncer_create", "gpud_fm_log_syncer_destroy", "gpud_fm_log_syncer_feed",
            "gpud_fm_nothing_to_do_from_store", "gpud_ring_checkpoint_bound", "gpud_ring_checkpoint", "gpud_ring_restore",
            "gpud_ring_checkpoint_stats", "gpud_ring_checkpoint_delta_bound", "gpud_ring_checkpoint_delta", "gpud_ring_restore_delta",
-           "gpud_ring_tier_open", "gpud_ring_tier_counts", "gpud_ring_tier_stats"]
+           "gpud_ring_tier_open", "gpud_ring_tier_counts", "gpud_ring_tier_stats", "gpud_ring_tier_checkpoint_bound", "gpud_ring_tier_checkpoint",
+           "gpud_ring_tier_checkpoint_delta_bound", "gpud_ring_tier_checkpoint_delta", "gpud_ring_tier_restore", "gpud_ring_tier_checkpoint_stats"]
 
 _lib = None
 
@@ -849,6 +850,12 @@ def lib() -> C.CDLL:
         "gpudh_ring_tier_plan": (i32, [i64, i32, i64, i64, vp, i64, vp, i64, vp, vp]),
         "gpudh_ring_tier_split": (i32, [i64, i64, i32, i64, i64, vp, vp, i64, vp, i64, vp, vp, vp, i64, C.POINTER(i64), C.POINTER(i64)]),
         "gpudh_ring_tier_row": (i32, [vp, i64, vp, i64, C.POINTER(i64)]), "gpudh_ring_tier_group": (i32, [vp, i32]),
+        "gpud_ring_tier_checkpoint_bound": (i32, [vp, C.POINTER(i64)]), "gpud_ring_tier_checkpoint": (i32, [vp, vp, i64, C.POINTER(i64)]),
+        "gpud_ring_tier_checkpoint_delta_bound": (i32, [vp, C.POINTER(i64)]),
+        "gpud_ring_tier_checkpoint_delta": (i32, [vp, vp, i64, C.POINTER(i64)]),
+        "gpud_ring_tier_restore": (i32, [vp, i64, vp, vp, i32]),
+        "gpud_ring_tier_checkpoint_stats": (i32, [vp, C.POINTER(C.c_float), C.POINTER(C.c_float), C.POINTER(i64)]),
+        "gpudh_ring_tier_chain_plan": (i32, [i32, i32, i64, i64, i64, vp, vp, i32, vp, i64, C.POINTER(i64), vp, C.c_char_p, i32]),
         "gpud_kmsg_scan": (i32, [vp, i32, vp, i64, i32, C.POINTER(XidHit), i64, C.POINTER(i64), C.POINTER(i64)]),
         "gpud_kmsg_scan_sharded": (i32, [vp, vp, i64, i32, C.POINTER(XidHit), i64, C.POINTER(i64), C.POINTER(i64)]),
         "gpud_kmsg_scan_device": (i32, [vp, i32, vp, i64, i32, C.POINTER(XidHit), i64, C.POINTER(i64), C.POINTER(i64), vp]),
@@ -1433,6 +1440,38 @@ class Ring:
     def tier_group(self, max_fields: int):
         """test hook gpudh_ring_tier_group: at most max_fields fields per decoded group (0: the default)"""
         self.ctx._check(self._L.gpudh_ring_tier_group(self._h, max_fields))
+
+    # ---- tier checkpoints: the tier's rows as bytes that outlive the process, with a marker of their own ----
+    def tier_checkpoint_bound(self) -> int:
+        n = C.c_int64()
+        self.ctx._check(self._L.gpud_ring_tier_checkpoint_bound(self._h, C.byref(n)))
+        return n.value
+
+    def tier_checkpoint(self, out=None):
+        """gpud_ring_tier_checkpoint: the rows the tier holds; the tier marker moves to this blob.  out as for checkpoint()."""
+        return self._write_blob(self._L.gpud_ring_tier_checkpoint, self.tier_checkpoint_bound, out)
+
+    def tier_checkpoint_delta_bound(self) -> int:
+        n = C.c_int64()
+        self.ctx._check(self._L.gpud_ring_tier_checkpoint_delta_bound(self._h, C.byref(n)))
+        return n.value
+
+    def tier_checkpoint_delta(self, out=None):
+        """gpud_ring_tier_checkpoint_delta: the tier's rows since its marker, which then moves to this delta.  out as for checkpoint()."""
+        return self._write_blob(self._L.gpud_ring_tier_checkpoint_delta, self.tier_checkpoint_delta_bound, out)
+
+    def tier_restore(self, tier_bytes: int, blobs) -> None:
+        """gpud_ring_tier_restore: open this ring's tier of tier_bytes from a chain, a full tier checkpoint then its deltas in order"""
+        views = [_blob_ptr(b) for b in blobs]
+        ptrs = (C.c_void_p * max(1, len(views)))(*[src for _, src in views])
+        sizes = (C.c_int64 * max(1, len(views)))(*[len(mv) for mv, _ in views])
+        self.ctx._check(self._L.gpud_ring_tier_restore(self._h, tier_bytes, ptrs, sizes, len(views)))
+
+    def tier_checkpoint_stats(self):
+        """the last tier checkpoint or tier restore: (export + check device ms, check + load device ms, rows written or loaded)"""
+        enc, dec, rows = C.c_float(), C.c_float(), C.c_int64()
+        self.ctx._check(self._L.gpud_ring_tier_checkpoint_stats(self._h, C.byref(enc), C.byref(dec), C.byref(rows)))
+        return float(enc.value), float(dec.value), int(rows.value)
 
 
 def _blob_ptr(blob):

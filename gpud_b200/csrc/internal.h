@@ -111,6 +111,14 @@ struct gpud_tier {
   int64_t* d_rows = nullptr;  size_t rows_cap = 0;
   uint8_t* d_vdir = nullptr;  size_t vdir_cap = 0;
   unsigned long long* d_voffs = nullptr;  size_t voffs_cap = 0;
+  // The tier marker (DESIGN.md "Ring tier checkpoint format"): the next row and link of the last tier blob written or restored, apart
+  // from the ring's own chain marker.
+  bool ck_marked = false;
+  int64_t ck_next = 0;
+  uint64_t ck_link = 0;
+  bool ck_timed = false;           // gpud_ring_tier_checkpoint_stats: a tier checkpoint or restore has run
+  float ck_encode_ms = 0.f, ck_decode_ms = 0.f;
+  int64_t ck_rows = 0;             // ... rows the last of either wrote or loaded
 };
 // ring_ckpt.cu: after every push into a tiered ring, on its stream: the loss rule, then the encode of every row the push completed.
 int32_t gpud_tier_push(gpud_ring* r);

@@ -1041,6 +1041,50 @@ __global__ void __launch_bounds__(256) k_tier_tail(const double* __restrict__ ri
   }
 }
 
+cudaError_t launch_gather(const gpud_ring* r, const int64_t* rows, int64_t n, int f0, int G, const unsigned long long* buf, const int64_t* slot,
+                          int64_t R, uint8_t* dir, unsigned long long* offs) {
+  const int grid = (int)std::min<int64_t>(((int64_t)G * n + 255) / 256, (int64_t)r->sm_count * 8);
+  k_tier_gather<<<grid, 256, 0, r->stream>>>(rows, n, f0, G, r->F, buf, slot, R, tier_rec_bytes(r->F), dir, offs);
+  return cudaGetLastError();
+}
+
+// Tier checkpoints (DESIGN.md "Ring tier checkpoint format") move whole rows between byte buffers: the export from the tier's byte ring
+// into a blob's packed rows section, the restore's load from the staged chain into a new tier's byte ring.  Row j of a copy is bytes
+// [src, src + n) of one buffer to [dst, dst + n) of the other, and its record's byte-offset word becomes dst.
+struct TierCopy { int64_t src, dst, n; };
+constexpr int kCopyThreads = 256;
+
+// One CTA per row, grid-stride over the rows: 16-byte copies where both offsets agree mod 16 (one lone word before the first boundary
+// at most), 8-byte ones otherwise; then thread 0 writes the offset word over the copied one.
+__global__ void __launch_bounds__(kCopyThreads) k_tier_copy(const TierCopy* __restrict__ rows, int64_t n_rows, const uint8_t* __restrict__ src,
+                                                            uint8_t* __restrict__ dst) {
+  for (int64_t j = blockIdx.x; j < n_rows; j += gridDim.x) {
+    const TierCopy c = rows[j];
+    const unsigned long long* s = reinterpret_cast<const unsigned long long*>(src + c.src);
+    unsigned long long* d = reinterpret_cast<unsigned long long*>(dst + c.dst);
+    const int64_t words = c.n >> 3;
+    int64_t w = 0;
+    if (((c.src ^ c.dst) & 15) == 0) {
+      const int64_t lead = (c.src & 15) ? 1 : 0, n16 = (words - lead) >> 1;
+      if (lead && threadIdx.x == 0) d[0] = __ldg(s);
+      const uint4* s16 = reinterpret_cast<const uint4*>(s + lead);
+      uint4* d16 = reinterpret_cast<uint4*>(d + lead);
+      for (int64_t i = threadIdx.x; i < n16; i += blockDim.x) d16[i] = __ldg(s16 + i);
+      w = lead + 2 * n16;
+    }
+    for (int64_t i = w + threadIdx.x; i < words; i += blockDim.x) d[i] = __ldg(s + i);
+    __syncthreads();
+    if (threadIdx.x == 0) reinterpret_cast<int64_t*>(d)[1] = c.dst;
+  }
+}
+
+cudaError_t launch_copy(const gpud_ring* r, const TierCopy* rows, int64_t n_rows, const void* src, void* dst) {
+  if (n_rows == 0) return cudaSuccess;
+  const int grid = (int)std::min<int64_t>(n_rows, (int64_t)r->sm_count * 8);
+  k_tier_copy<<<grid, kCopyThreads, 0, r->stream>>>(rows, n_rows, (const uint8_t*)src, (uint8_t*)dst);
+  return cudaGetLastError();
+}
+
 }  // namespace
 
 void gpud_tier_free(gpud_tier* t) {
@@ -1115,9 +1159,7 @@ int32_t gpud_tier_decode(gpud_ring* r, const std::vector<int64_t>& rows, int64_t
   GPUD_CUDA(r->ctx, cudaEventRecord(t->ev_dec[0], r->stream));
   if (n > 0) {
     GPUD_CUDA(r->ctx, cudaMemcpyAsync(t->d_rows, rows.data(), n * sizeof(int64_t), cudaMemcpyHostToDevice, r->stream));
-    const int grid = (int)std::min<int64_t>((units + 255) / 256, (int64_t)r->sm_count * 8);
-    k_tier_gather<<<grid, 256, 0, r->stream>>>(t->d_rows, n, f0, G, r->F, t->d_buf, t->d_slot, t->slots, t->rec_bytes, t->d_vdir, t->d_voffs);
-    GPUD_CUDA(r->ctx, cudaGetLastError());
+    GPUD_CUDA(r->ctx, launch_gather(r, t->d_rows, n, f0, G, t->d_buf, t->d_slot, t->slots, t->d_vdir, t->d_voffs));
     CkGeo g{};
     g.ring = t->d_vring; g.sample = t->d_vsmp;
     g.cap = vcap; g.start = 0; g.count = n * kBlock; g.nb = n;
@@ -1135,14 +1177,18 @@ int32_t gpud_tier_decode(gpud_ring* r, const std::vector<int64_t>& rows, int64_t
   return GPUD_OK;
 }
 
-extern "C" int32_t gpud_ring_tier_open(gpud_ring* r, int64_t tier_bytes) {
-  if (!r) return GPUD_E_INVALID;
-  if (r->tier) return gpud_fail(r->ctx, GPUD_E_STATE, "tier_open: the ring already has a tier");
-  const int64_t F = r->F, B = tier_bytes & ~(int64_t)7, rec = tier_rec_bytes(F), row_max = rec + 8 * F * kBlock;
-  if (r->cap < 2 * kBlock) return gpud_fail(r->ctx, GPUD_E_INVALID, "tier_open: capacity %lld is below %d", (long long)r->cap, 2 * kBlock);
+// tier_open's refusals of a ring's capacity and a tier's size (tier_restore's too).
+static int32_t tier_size_ok(gpud_ctx* ctx, int64_t cap, int64_t F, int64_t tier_bytes, const char* what) {
+  const int64_t row_max = tier_rec_bytes(F) + 8 * F * kBlock;
+  if (cap < 2 * kBlock) return gpud_fail(ctx, GPUD_E_INVALID, "%s: capacity %lld is below %d", what, (long long)cap, 2 * kBlock);
   if (tier_bytes < row_max)
-    return gpud_fail(r->ctx, GPUD_E_INVALID, "tier_open: %lld bytes do not hold one row coded at 64 bits (%lld bytes)", (long long)tier_bytes, (long long)row_max);
-  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
+    return gpud_fail(ctx, GPUD_E_INVALID, "%s: %lld bytes do not hold one row coded at 64 bits (%lld bytes)", what, (long long)tier_bytes, (long long)row_max);
+  return GPUD_OK;
+}
+
+// A tier of tier_bytes for the ring, its control word set to c0; nothing is placed or encoded.  On failure nothing stays allocated.
+static int32_t tier_new(gpud_ring* r, int64_t tier_bytes, const gpud_tier_ctl& c0, gpud_tier** out, const char* what) {
+  const int64_t F = r->F, B = tier_bytes & ~(int64_t)7, rec = tier_rec_bytes(F), row_max = rec + 8 * F * kBlock;
   gpud_tier* t = new gpud_tier();
   t->bytes = B;
   t->rec_bytes = rec;
@@ -1157,16 +1203,26 @@ extern "C" int32_t gpud_ring_tier_open(gpud_ring* r, int64_t tier_bytes) {
   if (e == cudaSuccess) e = cudaMalloc(&t->d_csum, (size_t)F * 8);
   if (e == cudaSuccess) e = cudaMalloc(&t->d_rowsz, (size_t)(r->cap / kBlock + 1) * 8);
   for (int i = 0; i < 2 && e == cudaSuccess; ++i) e = cudaEventCreate(&t->ev_enc[i]);
-  // the tier starts at the first row wholly in the ring: the rows the ring already completed are encoded now, as a push would
-  const int64_t whole = (r->total - ring_count(r) + kBlock - 1) / kBlock;
-  const gpud_tier_ctl c0{whole, whole, 0, 0, 0, 0, 0, 0};
   if (e == cudaSuccess) e = cudaMemcpyAsync(t->d_ctl, &c0, sizeof c0, cudaMemcpyHostToDevice, r->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(r->stream);
   if (e != cudaSuccess) {
     gpud_tier_free(t);
     cudaGetLastError();
-    return gpud_fail(r->ctx, e == cudaErrorMemoryAllocation ? GPUD_E_NOMEM : GPUD_E_CUDA, "tier_open: %s", cudaGetErrorString(e));
+    return gpud_fail(r->ctx, e == cudaErrorMemoryAllocation ? GPUD_E_NOMEM : GPUD_E_CUDA, "%s: %s", what, cudaGetErrorString(e));
   }
+  *out = t;
+  return GPUD_OK;
+}
+
+extern "C" int32_t gpud_ring_tier_open(gpud_ring* r, int64_t tier_bytes) {
+  if (!r) return GPUD_E_INVALID;
+  if (r->tier) return gpud_fail(r->ctx, GPUD_E_STATE, "tier_open: the ring already has a tier");
+  { const int32_t rc = tier_size_ok(r->ctx, r->cap, r->F, tier_bytes, "tier_open"); if (rc) return rc; }
+  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
+  // the tier starts at the first row wholly in the ring: the rows the ring already completed are encoded now, as a push would
+  const int64_t whole = (r->total - ring_count(r) + kBlock - 1) / kBlock;
+  gpud_tier* t = nullptr;
+  { const int32_t rc = tier_new(r, tier_bytes, gpud_tier_ctl{whole, whole, 0, 0, 0, 0, 0, 0}, &t, "tier_open"); if (rc) return rc; }
   t->next = whole;
   r->tier = t;
   return gpud_tier_push(r);
@@ -1256,5 +1312,447 @@ extern "C" int32_t gpudh_ring_tier_plan(int64_t cap, int32_t F, int64_t tier_byt
     int64_t* o = state + 6 * (i + 1);
     o[0] = c.first; o[1] = c.next; o[2] = c.used; o[3] = lost; o[4] = c.head; o[5] = c.tail;
   }
+  return GPUD_OK;
+}
+
+// ---- tier checkpoints (DESIGN.md "Ring tier checkpoint format") --------------------------------------------------------------------
+// A tier blob holds rows [from, next) of the tier as they lie in its byte ring, packed, each record's byte-offset word rewritten to the
+// row's offset in the rows section, then per field the checkpoint checksum of its samples.  The writer exports the rows on the device
+// (k_tier_copy), checks them with the decode's check pass (k_tier_gather over the export, k_ckpt_unpack<false>) and copies them out
+// once.  The restore checks a whole chain on the host (tier_chain_plan, which also places its rows), stages every blob's rows, runs the
+// check pass over each blob and over the rows the ring also holds, then loads the kept rows into a new tier (k_tier_copy).  The tier's
+// own marker follows its blobs; the ring's chain marker is never touched.
+namespace {
+
+constexpr char kTierMagic[2][8] = {{'G', 'P', 'U', 'D', 'R', 'T', 'K', '1'}, {'G', 'P', 'U', 'D', 'R', 'T', 'D', '1'}};   // [delta]
+// header words at their byte offsets (i64 unless noted); [kThEnd, 128) is zero
+enum : int64_t { kThFirst = 32, kThNext = 40, kThFrom = 48, kThPrevNext = 56, kThLost = 64, kThPrevLink = 72, kThRowsLen = 80, kThSumsLen = 88,
+                 kThEnd = 96 };
+
+uint64_t tier_link(uint64_t prev, int64_t next, int64_t first, const uint64_t* csum, int64_t F) {
+  uint64_t h = mix64(prev + kGolden);
+  h = mix64(h + (uint64_t)next);
+  h = mix64(h + (uint64_t)first);
+  for (int64_t f = 0; f < F; ++f) h = mix64(h + csum[f]);
+  return h;
+}
+
+// The check pass's geometry over n packed rows of F fields: unit f n + j is row j's block of field f (k_tier_gather's numbering), and
+// sample i = 0 of the field checksum is the first row's first sample.  Nothing is stored.
+CkGeo rows_geo(int64_t F, int64_t n) {
+  CkGeo g{};
+  g.cap = n * kBlock; g.start = 0; g.count = n * kBlock; g.nb = n; g.F = (int)F;
+  return g;
+}
+
+int32_t scratch_fail(gpud_ring* r, cudaError_t e, const char* what) {
+  return gpud_fail(r->ctx, e == cudaErrorMemoryAllocation ? GPUD_E_NOMEM : GPUD_E_CUDA, "%s: %s", what, cudaGetErrorString(e));
+}
+
+// What a tier blob of the ring would hold now: rows [from, next) with from = first (a base) or max(first, marker next) (a delta), and
+// where each lies in the byte ring (src) and will lie in the rows section (dst).  Synchronises the ring's stream.
+struct TierSpan {
+  int64_t first = 0, next = 0, from = 0, prev_next = 0, lost = 0, rows_len = 0;
+  uint64_t prev_link = 0;
+  std::vector<TierCopy> rows;
+};
+
+int32_t tier_span_of(gpud_ring* r, bool delta, TierSpan* s, const char* what) {
+  gpud_tier* t = r->tier;
+  if (!t) return gpud_fail(r->ctx, GPUD_E_STATE, "%s: the ring has no tier", what);
+  if (delta && !t->ck_marked)
+    return gpud_fail(r->ctx, GPUD_E_STATE, "%s: no tier checkpoint written or restored on this ring yet: write a full tier checkpoint", what);
+  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
+  { const int32_t rc = gpud_tier_span(r, &s->first, &s->next); if (rc) return rc; }
+  s->from = delta ? std::max(s->first, t->ck_next) : s->first;
+  s->prev_next = delta ? t->ck_next : 0;
+  s->prev_link = delta ? t->ck_link : 0;
+  s->lost = t->lost;
+  // the slot entries {offset, bytes} of rows [from, next): slots from % R on, wrapping at most once
+  const int64_t n = s->next - s->from, R = t->slots;
+  std::vector<int64_t> slot(2 * std::max<int64_t>(n, 1));
+  if (n > 0) {
+    const int64_t k0 = s->from % R, n1 = std::min(n, R - k0);
+    GPUD_CUDA(r->ctx, cudaMemcpy(slot.data(), t->d_slot + 2 * k0, 16 * n1, cudaMemcpyDeviceToHost));
+    if (n > n1) GPUD_CUDA(r->ctx, cudaMemcpy(slot.data() + 2 * n1, t->d_slot, 16 * (n - n1), cudaMemcpyDeviceToHost));
+  }
+  s->rows.resize(n);
+  int64_t off = 0;
+  for (int64_t j = 0; j < n; ++j) {
+    s->rows[j] = TierCopy{slot[2 * j], off, slot[2 * j + 1]};
+    off += slot[2 * j + 1];
+  }
+  s->rows_len = off;
+  return GPUD_OK;
+}
+
+int32_t tier_blob_bound(gpud_ring* r, bool delta, int64_t* bytes) {
+  if (!r || !bytes) return GPUD_E_INVALID;
+  TierSpan s;
+  { const int32_t rc = tier_span_of(r, delta, &s, delta ? "tier_checkpoint_delta" : "tier_checkpoint"); if (rc) return rc; }
+  *bytes = kHeaderBytes + s.rows_len + 8 * r->F;
+  return GPUD_OK;
+}
+
+// Both kinds of tier blob: the export, its check pass and one copy out, then the header and the checksums; the tier marker moves to it.
+int32_t write_tier_blob(gpud_ring* r, bool delta, void* out_v, int64_t cap, int64_t* n_bytes) {
+  if (!r || !n_bytes || cap < 0 || (cap > 0 && !out_v)) return GPUD_E_INVALID;
+  uint8_t* out = (uint8_t*)out_v;
+  const char* what = delta ? "tier_checkpoint_delta" : "tier_checkpoint";
+  TierSpan s;
+  { const int32_t rc = tier_span_of(r, delta, &s, what); if (rc) return rc; }
+  gpud_tier* t = r->tier;
+  const int64_t F = r->F, n = s.next - s.from, size = kHeaderBytes + s.rows_len + 8 * F;
+  *n_bytes = size;
+  if (cap < size) return gpud_fail(r->ctx, GPUD_E_CAPACITY, "%s needs %lld bytes", what, (long long)size);
+  bool pinned = false;
+  { const int32_t rc = host_pinned(r, out, &pinned); if (rc) return rc; }
+  std::vector<uint64_t> csum(F, 0);
+  float ms = 0.f;
+  CallScratch sc;
+  unsigned long long *d_rows_sec = nullptr, *d_offs = nullptr, *d_csum = nullptr;
+  if (n > 0) {
+    // the packed rows' slot table: row j (numbered from 0) at its section offset
+    std::vector<int64_t> idx(n), slot2(2 * n);
+    for (int64_t j = 0; j < n; ++j) { idx[j] = j; slot2[2 * j] = s.rows[j].dst; slot2[2 * j + 1] = s.rows[j].n; }
+    TierCopy* d_copy = nullptr;
+    int64_t *d_idx = nullptr, *d_slot2 = nullptr;
+    uint8_t* d_dir = nullptr;
+    cudaEvent_t ev[2];
+    cudaError_t e = sc.alloc(&d_rows_sec, s.rows_len / 8);
+    if (e == cudaSuccess) e = sc.alloc(&d_copy, n);
+    if (e == cudaSuccess) e = sc.alloc(&d_idx, n);
+    if (e == cudaSuccess) e = sc.alloc(&d_slot2, 2 * n);
+    if (e == cudaSuccess) e = sc.alloc(&d_dir, F * n);
+    if (e == cudaSuccess) e = sc.alloc(&d_offs, F * n);
+    if (e == cudaSuccess) e = sc.alloc(&d_csum, F);
+    for (int i = 0; i < 2 && e == cudaSuccess; ++i) e = sc.event(&ev[i]);
+    if (e != cudaSuccess) return scratch_fail(r, e, what);
+    GPUD_CUDA(r->ctx, cudaMemcpyAsync(d_copy, s.rows.data(), n * sizeof(TierCopy), cudaMemcpyHostToDevice, r->stream));
+    GPUD_CUDA(r->ctx, cudaMemcpyAsync(d_idx, idx.data(), n * 8, cudaMemcpyHostToDevice, r->stream));
+    GPUD_CUDA(r->ctx, cudaMemcpyAsync(d_slot2, slot2.data(), n * 16, cudaMemcpyHostToDevice, r->stream));
+    GPUD_CUDA(r->ctx, cudaMemsetAsync(d_csum, 0, F * 8, r->stream));
+    GPUD_CUDA(r->ctx, cudaEventRecord(ev[0], r->stream));
+    GPUD_CUDA(r->ctx, launch_copy(r, d_copy, n, t->d_buf, d_rows_sec));
+    GPUD_CUDA(r->ctx, launch_gather(r, d_idx, n, 0, (int)F, d_rows_sec, d_slot2, n, d_dir, d_offs));
+    GPUD_CUDA(r->ctx, launch_unpack<false>(r, rows_geo(F, n), d_dir, d_offs, d_rows_sec, d_csum));
+    GPUD_CUDA(r->ctx, cudaEventRecord(ev[1], r->stream));
+    GPUD_CUDA(r->ctx, cudaMemcpyAsync(csum.data(), d_csum, F * 8, cudaMemcpyDeviceToHost, r->stream));
+    GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));
+    GPUD_CUDA(r->ctx, cudaEventElapsedTime(&ms, ev[0], ev[1]));
+    { const int32_t rc = copy_out(r, out + kHeaderBytes, d_rows_sec, (size_t)s.rows_len, pinned); if (rc) return rc; }
+  }
+  memset(out, 0, kHeaderBytes);
+  memcpy(out, kTierMagic[delta], 8);
+  put<uint32_t>(out, 8, kVersion);
+  put<uint32_t>(out, 12, (uint32_t)F);
+  put<uint32_t>(out, 16, (uint32_t)r->W);
+  put<int64_t>(out, 24, r->cap);
+  put<int64_t>(out, kThFirst, s.first);
+  put<int64_t>(out, kThNext, s.next);
+  put<int64_t>(out, kThFrom, s.from);
+  put<int64_t>(out, kThPrevNext, s.prev_next);
+  put<int64_t>(out, kThLost, s.lost);
+  put<uint64_t>(out, kThPrevLink, s.prev_link);
+  put<int64_t>(out, kThRowsLen, s.rows_len);
+  put<int64_t>(out, kThSumsLen, 8 * F);
+  memcpy(out + kHeaderBytes + s.rows_len, csum.data(), 8 * F);
+  t->ck_marked = true;
+  t->ck_next = s.next;
+  t->ck_link = tier_link(s.prev_link, s.next, s.first, csum.data(), F);
+  t->ck_timed = true;
+  t->ck_encode_ms = ms;
+  t->ck_rows = n;
+  return GPUD_OK;
+}
+
+// One blob of a chain whose frame checked out: its header words, its rows [from, next) at off[j] of its rows section, and its link.
+struct TierBlob {
+  int64_t first = 0, next = 0, from = 0, prev_next = 0, lost = 0, rows_len = 0;
+  uint64_t prev_link = 0, link = 0;
+  const uint8_t *rows = nullptr, *sums = nullptr;
+  std::vector<int64_t> off, size;
+};
+
+// A chain checked against a ring of F fields, window W, capacity cap and `total` samples, and its rows placed in a new tier of
+// tier_bytes: the control word and slot table after placing rows [last first, last next) oldest first, and where each of those rows
+// went (-1: placed, then evicted by a newer one).
+struct TierPlan {
+  std::vector<TierBlob> blobs;
+  int64_t R = 0, whole = 0;
+  gpud_tier_ctl c{};
+  std::vector<int64_t> slot, place;
+  std::vector<int> blob_of;                     // the blob that holds each of rows [last first, last next)
+  std::vector<int64_t> row_of;                  // ... and its index in that blob's rows
+};
+
+// One blob's frame: magic, version and header padding; F, W and CAP; section lengths; the header words; its place in the chain after
+// blob i - 1; then every row: its record's first sample and offset word, its directory and word offsets, and the section filled.
+int32_t tier_blob_frame(gpud_ctx* ctx, int64_t F, int64_t W, int64_t cap, const uint8_t* in, int64_t n_bytes, int i, const TierBlob* prev,
+                        TierBlob* b) {
+  const char* what = "tier_restore";
+  if (!in || n_bytes < kHeaderBytes || (memcmp(in, kTierMagic[0], 8) != 0 && memcmp(in, kTierMagic[1], 8) != 0))
+    return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d is not a ring tier checkpoint", what, i);
+  const bool delta = memcmp(in, kTierMagic[1], 8) == 0;
+  if (get<uint32_t>(in, 8) != kVersion)
+    return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d: version %u, this library reads %u", what, i, get<uint32_t>(in, 8), kVersion);
+  for (int k = 20; k < kHeaderBytes; k = k == 23 ? (int)kThEnd : k + 1)
+    if (in[k]) return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d: header byte %d is not zero", what, i, k);
+  if (get<uint32_t>(in, 12) != (uint32_t)F) return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d: n_fields %u, the ring has %lld", what, i, get<uint32_t>(in, 12), (long long)F);
+  if (get<uint32_t>(in, 16) != (uint32_t)W) return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d: window %u, the ring has %lld", what, i, get<uint32_t>(in, 16), (long long)W);
+  if (get<int64_t>(in, 24) != cap)
+    return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d: capacity %lld, the ring has %lld", what, i, (long long)get<int64_t>(in, 24), (long long)cap);
+  b->rows_len = get<int64_t>(in, kThRowsLen);
+  const int64_t sums_len = get<int64_t>(in, kThSumsLen);
+  if (b->rows_len < 0 || (b->rows_len & 7) || b->rows_len > n_bytes || sums_len != 8 * F || kHeaderBytes + b->rows_len + sums_len != n_bytes)
+    return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d: section lengths do not add up to the %lld bytes given", what, i, (long long)n_bytes);
+  b->first = get<int64_t>(in, kThFirst); b->next = get<int64_t>(in, kThNext); b->from = get<int64_t>(in, kThFrom);
+  b->prev_next = get<int64_t>(in, kThPrevNext); b->lost = get<int64_t>(in, kThLost); b->prev_link = get<uint64_t>(in, kThPrevLink);
+  const bool words_ok = b->first >= 0 && b->first <= b->next && b->next <= ((int64_t)1 << 52) && b->lost >= 0 &&
+                        (delta ? b->prev_next <= b->next && b->from == std::max(b->first, b->prev_next) : b->prev_next == 0 && b->prev_link == 0 && b->from == b->first);
+  if (!words_ok)
+    return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d: first %lld, next %lld, from %lld, prev_next %lld and lost %lld disagree", what, i,
+                     (long long)b->first, (long long)b->next, (long long)b->from, (long long)b->prev_next, (long long)b->lost);
+  // its place in the chain
+  if (i == 0 && delta) return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob 0 is a delta: a chain starts with a full tier checkpoint", what);
+  if (i > 0 && !delta) return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d is a full tier checkpoint: only blob 0 may be", what, i);
+  if (prev) {
+    if (b->prev_link != prev->link)
+      return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d follows link %016llx, blob %d's is %016llx (out of order, or another chain)", what, i,
+                       (unsigned long long)b->prev_link, i - 1, (unsigned long long)prev->link);
+    if (b->prev_next != prev->next)
+      return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d follows row %lld, blob %d ends at row %lld", what, i, (long long)b->prev_next, i - 1, (long long)prev->next);
+    if (b->first < prev->first || b->lost < prev->lost)
+      return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d starts at row %lld with %lld lost, before blob %d's row %lld with %lld lost", what, i, (long long)b->first,
+                       (long long)b->lost, i - 1, (long long)prev->first, (long long)prev->lost);
+  }
+  // the rows: every address comes from the directories, which the offset words must agree with
+  b->rows = in + kHeaderBytes;
+  b->sums = in + kHeaderBytes + b->rows_len;
+  const int64_t rec = tier_rec_bytes(F), dir_at = kTierRecHead, woff_at = kTierRecHead + pad8(F);
+  int64_t off = 0;
+  for (int64_t row = b->from; row < b->next; ++row) {
+    if (off + rec > b->rows_len) return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d: row %lld is truncated", what, i, (long long)row);
+    const uint8_t* p = b->rows + off;
+    if (get<int64_t>(p, 0) != row * kBlock)
+      return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d: row %lld's record starts at sample %lld", what, i, (long long)row, (long long)get<int64_t>(p, 0));
+    if (get<int64_t>(p, 8) != off)
+      return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d: row %lld's offset word is %lld, the row is at %lld", what, i, (long long)row, (long long)get<int64_t>(p, 8),
+                       (long long)off);
+    int64_t words = 0;
+    for (int64_t f = 0; f < F; ++f) {
+      const int w = p[dir_at + f] & 127;
+      if (w > 64) return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d: row %lld field %lld has width %d", what, i, (long long)row, (long long)f, w);
+      const uint32_t wo = get<uint32_t>(p, woff_at + 4 * f);
+      if (wo != (uint64_t)words)
+        return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d: row %lld field %lld's word offset is %u, its directory gives %lld", what, i, (long long)row, (long long)f, wo,
+                         (long long)words);
+      words += 1 + ((kBlock - 1) * (int64_t)w + 63) / 64;
+    }
+    bool pad_ok = true;
+    for (int64_t k = F; k < pad8(F); ++k) pad_ok = pad_ok && p[dir_at + k] == 0;
+    for (int64_t k = 4 * F; k < pad8(4 * F); ++k) pad_ok = pad_ok && p[woff_at + k] == 0;
+    if (!pad_ok) return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d: row %lld's record padding is not zero", what, i, (long long)row);
+    const int64_t size = rec + 8 * words;
+    if (off + size > b->rows_len) return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d: row %lld is truncated", what, i, (long long)row);
+    b->off.push_back(off);
+    b->size.push_back(size);
+    off += size;
+  }
+  if (off != b->rows_len)
+    return gpud_fail(ctx, GPUD_E_INVALID, "%s: blob %d: the rows section has %lld bytes after its last row", what, i, (long long)(b->rows_len - off));
+  std::vector<uint64_t> sums(F);
+  memcpy(sums.data(), b->sums, 8 * F);
+  b->link = tier_link(b->prev_link, b->next, b->first, sums.data(), F);
+  return GPUD_OK;
+}
+
+// The whole chain, host only: tier_open's size rules, every blob's frame in chain order, the join with the ring, then the placement.
+int32_t tier_chain_plan(gpud_ctx* ctx, int64_t F, int64_t W, int64_t cap, int64_t total, int64_t tier_bytes, const void* const* blobs, const int64_t* n_bytes,
+                        int32_t n_blobs, TierPlan* p) {
+  const char* what = "tier_restore";
+  { const int32_t rc = tier_size_ok(ctx, cap, F, tier_bytes, what); if (rc) return rc; }
+  p->blobs.resize(n_blobs);
+  for (int32_t i = 0; i < n_blobs; ++i) {
+    const int32_t rc = tier_blob_frame(ctx, F, W, cap, (const uint8_t*)blobs[i], n_bytes[i], i, i ? &p->blobs[i - 1] : nullptr, &p->blobs[i]);
+    if (rc) return rc;
+  }
+  const TierBlob& last = p->blobs.back();
+  p->whole = (total - std::min(total, cap) + kBlock - 1) / kBlock;
+  if (last.next * kBlock > total)
+    return gpud_fail(ctx, GPUD_E_INVALID, "%s: the chain holds samples up to %lld, the ring has %lld", what, (long long)(last.next * kBlock), (long long)total);
+  if (last.next < p->whole)
+    return gpud_fail(ctx, GPUD_E_INVALID, "%s: the chain ends at row %lld, before the ring's first whole row %lld: the samples between are in neither", what,
+                     (long long)last.next, (long long)p->whole);
+  // rows [last first, last next), oldest first, each from the last blob that holds it (the blobs' rows are disjoint and ascending)
+  const int64_t B = tier_bytes & ~(int64_t)7, n = last.next - last.first;
+  p->R = tier_slots(B, F);
+  p->slot.assign(2 * p->R, 0);
+  p->place.assign(n, -1);
+  p->blob_of.assign(n, 0);
+  p->row_of.assign(n, 0);
+  p->c = gpud_tier_ctl{last.first, last.first, 0, 0, 0, 0, 0, 0};
+  int bi = 0;
+  for (int64_t k = last.first; k < last.next; ++k) {
+    while (p->blobs[bi].next <= k) ++bi;
+    const TierBlob& b = p->blobs[bi];
+    p->blob_of[k - last.first] = bi;
+    p->row_of[k - last.first] = k - b.from;
+    p->place[k - last.first] = gpud_tier_place(p->c, p->slot.data(), p->R, B, b.size[k - b.from]);
+  }
+  for (int64_t k = last.first; k < p->c.first; ++k) p->place[k - last.first] = -1;
+  return GPUD_OK;
+}
+
+}  // namespace
+
+extern "C" int32_t gpud_ring_tier_checkpoint_bound(gpud_ring* r, int64_t* bytes) { return tier_blob_bound(r, false, bytes); }
+extern "C" int32_t gpud_ring_tier_checkpoint_delta_bound(gpud_ring* r, int64_t* bytes) { return tier_blob_bound(r, true, bytes); }
+extern "C" int32_t gpud_ring_tier_checkpoint(gpud_ring* r, void* out, int64_t cap, int64_t* n_bytes) { return write_tier_blob(r, false, out, cap, n_bytes); }
+extern "C" int32_t gpud_ring_tier_checkpoint_delta(gpud_ring* r, void* out, int64_t cap, int64_t* n_bytes) {
+  return write_tier_blob(r, true, out, cap, n_bytes);
+}
+
+extern "C" int32_t gpud_ring_tier_restore(gpud_ring* r, int64_t tier_bytes, const void* const* blobs, const int64_t* n_bytes, int32_t n_blobs) {
+  if (!r || n_blobs < 1 || !blobs || !n_bytes) return GPUD_E_INVALID;
+  const char* what = "tier_restore";
+  if (r->tier) return gpud_fail(r->ctx, GPUD_E_STATE, "%s: the ring already has a tier", what);
+  const int64_t F = r->F;
+  TierPlan p;
+  { const int32_t rc = tier_chain_plan(r->ctx, F, r->W, r->cap, r->total, tier_bytes, blobs, n_bytes, n_blobs, &p); if (rc) return rc; }
+  const TierBlob& last = p.blobs.back();
+  GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
+  GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));
+  // staging: every blob's rows section, one after the other; staged row q (all blobs' rows in chain order) at stage_off[q]
+  std::vector<int64_t> blob_q0(n_blobs + 1, 0), blob_at(n_blobs + 1, 0), sslot;
+  for (int32_t i = 0; i < n_blobs; ++i) {
+    blob_q0[i + 1] = blob_q0[i] + (int64_t)p.blobs[i].off.size();
+    blob_at[i + 1] = blob_at[i] + p.blobs[i].rows_len;
+    for (size_t j = 0; j < p.blobs[i].off.size(); ++j) {
+      sslot.push_back(blob_at[i] + p.blobs[i].off[j]);
+      sslot.push_back(p.blobs[i].size[j]);
+    }
+  }
+  const int64_t Q = blob_q0[n_blobs], stage_bytes_all = blob_at[n_blobs];
+  // the rows held by both the chain and the ring: [ov0, last next), staged rows q_ov.. of the last blobs
+  const int64_t ov0 = std::max(p.whole, last.first), n_ov = last.next - ov0;
+  const int64_t q_ov = n_ov > 0 ? blob_q0[p.blob_of[ov0 - last.first]] + p.row_of[ov0 - last.first] : 0;
+  CallScratch sc;
+  unsigned long long *d_stage = nullptr, *d_offs = nullptr, *d_csum = nullptr, *d_words = nullptr;
+  int64_t *d_idx = nullptr, *d_sslot = nullptr;
+  uint8_t* d_dir = nullptr;
+  cudaEvent_t ev[4];
+  std::vector<int64_t> idx(std::max<int64_t>(Q, 1));
+  for (int64_t q = 0; q < Q; ++q) idx[q] = q;
+  const int64_t units = F * (Q + n_ov);
+  cudaError_t e = sc.alloc(&d_stage, stage_bytes_all / 8);
+  if (e == cudaSuccess) e = sc.alloc(&d_idx, Q);
+  if (e == cudaSuccess) e = sc.alloc(&d_sslot, 2 * Q);
+  if (e == cudaSuccess) e = sc.alloc(&d_dir, units + F * n_ov);
+  if (e == cudaSuccess) e = sc.alloc(&d_offs, units);
+  if (e == cudaSuccess) e = sc.alloc(&d_words, F * n_ov);
+  if (e == cudaSuccess) e = sc.alloc(&d_csum, F * (n_blobs + 2));
+  for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = sc.event(&ev[i]);
+  if (e != cudaSuccess) return scratch_fail(r, e, what);
+  for (int32_t i = 0; i < n_blobs; ++i) {
+    bool pinned = false;
+    { const int32_t rc = host_pinned(r, p.blobs[i].rows, &pinned); if (rc) return rc; }
+    const int32_t rc = copy_in(r, (uint8_t*)d_stage + blob_at[i], p.blobs[i].rows, (size_t)p.blobs[i].rows_len, pinned);
+    if (rc) return rc;
+  }
+  if (Q > 0) {
+    GPUD_CUDA(r->ctx, cudaMemcpyAsync(d_idx, idx.data(), Q * 8, cudaMemcpyHostToDevice, r->stream));
+    GPUD_CUDA(r->ctx, cudaMemcpyAsync(d_sslot, sslot.data(), Q * 16, cudaMemcpyHostToDevice, r->stream));
+  }
+  GPUD_CUDA(r->ctx, cudaMemsetAsync(d_csum, 0, F * (n_blobs + 2) * 8, r->stream));
+  // the check pass: each blob's rows decoded against its checksums, and the rows the ring also holds decoded and re-encoded from it
+  GPUD_CUDA(r->ctx, cudaEventRecord(ev[0], r->stream));
+  for (int32_t i = 0; i < n_blobs; ++i) {
+    const int64_t n = blob_q0[i + 1] - blob_q0[i];
+    if (n == 0) continue;
+    GPUD_CUDA(r->ctx, launch_gather(r, d_idx + blob_q0[i], n, 0, (int)F, d_stage, d_sslot, Q, d_dir + F * blob_q0[i], d_offs + F * blob_q0[i]));
+    GPUD_CUDA(r->ctx, launch_unpack<false>(r, rows_geo(F, n), d_dir + F * blob_q0[i], d_offs + F * blob_q0[i], d_stage, d_csum + F * i));
+  }
+  if (n_ov > 0) {
+    uint8_t* dir_ov = d_dir + F * Q;
+    GPUD_CUDA(r->ctx, launch_gather(r, d_idx + q_ov, n_ov, 0, (int)F, d_stage, d_sslot, Q, dir_ov, d_offs + F * Q));
+    GPUD_CUDA(r->ctx, launch_unpack<false>(r, rows_geo(F, n_ov), dir_ov, d_offs + F * Q, d_stage, d_csum + F * n_blobs));
+    GPUD_CUDA(r->ctx, launch_size(r, ckpt_geo(r, ov0 * kBlock, n_ov * kBlock), dir_ov + F * n_ov, d_words, d_csum + F * (n_blobs + 1)));
+  }
+  GPUD_CUDA(r->ctx, cudaEventRecord(ev[1], r->stream));
+  std::vector<uint64_t> csum(F * (n_blobs + 2));
+  GPUD_CUDA(r->ctx, cudaMemcpyAsync(csum.data(), d_csum, csum.size() * 8, cudaMemcpyDeviceToHost, r->stream));
+  GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));
+  for (int32_t i = 0; i < n_blobs; ++i)
+    for (int64_t f = 0; f < F; ++f)
+      if (csum[F * i + f] != get<uint64_t>(p.blobs[i].sums, 8 * f))
+        return gpud_fail(r->ctx, GPUD_E_INVALID, "%s: blob %d: checksum mismatch in field %lld: the blob is corrupt", what, i, (long long)f);
+  for (int64_t f = 0; f < F && n_ov > 0; ++f)
+    if (csum[F * n_blobs + f] != csum[F * (n_blobs + 1) + f])
+      return gpud_fail(r->ctx, GPUD_E_INVALID, "%s: rows [%lld, %lld) of the chain differ from the ring's samples in field %lld: the chain is from another ring",
+                       what, (long long)ov0, (long long)last.next, (long long)f);
+  float ms_check = 0.f, ms_load = 0.f;
+  GPUD_CUDA(r->ctx, cudaEventElapsedTime(&ms_check, ev[0], ev[1]));
+  // the load: the kept rows from the staging to where the placement put them, into a new tier with the placement's slot table
+  std::vector<TierCopy> kept;
+  for (int64_t k = p.c.first; k < last.next; ++k) {
+    const int64_t a = k - last.first;
+    const int64_t q = blob_q0[p.blob_of[a]] + p.row_of[a];
+    kept.push_back(TierCopy{sslot[2 * q], p.place[a], sslot[2 * q + 1]});
+  }
+  TierCopy* d_kept = nullptr;
+  e = sc.alloc(&d_kept, kept.size());
+  if (e != cudaSuccess) return scratch_fail(r, e, what);
+  gpud_tier* t = nullptr;
+  { const int32_t rc = tier_new(r, tier_bytes, p.c, &t, what); if (rc) return rc; }
+  e = cudaMemcpyAsync(t->d_slot, p.slot.data(), p.slot.size() * 8, cudaMemcpyHostToDevice, r->stream);
+  if (e == cudaSuccess && !kept.empty()) e = cudaMemcpyAsync(d_kept, kept.data(), kept.size() * sizeof(TierCopy), cudaMemcpyHostToDevice, r->stream);
+  if (e == cudaSuccess) e = cudaEventRecord(ev[2], r->stream);
+  if (e == cudaSuccess) e = launch_copy(r, d_kept, (int64_t)kept.size(), d_stage, t->d_buf);
+  if (e == cudaSuccess) e = cudaEventRecord(ev[3], r->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(r->stream);
+  if (e == cudaSuccess) e = cudaEventElapsedTime(&ms_load, ev[2], ev[3]);
+  if (e != cudaSuccess) {
+    gpud_tier_free(t);
+    return gpud_fail(r->ctx, GPUD_E_CUDA, "%s: %s", what, cudaGetErrorString(e));
+  }
+  t->next = last.next;
+  t->lost = last.lost;
+  t->ck_marked = true;
+  t->ck_next = last.next;
+  t->ck_link = last.link;
+  t->ck_timed = true;
+  t->ck_decode_ms = ms_check + ms_load;
+  t->ck_rows = (int64_t)kept.size();
+  r->tier = t;
+  // rows [last next, total / 1024) from the ring, as the open encodes them
+  return gpud_tier_push(r);
+}
+
+extern "C" int32_t gpud_ring_tier_checkpoint_stats(gpud_ring* r, float* encode_ms, float* decode_ms, int64_t* rows) {
+  if (!r) return GPUD_E_INVALID;
+  if (!r->tier || !r->tier->ck_timed) return gpud_fail(r->ctx, GPUD_E_STATE, "tier_checkpoint_stats: no tier checkpoint or restore on this ring yet");
+  if (encode_ms) *encode_ms = r->tier->ck_encode_ms;
+  if (decode_ms) *decode_ms = r->tier->ck_decode_ms;
+  if (rows) *rows = r->tier->ck_rows;
+  return GPUD_OK;
+}
+
+// Test hook (include/gpud_b200_hooks.h): tier_restore's host verdict and placement, without a ring or a device.
+extern "C" int32_t gpudh_ring_tier_chain_plan(int32_t n_fields, int32_t window, int64_t cap, int64_t total, int64_t tier_bytes, const void* const* blobs,
+                                              const int64_t* n_bytes, int32_t n_blobs, int64_t* row_off, int64_t row_cap, int64_t* n_rows, int64_t* state,
+                                              char* msg, int32_t msg_cap) {
+  if (n_fields < 1 || n_blobs < 1 || !blobs || !n_bytes || !n_rows || !state || row_cap < 0 || (row_cap > 0 && !row_off)) return GPUD_E_INVALID;
+  gpud_ctx ctx;
+  TierPlan p;
+  const int32_t rc = tier_chain_plan(&ctx, n_fields, window, cap, total, tier_bytes, blobs, n_bytes, n_blobs, &p);
+  if (msg && msg_cap > 0) snprintf(msg, msg_cap, "%s", ctx.last_error.c_str());
+  if (rc) return rc;
+  const int64_t n = (int64_t)p.place.size();
+  *n_rows = n;
+  if (row_cap < n) return GPUD_E_CAPACITY;
+  std::copy(p.place.begin(), p.place.end(), row_off);
+  const int64_t s[6] = {p.c.first, p.c.next, p.c.used, p.blobs.back().lost, p.c.head, p.c.tail};
+  std::copy(s, s + 6, state);
   return GPUD_OK;
 }

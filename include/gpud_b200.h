@@ -421,7 +421,8 @@ int32_t gpud_ring_checkpoint_stats(gpud_ring* ring, float* encode_ms, float* dec
  * On a tiered ring gpud_ring_reduce_ranges and gpud_ring_reduce_range_sets take any range with len >= 1, first + len <= total and
  * first >= min(total - count, first_sample) (gpud_ring_tier_counts), with the same definitions and every other refusal unchanged;
  * min / max / p99 / n_over equal bit for bit what a ring of a CAP that holds all those samples gives.  gpud_rings_reduce_range_sets,
- * gpud_box_query, checkpoints and deltas ignore the tier (a restored ring has none; restore into a tiered ring -> GPUD_E_STATE).
+ * gpud_box_query, checkpoints and deltas ignore the tier (a restored ring has none until gpud_ring_tier_restore below; restore into a
+ * tiered ring -> GPUD_E_STATE).
  * Open: once per ring (again -> GPUD_E_STATE); allocates tier_bytes (rounded down to 8) for the rows, plus 8 KiB per field and 16 B
  * per row it could hold, on the ring's device until gpud_ring_destroy.  CAP < 2048, or tier_bytes below one row coded at 64 bits and
  * its record (8192 F + 16 + pad8(F) + pad8(4 F)) -> GPUD_E_INVALID; a failed allocation -> GPUD_E_NOMEM / GPUD_E_CUDA with the ring
@@ -433,6 +434,38 @@ int32_t gpud_ring_tier_counts(gpud_ring* ring, int64_t* first_sample, int64_t* n
 /* Synchronise the ring's stream: device ms of the last encode (the last push that completed a row; 0 before one), of the last range
  * call's decode (0 if none touched the tier), and the blocks of that encode by mode ([2]: RAW, INT).  GPUD_E_STATE without a tier. */
 int32_t gpud_ring_tier_stats(gpud_ring* ring, float* encode_ms, float* decode_ms, int64_t* blocks_by_mode);
+/* Tier checkpoints (DESIGN.md §2 "Tier", format: DESIGN.md "Ring tier checkpoint format"): the tier's rows as bytes that outlive the
+ * process, so that a restarted daemon keeps its history beyond CAP.  A full tier checkpoint holds the rows [first, next) the tier holds,
+ * a tier delta the rows [max(first, marker next), next) and the header's first, next and lost count.  The rows are copied as the tier
+ * coded them, with no re-encode.  Each tier keeps a tier marker (next row and link of the last tier blob it wrote or was restored from),
+ * apart from the ring's chain marker, which tier calls never read or move; ring checkpoints and deltas are unchanged by a tier.
+ * Exact size of the next full tier checkpoint / tier delta.  Synchronises the ring's stream; no tier -> GPUD_E_STATE. */
+int32_t gpud_ring_tier_checkpoint_bound(gpud_ring* ring, int64_t* bytes);
+/* Synchronise the ring's stream, then write the tier's rows into out (pageable or pinned) and set the tier marker.  No tier
+ * -> GPUD_E_STATE; cap too small -> GPUD_E_CAPACITY with *n_bytes = the exact size, nothing else changes.  Synchronous. */
+int32_t gpud_ring_tier_checkpoint(gpud_ring* ring, void* out, int64_t cap, int64_t* n_bytes);
+int32_t gpud_ring_tier_checkpoint_delta_bound(gpud_ring* ring, int64_t* bytes);
+/* As gpud_ring_tier_checkpoint, for the rows since the tier marker (none new: a valid delta of header and checksums).  No tier, or
+ * no tier marker yet -> GPUD_E_STATE (write a full tier checkpoint).  Rows evicted or lost since the marker need nothing: the restore
+ * drops every row below the last blob's first. */
+int32_t gpud_ring_tier_checkpoint_delta(gpud_ring* ring, void* out, int64_t cap, int64_t* n_bytes);
+/* Open the tier of a ring that has none from a chain: blobs[0] a full tier checkpoint, then its deltas in order, n_bytes[i] each
+ * (pageable or pinned).  Restore the ring's own chain first (gpud_ring_restore, _restore_delta), then its tier.  The tier is what
+ * gpud_ring_tier_open(tier_bytes) would give, except that it also holds the chain's rows [last first, last next), placed oldest first
+ * as pushes place rows (a smaller tier_bytes keeps the newest of them); rows [last next, total / 1024) are then encoded from the ring.
+ * The lost count carries over and the tier marker is the chain's last blob.  With tier_bytes >= the original's bytes_used the tier
+ * holds every row the original held.  Every refusal comes before the tier exists and leaves the ring without one, nothing allocated,
+ * gpud_last_error naming the blob, row or field: a tier already -> GPUD_E_STATE; tier_bytes or CAP that gpud_ring_tier_open refuses,
+ * malformed bytes (magic, version, header padding, F / W / CAP not the ring's, section lengths, a record not at sample 1024 row or with
+ * another offset word, a width above 64, padding, word offsets that are not the directory's prefix sums, rows that do not fill their
+ * section), a broken chain (blob 0 not a full one, a later one not a delta or not following its predecessor's link and next), a chain
+ * that does not join the ring (next row past the ring's total, or before its first whole row), a checksum mismatch of any blob's rows,
+ * or the rows both the chain and the ring hold differing (a chain from another ring) -> GPUD_E_INVALID.  Synchronous. */
+int32_t gpud_ring_tier_restore(gpud_ring* ring, int64_t tier_bytes, const void* const* blobs, const int64_t* n_bytes, int32_t n_blobs);
+/* The last tier checkpoint or tier restore: device ms of the checkpoint's export and check pass, of the restore's check pass and
+ * load, and the rows the last of them wrote or loaded into the tier.  Any pointer may be NULL; GPUD_E_STATE without a tier or before
+ * the first. */
+int32_t gpud_ring_tier_checkpoint_stats(gpud_ring* ring, float* encode_ms, float* decode_ms, int64_t* rows);
 
 /* ------------------------------------------------------------------------------------------------
  * components.Component (components/types.go:20-66) for the three paths this library replaces, as objects: what a Go file that

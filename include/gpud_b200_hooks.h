@@ -98,6 +98,14 @@ int32_t gpudh_ring_tier_split(int64_t total, int64_t cap, int32_t n_fields, int6
 int32_t gpudh_ring_tier_row(gpud_ring* r, int64_t row, void* out, int64_t cap, int64_t* n_bytes);
 /* At most max_fields fields per decoded group of a range call that reaches the tier (0: as many as 1 GiB of decoded rows allows). */
 int32_t gpudh_ring_tier_group(gpud_ring* r, int32_t max_fields);
+/* gpud_ring_tier_restore's host work, without a ring or a device: the verdict on a chain of n_blobs tier blobs for a ring of n_fields
+ * fields, window, capacity cap and `total` samples restoring into tier_bytes (every refusal but GPUD_E_STATE and the check pass's),
+ * its text into msg (msg_cap bytes, may be NULL), and the placement of the chain's rows [last first, last next): *n_rows of them,
+ * row_off[k - last first] the byte offset row k went to or -1 if a newer row evicted it (GPUD_E_CAPACITY if row_cap is smaller), and
+ * state[6] = {first row, next row, bytes in use, rows lost, head, tail} after it, before rows are encoded from the ring. */
+int32_t gpudh_ring_tier_chain_plan(int32_t n_fields, int32_t window, int64_t cap, int64_t total, int64_t tier_bytes, const void* const* blobs,
+                                   const int64_t* n_bytes, int32_t n_blobs, int64_t* row_off, int64_t row_cap, int64_t* n_rows, int64_t* state,
+                                   char* msg, int32_t msg_cap);
 /* the host plan of one gpud_ring_windows_reduce of a handle of span x W samples every hop x W (P) on a ring of `total` pushed
  * samples and capacity cap, its history of at most `history` windows now holding [first, next), reseed = 1 when the handle re-seeds
  * its EMA at window next (opened, or restarted with nothing reduced since).  out[8] as gpudh_ring_stream_plan; ema[5] = {physical
