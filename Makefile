@@ -3,12 +3,12 @@ NVCC ?= /usr/local/cuda/bin/nvcc
 ARCH := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xcompiler -Wall -Xptxas -v
 SRC := gpud_b200/csrc
-OBJS := $(SRC)/api.o $(SRC)/ring.o $(SRC)/ring_ckpt.o $(SRC)/select.o $(SRC)/ranges.o $(SRC)/box_query.o $(SRC)/kmsg_scan.o $(SRC)/kmsg_dedup.o $(SRC)/ib_scan.o $(SRC)/fabric.o $(SRC)/catalog.o $(SRC)/host_component.o $(SRC)/component_abi.o $(SRC)/kmsg_stateful.o $(SRC)/poller.o $(SRC)/store_sqlite.o
+OBJS := $(SRC)/api.o $(SRC)/ring.o $(SRC)/ring_ckpt.o $(SRC)/tier.o $(SRC)/select.o $(SRC)/ranges.o $(SRC)/box_query.o $(SRC)/kmsg_scan.o $(SRC)/kmsg_dedup.o $(SRC)/ib_scan.o $(SRC)/fabric.o $(SRC)/catalog.o $(SRC)/host_component.o $(SRC)/component_abi.o $(SRC)/kmsg_stateful.o $(SRC)/poller.o $(SRC)/store_sqlite.o
 LIB := gpud_b200/libgpud_b200.so
 
 all: $(LIB) gpud_b200/gpud-scan oracle
 
-$(SRC)/%.o: $(SRC)/%.cu $(SRC)/internal.h $(SRC)/segsel.h $(SRC)/catalog.h include/gpud_b200.h
+$(SRC)/%.o: $(SRC)/%.cu $(SRC)/internal.h $(SRC)/segsel.h $(SRC)/ckpt.h $(SRC)/catalog.h include/gpud_b200.h
 	$(NVCC) $(NVFLAGS) -c $< -o $@ 2> $@.ptxas.log || (cat $@.ptxas.log; exit 1)
 
 $(SRC)/catalog.o: $(SRC)/catalog.cpp $(SRC)/catalog.h $(SRC)/catalog_data.inc include/gpud_b200.h

@@ -80,10 +80,10 @@ struct gpud_ring {
   bool ck_marked = false;
   int64_t ck_total = 0, ck_gen = 0;                    // ... total and handle_gen at the marker
   uint64_t ck_link = 0;                                // ... and that blob's chain link
-  gpud_tier* tier = nullptr;                           // gpud_ring_tier_open: the delta-coded tier of older samples (ring_ckpt.cu)
+  gpud_tier* tier = nullptr;                           // gpud_ring_tier_open: the delta-coded tier of older samples (tier.cu)
 };
 
-// The tier of a ring (ring_ckpt.cu, DESIGN.md §2 "Tier"): block rows k = samples [1024 k, 1024 (k + 1)) of every field, each coded as
+// The tier of a ring (tier.cu, DESIGN.md §2 "Tier"): block rows k = samples [1024 k, 1024 (k + 1)) of every field, each coded as
 // the checkpoint codes a block, kept in a byte ring of whole rows.  Placement and eviction run on the device (only it knows the coded
 // sizes): the control word below, the slot table {byte offset, bytes} of row k at slot k % slots and the row records live there.  The
 // host knows which rows were encoded (next) and lost; a query reads the control word to learn the rows still held.
@@ -120,12 +120,12 @@ struct gpud_tier {
   float ck_encode_ms = 0.f, ck_decode_ms = 0.f;
   int64_t ck_rows = 0;             // ... rows the last of either wrote or loaded
 };
-// ring_ckpt.cu: after every push into a tiered ring, on its stream: the loss rule, then the encode of every row the push completed.
+// tier.cu: after every push into a tiered ring, on its stream: the loss rule, then the encode of every row the push completed.
 int32_t gpud_tier_push(gpud_ring* r);
 void gpud_tier_free(gpud_tier* t);
-// ring_ckpt.cu: synchronise the ring's stream and read the rows the tier holds, [*first, *next).
-int32_t gpud_tier_span(gpud_ring* r, int64_t* first, int64_t* next);
-// ring_ckpt.cu: fields [f0, f0 + G) of rows[0, n_rows) (each held by the tier, ascending) into virtual rows 0 .. n_rows - 1 of a ring
+// tier.cu: synchronise the ring's stream and read the tier's control word (the rows it holds, [first, next), and its bytes in use).
+int32_t gpud_tier_read_ctl(gpud_ring* r, gpud_tier_ctl* c);
+// tier.cu: fields [f0, f0 + G) of rows[0, n_rows) (each held by the tier, ascending) into virtual rows 0 .. n_rows - 1 of a ring
 // of G fields and capacity vcap, then the first tail_n samples of row rows_tail (not yet coded) from the ring itself into virtual row
 // n_rows; the sample ring by k_ring_append's rule.  The virtual ring and its sample ring are the tier's scratch (*vring, *vsmp).
 int32_t gpud_tier_decode(gpud_ring* r, const std::vector<int64_t>& rows, int64_t rows_tail, int64_t tail_n, int f0, int G, int64_t vcap,

@@ -319,10 +319,10 @@ int32_t reduce_subset(const gpud_ring_view& v, int64_t home_total, const std::ve
 static int32_t reduce_sets_tier(gpud_ring* r, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets,
                                 double* out_f64, uint32_t* out_n_over) {
   gpud_tier* t = r->tier;
-  int64_t t_first = 0, t_next = 0;
-  { int32_t rc = gpud_tier_span(r, &t_first, &t_next); if (rc) return rc; }
+  gpud_tier_ctl c;
+  { int32_t rc = gpud_tier_read_ctl(r, &c); if (rc) return rc; }
   TierSplit sp;
-  { int32_t rc = tier_split(r->ctx, r->total, r->cap, r->F, t_first, t_next, first, len, n_ranges, set_off, n_sets, &sp); if (rc) return rc; }
+  { int32_t rc = tier_split(r->ctx, r->total, r->cap, r->F, c.first, c.next, first, len, n_ranges, set_off, n_sets, &sp); if (rc) return rc; }
   if (sp.rows.empty()) return reduce_sets(gpud_view(r), r->total, nullptr, 1, nullptr, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over, &r->ranges);
   std::vector<int64_t> ids[2];
   for (int64_t s = 0; s < n_sets; ++s) ids[sp.route[s]].push_back(s);
@@ -348,8 +348,8 @@ static int32_t reduce_sets_tier(gpud_ring* r, const int64_t* first, const int64_
   // the virtual ring: rows held by the tier are decoded, the newest one (partial) is copied from the ring
   std::vector<int64_t> dec(sp.rows);
   int64_t tail_n = 0;
-  if (dec.back() == t_next) {
-    tail_n = r->total - t_next * GPUD_TIER_ROW;
+  if (dec.back() == c.next) {
+    tail_n = r->total - c.next * GPUD_TIER_ROW;
     dec.pop_back();
   }
   const int64_t vcap = (int64_t)sp.rows.size() * GPUD_TIER_ROW;
@@ -361,7 +361,7 @@ static int32_t reduce_sets_tier(gpud_ring* r, const int64_t* first, const int64_
   for (int f0 = 0; f0 < F; f0 += G) {
     const int g = std::min(G, F - f0);
     double *vring = nullptr, *vsmp = nullptr;
-    { int32_t rc = gpud_tier_decode(r, dec, t_next, tail_n, f0, g, vcap, smp_shift, smp_slots, &vring, &vsmp); if (rc) return rc; }
+    { int32_t rc = gpud_tier_decode(r, dec, c.next, tail_n, f0, g, vcap, smp_shift, smp_slots, &vring, &vsmp); if (rc) return rc; }
     gpud_ring_view v = gpud_view(r);   // the virtual ring: fields [f0, f0 + g) of the decoded rows
     v.F = g;
     v.cap = vcap;
