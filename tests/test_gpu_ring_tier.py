@@ -4,7 +4,8 @@ EMA within oracle/SPEC.md's tolerance), on NVML-like uint32 rows pushed raw (INT
 straddling its boundary with the ring, wholly in the ring, 1 sample, <= 1024, > 1024 and > CAP.  Every row's bytes against the host
 model (tests/ring_tier.py), its placement and tier_counts after every push against the model's, refusals before the tier with
 nothing written, every push entry point and raw dtype giving the same bytes, a tiered ring's reduce, handles and checkpoints equal to
-an untiered twin's, and forced small field groups giving the same answers.  Run on an H100: pytest -m gpu."""
+an untiered twin's, and forced small field groups giving the same answers.  The range path's routes on the decoded ring, wide rows,
+natural field groups and capacities that are not a multiple of 1024 are test_gpu_tier_paths.py's.  Run on an H100: pytest -m gpu."""
 import ctypes as C
 
 import numpy as np
