@@ -849,6 +849,8 @@ def lib() -> C.CDLL:
         "gpud_ring_tier_stats": (i32, [vp, C.POINTER(C.c_float), C.POINTER(C.c_float), vp]),
         "gpudh_ring_tier_plan": (i32, [i64, i32, i64, i64, vp, i64, vp, i64, vp, vp]),
         "gpudh_ring_tier_split": (i32, [i64, i64, i32, i64, i64, vp, vp, i64, vp, i64, vp, vp, vp, i64, C.POINTER(i64), C.POINTER(i64)]),
+        "gpudh_rings_tier_split": (i32, [vp, i32, i64, vp, vp, vp, vp, vp, i64, vp, i64, vp, vp, vp, C.POINTER(C.c_int32), vp, vp, vp, vp, vp, i64,
+                                         C.POINTER(i64)]),
         "gpudh_ring_tier_row": (i32, [vp, i64, vp, i64, C.POINTER(i64)]), "gpudh_ring_tier_group": (i32, [vp, i32]),
         "gpud_ring_tier_checkpoint_bound": (i32, [vp, C.POINTER(i64)]), "gpud_ring_tier_checkpoint": (i32, [vp, vp, i64, C.POINTER(i64)]),
         "gpud_ring_tier_checkpoint_delta_bound": (i32, [vp, C.POINTER(i64)]),

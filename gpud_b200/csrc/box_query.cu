@@ -503,7 +503,7 @@ static int32_t box_local_sets(gpud_box_query* q) {
   const int64_t nm = (int64_t)mine.size();
   std::vector<double> o;
   std::vector<uint32_t> nv;
-  const int32_t rc = reduce_subset(gpud_view(r), r->total, sets, q->first.data(), q->len.data(), q->set_off.data(), nullptr, &q->local, o, nv);
+  const int32_t rc = reduce_subset(gpud_view(r), ring_table(&r, 1), sets, nullptr, q->first.data(), q->len.data(), q->set_off.data(), &q->local, o, nv);
   if (rc) return rc;
   for (int f = 0; f < F; ++f)
     for (int64_t k = 0; k < nm; ++k) {

@@ -101,16 +101,10 @@ struct gpud_tier {
   unsigned long long *d_words = nullptr, *d_offs = nullptr, *d_csum = nullptr;
   int64_t* d_rowsz = nullptr;
   int64_t units_cap = 0;
-  cudaEvent_t ev_enc[2] = {nullptr, nullptr}, ev_dec[2] = {nullptr, nullptr};
+  cudaEvent_t ev_enc[2] = {nullptr, nullptr};
   bool enc_timed = false;
-  float dec_ms = 0.f;              // the last query's decode, all its field groups
+  float dec_ms = 0.f;              // the last range call homed on this ring that decoded: all its decode, every field group
   int group_max = 0;               // > 0: at most this many fields per decoded group (gpudh_ring_tier_group)
-  // query scratch, grown on demand: the virtual ring, its sample ring, the rows to decode and their directory
-  double* d_vring = nullptr;  size_t vring_cap = 0;
-  double* d_vsmp = nullptr;  size_t vsmp_cap = 0;
-  int64_t* d_rows = nullptr;  size_t rows_cap = 0;
-  uint8_t* d_vdir = nullptr;  size_t vdir_cap = 0;
-  unsigned long long* d_voffs = nullptr;  size_t voffs_cap = 0;
   // The tier marker (DESIGN.md "Ring tier checkpoint format"): the next row and link of the last tier blob written or restored, apart
   // from the ring's own chain marker.
   bool ck_marked = false;
@@ -125,11 +119,21 @@ int32_t gpud_tier_push(gpud_ring* r);
 void gpud_tier_free(gpud_tier* t);
 // tier.cu: synchronise the ring's stream and read the tier's control word (the rows it holds, [first, next), and its bytes in use).
 int32_t gpud_tier_read_ctl(gpud_ring* r, gpud_tier_ctl* c);
-// tier.cu: fields [f0, f0 + G) of rows[0, n_rows) (each held by the tier, ascending) into virtual rows 0 .. n_rows - 1 of a ring
-// of G fields and capacity vcap, then the first tail_n samples of row rows_tail (not yet coded) from the ring itself into virtual row
-// n_rows; the sample ring by k_ring_append's rule.  The virtual ring and its sample ring are the tier's scratch (*vring, *vsmp).
-int32_t gpud_tier_decode(gpud_ring* r, const std::vector<int64_t>& rows, int64_t rows_tail, int64_t tail_n, int f0, int G, int64_t vcap,
-                         int smp_shift, int64_t smp_slots, double** vring, double** vsmp);
+// A slot of a virtual box (ranges.cu): a ring of G fields and capacity vcap at `ring` [G][vcap], its sample ring at `sample`
+// [G][smp_slots] kept by k_ring_append's rule.
+struct gpud_vslot { double* ring; double* sample; int64_t vcap; int smp_shift; int64_t smp_slots; };
+// tier.cu: fields [f0, f0 + G) of rows d_rows[0, n) of ring o's tier (each held, ascending) decoded into virtual columns
+// [vcol0, vcol0 + 1024 n) of slot s, on ring h's device and stream: o's coded rows are read in place (through the peer mapping when
+// o lives on another device), dir / offs [G n] are h's scratch and csum [G] takes the field sums no one reads.
+cudaError_t gpud_tier_decode(const gpud_ring* h, const gpud_ring* o, const int64_t* d_rows, int64_t n, int f0, int G, const gpud_vslot& s,
+                             int64_t vcol0, uint8_t* dir, unsigned long long* offs, unsigned long long* csum);
+// A run of samples copied from a ring into its virtual slot: samples [first, first + n) of the ring's push order to virtual columns
+// vcol.., where n is the next run's off minus this one's (the last: up to n_samples); off counts the samples of the runs before it.
+struct gpud_tier_run { int64_t first, vcol, off; };
+// tier.cu: fields [f0, f0 + G) of the n_runs runs d_runs (n_samples samples in all) from ring o into slot s, in one launch on ring h's
+// device and stream, the sample ring by k_ring_append's rule.
+cudaError_t gpud_tier_copy_runs(const gpud_ring* h, const gpud_ring* o, const gpud_tier_run* d_runs, int64_t n_runs, int64_t n_samples, int f0, int G,
+                                const gpud_vslot& s);
 // The placement of one row of s bytes (host plan and device encode): the oldest rows go until [off, off + s) overlaps none held.
 __host__ __device__ inline int64_t gpud_tier_place(gpud_tier_ctl& c, int64_t* slot, int64_t R, int64_t B, int64_t s) {
   for (;;) {
@@ -184,7 +188,8 @@ struct gpud_ring_windows {
 };
 
 // What the range launchers (ring.cu, select.cu, ranges.cu, box_query.cu) read of a ring; owns nothing.  gpud_view gives a real ring's;
-// the tier's decoded virtual ring and the box query's dense and pivot buffers are views of their own, with the ring's config.
+// a slot of a range call's virtual box (rows decoded from tiers or copied from rings) and the box query's dense and pivot buffers are
+// views of their own, with the ring's config.
 struct gpud_ring_view {
   gpud_ctx* ctx; int dev; cudaStream_t stream; int sm_count;                         // where the launches run
   int F; int64_t cap; double alpha; int q_num, q_den;                                // the ring's config

@@ -1,5 +1,5 @@
 // ranges.cu — sets of sample ranges of one ring or of several: gpud_ring_reduce_ranges, gpud_ring_reduce_range_sets and
-// gpud_rings_reduce_range_sets, their plan, their driver over the segment select (segsel.h), and the ranges that reach into the tier.
+// gpud_rings_reduce_range_sets, their plan, their driver over the segment select (segsel.h), and the ranges that reach into tiers.
 #include <algorithm>
 
 #include "segsel.h"
@@ -18,12 +18,18 @@ constexpr int64_t kRangesBatchBytes = (int64_t)1 << 30;
 // slot ring_of[i] of n_rings (ring_of NULL: all in slot 0, the home ring), which has pushed totals[ring_of[i]] samples; every ring has
 // capacity cap.  set_off NULL: every range is a set of its own (n_sets = n).  A refusal names the range or the set in ctx's last error
 // (ctx may be NULL).
-int32_t ranges_plan(gpud_ctx* ctx, const int64_t* totals, int n_rings, const int32_t* ring_of, int64_t cap, int F, int q_num, int q_den, double alpha,
-                    int smp_shift, const int64_t* first, const int64_t* len, int64_t n, const int64_t* set_off, int64_t n_sets, RangesPlan* pl) {
+int32_t ranges_check(gpud_ctx* ctx, const int64_t* totals, int n_rings, const int32_t* ring_of, int64_t cap, const int64_t* lo, const int64_t* first,
+                     const int64_t* len, int64_t n, const int64_t* set_off, int64_t n_sets) {
   for (int64_t i = 0; i < n; ++i) {
     const int32_t k = ring_of ? ring_of[i] : 0;
     if (k < 0 || k >= n_rings) return gpud_fail(ctx, GPUD_E_INVALID, "range %lld: ring_of is %d, not a ring of the call's %d", (long long)i, k, n_rings);
     const int64_t total = totals[k], count = total < cap ? total : cap;
+    if (lo && lo[k] >= 0) {                        // a tiered ring: its ring and its tier
+      if (len[i] < 1 || first[i] < lo[k] || first[i] > total - len[i])
+        return gpud_fail(ctx, GPUD_E_INVALID, "range %lld: samples [%lld, +%lld) are not all in ring %d's reach [%lld, %lld) (its tier and its ring)",
+                         (long long)i, (long long)first[i], (long long)len[i], k, (long long)lo[k], (long long)total);
+      continue;
+    }
     if (len[i] < 1 || first[i] < total - count || first[i] > total - len[i])
       return gpud_fail(ctx, GPUD_E_INVALID, "range %lld: samples [%lld, +%lld) are not all in ring %d (pushed %lld, held %lld)", (long long)i,
                        (long long)first[i], (long long)len[i], k, (long long)total, (long long)count);
@@ -43,6 +49,12 @@ int32_t ranges_plan(gpud_ctx* ctx, const int64_t* totals, int n_rings, const int
       if (m > (int64_t)UINT32_MAX) return gpud_fail(ctx, GPUD_E_INVALID, "set %lld: more than UINT32_MAX samples (its n_over is 32-bit)", (long long)s);
     }
   }
+  return GPUD_OK;
+}
+
+int32_t ranges_plan(gpud_ctx* ctx, const int64_t* totals, int n_rings, const int32_t* ring_of, int64_t cap, int F, int q_num, int q_den, double alpha,
+                    int smp_shift, const int64_t* first, const int64_t* len, int64_t n, const int64_t* set_off, int64_t n_sets, RangesPlan* pl) {
+  { int32_t rc = ranges_check(ctx, totals, n_rings, ring_of, cap, nullptr, first, len, n, set_off, n_sets); if (rc) return rc; }
   pl->start.resize(n);
   pl->route.assign(n_sets, 0);
   pl->batch0.assign(1, 0);
@@ -108,7 +120,9 @@ void gpud_ranges_state_free(gpud_ranges_state* s) {
   if (!s) return;
   gpud_range_state_free(s->seg);
   cudaFree(s->d_short); cudaFree(s->d_pieces); cudaFree(s->d_srcs); cudaFree(s->d_tile); cudaFree(s->d_tile_piece); cudaFree(s->d_out); cudaFree(s->d_nover);
+  cudaFree(s->d_vring); cudaFree(s->d_vsmp); cudaFree(s->d_rows); cudaFree(s->d_vdir); cudaFree(s->d_voffs); cudaFree(s->d_runs); cudaFree(s->d_vsum);
   for (auto& ev : s->ev) if (ev) cudaEventDestroy(ev);
+  for (auto& ev : s->ev_dec) if (ev) cudaEventDestroy(ev);
   delete s;
 }
 
@@ -132,23 +146,19 @@ cudaError_t ranges_scatter(const gpud_ring_view& v, const gpud_range_state* s, i
   return cudaGetLastError();
 }
 
-// The call behind both entry points, after their argument checks (and, for several rings, rings_check): every refusal comes from
-// ranges_plan, or the peer check after it, before any launch.  The kernels run on the home ring's device and stream, read through the
-// view v (the ring itself, or a buffer laid out as one: the tier's virtual ring), with the scratch *state (created on first use): the
-// home ring's own, or a box query's (gpud_box_query), which must leave the ring's untouched.  rings[1, n_rings) are the call's other rings.
-int32_t reduce_sets(const gpud_ring_view& v, int64_t home_total, gpud_ring* const* rings, int n_rings, const int32_t* ring_of, const int64_t* first,
-                    const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over,
-                    gpud_ranges_state** state) {
-  std::vector<int64_t> totals(n_rings, home_total);
-  std::vector<gpud_ring_src> src(n_rings, gpud_ring_src{v.d_ring, v.d_sample});
-  for (int i = 1; i < n_rings; ++i) {
-    totals[i] = rings[i]->total;
-    src[i] = {rings[i]->d_ring, rings[i]->d_sample};
+RingTable ring_table(gpud_ring* const* rings, int n_rings) {
+  RingTable t;
+  t.rings = rings;
+  for (int i = 0; i < n_rings; ++i) {
+    t.src.push_back({rings[i]->d_ring, rings[i]->d_sample});
+    t.total.push_back(rings[i]->total);
   }
-  RangesPlan pl;
-  { int32_t rc = ranges_plan(v.ctx, totals.data(), n_rings, ring_of, v.cap, v.F, v.q_num, v.q_den, v.alpha, v.smp_shift, first, len, n_ranges, set_off,
-                             n_sets, &pl); if (rc) return rc; }
-  // the last refusal: a ring whose device the home device cannot map.  Peer access is enabled only for a call that runs.
+  return t;
+}
+
+// The last refusal of a call over rings[1, n_rings): a ring whose device the home device cannot map (peer access is enabled only for
+// a call that runs); then the other rings' pushes are made complete before the first launch: the home stream waits for each one's.
+static int32_t rings_ready(const gpud_ring_view& v, gpud_ring* const* rings, int n_rings) {
   for (int i = 1; i < n_rings; ++i) {
     if (rings[i]->dev == v.dev) continue;
     const cudaError_t e = gpud_peer_enable(v.ctx, v.dev, rings[i]->dev);
@@ -156,10 +166,6 @@ int32_t reduce_sets(const gpud_ring_view& v, int64_t home_total, gpud_ring* cons
       return gpud_fail(v.ctx, GPUD_E_UNSUPPORTED, "ring %d: device %d cannot map device %d's memory as a peer", i, v.dev, rings[i]->dev);
     GPUD_CUDA(v.ctx, e);
   }
-  // a piece in a ring other than the home ring makes the call MULTI (internal.h); a call of one ring reads no ring table
-  bool multi = false;
-  for (const gpud_piece& q : pl.pieces) multi |= gpud_piece_ring(q) != 0;
-  // the other rings' pushes are complete before the first launch: the home stream waits for each one's stream
   for (int i = 1; i < n_rings; ++i) {
     gpud_ring* o = rings[i];
     if (o->stream == v.stream) continue;
@@ -171,6 +177,26 @@ int32_t reduce_sets(const gpud_ring_view& v, int64_t home_total, gpud_ring* cons
     cudaEventDestroy(ev);              // released once the wait has been satisfied
     if (e != cudaSuccess) return gpud_fail(v.ctx, GPUD_E_CUDA, "ring %d: waiting for its stream: %s", i, cudaGetErrorString(e));
   }
+  GPUD_CUDA(v.ctx, cudaSetDevice(v.dev));
+  return GPUD_OK;
+}
+
+// The call behind the entry points, after their argument checks (and, for several rings, rings_check): every refusal comes from
+// ranges_plan, or the peer check after it, before any launch.  The kernels run on the home ring's device and stream, read through the
+// view v (the ring itself, or a buffer laid out as one: a slot of a virtual box) and the ring table t, with the scratch *state (created
+// on first use): the home ring's own, or a box query's (gpud_box_query), which must leave the ring's untouched.
+int32_t reduce_sets(const gpud_ring_view& v, const RingTable& t, const int32_t* ring_of, const int64_t* first, const int64_t* len, int64_t n_ranges,
+                    const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over, gpud_ranges_state** state) {
+  const int n_rings = t.n();
+  std::vector<gpud_ring_src> src(t.src);
+  src[0] = {v.d_ring, v.d_sample};
+  RangesPlan pl;
+  { int32_t rc = ranges_plan(v.ctx, t.total.data(), n_rings, ring_of, v.cap, v.F, v.q_num, v.q_den, v.alpha, v.smp_shift, first, len, n_ranges, set_off,
+                             n_sets, &pl); if (rc) return rc; }
+  if (t.rings) { int32_t rc = rings_ready(v, t.rings, n_rings); if (rc) return rc; }
+  // a piece in a ring other than the home ring makes the call MULTI (internal.h); a call of one ring reads no ring table
+  bool multi = false;
+  for (const gpud_piece& q : pl.pieces) multi |= gpud_piece_ring(q) != 0;
   GPUD_CUDA(v.ctx, cudaSetDevice(v.dev));
   if (!*state) *state = new gpud_ranges_state();
   gpud_ranges_state* rs = *state;
@@ -238,56 +264,99 @@ int32_t reduce_sets(const gpud_ring_view& v, int64_t home_total, gpud_ring* cons
   return GPUD_OK;
 }
 
-// ---- ranges that reach into the tier (DESIGN.md §2 "Tier") -------------------------------------------------------------------
-// A tiered ring holds samples [lo, total) with lo = min(total - count, 1024 tier_first).  The sets whose ranges all lie in the ring go
-// through reduce_sets untouched.  Each other set's ranges cover block rows; those rows, merged and ascending, are decoded into a
-// virtual ring (row j at columns [1024 j, 1024 (j + 1)); the newest row, not yet coded, copied from the ring), and reduce_sets runs
-// on that buffer as on a ring of its own capacity with the ring's alpha, quantile and thresholds - in groups of fields, each as large
-// as kTierGroupBytes of decoded samples allow.
+// ---- ranges that reach into a tier (DESIGN.md §2 "Tier", "Box sets") ----------------------------------------------------------
+// A tiered ring holds samples [lo, total) with lo = min(total - count, 1024 tier_first).  The sets whose ranges all lie in their rings
+// go through reduce_sets untouched.  Each other set's ranges cover block rows of their rings; per ring, those rows, merged and
+// ascending, are one slot of a virtual box (row j at columns [1024 j, 1024 (j + 1))): rows the ring's tier holds are decoded, the
+// others copied from the ring (the newest row, not yet coded; rows below a tier shorter than its ring; every row of an untiered ring).
+// The slots share one capacity vcap, as the range kernels read every ring of a call with one geometry, and reduce_sets runs on the box
+// as on a call of as many rings with the home ring's alpha, quantile and thresholds - in groups of fields, each as large as
+// kTierGroupBytes of decoded samples over all slots allow.
 constexpr int64_t kTierGroupBytes = (int64_t)1 << 30;
 
+// What the split knows of ring k of a call: its pushed samples and, tiered, the rows [t_first, t_next) its tier holds.
+struct SplitRing { int64_t total; bool tiered; int64_t t_first, t_next; };
+
 struct TierSplit {
-  std::vector<int32_t> route;        // per set: 0 the ring, 1 the tier
-  std::vector<int64_t> rows;         // the block rows the tier sets read, ascending
-  std::vector<int64_t> vfirst;       // per range of a tier set: its first sample in the virtual ring (-1: a ring set's range)
-  int64_t vtotal = 0;                // samples of the virtual ring
+  std::vector<int32_t> route;                // per set: 0 its rings, 1 the virtual box
+  std::vector<int32_t> ring;                 // per slot: its ring, ascending
+  std::vector<std::vector<int64_t>> rows;    // per slot: the block rows the tier sets read in its ring, ascending
+  std::vector<std::vector<uint8_t>> dec;     // ... each one decoded from the ring's tier (1) or copied from the ring (0)
+  std::vector<int64_t> vtotal;               // per slot: its samples (its newest row may be partial)
+  std::vector<int32_t> vslot;                // per range of a tier set: its slot (-1: a ring set's range)
+  std::vector<int64_t> vfirst;               // ... and its first sample in that slot (-1)
+  int64_t vcap = 0;                          // the slots' capacity: the largest slot's rows x 1024
 };
 
-// Validation (every refusal of ranges_plan, against samples [lo, total)) and the split.  Pure host arithmetic.
-static int32_t tier_split(gpud_ctx* ctx, int64_t total, int64_t cap, int F, int64_t t_first, int64_t t_next, const int64_t* first, const int64_t* len,
+// Validation (every refusal of ranges_check, each range against its own ring's reach) and the split.  Pure host arithmetic.
+static int32_t tier_split(gpud_ctx* ctx, const std::vector<SplitRing>& rg, int64_t cap, const int32_t* ring_of, const int64_t* first, const int64_t* len,
                           int64_t n, const int64_t* set_off, int64_t n_sets, TierSplit* sp) {
-  const int64_t count = std::min(total, cap), lo = std::min(total - count, t_first * GPUD_TIER_ROW);
-  {
-    // ranges_plan's checks with a capacity that holds [lo, total): the same refusals, against the tier's reach
-    RangesPlan pl;
-    int32_t rc = ranges_plan(ctx, &total, 1, nullptr, std::max<int64_t>(1, total - lo), F, 99, 100, 0.5, 0, first, len, n, set_off, n_sets, &pl);
-    if (rc) return rc;
+  const int nr = (int)rg.size();
+  std::vector<int64_t> totals(nr), lo(nr), held(nr);
+  for (int k = 0; k < nr; ++k) {
+    totals[k] = rg[k].total;
+    held[k] = rg[k].total - std::min(rg[k].total, cap);   // the ring's first sample
+    lo[k] = rg[k].tiered ? std::min(held[k], rg[k].t_first * GPUD_TIER_ROW) : -1;
   }
+  { int32_t rc = ranges_check(ctx, totals.data(), nr, ring_of, cap, lo.data(), first, len, n, set_off, n_sets); if (rc) return rc; }
+  auto ring = [&](int64_t i) { return ring_of ? ring_of[i] : 0; };
   sp->route.assign(n_sets, 0);
-  sp->vfirst.assign(n, -1);
-  std::vector<std::pair<int64_t, int64_t>> iv;
+  std::vector<std::vector<std::pair<int64_t, int64_t>>> iv(nr);
   for (int64_t s = 0; s < n_sets; ++s) {
     const int64_t a = set_off ? set_off[s] : s, e = set_off ? set_off[s + 1] : s + 1;
-    for (int64_t i = a; i < e; ++i) sp->route[s] |= first[i] < total - count;
+    for (int64_t i = a; i < e; ++i) sp->route[s] |= first[i] < held[ring(i)];
     if (!sp->route[s]) continue;
-    for (int64_t i = a; i < e; ++i) iv.push_back({first[i] / GPUD_TIER_ROW, (first[i] + len[i] + GPUD_TIER_ROW - 1) / GPUD_TIER_ROW});
+    for (int64_t i = a; i < e; ++i) iv[ring(i)].push_back({first[i] / GPUD_TIER_ROW, (first[i] + len[i] + GPUD_TIER_ROW - 1) / GPUD_TIER_ROW});
   }
-  std::sort(iv.begin(), iv.end());
-  sp->rows.clear();
-  for (const auto& v : iv)
-    for (int64_t k = std::max(v.first, sp->rows.empty() ? v.first : sp->rows.back() + 1); k < v.second; ++k) sp->rows.push_back(k);
+  std::vector<int32_t> slot_of(nr, -1);
+  sp->ring.clear(); sp->rows.clear(); sp->dec.clear(); sp->vtotal.clear();
+  sp->vcap = 0;
+  for (int k = 0; k < nr; ++k) {
+    if (iv[k].empty()) continue;
+    std::sort(iv[k].begin(), iv[k].end());
+    std::vector<int64_t> rows;
+    for (const auto& v : iv[k])
+      for (int64_t j = std::max(v.first, rows.empty() ? v.first : rows.back() + 1); j < v.second; ++j) rows.push_back(j);
+    std::vector<uint8_t> dec(rows.size());
+    for (size_t j = 0; j < rows.size(); ++j) dec[j] = rg[k].tiered && rows[j] >= rg[k].t_first && rows[j] < rg[k].t_next;
+    const int64_t nrow = (int64_t)rows.size(), last = rows.back();
+    slot_of[k] = (int32_t)sp->ring.size();
+    sp->ring.push_back(k);
+    sp->vtotal.push_back((nrow - 1) * GPUD_TIER_ROW + std::min<int64_t>(GPUD_TIER_ROW, rg[k].total - last * GPUD_TIER_ROW));
+    sp->vcap = std::max(sp->vcap, nrow * GPUD_TIER_ROW);
+    sp->rows.push_back(std::move(rows));
+    sp->dec.push_back(std::move(dec));
+  }
+  sp->vslot.assign(n, -1);
+  sp->vfirst.assign(n, -1);
   for (int64_t s = 0; s < n_sets; ++s) {
     if (!sp->route[s]) continue;
     const int64_t a = set_off ? set_off[s] : s, e = set_off ? set_off[s + 1] : s + 1;
     for (int64_t i = a; i < e; ++i) {
-      const int64_t j = std::lower_bound(sp->rows.begin(), sp->rows.end(), first[i] / GPUD_TIER_ROW) - sp->rows.begin();
+      const int32_t v = slot_of[ring(i)];
+      const std::vector<int64_t>& rows = sp->rows[v];
+      const int64_t j = std::lower_bound(rows.begin(), rows.end(), first[i] / GPUD_TIER_ROW) - rows.begin();
+      sp->vslot[i] = v;
       sp->vfirst[i] = j * GPUD_TIER_ROW + first[i] % GPUD_TIER_ROW;
     }
   }
-  const int64_t nr = (int64_t)sp->rows.size();
-  sp->vtotal = nr * GPUD_TIER_ROW;
-  if (nr && sp->rows.back() == t_next) sp->vtotal -= GPUD_TIER_ROW - (total - t_next * GPUD_TIER_ROW);   // the newest row is partial
   return GPUD_OK;
+}
+
+// The runs slot v copies from its ring (total pushed, samples [held, total) in the ring): its rows not decoded, clipped to the ring's
+// samples, consecutive ones merged; appended to runs, *n their samples.
+static void slot_runs(const TierSplit& sp, int v, int64_t total, int64_t held, std::vector<gpud_tier_run>& runs, int64_t* n) {
+  const size_t r0 = runs.size();
+  *n = 0;
+  for (size_t j = 0; j < sp.rows[v].size(); ++j) {
+    if (sp.dec[v][j]) continue;
+    const int64_t row = sp.rows[v][j] * GPUD_TIER_ROW, a = std::max(row, held), b = std::min(row + GPUD_TIER_ROW, total);
+    if (b <= a) continue;
+    const int64_t vcol = (int64_t)j * GPUD_TIER_ROW + (a - row);
+    const bool joins = runs.size() > r0 && runs.back().first + (*n - runs.back().off) == a && runs.back().vcol + (*n - runs.back().off) == vcol;
+    if (!joins) runs.push_back({a, vcol, *n});
+    *n += b - a;
+  }
 }
 
 // results [5][G][n_sub] / [G][n_sub] of sets ids[] and fields [f0, f0 + G) into the caller's [5][F][n_sets] / [F][n_sets]
@@ -301,87 +370,152 @@ static void tier_scatter(const std::vector<double>& f64, const std::vector<uint3
     for (int64_t j = 0; j < m; ++j) out_n_over[(int64_t)(f0 + f) * n_sets + ids[j]] = nov[(int64_t)f * m + j];
 }
 
-int32_t reduce_subset(const gpud_ring_view& v, int64_t home_total, const std::vector<int64_t>& ids, const int64_t* first, const int64_t* len,
-                      const int64_t* set_off, const std::vector<int64_t>* vfirst, gpud_ranges_state** state, std::vector<double>& f64,
-                      std::vector<uint32_t>& nov) {
+int32_t reduce_subset(const gpud_ring_view& v, const RingTable& t, const std::vector<int64_t>& ids, const int32_t* ring_of, const int64_t* first,
+                      const int64_t* len, const int64_t* set_off, gpud_ranges_state** state, std::vector<double>& f64, std::vector<uint32_t>& nov) {
   std::vector<int64_t> sf, sl, so(1, 0);
+  std::vector<int32_t> sr;
   for (int64_t s : ids) {
     const int64_t a = set_off ? set_off[s] : s, e = set_off ? set_off[s + 1] : s + 1;
-    for (int64_t i = a; i < e; ++i) { sf.push_back(vfirst ? (*vfirst)[i] : first[i]); sl.push_back(len[i]); }
+    for (int64_t i = a; i < e; ++i) {
+      sf.push_back(first[i]);
+      sl.push_back(len[i]);
+      if (ring_of) sr.push_back(ring_of[i]);
+    }
     so.push_back((int64_t)sf.size());
   }
   const int64_t m = (int64_t)ids.size();
   f64.assign(5 * (size_t)v.F * m, 0.0);
   nov.assign((size_t)v.F * m, 0u);
-  return reduce_sets(v, home_total, nullptr, 1, nullptr, sf.data(), sl.data(), (int64_t)sf.size(), so.data(), m, f64.data(), nov.data(), state);
+  return reduce_sets(v, t, ring_of ? sr.data() : nullptr, sf.data(), sl.data(), (int64_t)sf.size(), so.data(), m, f64.data(), nov.data(), state);
 }
 
-static int32_t reduce_sets_tier(gpud_ring* r, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets,
-                                double* out_f64, uint32_t* out_n_over) {
-  gpud_tier* t = r->tier;
-  gpud_tier_ctl c;
-  { int32_t rc = gpud_tier_read_ctl(r, &c); if (rc) return rc; }
+// Device scratch of the virtual box, grown on the home ring: a failed allocation is GPUD_E_CUDA and leaves every ring usable.
+template <typename T>
+static int32_t vbox_grow(gpud_ctx* ctx, T** p, size_t* cap, size_t need) {
+  const cudaError_t e = gpud_grow(p, cap, std::max<size_t>(1, need));
+  if (e == cudaSuccess) return GPUD_OK;
+  cudaGetLastError();
+  return gpud_fail(ctx, GPUD_E_CUDA, "reduce_range_sets: the virtual box's %zu-element scratch: %s", need, cudaGetErrorString(e));
+}
+
+// The call behind gpud_rings_reduce_range_sets, and behind the one-ring calls as its n_rings = 1 case (set_off NULL: every range is a
+// set, n_sets = n_ranges), after their argument checks and rings_check.  A call none of whose rings has a tier is reduce_sets; so is a
+// call with no set that reaches a tier, once each tiered ring's control word has been read (one synchronisation of its stream).
+static int32_t reduce_box(gpud_ring* const* rings, int n_rings, const int32_t* ring_of, const int64_t* first, const int64_t* len, int64_t n_ranges,
+                          const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over) {
+  gpud_ring* h = rings[0];
+  gpud_ctx* ctx = h->ctx;
+  RingTable rt = ring_table(rings, n_rings);
+  std::vector<SplitRing> rg(n_rings);
+  bool tiered = false;
+  for (int k = 0; k < n_rings; ++k) {
+    rg[k] = {rings[k]->total, rings[k]->tier != nullptr, 0, 0};
+    if (!rings[k]->tier) continue;
+    tiered = true;
+    gpud_tier_ctl c;
+    { int32_t rc = gpud_tier_read_ctl(rings[k], &c); if (rc) return rc; }
+    rg[k].t_first = c.first;
+    rg[k].t_next = c.next;
+  }
   TierSplit sp;
-  { int32_t rc = tier_split(r->ctx, r->total, r->cap, r->F, c.first, c.next, first, len, n_ranges, set_off, n_sets, &sp); if (rc) return rc; }
-  if (sp.rows.empty()) return reduce_sets(gpud_view(r), r->total, nullptr, 1, nullptr, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over, &r->ranges);
+  if (tiered) { int32_t rc = tier_split(ctx, rg, h->cap, ring_of, first, len, n_ranges, set_off, n_sets, &sp); if (rc) return rc; }
+  if (sp.ring.empty()) return reduce_sets(gpud_view(h), rt, ring_of, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over, &h->ranges);
+  { int32_t rc = rings_ready(gpud_view(h), rings, n_rings); if (rc) return rc; }
+  rt.rings = nullptr;                              // ready: the subsets below wait for nothing more
   std::vector<int64_t> ids[2];
   for (int64_t s = 0; s < n_sets; ++s) ids[sp.route[s]].push_back(s);
-  const int F = r->F;
+  const int F = h->F, ns = (int)sp.ring.size();
+  // the virtual box's geometry and field groups
+  const int64_t vcap = sp.vcap;
+  const int smp_shift = ring_smp_shift(vcap);
+  const int64_t smp_slots = (vcap + (1ll << smp_shift) - 1) >> smp_shift, per_field = 8 * (vcap + smp_slots) * ns;
+  int G = (int)std::max<int64_t>(1, std::min<int64_t>(F, kTierGroupBytes / per_field));
+  if (h->tier && h->tier->group_max > 0) G = std::min(G, h->tier->group_max);
+  // per slot: its decoded rows (one list over all slots, rows [d0[v], d0[v + 1])) at virtual column dcol[v], and its ring runs
+  // (runs [r0[v], r0[v + 1]), rn[v] samples)
+  std::vector<int64_t> drows, d0(ns + 1, 0), dcol(ns, 0), r0(ns + 1, 0), rn(ns, 0);
+  std::vector<gpud_tier_run> runs;
+  for (int v = 0; v < ns; ++v) {
+    const gpud_ring* o = rings[sp.ring[v]];
+    for (size_t j = 0; j < sp.rows[v].size(); ++j) {
+      if (!sp.dec[v][j]) continue;
+      if ((int64_t)drows.size() == d0[v]) dcol[v] = (int64_t)j * GPUD_TIER_ROW;   // a tier's rows are consecutive in the slot
+      drows.push_back(sp.rows[v][j]);
+    }
+    d0[v + 1] = (int64_t)drows.size();
+    slot_runs(sp, v, o->total, o->total - ring_count(o), runs, &rn[v]);
+    r0[v + 1] = (int64_t)runs.size();
+  }
+  GPUD_CUDA(ctx, cudaSetDevice(h->dev));
+  if (!h->ranges) h->ranges = new gpud_ranges_state();
+  gpud_ranges_state* rs = h->ranges;
+  { int32_t rc = vbox_grow(ctx, &rs->d_vring, &rs->vring_cap, (size_t)ns * G * vcap); if (rc) return rc; }
+  { int32_t rc = vbox_grow(ctx, &rs->d_vsmp, &rs->vsmp_cap, (size_t)ns * G * smp_slots); if (rc) return rc; }
+  { int32_t rc = vbox_grow(ctx, &rs->d_rows, &rs->rows_cap, drows.size()); if (rc) return rc; }
+  { int32_t rc = vbox_grow(ctx, &rs->d_vdir, &rs->vdir_cap, (size_t)G * drows.size()); if (rc) return rc; }
+  { int32_t rc = vbox_grow(ctx, &rs->d_voffs, &rs->voffs_cap, (size_t)G * drows.size()); if (rc) return rc; }
+  { int32_t rc = vbox_grow(ctx, &rs->d_runs, &rs->runs_cap, runs.size()); if (rc) return rc; }
+  { int32_t rc = vbox_grow(ctx, &rs->d_vsum, &rs->vsum_cap, (size_t)G); if (rc) return rc; }
+  for (auto& e : rs->ev_dec) if (!e) GPUD_CUDA(ctx, cudaEventCreate(&e));
   cudaEvent_t ev[2] = {};
-  for (auto& e : ev) GPUD_CUDA(r->ctx, cudaEventCreate(&e));
+  for (auto& e : ev) GPUD_CUDA(ctx, cudaEventCreate(&e));
   struct EvFree { cudaEvent_t* e; ~EvFree() { for (int i = 0; i < 2; ++i) if (e[i]) cudaEventDestroy(e[i]); } } ev_free{ev};
-  GPUD_CUDA(r->ctx, cudaEventRecord(ev[0], r->stream));
+  GPUD_CUDA(ctx, cudaEventRecord(ev[0], h->stream));
+  if (!drows.empty()) GPUD_CUDA(ctx, cudaMemcpyAsync(rs->d_rows, drows.data(), drows.size() * sizeof(int64_t), cudaMemcpyHostToDevice, h->stream));
+  if (!runs.empty()) GPUD_CUDA(ctx, cudaMemcpyAsync(rs->d_runs, runs.data(), runs.size() * sizeof(gpud_tier_run), cudaMemcpyHostToDevice, h->stream));
   int64_t open = 0;
   int reasons[GPUD_RANGE_N_OPEN_REASONS] = {};
   auto tally = [&]() {
-    open += r->ranges->open;
-    for (int i = 0; i < GPUD_RANGE_N_OPEN_REASONS; ++i) reasons[i] += r->ranges->reasons[i];
+    open += h->ranges->open;
+    for (int i = 0; i < GPUD_RANGE_N_OPEN_REASONS; ++i) reasons[i] += h->ranges->reasons[i];
   };
   std::vector<double> f64;
   std::vector<uint32_t> nov;
   if (!ids[0].empty()) {
-    int32_t rc = reduce_subset(gpud_view(r), r->total, ids[0], first, len, set_off, nullptr, &r->ranges, f64, nov);
+    int32_t rc = reduce_subset(gpud_view(h), rt, ids[0], ring_of, first, len, set_off, &h->ranges, f64, nov);
     if (rc) return rc;
     tier_scatter(f64, nov, ids[0], 0, F, F, n_sets, out_f64, out_n_over);
     tally();
   }
-  // the virtual ring: rows held by the tier are decoded, the newest one (partial) is copied from the ring
-  std::vector<int64_t> dec(sp.rows);
-  int64_t tail_n = 0;
-  if (dec.back() == c.next) {
-    tail_n = r->total - c.next * GPUD_TIER_ROW;
-    dec.pop_back();
-  }
-  const int64_t vcap = (int64_t)sp.rows.size() * GPUD_TIER_ROW;
-  const int smp_shift = ring_smp_shift(vcap);
-  const int64_t smp_slots = (vcap + (1ll << smp_shift) - 1) >> smp_shift, per_field = 8 * (vcap + smp_slots);
-  int G = (int)std::max<int64_t>(1, std::min<int64_t>(F, kTierGroupBytes / per_field));
-  if (t->group_max > 0) G = std::min(G, t->group_max);
-  t->dec_ms = 0.f;
+  float dec_ms = 0.f;
   for (int f0 = 0; f0 < F; f0 += G) {
     const int g = std::min(G, F - f0);
-    double *vring = nullptr, *vsmp = nullptr;
-    { int32_t rc = gpud_tier_decode(r, dec, c.next, tail_n, f0, g, vcap, smp_shift, smp_slots, &vring, &vsmp); if (rc) return rc; }
-    gpud_ring_view v = gpud_view(r);   // the virtual ring: fields [f0, f0 + g) of the decoded rows
-    v.F = g;
-    v.cap = vcap;
-    v.d_ring = vring;
-    v.d_thr = r->d_thr + f0;
-    v.d_sample = vsmp;
-    v.smp_shift = smp_shift;
-    v.smp_slots = smp_slots;
-    int32_t rc = reduce_subset(v, sp.vtotal, ids[1], first, len, set_off, &sp.vfirst, &r->ranges, f64, nov);
+    // the group's slots, packed: slot v's fields at [v g, (v + 1) g) of the box's rows
+    std::vector<gpud_vslot> vs(ns);
+    RingTable vt;
+    vt.total = sp.vtotal;
+    for (int v = 0; v < ns; ++v) {
+      vs[v] = {rs->d_vring + (size_t)v * g * vcap, rs->d_vsmp + (size_t)v * g * smp_slots, vcap, smp_shift, smp_slots};
+      vt.src.push_back({vs[v].ring, vs[v].sample});
+    }
+    GPUD_CUDA(ctx, cudaEventRecord(rs->ev_dec[0], h->stream));
+    for (int v = 0; v < ns; ++v) {
+      const gpud_ring* o = rings[sp.ring[v]];
+      GPUD_CUDA(ctx, gpud_tier_decode(h, o, rs->d_rows + d0[v], d0[v + 1] - d0[v], f0, g, vs[v], dcol[v], rs->d_vdir + (size_t)g * d0[v],
+                                      rs->d_voffs + (size_t)g * d0[v], rs->d_vsum));
+      GPUD_CUDA(ctx, gpud_tier_copy_runs(h, o, rs->d_runs + r0[v], r0[v + 1] - r0[v], rn[v], f0, g, vs[v]));
+    }
+    GPUD_CUDA(ctx, cudaEventRecord(rs->ev_dec[1], h->stream));
+    gpud_ring_view vv = gpud_view(h);   // the box: fields [f0, f0 + g) of every slot, slot 0 the view's own
+    vv.F = g;
+    vv.cap = vcap;
+    vv.d_ring = vs[0].ring;
+    vv.d_thr = h->d_thr + f0;
+    vv.d_sample = vs[0].sample;
+    vv.smp_shift = smp_shift;
+    vv.smp_slots = smp_slots;
+    int32_t rc = reduce_subset(vv, vt, ids[1], ns > 1 ? sp.vslot.data() : nullptr, sp.vfirst.data(), len, set_off, &h->ranges, f64, nov);
     if (rc) return rc;
     float ms = 0.f;
-    GPUD_CUDA(r->ctx, cudaEventElapsedTime(&ms, t->ev_dec[0], t->ev_dec[1]));
-    t->dec_ms += ms;
+    GPUD_CUDA(ctx, cudaEventElapsedTime(&ms, rs->ev_dec[0], rs->ev_dec[1]));
+    dec_ms += ms;
     tier_scatter(f64, nov, ids[1], f0, g, F, n_sets, out_f64, out_n_over);
     tally();
   }
+  if (h->tier) h->tier->dec_ms = dec_ms;
   // gpud_ring_ranges_stats reports the whole call: its events now bracket everything above
-  gpud_ranges_state* rs = r->ranges;
-  GPUD_CUDA(r->ctx, cudaEventRecord(ev[1], r->stream));
-  GPUD_CUDA(r->ctx, cudaEventSynchronize(ev[1]));
+  GPUD_CUDA(ctx, cudaEventRecord(ev[1], h->stream));
+  GPUD_CUDA(ctx, cudaEventSynchronize(ev[1]));
   std::swap(rs->ev[0], ev[0]);
   std::swap(rs->ev[1], ev[1]);
   rs->open = open;
@@ -389,20 +523,55 @@ static int32_t reduce_sets_tier(gpud_ring* r, const int64_t* first, const int64_
   return GPUD_OK;
 }
 
-// Test hook (include/gpud_b200_hooks.h): the split of one call on a tiered ring that holds rows [tier_first, tier_next).
+// Test hooks (include/gpud_b200_hooks.h): the split of one call over rings of totals[] pushed samples, ring k's tier holding rows
+// [tier_first[k], tier_next[k]) (tier_first[k] < 0: no tier); gpudh_ring_tier_split is the one-ring case.
+extern "C" int32_t gpudh_rings_tier_split(const int64_t* totals, int32_t n_rings, int64_t cap, const int64_t* tier_first, const int64_t* tier_next,
+                                          const int32_t* ring_of, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off,
+                                          int64_t n_sets, int32_t* route, int32_t* vslot, int64_t* vfirst, int32_t* n_slots, int32_t* slot_ring,
+                                          int64_t* vtotal, int64_t* slot_rows, int64_t* rows, uint8_t* dec, int64_t rows_cap, int64_t* vcap) {
+  if (!totals || !tier_first || !tier_next || n_rings < 1 || n_rings > GPUD_PIECE_RINGS || cap < 2 || n_ranges < 0 || n_sets < 1 || !first || !len ||
+      !route || !vslot || !vfirst || !n_slots || !slot_ring || !vtotal || !slot_rows || !vcap || (n_rings > 1 && !ring_of))
+    return GPUD_E_INVALID;
+  if (!set_off && n_sets != n_ranges) return GPUD_E_INVALID;
+  std::vector<SplitRing> rg(n_rings);
+  for (int k = 0; k < n_rings; ++k) {
+    if (totals[k] < 0) return GPUD_E_INVALID;
+    rg[k] = {totals[k], tier_first[k] >= 0, std::max<int64_t>(0, tier_first[k]), tier_next[k]};
+  }
+  TierSplit sp;
+  if (tier_split(nullptr, rg, cap, ring_of, first, len, n_ranges, set_off, n_sets, &sp)) return GPUD_E_INVALID;
+  std::copy(sp.route.begin(), sp.route.end(), route);
+  std::copy(sp.vslot.begin(), sp.vslot.end(), vslot);
+  std::copy(sp.vfirst.begin(), sp.vfirst.end(), vfirst);
+  *n_slots = (int32_t)sp.ring.size();
+  *vcap = sp.vcap;
+  slot_rows[0] = 0;
+  for (size_t v = 0; v < sp.ring.size(); ++v) {
+    slot_ring[v] = sp.ring[v];
+    vtotal[v] = sp.vtotal[v];
+    slot_rows[v + 1] = slot_rows[v] + (int64_t)sp.rows[v].size();
+  }
+  if (slot_rows[sp.ring.size()] > rows_cap || (slot_rows[sp.ring.size()] && (!rows || !dec))) return GPUD_E_CAPACITY;
+  for (size_t v = 0; v < sp.ring.size(); ++v) {
+    std::copy(sp.rows[v].begin(), sp.rows[v].end(), rows + slot_rows[v]);
+    std::copy(sp.dec[v].begin(), sp.dec[v].end(), dec + slot_rows[v]);
+  }
+  return GPUD_OK;
+}
+
 extern "C" int32_t gpudh_ring_tier_split(int64_t total, int64_t cap, int32_t n_fields, int64_t tier_first, int64_t tier_next, const int64_t* first,
                                          const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets, int32_t* route, int64_t* vfirst,
                                          int64_t* rows, int64_t rows_cap, int64_t* n_rows, int64_t* vtotal) {
   if (total < 0 || cap < 2 || n_fields < 1 || n_ranges < 0 || n_sets < 1 || !first || !len || !route || !vfirst || !n_rows || !vtotal) return GPUD_E_INVALID;
   if (!set_off && n_sets != n_ranges) return GPUD_E_INVALID;
   TierSplit sp;
-  if (tier_split(nullptr, total, cap, n_fields, tier_first, tier_next, first, len, n_ranges, set_off, n_sets, &sp)) return GPUD_E_INVALID;
+  if (tier_split(nullptr, {SplitRing{total, true, tier_first, tier_next}}, cap, nullptr, first, len, n_ranges, set_off, n_sets, &sp)) return GPUD_E_INVALID;
   std::copy(sp.route.begin(), sp.route.end(), route);
   std::copy(sp.vfirst.begin(), sp.vfirst.end(), vfirst);
-  *n_rows = (int64_t)sp.rows.size();
-  *vtotal = sp.vtotal;
+  *n_rows = sp.ring.empty() ? 0 : (int64_t)sp.rows[0].size();
+  *vtotal = sp.ring.empty() ? 0 : sp.vtotal[0];
   if (*n_rows > rows_cap || (*n_rows && !rows)) return GPUD_E_CAPACITY;
-  std::copy(sp.rows.begin(), sp.rows.end(), rows);
+  if (*n_rows) std::copy(sp.rows[0].begin(), sp.rows[0].end(), rows);
   return GPUD_OK;
 }
 
@@ -412,8 +581,7 @@ extern "C" int32_t gpud_ring_reduce_ranges(gpud_ring* r, const int64_t* first, c
   if (!first || !len || !out_f64 || !out_n_over) return GPUD_E_INVALID;
   if (n_ranges > GPUD_RANGES_MAX_SEGMENTS / r->F)
     return gpud_fail(r->ctx, GPUD_E_INVALID, "%d fields x %lld ranges exceed GPUD_RANGES_MAX_SEGMENTS", r->F, (long long)n_ranges);
-  if (r->tier) return reduce_sets_tier(r, first, len, n_ranges, nullptr, n_ranges, out_f64, out_n_over);
-  return reduce_sets(gpud_view(r), r->total, nullptr, 1, nullptr, first, len, n_ranges, nullptr, n_ranges, out_f64, out_n_over, &r->ranges);
+  return reduce_box(&r, 1, nullptr, first, len, n_ranges, nullptr, n_ranges, out_f64, out_n_over);
 }
 
 // The refusals of a call over several rings beyond those of one ring (DESIGN.md §2 "Box sets"): one ctx and the home ring's config bit
@@ -444,17 +612,11 @@ extern "C" int32_t gpud_rings_reduce_range_sets(gpud_ring* const* rings, int32_t
   if (n_sets > GPUD_RANGES_MAX_SEGMENTS / r->F)
     return gpud_fail(r->ctx, GPUD_E_INVALID, "%d fields x %lld sets exceed GPUD_RANGES_MAX_SEGMENTS", r->F, (long long)n_sets);
   { int32_t rc = rings_check(rings, n_rings); if (rc) return rc; }
-  return reduce_sets(gpud_view(r), r->total, rings, n_rings, ring_of, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over, &r->ranges);
+  return reduce_box(rings, n_rings, ring_of, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over);
 }
 
 extern "C" int32_t gpud_ring_reduce_range_sets(gpud_ring* r, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets,
                                                double* out_f64, uint32_t* out_n_over) {
-  if (r && r->tier && n_sets > 0 && n_ranges >= 0) {
-    if (!first || !len || !set_off || !out_f64 || !out_n_over) return GPUD_E_INVALID;
-    if (n_sets > GPUD_RANGES_MAX_SEGMENTS / r->F)
-      return gpud_fail(r->ctx, GPUD_E_INVALID, "%d fields x %lld sets exceed GPUD_RANGES_MAX_SEGMENTS", r->F, (long long)n_sets);
-    return reduce_sets_tier(r, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over);
-  }
   return gpud_rings_reduce_range_sets(&r, 1, nullptr, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over);
 }
 

@@ -109,7 +109,12 @@ struct RangesPlan {
 };
 // The sample ring's shift of a ring of capacity cap (gpud_ring_create).
 int ring_smp_shift(int64_t cap);
-// Validation, the physical columns, the pieces, the routes, the tile list and the batches of a call (ranges.cu).
+// The refusals of a call's ranges and sets (ranges.cu): range i must lie in [lo_k, totals[k]) of its ring k, lo_k = total - min(total,
+// cap) (the ring's samples) or, with lo given and lo[k] >= 0, lo[k] (a tiered ring's reach).
+int32_t ranges_check(gpud_ctx* ctx, const int64_t* totals, int n_rings, const int32_t* ring_of, int64_t cap, const int64_t* lo, const int64_t* first,
+                     const int64_t* len, int64_t n, const int64_t* set_off, int64_t n_sets);
+// Validation (ranges_check against the rings' own samples), the physical columns, the pieces, the routes, the tile list and the batches
+// of a call (ranges.cu).
 int32_t ranges_plan(gpud_ctx* ctx, const int64_t* totals, int n_rings, const int32_t* ring_of, int64_t cap, int F, int q_num, int q_den, double alpha,
                     int smp_shift, const int64_t* first, const int64_t* len, int64_t n, const int64_t* set_off, int64_t n_sets, RangesPlan* pl);
 
@@ -128,17 +133,38 @@ struct gpud_ranges_state {
   bool seg_last = false;          // seg holds the last batch of the last call (that call had a long set)
   int64_t open = 0;
   int reasons[GPUD_RANGE_N_OPEN_REASONS] = {};
+  // The virtual box of a call that reaches a tier (ranges.cu, DESIGN.md §2 "Tier"): its slots' samples [slots][G][vcap] and sample
+  // rings [slots][G][smp_slots], the tier rows to decode and their directories and block offsets, the ring runs to copy, the decode's
+  // unread field sums, and events around each group's decode.
+  double* d_vring = nullptr;  size_t vring_cap = 0;
+  double* d_vsmp = nullptr;  size_t vsmp_cap = 0;
+  int64_t* d_rows = nullptr;  size_t rows_cap = 0;
+  uint8_t* d_vdir = nullptr;  size_t vdir_cap = 0;
+  unsigned long long* d_voffs = nullptr;  size_t voffs_cap = 0;
+  gpud_tier_run* d_runs = nullptr;  size_t runs_cap = 0;
+  unsigned long long* d_vsum = nullptr;  size_t vsum_cap = 0;
+  cudaEvent_t ev_dec[2] = {};
 };
 
-// The sets of a call over home ring v (home_total samples pushed) and rings[1, n_rings), into out_f64 [5][F][n_sets] / out_n_over
-// [F][n_sets], on the scratch *state (created on first use).  ranges.cu says the rest.
-int32_t reduce_sets(const gpud_ring_view& v, int64_t home_total, gpud_ring* const* rings, int n_rings, const int32_t* ring_of, const int64_t* first,
-                    const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over,
-                    gpud_ranges_state** state);
-// The sets ids[] of a call reduced as a call of their own over v (one ring), on *state: their ranges (first[i] or, with vfirst,
-// vfirst[i]) and set offsets, into f64 [5][F][ids] / nov [F][ids].
-int32_t reduce_subset(const gpud_ring_view& v, int64_t home_total, const std::vector<int64_t>& ids, const int64_t* first, const int64_t* len,
-                      const int64_t* set_off, const std::vector<int64_t>* vfirst, gpud_ranges_state** state, std::vector<double>& f64,
-                      std::vector<uint32_t>& nov);
+// The ring table of a call: slot k's samples and sample ring (slot 0: the view's own, which the table's entry 0 need not repeat) and
+// its pushed samples.  `rings` (may be NULL) are real rings behind slots 1.., whose devices the home device must map and whose streams
+// it waits for; a virtual box has none.
+struct RingTable {
+  std::vector<gpud_ring_src> src;
+  std::vector<int64_t> total;
+  gpud_ring* const* rings = nullptr;
+  int n() const { return (int)total.size(); }
+};
+// The table of rings[0, n_rings), rings[0] the home ring.
+RingTable ring_table(gpud_ring* const* rings, int n_rings);
+
+// The sets of a call over table t (slot 0 the view v's ring), into out_f64 [5][F][n_sets] / out_n_over [F][n_sets], on the scratch
+// *state (created on first use).  ranges.cu says the rest.
+int32_t reduce_sets(const gpud_ring_view& v, const RingTable& t, const int32_t* ring_of, const int64_t* first, const int64_t* len, int64_t n_ranges,
+                    const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over, gpud_ranges_state** state);
+// The sets ids[] of a call (set_off NULL: every range a set) reduced as a call of their own over v and table t, on *state: range i in
+// slot ring_of[i] (ring_of NULL: all in slot 0) from sample first[i], len[i] samples, into f64 [5][F][ids] / nov [F][ids].
+int32_t reduce_subset(const gpud_ring_view& v, const RingTable& t, const std::vector<int64_t>& ids, const int32_t* ring_of, const int64_t* first,
+                      const int64_t* len, const int64_t* set_off, gpud_ranges_state** state, std::vector<double>& f64, std::vector<uint32_t>& nov);
 // The results of a select's n_long segments (s->d_out [5][F n_long], s->d_nover) into columns geo[j].id of out [5][F][n_out] / nover [F][n_out].
 cudaError_t ranges_scatter(const gpud_ring_view& v, const gpud_range_state* s, int64_t n_long, int64_t n_out, double* out, uint32_t* nover);

@@ -3,7 +3,9 @@
 // decides its mode and width, k_ckpt_pack writes it).  A row is its record - first sample, byte offset, the F directory bytes and the
 // F block word offsets from the end of the record - then the blocks in field order.  k_tier_place lays the rows one push completed
 // into the byte ring (gpud_tier_place), writes their records and each block's word offset for k_ckpt_pack.  A decode gathers the
-// directory and offsets of the rows it wants from their records (k_tier_gather) and runs k_ckpt_unpack<true> into a virtual ring.
+// directory and offsets of the rows it wants from their records (k_tier_gather) and runs k_ckpt_unpack<true> into a slot of a range
+// call's virtual box, on the device of the call's home ring, which may be another than the tier's; k_tier_ring_runs fills the slot's
+// rows the tier does not hold from the ring.
 #include "ckpt.h"
 
 namespace {
@@ -105,13 +107,21 @@ __global__ void __launch_bounds__(256) k_tier_gather(const int64_t* __restrict__
   }
 }
 
-// The tail of the virtual ring: samples [first, first + n) of fields [f0, f0 + G) from the ring to virtual columns vcol0.., with the
-// sample ring kept as k_ring_append keeps it.
-__global__ void __launch_bounds__(256) k_tier_tail(const double* __restrict__ ring, int64_t cap, int64_t first, int64_t n, int f0, int G, double* __restrict__ vring,
-                                                   int64_t vcap, int64_t vcol0, double* __restrict__ vsmp, int smp_shift, int64_t smp_half, int64_t smp_slots) {
+// Ring samples into a virtual slot: the n samples of the runs (gpud_tier_run, ascending off) of fields [f0, f0 + G) from the ring to
+// their virtual columns, with the sample ring kept as k_ring_append keeps it.  The newest row, not yet coded, is one run; an untiered
+// ring's rows, or rows a tier does not hold, are the others.
+__global__ void __launch_bounds__(256) k_tier_ring_runs(const double* __restrict__ ring, int64_t cap, const gpud_tier_run* __restrict__ runs, int64_t n_runs,
+                                                        int64_t n, int f0, int G, double* __restrict__ vring, int64_t vcap, double* __restrict__ vsmp,
+                                                        int smp_shift, int64_t smp_half, int64_t smp_slots) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < (int64_t)G * n; i += (int64_t)gridDim.x * blockDim.x) {
-    const int64_t f = i / n, t = i - f * n, c = vcol0 + t;
-    const double x = ring[(f0 + f) * cap + (first + t) % cap];
+    const int64_t f = i / n, t = i - f * n;
+    int64_t lo = 0, hi = n_runs;                   // the run of sample t: the last whose off <= t
+    while (hi - lo > 1) {
+      const int64_t mid = (lo + hi) >> 1;
+      if (__ldg(&runs[mid].off) <= t) lo = mid; else hi = mid;
+    }
+    const int64_t d = t - __ldg(&runs[lo].off), c = __ldg(&runs[lo].vcol) + d;
+    const double x = ring[(f0 + f) * cap + (__ldg(&runs[lo].first) + d) % cap];
     vring[f * vcap + c] = x;
     if ((c & ((1ll << smp_shift) - 1)) == smp_half) vsmp[f * smp_slots + (c >> smp_shift)] = x;
   }
@@ -215,9 +225,8 @@ cudaError_t launch_copy(const gpud_ring* r, const TierCopy* rows, int64_t n_rows
 void gpud_tier_free(gpud_tier* t) {
   if (!t) return;
   cudaFree(t->d_buf); cudaFree(t->d_slot); cudaFree(t->d_ctl); cudaFree(t->d_dir); cudaFree(t->d_words); cudaFree(t->d_offs); cudaFree(t->d_csum);
-  cudaFree(t->d_rowsz); cudaFree(t->d_vring); cudaFree(t->d_vsmp); cudaFree(t->d_rows); cudaFree(t->d_vdir); cudaFree(t->d_voffs);
+  cudaFree(t->d_rowsz);
   for (auto& e : t->ev_enc) if (e) cudaEventDestroy(e);
-  for (auto& e : t->ev_dec) if (e) cudaEventDestroy(e);
   delete t;
 }
 
@@ -259,37 +268,26 @@ int32_t gpud_tier_read_ctl(gpud_ring* r, gpud_tier_ctl* c) {
   return GPUD_OK;
 }
 
-int32_t gpud_tier_decode(gpud_ring* r, const std::vector<int64_t>& rows, int64_t rows_tail, int64_t tail_n, int f0, int G, int64_t vcap,
-                         int smp_shift, int64_t smp_slots, double** vring, double** vsmp) {
-  gpud_tier* t = r->tier;
-  const int64_t n = (int64_t)rows.size(), units = (int64_t)G * n;
-  GPUD_CUDA(r->ctx, gpud_grow(&t->d_vring, &t->vring_cap, (size_t)G * vcap));
-  GPUD_CUDA(r->ctx, gpud_grow(&t->d_vsmp, &t->vsmp_cap, (size_t)G * smp_slots));
-  GPUD_CUDA(r->ctx, gpud_grow(&t->d_rows, &t->rows_cap, std::max<size_t>(1, n)));
-  GPUD_CUDA(r->ctx, gpud_grow(&t->d_vdir, &t->vdir_cap, std::max<size_t>(1, units)));
-  GPUD_CUDA(r->ctx, gpud_grow(&t->d_voffs, &t->voffs_cap, std::max<size_t>(1, units)));
-  for (auto& e : t->ev_dec) if (!e) GPUD_CUDA(r->ctx, cudaEventCreate(&e));
-  *vring = t->d_vring;
-  *vsmp = t->d_vsmp;
-  const int64_t half = (1ll << smp_shift) >> 1;
-  GPUD_CUDA(r->ctx, cudaEventRecord(t->ev_dec[0], r->stream));
-  if (n > 0) {
-    GPUD_CUDA(r->ctx, cudaMemcpyAsync(t->d_rows, rows.data(), n * sizeof(int64_t), cudaMemcpyHostToDevice, r->stream));
-    GPUD_CUDA(r->ctx, launch_gather(r, t->d_rows, n, f0, G, t->d_buf, t->d_slot, t->slots, t->d_vdir, t->d_voffs));
-    CkGeo g = rows_geo(G, n);
-    g.ring = t->d_vring; g.sample = t->d_vsmp; g.cap = vcap;
-    g.smp_half = half; g.smp_slots = smp_slots; g.smp_shift = smp_shift;
-    // the field sums k_ckpt_unpack re-forms land in the encode's scratch, which no one reads
-    GPUD_CUDA(r->ctx, launch_unpack(r, true, g, t->d_vdir, t->d_voffs, t->d_buf, t->d_csum));
-  }
-  if (tail_n > 0) {
-    const int grid = (int)std::min<int64_t>(((int64_t)G * tail_n + 255) / 256, (int64_t)r->sm_count * 8);
-    k_tier_tail<<<grid, 256, 0, r->stream>>>(r->d_ring, r->cap, rows_tail * kBlock, tail_n, f0, G, t->d_vring, vcap, n * kBlock, t->d_vsmp, smp_shift, half,
-                                             smp_slots);
-    GPUD_CUDA(r->ctx, cudaGetLastError());
-  }
-  GPUD_CUDA(r->ctx, cudaEventRecord(t->ev_dec[1], r->stream));
-  return GPUD_OK;
+cudaError_t gpud_tier_decode(const gpud_ring* h, const gpud_ring* o, const int64_t* d_rows, int64_t n, int f0, int G, const gpud_vslot& s,
+                             int64_t vcol0, uint8_t* dir, unsigned long long* offs, unsigned long long* csum) {
+  if (n == 0) return cudaSuccess;
+  const gpud_tier* t = o->tier;
+  // the gather and the unpack run on h; every ring of a call has h's F, so o's records have h's layout
+  const cudaError_t e = launch_gather(h, d_rows, n, f0, G, t->d_buf, t->d_slot, t->slots, dir, offs);
+  if (e != cudaSuccess) return e;
+  CkGeo g = rows_geo(G, n);
+  g.ring = s.ring; g.sample = s.sample; g.cap = s.vcap; g.start = vcol0;
+  g.smp_half = (1ll << s.smp_shift) >> 1; g.smp_slots = s.smp_slots; g.smp_shift = s.smp_shift;
+  return launch_unpack(h, true, g, dir, offs, t->d_buf, csum);
+}
+
+cudaError_t gpud_tier_copy_runs(const gpud_ring* h, const gpud_ring* o, const gpud_tier_run* d_runs, int64_t n_runs, int64_t n_samples, int f0, int G,
+                                const gpud_vslot& s) {
+  if (n_runs == 0 || n_samples == 0) return cudaSuccess;
+  const int grid = (int)std::min<int64_t>(((int64_t)G * n_samples + 255) / 256, (int64_t)h->sm_count * 8);
+  k_tier_ring_runs<<<grid, 256, 0, h->stream>>>(o->d_ring, o->cap, d_runs, n_runs, n_samples, f0, G, s.ring, s.vcap, s.sample, s.smp_shift,
+                                                (1ll << s.smp_shift) >> 1, s.smp_slots);
+  return cudaGetLastError();
 }
 
 // tier_open's refusals of a ring's capacity and a tier's size (tier_restore's too).

@@ -320,8 +320,17 @@ int32_t gpud_ring_reduce_range_sets(gpud_ring* ring, const int64_t* first, const
  * kernels run on its device and stream with its scratch, and its gpud_ring_ranges_stats reports the call.  Rings on other devices are
  * read in place through peer mappings, which the call enables once per device pair.  Before its first launch the home stream waits
  * for every other ring's stream; nothing else of the other rings changes.  Synchronous.
+ * Tiers (gpud_ring_tier_open below): rings of one call may mix tiered and untiered, the home ring either.  Range i on a tiered ring k is
+ * valid when len >= 1, first + len <= total_k and first >= lo_k = min(total_k - count_k, first_sample_k) (gpud_ring_tier_counts), the
+ * rule of gpud_ring_reduce_ranges on that ring; the definitions and the exactness are unchanged (min / max / p99 / n_over bit for bit
+ * what untiered rings that hold every sample give).  The call reads each tiered ring's control word, synchronising its stream once.
+ * A set with a range before its ring's own samples reads the rows its tier sets cover from a virtual box on the home device: rows a
+ * tier holds decoded there (other rings' coded rows read in place), the others copied from their ring, in groups of fields that keep it
+ * near 1 GiB; its scratch is kept on the home ring, whose gpud_ring_ranges_stats and, tiered, gpud_ring_tier_stats decode time report
+ * the whole call.  A failed allocation -> GPUD_E_CUDA, every ring usable.  A call with no such set launches what it would without tiers.
  * Every refusal comes before any launch, writes nothing and names the ring, range or set in gpud_last_error: what
- * gpud_ring_reduce_range_sets refuses (each range checked against its own ring's counts); n_rings < 1 or > 32768, a NULL ring, ring_of[i] outside
+ * gpud_ring_reduce_range_sets refuses (each range checked against its own ring's counts, or a tiered ring's reach [lo_k, total_k),
+ * which the message names); n_rings < 1 or > 32768, a NULL ring, ring_of[i] outside
  * [0, n_rings), or a ring of another ctx -> GPUD_E_INVALID; a config that differs from the home ring's, compared as gpud_ring_restore
  * compares it -> GPUD_E_INVALID naming the field; a ring on a device the home device cannot map as a peer -> GPUD_E_UNSUPPORTED. */
 int32_t gpud_rings_reduce_range_sets(gpud_ring* const* rings, int32_t n_rings, const int32_t* ring_of, const int64_t* first,
@@ -420,9 +429,9 @@ int32_t gpud_ring_checkpoint_stats(gpud_ring* ring, float* encode_ms, float* dec
  * row wholly in the ring, so the tier and the ring always hold one contiguous run of the push order.
  * On a tiered ring gpud_ring_reduce_ranges and gpud_ring_reduce_range_sets take any range with len >= 1, first + len <= total and
  * first >= min(total - count, first_sample) (gpud_ring_tier_counts), with the same definitions and every other refusal unchanged;
- * min / max / p99 / n_over equal bit for bit what a ring of a CAP that holds all those samples gives.  gpud_rings_reduce_range_sets,
- * gpud_box_query, checkpoints and deltas ignore the tier (a restored ring has none until gpud_ring_tier_restore below; restore into a
- * tiered ring -> GPUD_E_STATE).
+ * min / max / p99 / n_over equal bit for bit what a ring of a CAP that holds all those samples gives.  Both are the n_rings = 1 case of
+ * gpud_rings_reduce_range_sets, which takes the same reach on each tiered ring of a call.  gpud_box_query, checkpoints and deltas
+ * ignore the tier (a restored ring has none until gpud_ring_tier_restore below; restore into a tiered ring -> GPUD_E_STATE).
  * Open: once per ring (again -> GPUD_E_STATE); allocates tier_bytes (rounded down to 8) for the rows, plus 8 KiB per field and 16 B
  * per row it could hold, on the ring's device until gpud_ring_destroy.  CAP < 2048, or tier_bytes below one row coded at 64 bits and
  * its record (8192 F + 16 + pad8(F) + pad8(4 F)) -> GPUD_E_INVALID; a failed allocation -> GPUD_E_NOMEM / GPUD_E_CUDA with the ring
@@ -432,7 +441,8 @@ int32_t gpud_ring_tier_open(gpud_ring* ring, int64_t tier_bytes);
  * and *rows_lost_total rows were lost since the open.  Any pointer may be NULL; GPUD_E_STATE without a tier. */
 int32_t gpud_ring_tier_counts(gpud_ring* ring, int64_t* first_sample, int64_t* next_sample, int64_t* bytes_used, int64_t* rows_lost_total);
 /* Synchronise the ring's stream: device ms of the last encode (the last push that completed a row; 0 before one), of the last range
- * call's decode (0 if none touched the tier), and the blocks of that encode by mode ([2]: RAW, INT).  GPUD_E_STATE without a tier. */
+ * call homed on this ring that decoded (every ring's rows it decoded; 0 before one), and the blocks of that encode by mode ([2]: RAW,
+ * INT).  GPUD_E_STATE without a tier. */
 int32_t gpud_ring_tier_stats(gpud_ring* ring, float* encode_ms, float* decode_ms, int64_t* blocks_by_mode);
 /* Tier checkpoints (DESIGN.md §2 "Tier", format: DESIGN.md "Ring tier checkpoint format"): the tier's rows as bytes that outlive the
  * process, so that a restarted daemon keeps its history beyond CAP.  A full tier checkpoint holds the rows [first, next) the tier holds,

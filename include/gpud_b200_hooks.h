@@ -93,6 +93,17 @@ int32_t gpudh_ring_tier_plan(int64_t cap, int32_t n_fields, int64_t tier_bytes, 
 int32_t gpudh_ring_tier_split(int64_t total, int64_t cap, int32_t n_fields, int64_t tier_first, int64_t tier_next, const int64_t* first,
                               const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets, int32_t* route, int64_t* vfirst,
                               int64_t* rows, int64_t rows_cap, int64_t* n_rows, int64_t* vtotal);
+/* The split of one gpud_rings_reduce_range_sets (set_off NULL: every range a set, n_sets = n_ranges) over n_rings rings of capacity
+ * cap: ring k has pushed totals[k] samples and its tier holds rows [tier_first[k], tier_next[k]) (tier_first[k] < 0: no tier).
+ * route[s] = 0 (its rings, the driver as it is) or 1 (the virtual box); per range of a tier set its slot vslot[i] and first sample
+ * vfirst[i] there (-1 otherwise); *n_slots slots, slot v holding ring slot_ring[v]'s rows rows[slot_rows[v] .. slot_rows[v + 1]),
+ * ascending, each decoded from the tier (dec 1) or copied from the ring (dec 0), and vtotal[v] samples; *vcap the slots' capacity.
+ * slot_ring and vtotal take n_rings entries, slot_rows n_rings + 1; GPUD_E_CAPACITY if rows_cap is below the rows, GPUD_E_INVALID for
+ * what the call refuses. */
+int32_t gpudh_rings_tier_split(const int64_t* totals, int32_t n_rings, int64_t cap, const int64_t* tier_first, const int64_t* tier_next,
+                               const int32_t* ring_of, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off,
+                               int64_t n_sets, int32_t* route, int32_t* vslot, int64_t* vfirst, int32_t* n_slots, int32_t* slot_ring,
+                               int64_t* vtotal, int64_t* slot_rows, int64_t* rows, uint8_t* dec, int64_t rows_cap, int64_t* vcap);
 /* Row `row` of the tier as it lies in its byte ring: the record, then the blocks (*n_bytes; GPUD_E_CAPACITY if cap is smaller, a row
  * the tier does not hold -> GPUD_E_INVALID).  Synchronises. */
 int32_t gpudh_ring_tier_row(gpud_ring* r, int64_t row, void* out, int64_t cap, int64_t* n_bytes);
