@@ -1,7 +1,7 @@
 """The whole-range order statistic (gpud_ring_reduce_range) against the oracle and against the numpy model of its routes
 (test_range_paths_model.py), on the fields of range_cases.py: one field per route in every ring, so the fields the radix select
 redoes sit at non-contiguous indices.  Values: min / max / the order statistic / n_over bit for bit, mean and EMA within
-oracle/SPEC.md's tolerance (the C oracle, a port of pyoracle.window_aggregates, over one window of the whole range).  Routes, for
+the rounding budget of mean_ema_ref.py (its extended-precision reference over one window of the whole range).  Routes, for
 sampled ranges: range_stats' count of fields redone and their reasons, and the pivots, list fill and per-window class counts the
 pass left in the ring's scratch (gpudh_ring_range_scratch), all exactly as the model predicts.  A fault there usually costs only
 time, since the radix select still finds the right value; these checks see it.  Run on an H100: pytest -m gpu."""
@@ -10,8 +10,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from oracle import coracle
 from oracle import pyoracle as O
+import mean_ema_ref as R
 import range_cases as RC
 from test_range_paths_model import model_ring
 
@@ -71,19 +71,12 @@ def _run(env, cap, pushed, last_n, q_num, q_den, xs):
         scratch = _scratch(L, r, F)
     finally:
         r.close()
-    want = coracle.windows_fields(xs, n, thr, min(2.0 / (W + 1.0), 0.9999), q_num, q_den)
+    want = R.windows_fields(xs, n, thr, min(2.0 / (W + 1.0), 0.9999), q_num, q_den)
     for k in ("min", "max", "p99"):
         bad = np.flatnonzero(got[k].view(np.uint64) != want[k][:, 0].view(np.uint64))
         assert bad.size == 0, (k, bad.tolist(), got[k][bad[0]], want[k][bad[0], 0])
     assert np.array_equal(got["n_over"], want["n_over"][:, 0])
-    with np.errstate(invalid="ignore", over="ignore"):
-        scale = np.array([np.abs(x[np.isfinite(x)]).max(initial=0.0) for x in xs])
-        for k in ("mean", "ema"):
-            a, b = got[k], want[k][:, 0]
-            same = (a.view(np.uint64) == b.view(np.uint64)) | (np.isnan(a) & np.isnan(b))
-            close = np.isfinite(a) & np.isfinite(b) & (np.abs(a - b) <= 1e-6 * np.maximum(np.abs(b), scale))
-            bad = np.flatnonzero(~(same | close))
-            assert bad.size == 0, (k, bad.tolist(), a[bad[0]], b[bad[0]])
+    R.check_mean_ema(got, R.select(want, (slice(None), 0)))
     return got, stats, reasons, scratch
 
 

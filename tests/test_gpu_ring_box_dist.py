@@ -4,7 +4,8 @@ driver steps every rank and "all-gathers" with device-to-device copies into one 
   - every round's send size is equal on all ranks, and every rank's result is the same bit for bit;
   - the result equals gpud_rings_reduce_range_sets over the same rings in one process: min / max / p99 / n_over bit for bit for every
     set, all six outputs for sets local to one rank and spread sets of up to 1024 samples (one of odd length first, so the dense
-    columns after it start odd); mean and EMA of long spread sets, and everything, against the C oracle on each concatenation;
+    columns after it start odd); mean and EMA of long spread sets, on both sides, within the rounding budget of mean_ema_ref.py's
+    reference on each concatenation, and everything against the reference;
   - every radix-select reason forced in sets spread over ranks (tests/range_cases.py), with the reasons and every pivot equal to the
     one-process call's; a call of three long-route batches;
   - every refusal reaches every rank at the same step with the same code and message: differing arguments, a range invalid on one
@@ -32,6 +33,7 @@ from test_gpu_segment_paths import _scratch
 from test_gpu_ring_range_sets import _bits, _push
 from test_gpu_ring_ranges import OPS, _alpha, _fields, _thr
 from test_gpu_window_paths import _check
+import mean_ema_ref as R
 
 pytestmark = pytest.mark.gpu
 
@@ -152,7 +154,7 @@ def test_simulated_ranks_against_one_process_and_oracle(env, n_rings, W, q, alph
         cols = slice(None) if op in ("min", "max", "p99", "n_over") else ~long_spread
         bad = np.argwhere(res[0][op][:, cols] != one[op][:, cols])
         assert bad.size == 0, (op, bad[:5].tolist())
-    _check(qs[0].result(), _want(xs, olds, ring_of, first, length, set_off, thr, _alpha(W, alpha), q), np.concatenate(xs, axis=1))
+    _check(qs[0].result(), _want(xs, olds, ring_of, first, length, set_off, thr, _alpha(W, alpha), q))
     for k, qq in enumerate(qs):
         st = qq.stats()
         assert st["rounds"] == len(sizes) and st["bytes_sent"] == sum(sizes)
@@ -295,7 +297,7 @@ def test_radix_reasons_spread_over_ranks(env, n_rings):
         qq.close()
     held = [x[:, o:] for x, o in zip(xs, olds)]
     _check({k: v.view(np.float64) if k != "n_over" else v for k, v in got.items()},
-           _want(held, olds, ring_of, first, length, set_off, thr, _alpha(1000, 0.0), q), np.concatenate(held, axis=1))
+           _want(held, olds, ring_of, first, length, set_off, thr, _alpha(1000, 0.0), q))
     for r in rings:
         r.close()
 
@@ -308,11 +310,14 @@ def test_three_batches(env):
     rng = np.random.default_rng(3)
     total = cap + 12345
     rings = [g.Ring(ctx, F, cap, 1000, thresholds=np.full(F, 60.0)) for _ in range(2)]
+    hist = np.empty((F, total))                                       # the pushed samples, for the reference
     for a in range(0, total, 1 << 18):
         rows = rng.normal(60.0, 3.0, (min(1 << 18, total - a), F)).astype(np.float32)
+        hist[:, a:a + rows.shape[0]] = rows.T
         for r in rings:
             r.push(rows)
     lo = total - cap
+    hist = hist[:, lo:]
     sets, whole = [], []
     for i in range(140):
         a = int(rng.integers(lo, total - cap + 1)) if rng.random() < 0.2 else lo
@@ -326,9 +331,13 @@ def test_three_batches(env):
     want = _bits(rings[0].reduce_ranges([w[0] for w in whole], [w[1] for w in whole]))
     for op in ("min", "max", "p99", "n_over"):
         assert np.array_equal(got[op], want[op]), op
-    for op in ("mean", "ema"):
-        a, b = got[op].view(np.float64), want[op].view(np.float64)
-        assert np.allclose(a, b, rtol=1e-9, atol=1e-9 * 60.0), op
+    # mean and EMA fold in another order than the uncut range's: both against the reference on every field
+    ref = {}
+    for a in sorted({w[0] for w in whole}):
+        ref[a] = R.select(R.windows_fields(hist[:, a - lo:a - lo + cap], cap, np.full(F, 60.0), _alpha(1000, 0.0)), (slice(None), 0))
+    want_ref = R.stack([ref[w[0]] for w in whole])
+    for side, d in (("box", got), ("one ring", want)):
+        R.check_mean_ema({op: d[op].view(np.float64) for op in ("mean", "ema")}, want_ref, what=side)
     assert len(sizes) >= 1 + 3 * 3                                    # the header, then samples / summaries / lists of three batches
     for q in qs:
         q.close()
@@ -388,10 +397,13 @@ def _worker(rank, world, init, backend="gloo"):
             if not np.array_equal(got[op][:, cols], want[op][:, cols]):
                 print("rank 0:", op, "differs from the one-process call", file=sys.stderr)
                 ok = False
-        for op in ("mean", "ema"):
-            a, b = got[op].view(np.float64)[:, long_spread], want[op].view(np.float64)[:, long_spread]
-            if not np.allclose(a, b, rtol=1e-9, atol=1e-7, equal_nan=True):
-                print("rank 0:", op, "of long spread sets is off", file=sys.stderr)
+        ref = R.select(_want([_fields(F, t, np.random.default_rng([k, 5])) for k, t in enumerate(totals)], [0] * world, *args, thr,
+                             _alpha(W, 0.0), (0, 0)), (slice(None), long_spread))
+        for side, d in (("box", got), ("one process", want)):
+            try:
+                R.check_mean_ema({op: d[op].view(np.float64)[:, long_spread] for op in ("mean", "ema")}, ref, what=side)
+            except AssertionError as e:
+                print("rank 0: mean / EMA of long spread sets:", e, file=sys.stderr)
                 ok = False
         for r in rings[1:]:
             r.close()

@@ -1,5 +1,5 @@
 """gpud_rings_reduce_range_sets (DESIGN.md §2 "Box sets") against the C oracle: sets whose ranges lie in 2 to 8 rings of one config,
-with different totals (some wrapped, some not).  Every set is compared with oracle.coracle.windows_fields on its ranges' samples
+with different totals (some wrapped, some not).  Every set is compared with mean_ema_ref.windows_fields on its ranges' samples
 concatenated in the order given, W = their total: min / max / p99 / n_over bit for bit, mean and EMA within oracle/SPEC.md's tolerance.
 Covered: short and long sets, tiles across a join of two rings, singleton sets in every ring (equal to that ring's reduce_ranges in all
 six outputs, and its pivots taken from that ring's own sample ring), one-ring calls (equal to reduce_range_sets), sets cut across rings that hold
@@ -13,7 +13,7 @@ import pytest
 
 import range_cases as RC
 import test_segment_paths_model as M
-from oracle import coracle
+import mean_ema_ref as R
 from test_gpu_ring_range_sets import _bits, _push
 from test_gpu_ring_ranges import OPS, _alpha, _fields, _thr
 from test_gpu_segment_paths import _scratch
@@ -44,8 +44,8 @@ def _want(xs, olds, ring_of, first, length, set_off, thr, alpha, q):
     for s in range(len(set_off) - 1):
         c = np.concatenate([xs[k][:, f - olds[k]:f - olds[k] + n] for k, f, n in
                             zip(ring_of[set_off[s]:set_off[s + 1]], first[set_off[s]:set_off[s + 1]], length[set_off[s]:set_off[s + 1]])], axis=1)
-        cols.append(coracle.windows_fields(np.ascontiguousarray(c), c.shape[1], thr, alpha, q[0], q[1]))
-    return {k: np.concatenate([c[k] for c in cols], axis=1) for k in OPS}
+        cols.append(R.windows_fields(np.ascontiguousarray(c), c.shape[1], thr, alpha, q[0], q[1]))
+    return {k: np.concatenate([c[k] for c in cols], axis=1) for k in cols[0]}
 
 
 def _sets(sets):
@@ -97,7 +97,7 @@ def _mixed(g, ctx, devs, W, q, alpha):
     sets = [sets[i] for i in order]
     ring_of, first, length, set_off = _sets(sets)
     got = g.rings_reduce_range_sets(rings, ring_of, first, length, set_off)
-    _check(got, _want(xs, olds, ring_of, first, length, set_off, thr, _alpha(W, alpha), q), np.concatenate(xs, axis=1))
+    _check(got, _want(xs, olds, ring_of, first, length, set_off, thr, _alpha(W, alpha), q))
     ms, n_radix, why = rings[0].ranges_stats()                        # the home ring reports the call
     assert ms > 0 and n_radix == sum(why.values())
     # singleton sets: their own ring's reduce_ranges, all six outputs bit for bit
@@ -228,7 +228,7 @@ def test_radix_reasons_across_rings(env, cap, n):
     for r in rings:
         r.close()
     held = [x[:, o:] for x, o in zip(xs, olds)]
-    _check(got, _want(held, olds, ring_of, first, length, set_off, thr, _alpha(1000, 0.0), q), np.concatenate(held, axis=1))
+    _check(got, _want(held, olds, ring_of, first, length, set_off, thr, _alpha(1000, 0.0), q))
     expect = {}
     for route, _ in built:
         if route in M.OPEN:

@@ -1,6 +1,6 @@
 """Hopping stream windows (gpud_ring_windows_open_hop) against the C oracle.  The whole pushed stream is kept on the host; after each
-reduce every window of the handle's history is compared with oracle.coracle.windows_fields: min / max / p99 / n_over bit for bit
-and the mean within oracle/SPEC.md's tolerance from W = L run on each window's own samples, the EMA within tolerance from W = P run
+reduce every window of the handle's history is compared with mean_ema_ref.windows_fields: min / max / p99 / n_over bit for bit
+and the mean within its rounding budget from W = L run on each window's own samples, the EMA within budget from W = P run
 over the stream from the handle's EMA seed on, read at the windows' ends.  Shapes with L <= 1024 (the window kernel) and L > 1024
 (the segment select), P <= 1024 and P > 1024, CAP not a multiple of L or P, hop = span; pushes of 1, P - 1, P, L, CAP and more;
 loss, restart and eviction; alpha = 0.9999 through +inf and -inf; the select's radix reasons through the stats; and cross-checks
@@ -8,7 +8,7 @@ against tumbling handles, gpud_ring_reduce_range, and a ring without handles.  R
 import numpy as np
 import pytest
 
-from oracle import coracle
+import mean_ema_ref as R
 from test_gpu_window_paths import _check
 from test_gpu_ring_stream import _stream, _thresholds
 import test_ring_windows_model as WM
@@ -70,10 +70,12 @@ class HRun:
     def want(self, first, nxt):
         alpha = self.alpha if self.alpha > 0 else min(2.0 / (self.W + 1.0), 0.9999)   # the ring's alpha
         xs = np.concatenate([self.x[:, k * self.P:k * self.P + self.L] for k in range(first, nxt)], axis=1)
-        want = coracle.windows_fields(xs, self.L, self.thr, alpha, self.q[0], self.q[1])
+        want = R.windows_fields(xs, self.L, self.thr, alpha, self.q[0], self.q[1])
         src = self.x[:, self.seed_w * self.P:(nxt - 1) * self.P + self.L]
-        ema = coracle.windows_fields(src, self.P, self.thr, alpha, self.q[0], self.q[1])["ema"]
-        want["ema"] = ema[:, [k - self.seed_w + self.p - 1 for k in range(first, nxt)]]
+        ema = R.windows_fields(src, self.P, self.thr, alpha, self.q[0], self.q[1])
+        ends = [k - self.seed_w + self.p - 1 for k in range(first, nxt)]
+        for key in ("ema", "ema_err", "ema_exempt"):
+            want[key] = ema[key][:, ends]
         return want, src
 
     def check(self):
@@ -82,7 +84,7 @@ class HRun:
             return
         want, src = self.want(first, nxt)
         got = {k: self.h.read(k, first, nxt - first) for k in OPS}
-        _check(got, want, src)
+        _check(got, want)
 
     def close(self):
         self.h.close()

@@ -12,7 +12,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from oracle import coracle
+import mean_ema_ref as R
 import ring_ingest as RI
 from test_range_paths_model import model_ring
 
@@ -297,10 +297,11 @@ def test_busy_caller_stream_and_stream_switch(env):
         check(env, ring, model, "own stream")
         got = ring.reduce_all()
         sel = [0, 1, 31, 32, 2048, F - 1]
-        want = coracle.windows_fields(model.chronological(sel), 1000, thr[sel])
+        want = R.windows_fields(model.chronological(sel), 1000, thr[sel])
         for k in ("min", "max", "p99"):
             assert np.array_equal(got[k][sel].view(np.uint64), want[k].view(np.uint64)), k
         assert np.array_equal(got["n_over"][sel], want["n_over"])
+        R.check_mean_ema({k: got[k][sel] for k in ("mean", "ema")}, want)
     finally:
         ring.close()
 
@@ -330,10 +331,11 @@ def test_bench_e2e_transport_quarter_ring(env):
         got = ring.reduce_all()
         sel = [0, 1, 255, 256, 511]
         x = model.chronological(sel)
-        want = coracle.windows_fields(x, W, thr[sel])
+        want = R.windows_fields(x, W, thr[sel])
         for k in ("min", "max", "p99"):
             assert np.array_equal(got[k][sel].view(np.uint64), want[k].view(np.uint64)), k
         assert np.array_equal(got["n_over"][sel], want["n_over"])
+        R.check_mean_ema({k: got[k][sel] for k in ("mean", "ema")}, want)
         ring.reduce_range(0)
         assert ring.range_stats()[2] == 0, ring.range_open_reasons
         piv = np.empty((F, 2), dtype=np.float64)

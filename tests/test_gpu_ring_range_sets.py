@@ -1,4 +1,4 @@
-"""gpud_ring_reduce_range_sets against the C oracle.  Every set of a call is compared with oracle.coracle.windows_fields run on its
+"""gpud_ring_reduce_range_sets against the C oracle.  Every set of a call is compared with mean_ema_ref.windows_fields run on its
 ranges' samples concatenated in the order given, with W = their total and the ring's alpha: min / max / p99 / n_over bit for bit, mean
 and EMA within oracle/SPEC.md's tolerance.  Covered: singleton sets (equal to gpud_ring_reduce_ranges in all six outputs), sets of
 many 1-sample ranges short and long, joins at lane 0 / 31, mid-row and at a tile edge +-1, pieces across the physical end of a wrapped
@@ -13,7 +13,7 @@ import pytest
 
 import range_cases as RC
 import test_segment_paths_model as M
-from oracle import coracle
+import mean_ema_ref as R
 from test_gpu_ring_ranges import OPS, _alpha, _fields, _thr
 from test_gpu_segment_paths import _check_scratch, _scratch
 from test_gpu_window_paths import _check
@@ -43,8 +43,8 @@ def _want(x, oldest, first, length, set_off, thr, alpha, q):
     cols = []
     for s in range(len(set_off) - 1):
         c = _concat(x, oldest, first, length, set_off, s)
-        cols.append(coracle.windows_fields(np.ascontiguousarray(c), c.shape[1], thr, alpha, q[0], q[1]))
-    return {k: np.concatenate([c[k] for c in cols], axis=1) for k in OPS}
+        cols.append(R.windows_fields(np.ascontiguousarray(c), c.shape[1], thr, alpha, q[0], q[1]))
+    return {k: np.concatenate([c[k] for c in cols], axis=1) for k in cols[0]}
 
 
 def _sets(pieces):
@@ -91,7 +91,7 @@ def test_sets_against_oracle(env, W, q, alpha):
     sets = [sets[i] for i in order]
     first, length, set_off = _sets(sets)
     got = r.reduce_range_sets(first, length, set_off)
-    _check(got, _want(x[:, lo:], lo, first, length, set_off, thr, _alpha(W, alpha), q), x[:, lo:])
+    _check(got, _want(x[:, lo:], lo, first, length, set_off, thr, _alpha(W, alpha), q))
     ms, n_radix, why = r.ranges_stats()
     assert ms > 0 and n_radix == sum(why.values())
     # singleton sets: gpud_ring_reduce_ranges' answer, all six outputs bit for bit
@@ -109,7 +109,7 @@ def test_sets_against_oracle(env, W, q, alpha):
     b0, b1 = _bits(a0), _bits(a1)
     for k in ("min", "max", "p99", "n_over"):
         assert np.array_equal(b0[k], b1[k]), k
-    _check(a1, _want(x[:, lo:], lo, f1, l1, o1, thr, _alpha(W, alpha), q), x[:, lo:])
+    _check(a1, _want(x[:, lo:], lo, f1, l1, o1, thr, _alpha(W, alpha), q))
     r.close()
 
 
@@ -192,7 +192,7 @@ def test_radix_reasons(env, cap, n):
     scr = _scratch(L, r)
     r.close()
     xs = x[:, oldest:]
-    _check(got, _want(xs, oldest, first, length, set_off, thr, _alpha(1000, 0.0), q), xs)
+    _check(got, _want(xs, oldest, first, length, set_off, thr, _alpha(1000, 0.0), q))
     expect = {}
     for route, _ in built:
         if route in M.OPEN:

@@ -1,7 +1,7 @@
-"""gpud_ring_reduce_ranges against the C oracle.  Every range of a call is compared with oracle.coracle.windows_fields run on that
-range's own samples with W = its length and the ring's alpha: min / max / p99 / n_over bit for bit, mean and EMA within oracle/SPEC.md's
-tolerance.  Lengths on both sides of 1024 (the short route and the long one), 64 Ki and the whole ring, ranges across the physical end
-after the ring has wrapped several times, overlapping, duplicate and unsorted ranges in one call, W = 1000 / 1 / 999 with quantiles
+"""gpud_ring_reduce_ranges against the C oracle.  Every range of a call is compared with mean_ema_ref.windows_fields run on that
+range's own samples with W = its length and the ring's alpha: min / max / p99 / n_over bit for bit (the C oracle's), mean and EMA
+within the rounding budget of their extended-precision reference.  Lengths on both sides of 1024 (the short route and the long
+one), 64 Ki and the whole ring, ranges across the physical end after the ring has wrapped several times, overlapping, duplicate and unsorted ranges in one call, W = 1000 / 1 / 999 with quantiles
 other than 99/100, fields of constants, signed zeros, infinities, NaN of both signs, monotone counters and ties, alpha = 0.9999 through
 +inf and -inf, and every radix-select reason, forced with data built against the long route's pivots (tests/range_cases.py).
 Cross-checks: gpud_ring_reduce_range, span and hop handles, gpud_ring_reduce's tumbling windows, and that none of them, nor
@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 
 import range_cases as RC
-from oracle import coracle
+import mean_ema_ref as R
 from test_gpu_window_paths import _check
 
 pytestmark = pytest.mark.gpu
@@ -33,9 +33,9 @@ def _alpha(W, alpha):
 
 
 def _want(x, first0, firsts, lens, thr, alpha, q):
-    """the oracle on each range's own samples (x holds samples first0 ..), stacked into [F][n]"""
-    cols = [coracle.windows_fields(x[:, f - first0:f - first0 + n], int(n), thr, alpha, q[0], q[1]) for f, n in zip(firsts, lens)]
-    return {k: np.concatenate([c[k] for c in cols], axis=1) for k in OPS}
+    """the reference on each range's own samples (x holds samples first0 ..), stacked into [F][n]"""
+    cols = [R.windows_fields(x[:, f - first0:f - first0 + n], int(n), thr, alpha, q[0], q[1]) for f, n in zip(firsts, lens)]
+    return {k: np.concatenate([c[k] for c in cols], axis=1) for k in cols[0]}
 
 
 def _fields(F, n, rng):
@@ -102,7 +102,7 @@ def test_lengths_positions_and_data(env, W, q, alpha):
     firsts, lens = np.array(firsts)[order], np.array(lens)[order]
     got = r.reduce_ranges(firsts, lens)
     want = _want(x[:, lo:], lo, firsts, lens, thr, _alpha(W, alpha), q)
-    _check(got, want, x[:, lo:])
+    _check(got, want)
     ms, n_radix, why = r.ranges_stats()
     assert ms > 0 and n_radix == sum(why.values())
     r.close()
@@ -147,7 +147,7 @@ def test_radix_reasons(env, cap, n, at):
     r.push(np.ascontiguousarray(x.T))
     got = r.reduce_ranges([first, first], [n, n])                  # twice: each copy is its own segment
     want = _want(x[:, first:], first, [first, first], [n, n], thr, _alpha(1000, 0.0), q)
-    _check(got, want, x[:, first:])
+    _check(got, want)
     _, n_radix, why = r.ranges_stats()
     expect = {}
     for route, _ in built:
@@ -188,7 +188,9 @@ def test_cross_checks(env):
         for k in ("min", "max", "p99", "n_over"):
             assert np.array_equal(h.read(k, first, nxt - first).view(np.uint64 if k != "n_over" else np.uint32),
                                   b[k].view(np.uint64 if k != "n_over" else np.uint32)), (h.L, h.P, k)
-        assert np.allclose(h.read("mean", first, nxt - first), b["mean"], rtol=1e-6, atol=1e-6 * 2.0 ** 53, equal_nan=True)
+        want = _want(x, 0, ks * h.P, np.full(len(ks), h.L), thr, _alpha(W, 0.0), (0, 0))
+        R.check_mean_ema({"mean": h.read("mean", first, nxt - first)}, want, keys=("mean",), what=("handle", h.L, h.P))
+        R.check_mean_ema(b, want, keys=("mean",), what=("ranges", h.L, h.P))
     # the ring's tumbling windows
     r.reduce()
     red = {k: r.read(k) for k in OPS}

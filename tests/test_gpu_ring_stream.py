@@ -1,14 +1,14 @@
 """Stream windows of the ring against the C oracle.  The whole pushed stream is kept on the host; after each stream reduce every
-window of the history is compared with oracle.coracle.windows_fields run over the stream from the history's EMA seed (the window
-the stream was opened or last restarted at) on: min / max / p99 / n_over bit for bit, mean and EMA within oracle/SPEC.md's
-tolerance.  Push sizes around W and CAP (and past CAP, which loses windows), the window loop's instantiations (W = 1000, 1024,
+window of the history is compared with mean_ema_ref.windows_fields run over the stream from the history's EMA seed (the window
+the stream was opened or last restarted at) on: min / max / p99 / n_over bit for bit, mean and EMA within their rounding
+budget.  Push sizes around W and CAP (and past CAP, which loses windows), the window loop's instantiations (W = 1000, 1024,
 960, 999, 1, 7) with windows that wrap the physical end of the ring, the EMA carried over many calls (also at alpha = 0.9999
 through an infinite sample), eviction past the history, and the ring's other reduces left exactly as they are.
 Run on an H100: pytest -m gpu."""
 import numpy as np
 import pytest
 
-from oracle import coracle
+import mean_ema_ref as R
 from test_gpu_window_paths import _check
 import window_cases as WC
 
@@ -91,10 +91,10 @@ class Run:
         if nxt == first:
             return
         a = self.seed_w * self.W
-        want = coracle.windows_fields(self.x[:, a:nxt * self.W], self.W, self.thr, self.alpha)
+        want = R.windows_fields(self.x[:, a:nxt * self.W], self.W, self.thr, self.alpha)
         want = {k: v[:, first - self.seed_w:] for k, v in want.items()}
         got = {k: self.r.stream_read(k, first, nxt - first) for k in OPS}
-        _check(got, want, self.x[:, a:nxt * self.W])
+        _check(got, want)
 
     def close(self):
         self.r.close()

@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 
 import ring_tier as T
-from oracle import coracle
+import mean_ema_ref as R
 from test_gpu_ring_ranges import OPS, _fields, _thr
 from test_gpu_window_paths import _check
 
@@ -70,8 +70,8 @@ def _oracle(x, first, length, set_off, thr, alpha):
     cols = []
     for s in range(len(set_off) - 1):
         c = np.concatenate([x[:, f:f + n] for f, n in zip(first[set_off[s]:set_off[s + 1]], length[set_off[s]:set_off[s + 1]])], axis=1)
-        cols.append(coracle.windows_fields(np.ascontiguousarray(c), c.shape[1], thr, alpha))
-    return {k: np.concatenate([c[k] for c in cols], axis=1) for k in OPS}
+        cols.append(R.windows_fields(np.ascontiguousarray(c), c.shape[1], thr, alpha))
+    return {k: np.concatenate([c[k] for c in cols], axis=1) for k in cols[0]}
 
 
 def _bitwise(a, b, keys=OPS):
@@ -109,8 +109,7 @@ def test_ranges_against_large_ring_and_oracle(env, kind, cap):
     length = np.array([n for _, n in cases], dtype=np.int64)
     got = r.reduce_ranges(first, length)
     want = big.reduce_ranges(first, length)
-    _check(got, want, x)
-    _check(got, _oracle(x, first, length, np.arange(len(first) + 1), thr, alpha), x)
+    _check(got, _oracle(x, first, length, np.arange(len(first) + 1), thr, alpha))
     assert _bitwise(got, want)                     # mean and EMA too: tiles follow the concatenated samples, not their columns
     ms, _, _ = r.ranges_stats()
     enc, dec, blocks = r.tier_stats()
@@ -122,8 +121,7 @@ def test_ranges_against_large_ring_and_oracle(env, kind, cap):
     set_off = np.array(sorted({0, len(sf)} | set(rng.integers(1, len(sf), 6).tolist())), dtype=np.int64)
     got = r.reduce_range_sets(sf, sl, set_off)
     want = big.reduce_range_sets(sf, sl, set_off)
-    _check(got, want, x)
-    _check(got, _oracle(x, sf, sl, set_off, thr, alpha), x)
+    _check(got, _oracle(x, sf, sl, set_off, thr, alpha))
     assert _bitwise(got, want)
     # small field groups give the same answers, bit for bit
     for G in (1, 3):
@@ -182,8 +180,8 @@ def test_row_bytes_placement_and_counts(env):
                                        C.c_void_p(f64.ctypes.data), C.c_void_p(nov.ctypes.data))
     assert rc == -1 and (f64 == 7.0).all()
     got = r.reduce_ranges([lo], [total - lo])
-    want = coracle.windows_fields(np.ascontiguousarray(rows.T[:, lo:].astype(np.float64)), total - lo, np.full(F, 1000.0), 0.01)
-    _check(got, {k_: want[k_] for k_ in OPS}, rows.T.astype(np.float64))
+    want = R.windows_fields(np.ascontiguousarray(rows.T[:, lo:].astype(np.float64)), total - lo, np.full(F, 1000.0), 0.01)
+    _check(got, want)
     r.close()
 
 

@@ -1,6 +1,6 @@
 """Stream windows of any span (gpud_ring_windows_*) against the C oracle.  The whole pushed stream is kept on the host; after each
-reduce every window of the handle's history is compared with oracle.coracle.windows_fields with W = L = span x W, run over the
-stream from the history's EMA seed on: min / max / p99 / n_over bit for bit, mean and EMA within oracle/SPEC.md's tolerance.
+reduce every window of the handle's history is compared with mean_ema_ref.windows_fields with W = L = span x W, run over the
+stream from the history's EMA seed on: min / max / p99 / n_over bit for bit, mean and EMA within their rounding budget.
 Spans 1, 2, 10, 600 and L = CAP; W = 1000, 1024, 999, 7 and 1, so that both the window kernel (L <= 1024) and the segment select
 (L > 1024) run, on odd starts too; push sizes around L and CAP with windows that wrap the physical end, loss and eviction; the EMA
 over many calls (alpha = 0.9999 through +inf); segments built to hit every route of the select and every reason it hands a segment
@@ -9,7 +9,7 @@ Run on an H100: pytest -m gpu."""
 import numpy as np
 import pytest
 
-from oracle import coracle
+import mean_ema_ref as R
 from test_gpu_window_paths import _check
 from test_gpu_ring_stream import _stream, _thresholds
 import range_cases as RC
@@ -67,10 +67,10 @@ class WRun:
         a = self.seed_w * self.L
         xs = self.x[:, a:nxt * self.L]
         alpha = self.alpha if self.alpha > 0 else min(2.0 / (self.W + 1.0), 0.9999)   # the ring's alpha, not the default for W = L
-        want = coracle.windows_fields(xs, self.L, self.thr, alpha, self.q[0], self.q[1])
+        want = R.windows_fields(xs, self.L, self.thr, alpha, self.q[0], self.q[1])
         want = {k: v[:, first - self.seed_w:] for k, v in want.items()}
         got = {k: self.h.read(k, first, nxt - first) for k in OPS}
-        _check(got, want, xs)
+        _check(got, want)
 
     def close(self):
         self.h.close()

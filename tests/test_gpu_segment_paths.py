@@ -14,7 +14,7 @@ import numpy as np
 import pytest
 
 import test_segment_paths_model as M
-from oracle import coracle
+import mean_ema_ref as R
 from test_gpu_ring_hop import HRun
 from test_gpu_ring_ranges import _alpha, _want
 from test_gpu_window_paths import _check
@@ -111,7 +111,7 @@ def test_range_segment_routes(env, q):
         scr = _scratch(L, r)
     finally:
         r.close()
-    _check(got, _want(x, oldest, firsts, M.RANGE_LENS, thr, _alpha(1000, 0.0), q), x)
+    _check(got, _want(x, oldest, firsts, M.RANGE_LENS, thr, _alpha(1000, 0.0), q))
     models, reasons, n_segs, n_rows = _range_models(x, oldest, firsts, M.RANGE_LENS, segs, cap, q)
     assert why == reasons and n_radix == sum(reasons.values()), (why, reasons)
     _check_scratch(scr, models, n_segs, n_rows)
@@ -194,7 +194,7 @@ def test_radix_chunks(env, case):
         scr = _scratch(L, r)
     finally:
         r.close()
-    _check(got, _want(x, 0, firsts, lens, thr, _alpha(1000, 0.0), q), x)
+    _check(got, _want(x, 0, firsts, lens, thr, _alpha(1000, 0.0), q))
     models, reasons, n_segs, n_rows = _range_models(x, 0, firsts, lens, segs, cap, q)
     assert n_radix == {600: 4800, 512: 4096, 513: 4097}[n_ranges] and why == reasons, (n_radix, why, reasons)
     _check_scratch(scr, models, n_segs, n_rows)
@@ -220,15 +220,13 @@ def test_long_route_batches(env):
     finally:
         r.close()
     # values: the oracle once per distinct range
-    want = {k: np.empty_like(got[k]) for k in OPS}
     distinct = {}
-    for i, key in enumerate(zip(firsts, lens)):
+    for key in zip(firsts, lens):
         if key not in distinct:
             a = key[0] - oldest
-            distinct[key] = coracle.windows_fields(x[:, a:a + key[1]], int(key[1]), thr, alpha, q[0], q[1])
-        for k in OPS:
-            want[k][:, i] = distinct[key][k][:, 0]
-    _check(got, want, x)
+            distinct[key] = R.windows_fields(x[:, a:a + key[1]], int(key[1]), thr, alpha, q[0], q[1])
+    want = R.stack([R.select(distinct[key], (slice(None), 0)) for key in zip(firsts, lens)])
+    _check(got, want)
     whole = [i for i, (f, n) in enumerate(zip(firsts, lens)) if n == cap]
     for k in OPS:
         col = got[k][:, whole].view(np.uint64 if k != "n_over" else np.uint32)
@@ -272,8 +270,8 @@ def test_short_route_branches(env, q):
             assert _scratch(L, r) == E_STATE                          # no long range in the call
             for i, (first, m, kinds) in enumerate(ranges):
                 xr = lap[:, first - base:first - base + m]
-                want = coracle.windows_fields(xr, m, thr, alpha, q[0], q[1])
-                _check({k: got[k][:, i:i + 1] for k in OPS}, want, xr)
+                want = R.windows_fields(xr, m, thr, alpha, q[0], q[1])
+                _check({k: got[k][:, i:i + 1] for k in OPS}, want)
     finally:
         r.close()
 
@@ -307,8 +305,8 @@ def test_short_route_ema(env):
         r.close()
     for i, (first, m) in enumerate(ranges):
         xr = x[:, first:first + m]
-        want = coracle.windows_fields(xr, m, thr, alpha, 0, 0)
-        _check({k: got[k][:, i:i + 1] for k in OPS}, want, xr)
+        want = R.windows_fields(xr, m, thr, alpha, 0, 0)
+        _check({k: got[k][:, i:i + 1] for k in OPS}, want)
         assert np.isposinf(got["ema"][0, i]) and np.isneginf(got["ema"][1, i])
         assert np.isnan(got["ema"][3, i]) or m == 1
 

@@ -51,7 +51,7 @@ def _against_twin_and_oracle(r, twin, ranges, x, thr, alpha, q):
     got = r.reduce_ranges(first, length)
     _, n_open, why = r.ranges_stats()
     assert _bitwise(got, twin.reduce_ranges(first, length))
-    _check(got, _want(x, 0, first, length, thr, alpha, q), x)
+    _check(got, _want(x, 0, first, length, thr, alpha, q))
     return got, n_open, why
 
 
@@ -139,7 +139,7 @@ def test_sets_of_pieces_in_the_tier(env):
     finally:
         r.close()
         twin.close()
-    _check(got, _want_sets(x, 0, first, length, set_off, thr, alpha, q), x)
+    _check(got, _want_sets(x, 0, first, length, set_off, thr, alpha, q))
     expect = {}
     for route, _ in built:
         if route in M.OPEN:
@@ -223,7 +223,7 @@ def test_configs1_natural_groups(env):
             first, length = _split_args(ranges)
             got = r.reduce_ranges(first, length)
             assert _bitwise(got, twin.reduce_ranges(first, length))
-            _check({k: v[sub] for k, v in got.items()}, _want(xs, 0, first, length, thr[sub], alpha, P99), xs)
+            _check({k: v[sub] for k, v in got.items()}, _want(xs, 0, first, length, thr[sub], alpha, P99))
             route, rows_v, _, _, vcap = TM.virtual(total, cap, 0, first, length)
             G = TM.group_size(F, vcap)
             if total == total_b:

@@ -217,8 +217,8 @@ KINDS = {
     "ext_neg_nan": lambda r, m, k: extreme(r, m, k, "neg_nan"),
     "ext_all_neg_nan": lambda r, m, k: extreme(r, m, k, "all_neg_nan"),
 }
-# kinds with samples that make the rest of a field's EMA infinite or NaN, or whose magnitude (DBL_MAX, 2^39 counters) sets the
-# field's mean / EMA tolerance (1e-6 max|x|, oracle/SPEC.md) far above a gauge's EMA: the rings keep them to every fourth field
+# kinds with samples that make the rest of a field's EMA infinite or NaN, or whose magnitude (DBL_MAX, 2^39 counters) dwarfs a
+# gauge's: the rings keep them to every fourth field, so that most fields' EMA stays finite and on a gauge's scale
 WIDE_KINDS = ("ext_inf", "ext_pos_nan", "ext_neg_nan", "ext_all_neg_nan", "ext_dbl_max", "tied_shuffled", "pos_pass",
               "pos_fail_before_T", "pos_fail_last", "pos_fail_first", "pos_fail_nan")
 # kinds the tail windows (the wrap window and the trailing partial window) cycle through
