@@ -17,10 +17,10 @@ $(SRC)/catalog.o: $(SRC)/catalog.cpp $(SRC)/catalog.h $(SRC)/catalog_data.inc in
 $(SRC)/host_component.o: $(SRC)/host_component.cpp $(SRC)/host_component.h $(SRC)/json_min.h include/gpud_b200.h
 	g++ -O2 -std=c++17 -fPIC -Wall -c $< -o $@
 
-$(SRC)/component_abi.o: $(SRC)/component_abi.cpp $(SRC)/host_component.h $(SRC)/internal.h include/gpud_b200.h
+$(SRC)/component_abi.o: $(SRC)/component_abi.cpp $(SRC)/host_component.h $(SRC)/internal.h $(SRC)/catalog.h include/gpud_b200.h
 	g++ -O2 -std=c++17 -fPIC -Wall -I/usr/local/cuda/include -c $< -o $@
 
-$(SRC)/poller.o: $(SRC)/poller.cpp $(SRC)/internal.h include/gpud_b200.h
+$(SRC)/poller.o: $(SRC)/poller.cpp $(SRC)/internal.h $(SRC)/catalog.h include/gpud_b200.h
 	g++ -O2 -std=c++17 -fPIC -Wall -I/usr/local/cuda/include -c $< -o $@
 
 $(SRC)/store_sqlite.o: $(SRC)/store_sqlite.cpp $(SRC)/host_component.h $(SRC)/json_min.h include/gpud_b200.h

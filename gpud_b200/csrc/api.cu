@@ -21,9 +21,9 @@ extern "C" int32_t gpud_ctx_create(const int32_t* cuda_devs, int32_t n, gpud_ctx
     }
     ctx->devs.push_back(cuda_devs[i]);
   }
-  ctx->scan.assign(n, nullptr);
-  ctx->comm.assign(n, nullptr);
-  ctx->fabric_tables.assign(n, nullptr);
+  ctx->scan.resize(n);
+  ctx->comm.resize(n);
+  ctx->fabric_tables.resize(n);
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, ctx->devs[0]) == cudaSuccess) ctx->sm_count = prop.multiProcessorCount;
   *out = ctx;
@@ -32,11 +32,11 @@ extern "C" int32_t gpud_ctx_create(const int32_t* cuda_devs, int32_t n, gpud_ctx
 
 extern "C" int32_t gpud_ctx_destroy(gpud_ctx* ctx) {
   if (!ctx) return GPUD_E_INVALID;
-  for (size_t i = 0; i < ctx->devs.size(); ++i) {
+  for (size_t i = 0; i < ctx->devs.size(); ++i) {   // each device's states go with that device current
     cudaSetDevice(ctx->devs[i]);
-    if (ctx->scan[i]) gpud_scan_state_free(ctx->scan[i]);
-    if (ctx->comm[i]) gpud_comm_state_free(ctx->comm[i]);
-    if (ctx->fabric_tables[i]) cudaFree(ctx->fabric_tables[i]);
+    ctx->scan[i].reset();
+    ctx->comm[i].reset();
+    ctx->fabric_tables[i].reset();
   }
   delete ctx;
   return GPUD_OK;
@@ -62,6 +62,11 @@ extern "C" int32_t gpud_host_alloc(int64_t bytes, void** out) {
 extern "C" int32_t gpud_host_free(void* p) {
   if (!p) return GPUD_E_INVALID;
   return cudaFreeHost(p) == cudaSuccess ? GPUD_OK : GPUD_E_CUDA;
+}
+
+// Test hook (include/gpud_b200_hooks.h): the live device buffers, pinned buffers, events and streams the library owns.
+extern "C" void gpudh_cuda_objects(int64_t out[4]) {
+  for (int i = 0; i < 4; ++i) out[i] = gpud_live[i];
 }
 
 // struct sizes for binding layout checks (ctypes / cgo): 0 hit, 1 fabric_raw, 2 fabric_local, 3 fabric_verdict, 4 ring_cfg,

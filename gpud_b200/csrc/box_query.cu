@@ -367,36 +367,36 @@ struct gpud_box_query {
   size_t b = 0;                        // the batch of the round in flight
   int32_t fail = 0;
   BoxPlan plan;
-  gpud_ranges_state* local = nullptr;  // the one-ring call's scratch for the sets this rank holds alone
-  gpud_range_state* seg = nullptr;     // the finish and radix-select state of the batch in flight
-  unsigned char* d_send = nullptr;  size_t send_cap = 0;
+  std::unique_ptr<gpud_ranges_state> local;  // the one-ring call's scratch for the sets this rank holds alone
+  std::unique_ptr<gpud_range_state> seg;     // the finish and radix-select state of the batch in flight
+  gpud_buf<unsigned char> d_send;
   int64_t send_bytes = 0;
-  double* d_dense = nullptr;  size_t dense_cap = 0;             // the short spread sets' samples
-  double* d_piv_smp = nullptr;  size_t piv_smp_cap = 0;         // the batch's pivot buffer [F][D]
-  BoxRun* d_runs = nullptr;  size_t runs_cap = 0;
-  BoxPick* d_picks = nullptr;  size_t picks_cap = 0;
-  gpud_short_range* d_short = nullptr;  size_t short_cap = 0;
-  int64_t* d_i64 = nullptr;  size_t i64_cap = 0;                // tables: pivot columns, launch bases, pp0, list / collect offsets
-  BoxLp* d_lp = nullptr;  size_t lp_cap = 0;
-  BoxPiece* d_pcs = nullptr;  size_t pcs_cap = 0;
-  int32_t* d_tile = nullptr;  size_t tile_cap = 0;
-  gpud_range_geo* d_lgeo = nullptr;  size_t lgeo_cap = 0;       // the tile launches' per-piece tables, then the radix select's per-rank table
-  gpud_piece* d_lpieces = nullptr;  size_t lpieces_cap = 0;     // ... and its pieces
-  double* d_t[5] = {};  size_t t_cap[5] = {};                   // the tile pass: min, max, mean, -, EMA partial [launches][F][tiles]
-  uint32_t* d_t_nover = nullptr;  size_t t_nover_cap = 0;
-  uint4* d_t_cls = nullptr;  size_t t_cls_cap = 0;
-  unsigned long long* d_llists = nullptr;  size_t llists_cap = 0;   // this rank's keys between the pivots [F][list_row]
-  unsigned* d_lfill = nullptr;  size_t lfill_cap = 0;           // ... and their fill (the pivots' fill counters)
-  unsigned* d_u32 = nullptr;  size_t u32_cap = 0;               // summed fill, each rank's fill, list slots
-  double* d_out = nullptr;  size_t out_cap = 0;                 // the result [5][F][n_sets]
-  uint32_t* d_nover = nullptr;  size_t nover_cap = 0;
+  gpud_buf<double> d_dense;                  // the short spread sets' samples
+  gpud_buf<double> d_piv_smp;                // the batch's pivot buffer [F][D]
+  gpud_buf<BoxRun> d_runs;
+  gpud_buf<BoxPick> d_picks;
+  gpud_buf<gpud_short_range> d_short;
+  gpud_buf<int64_t> d_i64;                   // tables: pivot columns, launch bases, pp0, list / collect offsets
+  gpud_buf<BoxLp> d_lp;
+  gpud_buf<BoxPiece> d_pcs;
+  gpud_buf<int32_t> d_tile;
+  gpud_buf<gpud_range_geo> d_lgeo;           // the tile launches' per-piece tables, then the radix select's per-rank table
+  gpud_buf<gpud_piece> d_lpieces;            // ... and its pieces
+  gpud_buf<double> d_t[5];                   // the tile pass: min, max, mean, -, EMA partial [launches][F][tiles]
+  gpud_buf<uint32_t> d_t_nover;
+  gpud_buf<uint4> d_t_cls;
+  gpud_buf<unsigned long long> d_llists;     // this rank's keys between the pivots [F][list_row]
+  gpud_buf<unsigned> d_lfill;                // ... and their fill (the pivots' fill counters)
+  gpud_buf<unsigned> d_u32;                  // summed fill, each rank's fill, list slots
+  gpud_buf<double> d_out;                    // the result [5][F][n_sets]
+  gpud_buf<uint32_t> d_nover;
   std::vector<int64_t> list_off;       // the lists round: each segment's place (-1: none)
   std::vector<int> ids;                // the segments the finish left open, sorted
   std::vector<int64_t> cand_off;       // the collect round: each open segment's place (-1: none)
   std::vector<double> local_out;       // the local sets' results, [n_local][F][6]
   std::vector<double> out;
   std::vector<uint32_t> nover;
-  cudaEvent_t ev[2] = {};
+  gpud_event ev[2];
   float device_ms = 0.f;
   int rounds = 0;
   int64_t bytes_sent = 0, radix = 0;
@@ -406,13 +406,6 @@ struct gpud_box_query {
 extern "C" void gpud_box_query_destroy(gpud_box_query* q) {
   if (!q) return;
   if (q->ring) cudaSetDevice(q->ring->dev);
-  gpud_ranges_state_free(q->local);
-  gpud_range_state_free(q->seg);
-  cudaFree(q->d_send); cudaFree(q->d_dense); cudaFree(q->d_piv_smp); cudaFree(q->d_runs); cudaFree(q->d_picks); cudaFree(q->d_short); cudaFree(q->d_i64);
-  cudaFree(q->d_lp); cudaFree(q->d_pcs); cudaFree(q->d_tile); cudaFree(q->d_lgeo); cudaFree(q->d_lpieces);
-  for (auto* p : q->d_t) cudaFree(p);
-  cudaFree(q->d_t_nover); cudaFree(q->d_t_cls); cudaFree(q->d_llists); cudaFree(q->d_lfill); cudaFree(q->d_u32); cudaFree(q->d_out); cudaFree(q->d_nover);
-  for (auto& ev : q->ev) if (ev) cudaEventDestroy(ev);
   delete q;
 }
 
@@ -484,7 +477,7 @@ static int64_t box_status(const gpud_box_query* q) { return q->ring->gen != q->g
 
 // Size the send buffer for `words` and zero its status words; the content follows.
 static cudaError_t box_send(gpud_box_query* q, int64_t words) {
-  BOX_CUDA(gpud_grow(&q->d_send, &q->send_cap, (size_t)words * 8));
+  BOX_CUDA(q->d_send.grow((size_t)words * 8));
   q->send_bytes = words * 8;
   return cudaMemsetAsync(q->d_send, 0, 16, q->ring->stream);
 }
@@ -503,7 +496,7 @@ static int32_t box_local_sets(gpud_box_query* q) {
   const int64_t nm = (int64_t)mine.size();
   std::vector<double> o;
   std::vector<uint32_t> nv;
-  const int32_t rc = reduce_subset(gpud_view(r), ring_table(&r, 1), sets, nullptr, q->first.data(), q->len.data(), q->set_off.data(), &q->local, o, nv);
+  const int32_t rc = reduce_subset(gpud_view(r), ring_table(&r, 1), sets, nullptr, q->first.data(), q->len.data(), q->set_off.data(), q->local, o, nv);
   if (rc) return rc;
   for (int f = 0; f < F; ++f)
     for (int64_t k = 0; k < nm; ++k) {
@@ -522,7 +515,7 @@ static cudaError_t box_samples(gpud_box_query* q) {
   const BoxPlan& bp = q->plan;
   const int F = r->F;
   BOX_CUDA(box_send(q, bp.samples_words(q->b)));
-  double* send = reinterpret_cast<double*>(q->d_send) + 2;
+  double* send = reinterpret_cast<double*>(q->d_send.get()) + 2;
   if (q->b == 0) {
     const size_t nl = q->local_out.size();
     if (nl) BOX_CUDA(cudaMemcpyAsync(send, q->local_out.data(), nl * 8, cudaMemcpyHostToDevice, r->stream));
@@ -531,7 +524,7 @@ static cudaError_t box_samples(gpud_box_query* q) {
     if (bp.row > 0) {
       BOX_CUDA(cudaMemsetAsync(send, 0, (size_t)F * bp.row * 8, r->stream));
       if (!runs.empty()) {
-        BOX_CUDA(gpud_grow(&q->d_runs, &q->runs_cap, runs.size()));
+        BOX_CUDA(q->d_runs.grow(runs.size()));
         BOX_CUDA(cudaMemcpyAsync(q->d_runs, runs.data(), runs.size() * sizeof(BoxRun), cudaMemcpyHostToDevice, r->stream));
         k_box_pack<<<box_grid(r, (int64_t)F * runs.size() * 32), 256, 0, r->stream>>>(r->d_ring, r->cap, F, q->d_runs, (int64_t)runs.size(), send, bp.row);
         BOX_CUDA(cudaGetLastError());
@@ -545,7 +538,7 @@ static cudaError_t box_samples(gpud_box_query* q) {
     for (size_t e = 0; e < B.eown.size(); ++e) if (B.eown[e] == q->rank) runs.push_back({B.ecol[e], B.epos[e], 1});
     BOX_CUDA(cudaMemsetAsync(send, 0, (size_t)F * B.row_s * 8, r->stream));
     if (!runs.empty()) {
-      BOX_CUDA(gpud_grow(&q->d_runs, &q->runs_cap, runs.size()));
+      BOX_CUDA(q->d_runs.grow(runs.size()));
       BOX_CUDA(cudaMemcpyAsync(q->d_runs, runs.data(), runs.size() * sizeof(BoxRun), cudaMemcpyHostToDevice, r->stream));
       k_box_pack<<<box_grid(r, (int64_t)F * runs.size() * 32), 256, 0, r->stream>>>(r->d_ring, r->cap, F, q->d_runs, (int64_t)runs.size(), send, B.row_s);
       BOX_CUDA(cudaGetLastError());
@@ -588,9 +581,9 @@ static cudaError_t box_shorts(gpud_box_query* q, const double* recv, int64_t wpr
     }
   if (shorts.empty()) return cudaSuccess;
   const int64_t base = 2 + (int64_t)kBoxLocalWords * F * (int64_t)bp.local.size();
-  BOX_CUDA(gpud_grow(&q->d_dense, &q->dense_cap, (size_t)F * bp.D + 8));   // slack: the 16-byte load of a set's last odd sample
-  BOX_CUDA(gpud_grow(&q->d_picks, &q->picks_cap, bp.picks.size()));
-  BOX_CUDA(gpud_grow(&q->d_short, &q->short_cap, shorts.size()));
+  BOX_CUDA(q->d_dense.grow((size_t)F * bp.D + 8));   // slack: the 16-byte load of a set's last odd sample
+  BOX_CUDA(q->d_picks.grow(bp.picks.size()));
+  BOX_CUDA(q->d_short.grow(shorts.size()));
   BOX_CUDA(cudaMemcpyAsync(q->d_picks, bp.picks.data(), bp.picks.size() * sizeof(BoxPick), cudaMemcpyHostToDevice, r->stream));
   BOX_CUDA(cudaMemcpyAsync(q->d_short, shorts.data(), shorts.size() * sizeof(gpud_short_range), cudaMemcpyHostToDevice, r->stream));
   k_box_assemble<<<box_grid(r, (int64_t)F * bp.picks.size() * 32), 256, 0, r->stream>>>(recv, wpr, base, F, bp.row, q->d_picks, (int64_t)bp.picks.size(),
@@ -607,18 +600,18 @@ static cudaError_t box_local_pass(gpud_box_query* q, const double* recv, int64_t
   const BoxBatch& B = q->plan.batches[q->b];
   const int F = r->F;
   const int64_t n_long = (int64_t)B.geo.size(), segs = (int64_t)F * n_long;
-  if (!q->seg) q->seg = new gpud_range_state();
-  gpud_range_state* s = q->seg;
+  if (!q->seg) q->seg = std::make_unique<gpud_range_state>();
+  gpud_range_state* s = q->seg.get();
   // the pivot buffer [F][D] and the pivots
   std::vector<BoxPick> picks;
   for (size_t e = 0; e < B.eown.size(); ++e) picks.push_back({B.eown[e], B.epos[e], (int64_t)e, 1});
-  BOX_CUDA(gpud_grow(&q->d_piv_smp, &q->piv_smp_cap, (size_t)F * B.D + 8));
-  BOX_CUDA(gpud_grow(&q->d_picks, &q->picks_cap, picks.size()));
+  BOX_CUDA(q->d_piv_smp.grow((size_t)F * B.D + 8));
+  BOX_CUDA(q->d_picks.grow(picks.size()));
   BOX_CUDA(cudaMemcpyAsync(q->d_picks, picks.data(), picks.size() * sizeof(BoxPick), cudaMemcpyHostToDevice, r->stream));
   k_box_assemble<<<box_grid(r, (int64_t)F * picks.size() * 32), 256, 0, r->stream>>>(recv, wpr, base, F, B.row_s, q->d_picks, (int64_t)picks.size(),
                                                                                    q->d_piv_smp, B.D);
   BOX_CUDA(cudaGetLastError());
-  BOX_CUDA(gpud_grow(&q->d_lfill, &q->lfill_cap, (size_t)segs));
+  BOX_CUDA(q->d_lfill.grow((size_t)segs));
   const gpud_ring_view pv = box_view(r, q->d_piv_smp, B.D);
   BOX_CUDA(sel_reserve(pv, s, B.geo.data(), n_long, B.rows, B.list_row, true, nullptr));
   BOX_CUDA(sel_pivots(pv, s, B.geo.data(), n_long, q->d_lfill, nullptr, nullptr, nullptr));
@@ -653,14 +646,14 @@ static cudaError_t box_local_pass(gpud_box_query* q, const double* recv, int64_t
   }
   const int64_t T = lb[n_launch];
   const size_t per = (size_t)F * std::max<int64_t>(1, T);
-  for (int i = 0; i < 5; ++i) if (i != 3) BOX_CUDA(gpud_grow(&q->d_t[i], &q->t_cap[i], per));
-  BOX_CUDA(gpud_grow(&q->d_t_nover, &q->t_nover_cap, per));
-  BOX_CUDA(gpud_grow(&q->d_t_cls, &q->t_cls_cap, per));
-  BOX_CUDA(gpud_grow(&q->d_llists, &q->llists_cap, (size_t)F * B.list_row));
-  BOX_CUDA(gpud_grow(&q->d_lgeo, &q->lgeo_cap, std::max<size_t>(1, lgeo.size())));
-  BOX_CUDA(gpud_grow(&q->d_tile, &q->tile_cap, std::max<size_t>(1, tile.size())));
-  BOX_CUDA(gpud_grow(&q->d_lp, &q->lp_cap, std::max<size_t>(1, lp.size())));
-  BOX_CUDA(gpud_grow(&q->d_i64, &q->i64_cap, (size_t)2 * n_launch + 2));
+  for (int i = 0; i < 5; ++i) if (i != 3) BOX_CUDA(q->d_t[i].grow(per));
+  BOX_CUDA(q->d_t_nover.grow(per));
+  BOX_CUDA(q->d_t_cls.grow(per));
+  BOX_CUDA(q->d_llists.grow((size_t)F * B.list_row));
+  BOX_CUDA(q->d_lgeo.grow(std::max<size_t>(1, lgeo.size())));
+  BOX_CUDA(q->d_tile.grow(std::max<size_t>(1, tile.size())));
+  BOX_CUDA(q->d_lp.grow(std::max<size_t>(1, lp.size())));
+  BOX_CUDA(q->d_i64.grow((size_t)2 * n_launch + 2));
   if (!lgeo.empty()) {
     BOX_CUDA(cudaMemcpyAsync(q->d_lgeo, lgeo.data(), lgeo.size() * sizeof(gpud_range_geo), cudaMemcpyHostToDevice, r->stream));
     BOX_CUDA(cudaMemcpyAsync(q->d_tile, tile.data(), tile.size() * sizeof(int32_t), cudaMemcpyHostToDevice, r->stream));
@@ -676,7 +669,7 @@ static cudaError_t box_local_pass(gpud_box_query* q, const double* recv, int64_t
   }
   // the summaries round
   BOX_CUDA(box_send(q, q->plan.summary_words(q->b)));
-  unsigned long long* send = reinterpret_cast<unsigned long long*>(q->d_send) + 2;
+  unsigned long long* send = reinterpret_cast<unsigned long long*>(q->d_send.get()) + 2;
   BOX_CUDA(cudaMemsetAsync(send + segs * kBoxSumWords, 0, (size_t)F * B.row_p * 8, r->stream));
   k_box_summarize<<<box_grid(r, segs), 256, 0, r->stream>>>(F, n_long, n_launch, q->d_i64, q->d_i64 + n_launch, q->d_lp, q->d_t[0], q->d_t[1], q->d_t[2],
                                                            q->d_t[4], q->d_t_nover, q->d_t_cls, q->d_lfill, r->alpha, send,
@@ -690,10 +683,10 @@ static cudaError_t box_fold(gpud_box_query* q, const unsigned long long* recv, i
   const BoxBatch& B = q->plan.batches[q->b];
   const int F = r->F, n = q->n_ranks;
   const int64_t n_long = (int64_t)B.geo.size(), segs = (int64_t)F * n_long;
-  gpud_range_state* s = q->seg;
-  BOX_CUDA(gpud_grow(&q->d_u32, &q->u32_cap, (size_t)segs * (n + 1)));
-  BOX_CUDA(gpud_grow(&q->d_pcs, &q->pcs_cap, B.pcs.size()));
-  BOX_CUDA(gpud_grow(&q->d_i64, &q->i64_cap, B.pp0.size() + (size_t)segs));
+  gpud_range_state* s = q->seg.get();
+  BOX_CUDA(q->d_u32.grow((size_t)segs * (n + 1)));
+  BOX_CUDA(q->d_pcs.grow(B.pcs.size()));
+  BOX_CUDA(q->d_i64.grow(B.pp0.size() + (size_t)segs));
   BOX_CUDA(cudaMemcpyAsync(q->d_pcs, B.pcs.data(), B.pcs.size() * sizeof(BoxPiece), cudaMemcpyHostToDevice, r->stream));
   BOX_CUDA(cudaMemcpyAsync(q->d_i64, B.pp0.data(), B.pp0.size() * sizeof(int64_t), cudaMemcpyHostToDevice, r->stream));
   unsigned* rfill = q->d_u32;
@@ -716,7 +709,7 @@ static cudaError_t box_fold(gpud_box_query* q, const unsigned long long* recv, i
 static cudaError_t box_finish(gpud_box_query* q) {
   const gpud_ring_view v = gpud_view(q->ring);
   const BoxBatch& B = q->plan.batches[q->b];
-  gpud_range_state* s = q->seg;
+  gpud_range_state* s = q->seg.get();
   // the open segments sorted: the finish appends them in any order, and every rank must lay them out alike
   BOX_CUDA(sel_finish(v, s, (int64_t)B.geo.size(), kBoxWp, B.rows, B.list_row, true, true, nullptr, nullptr, nullptr, &q->ids));
   if (q->ids.empty()) return cudaSuccess;
@@ -771,9 +764,9 @@ static cudaError_t box_radix_geo(gpud_box_query* q, int64_t* n_max) {
     *n_max = std::max(*n_max, g.n);
     geo[j] = g;
   }
-  BOX_CUDA(gpud_grow(&q->d_lgeo, &q->lgeo_cap, (size_t)n_long));
-  BOX_CUDA(gpud_grow(&q->d_lpieces, &q->lpieces_cap, std::max<size_t>(1, pieces.size())));
-  BOX_CUDA(gpud_grow(&q->d_i64, &q->i64_cap, (size_t)n_long + q->ids.size()));
+  BOX_CUDA(q->d_lgeo.grow((size_t)n_long));
+  BOX_CUDA(q->d_lpieces.grow(std::max<size_t>(1, pieces.size())));
+  BOX_CUDA(q->d_i64.grow((size_t)n_long + q->ids.size()));
   BOX_CUDA(cudaMemcpyAsync(q->d_lgeo, geo.data(), n_long * sizeof(gpud_range_geo), cudaMemcpyHostToDevice, r->stream));
   if (!pieces.empty()) BOX_CUDA(cudaMemcpyAsync(q->d_lpieces, pieces.data(), pieces.size() * sizeof(gpud_piece), cudaMemcpyHostToDevice, r->stream));
   return cudaMemcpyAsync(q->d_i64, p0.data(), n_long * sizeof(int64_t), cudaMemcpyHostToDevice, r->stream);
@@ -782,7 +775,7 @@ static cudaError_t box_radix_geo(gpud_box_query* q, int64_t* n_max) {
 // Round hist(b) (need 1) or collect(b) (need 2) of this rank, over its own pieces of the open segments.
 static cudaError_t box_radix_round(gpud_box_query* q, int need) {
   gpud_ring* r = q->ring;
-  gpud_range_state* s = q->seg;
+  gpud_range_state* s = q->seg.get();
   const int64_t n_long = (int64_t)q->plan.batches[q->b].geo.size();
   const int n_sel = (int)q->ids.size();
   const int* ids = reinterpret_cast<const int*>(s->d_open + 1);
@@ -791,7 +784,7 @@ static cudaError_t box_radix_round(gpud_box_query* q, int need) {
   const gpud_ring_view v = gpud_view(r);
   const int64_t words = q->send_bytes / 8;
   BOX_CUDA(box_send(q, words));
-  unsigned long long* send = reinterpret_cast<unsigned long long*>(q->d_send) + 2;
+  unsigned long long* send = reinterpret_cast<unsigned long long*>(q->d_send.get()) + 2;
   if (need == 1) {
     unsigned* hist = reinterpret_cast<unsigned*>(send);
     BOX_CUDA(cudaMemsetAsync(hist, 0, (size_t)(words - 2) * 8, r->stream));
@@ -806,7 +799,7 @@ static cudaError_t box_radix_round(gpud_box_query* q, int need) {
 // The batch's results into the call's [5][F][n_sets]: the open segments' answers (k_sel_final), then the scatter.
 static cudaError_t box_batch_end(gpud_box_query* q) {
   const gpud_ring_view v = gpud_view(q->ring);
-  gpud_range_state* s = q->seg;
+  gpud_range_state* s = q->seg.get();
   const int64_t n_long = (int64_t)q->plan.batches[q->b].geo.size();
   if (!q->ids.empty())
     BOX_CUDA(sel_final(v, s, (int64_t)v.F * n_long, reinterpret_cast<const int*>(s->d_open + 1), (int)q->ids.size()));
@@ -874,8 +867,8 @@ static int32_t box_advance(gpud_box_query* q, const void* recv, bool* done) {
   switch (q->sent) {
     case gpud_box_query::kHeader:
       if (!box_status(q)) local_rc = box_local_sets(q);
-      e = gpud_grow(&q->d_out, &q->out_cap, 5 * plane);
-      if (e == cudaSuccess) e = gpud_grow(&q->d_nover, &q->nover_cap, plane);
+      e = q->d_out.grow(5 * plane);
+      if (e == cudaSuccess) e = q->d_nover.grow(plane);
       q->b = 0;
       if (e == cudaSuccess) e = box_samples(q);
       q->sent = gpud_box_query::kSamples;
@@ -899,11 +892,11 @@ static int32_t box_advance(gpud_box_query* q, const void* recv, bool* done) {
         const BoxBatch& B = q->plan.batches[q->b];
         const int64_t segs = (int64_t)F * (int64_t)B.geo.size();
         e = box_send(q, 2 + lw);
-        if (e == cudaSuccess) e = gpud_grow(&q->d_i64, &q->i64_cap, (size_t)segs);
+        if (e == cudaSuccess) e = q->d_i64.grow((size_t)segs);
         if (e == cudaSuccess) e = cudaMemcpyAsync(q->d_i64, q->list_off.data(), segs * sizeof(int64_t), cudaMemcpyHostToDevice, r->stream);
         if (e == cudaSuccess) {
           k_box_pack_lists<<<box_grid(r, segs * 32), 256, 0, r->stream>>>(segs, (int64_t)B.geo.size(), q->d_i64, q->seg->d_geo, B.list_row, q->d_llists,
-                                                                        q->d_lfill, reinterpret_cast<unsigned long long*>(q->d_send) + 2);
+                                                                        q->d_lfill, reinterpret_cast<unsigned long long*>(q->d_send.get()) + 2);
           e = cudaGetLastError();
         }
         q->sent = gpud_box_query::kLists;
@@ -931,7 +924,7 @@ static int32_t box_advance(gpud_box_query* q, const void* recv, bool* done) {
       break;
     }
     case gpud_box_query::kHist: {
-      gpud_range_state* s = q->seg;
+      gpud_range_state* s = q->seg.get();
       const int n_sel = (int)q->ids.size();
       k_box_sum_hist<<<box_grid(r, (int64_t)n_sel * kBins), 256, 0, r->stream>>>(static_cast<const unsigned*>(recv), wpr, q->n_ranks, (int64_t)n_sel * kBins,
                                                                                 s->d_hist);
@@ -947,7 +940,7 @@ static int32_t box_advance(gpud_box_query* q, const void* recv, bool* done) {
       break;
     }
     case gpud_box_query::kCollect: {
-      gpud_range_state* s = q->seg;
+      gpud_range_state* s = q->seg.get();
       const int n_sel = (int)q->ids.size();
       const int64_t n_long = (int64_t)q->plan.batches[q->b].geo.size();
       k_box_merge_cand<<<box_grid(r, (int64_t)n_sel * 32), 256, 0, r->stream>>>(static_cast<const unsigned long long*>(recv), wpr, q->n_ranks, n_sel,
@@ -969,7 +962,7 @@ static int32_t box_advance(gpud_box_query* q, const void* recv, bool* done) {
   }
   // the round goes out whatever happened, with this rank's status in its first words
   const int64_t words[2] = {status, (int64_t)e};
-  if (!q->d_send || q->send_cap < 16) return gpud_fail(ctx, GPUD_E_CUDA, "box query: could not allocate its send buffer: %s", cudaGetErrorString(e));
+  if (!q->d_send || q->d_send.cap() < 16) return gpud_fail(ctx, GPUD_E_CUDA, "box query: could not allocate its send buffer: %s", cudaGetErrorString(e));
   cudaGetLastError();
   GPUD_CUDA(ctx, cudaMemcpyAsync(q->d_send, words, 16, cudaMemcpyHostToDevice, r->stream));
   GPUD_CUDA(ctx, cudaStreamSynchronize(r->stream));
@@ -988,10 +981,10 @@ extern "C" int32_t gpud_box_query_step(gpud_box_query* q, const void* dev_recv, 
     return gpud_fail(ctx, GPUD_E_INVALID, "box query: dev_recv must be %s", q->started ? "the gathered round" : "NULL on the first step");
   GPUD_CUDA(ctx, cudaSetDevice(r->dev));
   if (!q->started) {
-    for (auto& ev : q->ev) if (!ev) GPUD_CUDA(ctx, cudaEventCreate(&ev));
+    for (auto& ev : q->ev) GPUD_CUDA(ctx, ev.make());
     int64_t hdr[kHdrWords];
     const uint64_t args = box_args_hash(q->n_ranks, q->rank_of.data(), q->first.data(), q->len.data(), q->n_ranges, q->set_off.data(), q->n_sets);
-    GPUD_CUDA(ctx, gpud_grow(&q->d_send, &q->send_cap, sizeof hdr));
+    GPUD_CUDA(ctx, q->d_send.grow(sizeof hdr));
     box_header(r->F, r->W, r->cap, r->alpha, r->q_num, r->q_den, r->thr.data(), r->total, q->rank, q->n_ranks, args, box_status(q), 0, hdr);
     GPUD_CUDA(ctx, cudaMemcpy(q->d_send, hdr, sizeof hdr, cudaMemcpyHostToDevice));
     q->send_bytes = sizeof hdr;

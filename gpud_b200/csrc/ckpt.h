@@ -3,7 +3,7 @@
 #include <algorithm>
 #include <utility>
 
-#include "internal.h"
+#include "segsel.h"
 
 constexpr int kBlock = 1024;                        // samples per coded block
 constexpr int64_t kHeaderBytes = 128;               // of every blob, ring and tier
@@ -43,27 +43,6 @@ cudaError_t launch_pack(const gpud_ring* r, const CkGeo& g, const uint8_t* dir, 
 cudaError_t launch_unpack(const gpud_ring* r, bool store, const CkGeo& g, const uint8_t* dir, const unsigned long long* offs,
                           const unsigned long long* payload, unsigned long long* csum);
 
-// Device scratch and events of one call, released on every return path.
-struct CallScratch {
-  std::vector<void*> mem;
-  std::vector<cudaEvent_t> ev;
-  template <typename T>
-  cudaError_t alloc(T** p, size_t n) {
-    *p = nullptr;
-    const cudaError_t e = cudaMalloc(p, std::max<size_t>(n, 1) * sizeof(T));
-    if (e == cudaSuccess) mem.push_back(*p);
-    return e;
-  }
-  cudaError_t event(cudaEvent_t* e) {
-    const cudaError_t rc = cudaEventCreate(e);
-    if (rc == cudaSuccess) ev.push_back(*e);
-    return rc;
-  }
-  ~CallScratch() {
-    for (void* p : mem) cudaFree(p);
-    for (cudaEvent_t e : ev) cudaEventDestroy(e);
-  }
-};
 inline int32_t scratch_fail(gpud_ring* r, cudaError_t e, const char* what) {
   return gpud_fail(r->ctx, e == cudaErrorMemoryAllocation ? GPUD_E_NOMEM : GPUD_E_CUDA, "%s: %s", what, cudaGetErrorString(e));
 }

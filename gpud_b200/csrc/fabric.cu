@@ -188,23 +188,8 @@ static bool nccl_load(gpud_ctx* ctx) {
   return true;
 }
 
-struct gpud_comm_state {
-  void* comm = nullptr;
-  int n_ranks = 0, rank = 0;
-  cudaStream_t stream = nullptr;
-  gpud_fabric_raw* d_raw = nullptr;
-  gpud_fabric_local* d_send = nullptr;
-  gpud_fabric_local* d_all = nullptr;
-  gpud_fabric_verdict* d_verdict = nullptr;
-  unsigned* d_timeout = nullptr;         // set by the verdict kernel when the peer-store arrivals never completed
-};
-
-void gpud_comm_state_free(gpud_comm_state* c) {
-  if (!c) return;
-  if (c->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(c->comm);
-  cudaFree(c->d_raw); cudaFree(c->d_send); cudaFree(c->d_all); cudaFree(c->d_verdict); cudaFree(c->d_timeout);
-  if (c->stream) cudaStreamDestroy(c->stream);
-  delete c;
+gpud_comm_state::~gpud_comm_state() {
+  if (comm && g_nccl.CommDestroy) g_nccl.CommDestroy(comm);
 }
 
 static int32_t comm_scratch(gpud_ctx* ctx, int dev, gpud_comm_state** out) {
@@ -212,22 +197,19 @@ static int32_t comm_scratch(gpud_ctx* ctx, int dev, gpud_comm_state** out) {
   if (slot < 0) return gpud_fail(ctx, GPUD_E_INVALID, "device %d is not part of this ctx", dev);
   GPUD_CUDA(ctx, cudaSetDevice(dev));
   if (!ctx->comm[slot]) {
-    // built locally and published only once every allocation has succeeded: a half-initialised state must never be reused
-    gpud_comm_state* c = new gpud_comm_state();
-    cudaError_t e = cudaMalloc(&c->d_raw, sizeof(gpud_fabric_raw));
-    if (e == cudaSuccess) e = cudaMalloc(&c->d_send, sizeof(gpud_fabric_local));
-    if (e == cudaSuccess) e = cudaMalloc(&c->d_all, GPUD_MAX_GPUS * sizeof(gpud_fabric_local));
-    if (e == cudaSuccess) e = cudaMalloc(&c->d_verdict, sizeof(gpud_fabric_verdict));
-    if (e == cudaSuccess) e = cudaMalloc(&c->d_timeout, sizeof(unsigned));
+    auto c = std::make_unique<gpud_comm_state>();
+    cudaError_t e = c->d_raw.alloc(1);
+    if (e == cudaSuccess) e = c->d_send.alloc(1);
+    if (e == cudaSuccess) e = c->d_all.alloc(GPUD_MAX_GPUS);
+    if (e == cudaSuccess) e = c->d_verdict.alloc(1);
+    if (e == cudaSuccess) e = c->d_timeout.alloc(1);
     if (e == cudaSuccess) e = cudaMemset(c->d_timeout, 0, sizeof(unsigned));
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking);
-    if (e != cudaSuccess) {
-      gpud_comm_state_free(c);
+    if (e == cudaSuccess) e = c->stream.make();
+    if (e != cudaSuccess)
       return gpud_fail(ctx, e == cudaErrorMemoryAllocation ? GPUD_E_NOMEM : GPUD_E_CUDA, "fabric scratch on device %d: %s", dev, cudaGetErrorString(e));
-    }
-    ctx->comm[slot] = c;
+    ctx->comm[slot] = std::move(c);
   }
-  *out = ctx->comm[slot];
+  *out = ctx->comm[slot].get();
   return GPUD_OK;
 }
 
@@ -344,7 +326,7 @@ extern "C" int32_t gpud_fabric_gather_p2p(gpud_ctx* ctx, const gpud_fabric_raw* 
     int32_t rc = comm_scratch(ctx, ctx->devs[i], &cs[i]);
     if (rc) return rc;
     if (!ctx->fabric_tables[i]) {
-      GPUD_CUDA(ctx, cudaMalloc(&ctx->fabric_tables[i], sizeof(P2PTable)));
+      GPUD_CUDA(ctx, ctx->fabric_tables[i].alloc(1));
       GPUD_CUDA(ctx, cudaMemset(ctx->fabric_tables[i], 0, sizeof(P2PTable)));
       for (int j = 0; j < n; ++j) {
         if (j == i) continue;
@@ -365,7 +347,7 @@ extern "C" int32_t gpud_fabric_gather_p2p(gpud_ctx* ctx, const gpud_fabric_raw* 
     }
     for (int i = 0; i < n; ++i) {
       GPUD_CUDA(ctx, cudaSetDevice(ctx->devs[i]));
-      GPUD_CUDA(ctx, cudaMemset(&reinterpret_cast<P2PTable*>(ctx->fabric_tables[i])->arrivals, 0, sizeof(unsigned)));
+      GPUD_CUDA(ctx, cudaMemset(&ctx->fabric_tables[i]->arrivals, 0, sizeof(unsigned)));
     }
     ctx->fabric_epoch = 0;
   }
@@ -379,7 +361,7 @@ extern "C" int32_t gpud_fabric_gather_p2p(gpud_ctx* ctx, const gpud_fabric_raw* 
     dst.n = n;
     dst.epoch = epoch;
     for (int j = 0; j < n; ++j) {
-      P2PTable* t = reinterpret_cast<P2PTable*>(ctx->fabric_tables[j]);
+      P2PTable* t = ctx->fabric_tables[j];
       dst.p[j] = t->rec;
       dst.flag[j] = &t->arrivals;
     }
@@ -388,7 +370,7 @@ extern "C" int32_t gpud_fabric_gather_p2p(gpud_ctx* ctx, const gpud_fabric_raw* 
   }
   for (int i = 0; i < n; ++i) {
     GPUD_CUDA(ctx, cudaSetDevice(ctx->devs[i]));
-    P2PTable* t = reinterpret_cast<P2PTable*>(ctx->fabric_tables[i]);
+    P2PTable* t = ctx->fabric_tables[i];
     k_fabric_verdict<<<1, 32, 0, cs[i]->stream>>>(t->rec, n, at_least, &t->arrivals, epoch * (unsigned)n, cs[i]->d_verdict, cs[i]->d_timeout);
     GPUD_CUDA(ctx, cudaGetLastError());
     GPUD_CUDA(ctx, cudaMemcpyAsync(&verdicts[i], cs[i]->d_verdict, sizeof(gpud_fabric_verdict), cudaMemcpyDeviceToHost, cs[i]->stream));

@@ -82,14 +82,14 @@ extern "C" int32_t gpud_ib_scan(gpud_ctx* ctx, int32_t dev, const gpud_ib_snapsh
   for (int64_t s = 0; s < n_series; ++s)
     if (series_off[s] > series_off[s + 1] || series_off[s] < 0) return gpud_fail(ctx, GPUD_E_INVALID, "series offsets must ascend");
   GPUD_CUDA(ctx, cudaSetDevice(dev));
-  gpud_ib_snapshot* d_snaps = nullptr;
-  int64_t* d_off = nullptr;
-  gpud_ib_verdict* d_out = nullptr;
-  cudaStream_t st;
-  GPUD_CUDA(ctx, cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-  cudaError_t e = cudaMalloc(&d_snaps, std::max<size_t>(1, (size_t)total) * sizeof(gpud_ib_snapshot));
-  if (e == cudaSuccess) e = cudaMalloc(&d_off, (size_t)(n_series + 1) * sizeof(int64_t));
-  if (e == cudaSuccess) e = cudaMalloc(&d_out, (size_t)n_series * sizeof(gpud_ib_verdict));
+  gpud_stream st;
+  GPUD_CUDA(ctx, st.make());
+  gpud_buf<gpud_ib_snapshot> d_snaps;
+  gpud_buf<int64_t> d_off;
+  gpud_buf<gpud_ib_verdict> d_out;
+  cudaError_t e = d_snaps.alloc(std::max<size_t>(1, (size_t)total));
+  if (e == cudaSuccess) e = d_off.alloc((size_t)n_series + 1);
+  if (e == cudaSuccess) e = d_out.alloc((size_t)n_series);
   if (e == cudaSuccess && total) e = cudaMemcpyAsync(d_snaps, snaps, (size_t)total * sizeof(gpud_ib_snapshot), cudaMemcpyHostToDevice, st);
   if (e == cudaSuccess) e = cudaMemcpyAsync(d_off, series_off, (size_t)(n_series + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, st);
   if (e == cudaSuccess) {
@@ -99,8 +99,6 @@ extern "C" int32_t gpud_ib_scan(gpud_ctx* ctx, int32_t dev, const gpud_ib_snapsh
   }
   if (e == cudaSuccess) e = cudaMemcpyAsync(out, d_out, (size_t)n_series * sizeof(gpud_ib_verdict), cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  cudaFree(d_snaps); cudaFree(d_off); cudaFree(d_out);
-  cudaStreamDestroy(st);
   if (e != cudaSuccess) return gpud_fail(ctx, GPUD_E_CUDA, "gpud_ib_scan: %s", cudaGetErrorString(e));
   return GPUD_OK;
 }

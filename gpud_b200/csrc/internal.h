@@ -6,26 +6,160 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <algorithm>
+#include <atomic>
+#include <memory>
 #include <mutex>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "../../include/gpud_b200.h"
+#include "catalog.h"
 
-struct gpud_scan_state;   // kmsg_scan.cu
-struct gpud_comm_state;   // fabric.cu
+// ---- owners of the library's CUDA objects ------------------------------------------------------
+// Every device buffer, pinned buffer, event and stream the library keeps belongs to one of these, and its destructor releases it.
+// gpud_live counts the live ones by kind (gpudh_cuda_objects).
+enum { GPUD_LIVE_DEVICE, GPUD_LIVE_PINNED, GPUD_LIVE_EVENT, GPUD_LIVE_STREAM };
+inline std::atomic<int64_t> gpud_live[4];
+
+// An array of T in device memory (PINNED: page-locked host memory).  grow(n) keeps the array when it holds n elements already, else
+// frees it first (peak memory does not double) and allocates n; alloc(n) allocates exactly n (at least 1).  After a failure it is empty.
+template <typename T, bool PINNED = false>
+class gpud_buf {
+ public:
+  gpud_buf() = default;
+  gpud_buf(gpud_buf&& o) noexcept { *this = std::move(o); }
+  gpud_buf& operator=(gpud_buf&& o) noexcept {
+    reset();
+    std::swap(p_, o.p_);
+    std::swap(n_, o.n_);
+    return *this;
+  }
+  ~gpud_buf() { reset(); }
+  cudaError_t grow(size_t n) { return n <= n_ ? cudaSuccess : alloc(n); }
+  cudaError_t alloc(size_t n) {
+    reset();
+    n = std::max<size_t>(n, 1);   // an empty array still has an address
+    void* p = nullptr;
+    const cudaError_t e = PINNED ? cudaMallocHost(&p, n * sizeof(T)) : cudaMalloc(&p, n * sizeof(T));
+    if (e != cudaSuccess || !p) return e;
+    p_ = static_cast<T*>(p);
+    n_ = n;
+    ++gpud_live[PINNED ? GPUD_LIVE_PINNED : GPUD_LIVE_DEVICE];
+    return e;
+  }
+  void reset() {
+    if (!p_) return;
+    if (PINNED) cudaFreeHost(p_); else cudaFree(p_);
+    --gpud_live[PINNED ? GPUD_LIVE_PINNED : GPUD_LIVE_DEVICE];
+    p_ = nullptr;
+    n_ = 0;
+  }
+  operator T*() const { return p_; }
+  T* get() const { return p_; }
+  T* operator->() const { return p_; }
+  size_t cap() const { return n_; }
+
+ private:
+  T* p_ = nullptr;
+  size_t n_ = 0;
+};
+template <typename T>
+using gpud_pinned = gpud_buf<T, true>;
+
+// An event, created by the first make() (later ones keep it).
+class gpud_event {
+ public:
+  gpud_event() = default;
+  gpud_event(gpud_event&& o) noexcept { std::swap(e_, o.e_); }
+  gpud_event& operator=(gpud_event&& o) noexcept {
+    std::swap(e_, o.e_);
+    return *this;
+  }
+  ~gpud_event() {
+    if (e_) { cudaEventDestroy(e_); --gpud_live[GPUD_LIVE_EVENT]; }
+  }
+  cudaError_t make(unsigned flags = cudaEventDefault) {
+    if (e_) return cudaSuccess;
+    const cudaError_t e = cudaEventCreateWithFlags(&e_, flags);
+    if (e != cudaSuccess) e_ = nullptr; else ++gpud_live[GPUD_LIVE_EVENT];
+    return e;
+  }
+  operator cudaEvent_t() const { return e_; }
+
+ private:
+  cudaEvent_t e_ = nullptr;
+};
+
+// A non-blocking stream, created by make().
+class gpud_stream {
+ public:
+  gpud_stream() = default;
+  gpud_stream(const gpud_stream&) = delete;
+  ~gpud_stream() {
+    if (s_) { cudaStreamDestroy(s_); --gpud_live[GPUD_LIVE_STREAM]; }
+  }
+  cudaError_t make() {
+    if (s_) return cudaSuccess;
+    const cudaError_t e = cudaStreamCreateWithFlags(&s_, cudaStreamNonBlocking);
+    if (e != cudaSuccess) s_ = nullptr; else ++gpud_live[GPUD_LIVE_STREAM];
+    return e;
+  }
+  operator cudaStream_t() const { return s_; }
+
+ private:
+  cudaStream_t s_ = nullptr;
+};
+
 struct gpud_range_state;  // segsel.h
 struct gpud_ranges_state; // segsel.h
 struct gpud_ring_windows; // below
 struct gpud_tier;         // below
+struct ScanCounters;      // kmsg_scan.cu
+struct P2PTable;          // fabric.cu
+
+// A device's kmsg scan scratch (kmsg_scan.cu), created by its first scan.
+struct gpud_scan_state {
+  gpud_stream stream;
+  int dev = 0;
+  gpud_buf<gpud_tables> d_tables;
+  gpud_buf<uint8_t> d_buf;
+  gpud_buf<uint32_t> d_chunk_sep, d_chunk_local;
+  gpud_buf<unsigned long long> d_tile_base;
+  gpud_buf<unsigned long long> d_cands;
+  gpud_buf<unsigned long long> d_side;                        // family-sorted copy of short candidate lists
+  gpud_buf<gpud_xid_hit> d_hits;
+  gpud_buf<ScanCounters> d_counters;
+  gpud_pinned<ScanCounters> h_counters;
+  gpud_event ev[4];                                           // around filter / prefix / match of the last scan
+  bool phase_timing = false;                                  // record ev[1], ev[2] too (and give up the overlapped launches, see launch_chain)
+  bool last_phased = false;                                   // what the last scan recorded
+  gpud_pinned<uint8_t> h_stage[2];                            // pinned staging for pageable caller buffers
+  gpud_pinned<gpud_xid_hit> h_hits;                           // pinned landing buffer of the hit list
+  gpud_event ev_stage[2];
+};
+
+// A device's fabric scratch and NCCL communicator (fabric.cu), created by its first fabric call.
+struct gpud_comm_state {
+  gpud_stream stream;
+  void* comm = nullptr;
+  int n_ranks = 0, rank = 0;
+  gpud_buf<gpud_fabric_raw> d_raw;
+  gpud_buf<gpud_fabric_local> d_send;
+  gpud_buf<gpud_fabric_local> d_all;
+  gpud_buf<gpud_fabric_verdict> d_verdict;
+  gpud_buf<unsigned> d_timeout;          // set by the verdict kernel when the peer-store arrivals never completed
+  ~gpud_comm_state();                    // destroys the communicator before its buffers
+};
 
 struct gpud_ctx {
   std::vector<int> devs;
   std::mutex mu;
   std::string last_error;
-  std::vector<gpud_scan_state*> scan;   // per dev slot, lazily created
-  std::vector<gpud_comm_state*> comm;   // per dev slot
-  std::vector<void*> fabric_tables;     // per dev slot: device table [GPUD_MAX_GPUS] x 128 B (+flags) for p2p gather
+  std::vector<std::unique_ptr<gpud_scan_state>> scan;   // per dev slot, lazily created
+  std::vector<std::unique_ptr<gpud_comm_state>> comm;   // per dev slot
+  std::vector<gpud_buf<P2PTable>> fabric_tables;        // per dev slot: device table [GPUD_MAX_GPUS] x 128 B (+flags) for p2p gather
   int sm_count = 132;
   std::mutex fabric_mu;                 // gpud_fabric_gather_p2p: one gather at a time per ctx
   unsigned fabric_epoch = 0;            // gathers completed or begun on this ctx's tables (arrival counters expect epoch * n)
@@ -43,32 +177,32 @@ struct gpud_ring {
   int q_num = 99, q_den = 100;
   int64_t total = 0;
   int64_t gen = 0;                 // pushes and restores so far: a box query started before one of them is refused (box_query.cu)
-  double* d_ring = nullptr;
-  double* d_thr = nullptr;
-  double* d_pw = nullptr;
+  gpud_stream own_stream, copy_stream;   // first: released after everything queued on them
+  cudaStream_t stream = nullptr;          // own_stream, or the caller's (gpud_ring_set_stream)
+  gpud_buf<double> d_ring;
+  gpud_buf<double> d_thr;
+  gpud_buf<double> d_pw;
   int64_t nw_max = 0;
-  double* d_res[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-  uint32_t* d_nover = nullptr;
-  double* d_part = nullptr;
-  unsigned long long* d_cursor = nullptr;   // window-kernel work cursors: [0..1] gpud_ring_reduce, [2..3] the range pass
+  gpud_buf<double> d_res[5];
+  gpud_buf<uint32_t> d_nover;
+  gpud_buf<double> d_part;
+  gpud_buf<unsigned long long> d_cursor;   // window-kernel work cursors: [0..1] gpud_ring_reduce, [2..3] the range pass
   int64_t reduced_nw = -1;
-  cudaStream_t own_stream = nullptr, stream = nullptr;
-  double* h_stage[2] = {nullptr, nullptr};
-  double* d_stage[2] = {nullptr, nullptr};
-  cudaEvent_t ev_stage[2] = {nullptr, nullptr};    // d_stage[i] is free again (its append has run)
-  cudaEvent_t ev_copied[2] = {nullptr, nullptr};   // the H2D into d_stage[i] has landed
-  cudaStream_t copy_stream = nullptr;
+  gpud_pinned<double> h_stage[2];
+  gpud_buf<double> d_stage[2];
+  gpud_event ev_stage[2];          // d_stage[i] is free again (its append has run)
+  gpud_event ev_copied[2];         // the H2D into d_stage[i] has landed
   int64_t stage_rows = 0;
-  double* d_sample = nullptr;      // [F][smp_slots]: column c with c % 2^smp_shift == 2^smp_shift / 2 lives at slot c >> smp_shift (kept by the append kernel)
+  gpud_buf<double> d_sample;       // [F][smp_slots]: column c with c % 2^smp_shift == 2^smp_shift / 2 lives at slot c >> smp_shift (kept by the append kernel)
   int smp_shift = 0;
   int64_t smp_slots = 0;
   int sm_count = 132;
   int cta_reserve = 0;           // CTA slots the persistent window grid leaves free for kernels of other streams (gpud_ring_set_cta_reserve)
-  gpud_range_state* range = nullptr;                   // created by the first gpud_ring_reduce_range
-  gpud_ranges_state* ranges = nullptr;                 // created by the first gpud_ring_reduce_ranges
-  cudaEvent_t ev_k[3] = {nullptr, nullptr, nullptr};   // around the two kernels of the last reduce (bench roofline)
-  gpud_ring_windows* swin = nullptr;                   // the span-1 handle behind gpud_ring_stream_*, created by gpud_ring_stream_open
-  std::vector<gpud_ring_windows*> handles;             // open gpud_ring_windows_open handles (gpud_ring_destroy frees them)
+  std::unique_ptr<gpud_range_state> range;            // created by the first gpud_ring_reduce_range
+  std::unique_ptr<gpud_ranges_state> ranges;          // created by the first gpud_ring_reduce_ranges
+  gpud_event ev_k[3];                                  // around the two kernels of the last reduce (bench roofline)
+  std::unique_ptr<gpud_ring_windows> swin;             // the span-1 handle behind gpud_ring_stream_*, created by gpud_ring_stream_open
+  std::vector<std::unique_ptr<gpud_ring_windows>> handles;   // open gpud_ring_windows_open handles
   std::vector<double> thr;                             // [F] the thresholds as created (a checkpoint records their bits)
   bool ck_timed = false;                               // gpud_ring_checkpoint_stats: a checkpoint or restore has run
   float ck_encode_ms = 0.f, ck_decode_ms = 0.f;        // ... device ms of the last checkpoint's encode and the last restore's decode
@@ -80,7 +214,7 @@ struct gpud_ring {
   bool ck_marked = false;
   int64_t ck_total = 0, ck_gen = 0;                    // ... total and handle_gen at the marker
   uint64_t ck_link = 0;                                // ... and that blob's chain link
-  gpud_tier* tier = nullptr;                           // gpud_ring_tier_open: the delta-coded tier of older samples (tier.cu)
+  std::unique_ptr<gpud_tier> tier;                     // gpud_ring_tier_open: the delta-coded tier of older samples (tier.cu)
 };
 
 // The tier of a ring (tier.cu, DESIGN.md §2 "Tier"): block rows k = samples [1024 k, 1024 (k + 1)) of every field, each coded as
@@ -94,14 +228,14 @@ struct gpud_tier {
   int64_t rec_bytes = 0;           // a row record: first sample, byte offset, directory bytes [F] (padded), block word offsets u32 [F] (padded)
   int64_t slots = 0;               // rows the byte ring can hold at most (+ 1)
   int64_t next = 0, lost = 0;      // host: rows [.., next) have been encoded; rows lost since open
-  unsigned long long* d_buf = nullptr;   // the byte ring [B], then a sink of one row coded at 64 bits for rows evicted by their own push
-  int64_t* d_slot = nullptr;             // [slots][2]
-  gpud_tier_ctl* d_ctl = nullptr;
-  uint8_t* d_dir = nullptr;              // encode scratch for the rows one push completes, [F][rows]
-  unsigned long long *d_words = nullptr, *d_offs = nullptr, *d_csum = nullptr;
-  int64_t* d_rowsz = nullptr;
+  gpud_buf<unsigned long long> d_buf;    // the byte ring [B], then a sink of one row coded at 64 bits for rows evicted by their own push
+  gpud_buf<int64_t> d_slot;              // [slots][2]
+  gpud_buf<gpud_tier_ctl> d_ctl;
+  gpud_buf<uint8_t> d_dir;               // encode scratch for the rows one push completes, [F][rows]
+  gpud_buf<unsigned long long> d_words, d_offs, d_csum;
+  gpud_buf<int64_t> d_rowsz;
   int64_t units_cap = 0;
-  cudaEvent_t ev_enc[2] = {nullptr, nullptr};
+  gpud_event ev_enc[2];
   bool enc_timed = false;
   float dec_ms = 0.f;              // the last range call homed on this ring that decoded: all its decode, every field group
   int group_max = 0;               // > 0: at most this many fields per decoded group (gpudh_ring_tier_group)
@@ -116,7 +250,6 @@ struct gpud_tier {
 };
 // tier.cu: after every push into a tiered ring, on its stream: the loss rule, then the encode of every row the push completed.
 int32_t gpud_tier_push(gpud_ring* r);
-void gpud_tier_free(gpud_tier* t);
 // tier.cu: synchronise the ring's stream and read the tier's control word (the rows it holds, [first, next), and its bytes in use).
 int32_t gpud_tier_read_ctl(gpud_ring* r, gpud_tier_ctl* c);
 // A slot of a virtual box (ranges.cu): a ring of G fields and capacity vcap at `ring` [G][vcap], its sample ring at `sample`
@@ -169,19 +302,19 @@ struct gpud_ring_windows {
   int64_t first = 0, next = 0, lost = 0;
   bool reseed = true;                  // the next commit seeds the EMA with the ring's sample at window next's start (open, loss)
   int64_t ck_next = 0;                 // `next` at the ring's chain marker (ring_ckpt.cu)
-  double* d_hist = nullptr;            // [5][F][H] f64, aggregate GPUD_OP_MIN..GPUD_OP_P99
-  uint32_t* d_hist_nover = nullptr;    // [F][H]
-  double* d_ema = nullptr;             // [F] EMA at the last sample of window next - 1
-  double* d_sc = nullptr;              // L <= GPUD_MAX_WINDOW: [5][F][ceil(CAP / L)] window-pass output of the new windows: MIN, MAX,
+  gpud_buf<double> d_hist;             // [5][F][H] f64, aggregate GPUD_OP_MIN..GPUD_OP_P99
+  gpud_buf<uint32_t> d_hist_nover;     // [F][H]
+  gpud_buf<double> d_ema;              // [F] EMA at the last sample of window next - 1
+  gpud_buf<double> d_sc;               // L <= GPUD_MAX_WINDOW: [5][F][ceil(CAP / L)] window-pass output of the new windows: MIN, MAX,
                                        // MEAN, P99 and, in slot GPUD_OP_EMA, the EMA partials; [F][n_new] packed at the start of each
-  uint32_t* d_sc_nover = nullptr;      // [F][ceil(CAP / L)]
+  gpud_buf<uint32_t> d_sc_nover;       // [F][ceil(CAP / L)]
   int64_t sc_cols = 0;                 // ceil(CAP / L)
-  double* d_eq = nullptr;              // hop < span: [4][F][ceil(CAP / Wq)] the EMA pass over the new samples, per sub-window of Wq: MIN, MAX,
+  gpud_buf<double> d_eq;               // hop < span: [4][F][ceil(CAP / Wq)] the EMA pass over the new samples, per sub-window of Wq: MIN, MAX,
                                        // MEAN (unused) and the EMA partials; [F][n] packed at the start of each
-  uint32_t* d_eq_nover = nullptr;      // [F][ceil(CAP / Wq)] (unused)
+  gpud_buf<uint32_t> d_eq_nover;       // [F][ceil(CAP / Wq)] (unused)
   int64_t eq_cols = 0;                 // ceil(CAP / Wq)
-  gpud_range_state* seg = nullptr;     // L > GPUD_MAX_WINDOW: the segment select's scratch (select.cu), apart from the ring's own range call's
-  cudaEvent_t ev[2] = {nullptr, nullptr};   // around the device work of the last reduce that had new windows
+  std::unique_ptr<gpud_range_state> seg;   // L > GPUD_MAX_WINDOW: the segment select's scratch (select.cu), apart from the ring's own range call's
+  gpud_event ev[2];                    // around the device work of the last reduce that had new windows
   bool timed = false;                  // the last reduce had new windows and ran to the end
   int64_t seg_open = 0;                // ... segments it handed to the radix select (L > GPUD_MAX_WINDOW), over all its phases
   int seg_reasons[GPUD_RANGE_N_OPEN_REASONS] = {};   // ... and why, by GPUD_RANGE_OPEN_*
@@ -233,17 +366,6 @@ inline int gpud_dev_slot(gpud_ctx* ctx, int dev) {
   return -1;
 }
 
-// Device scratch that is grown on demand and kept: afterwards *p holds at least `need` elements (*cap counts them).
-template <typename T>
-inline cudaError_t gpud_grow(T** p, size_t* cap, size_t need) {
-  if (need <= *cap) return cudaSuccess;
-  cudaFree(*p);
-  *p = nullptr;
-  *cap = 0;
-  cudaError_t e = cudaMalloc(p, need * sizeof(T));
-  if (e == cudaSuccess) *cap = need;
-  return e;
-}
 
 // ---- device helpers --------------------------------------------------------------------------
 #ifdef __CUDACC__
@@ -265,9 +387,8 @@ __host__ __device__ __forceinline__ long long gpud_rank_from_top(long long n, in
 #endif
 
 // ring.cu: open a windows handle of the ring (gpud_ring_windows_open_hop's checks, history_windows <= 0: the default) without
-// registering it anywhere, and free one.  ring_ckpt.cu re-creates a checkpoint's handles through them.
-int32_t gpud_ring_windows_new(gpud_ring* r, int64_t span, int64_t hop, int64_t history_windows, gpud_ring_windows** out);
-void gpud_ring_windows_free(gpud_ring_windows* s);
+// registering it anywhere.  ring_ckpt.cu re-creates a checkpoint's handles through it.
+int32_t gpud_ring_windows_new(gpud_ring* r, int64_t span, int64_t hop, int64_t history_windows, std::unique_ptr<gpud_ring_windows>* out);
 
 // ring.cu: the window pass and the EMA carry over chronological samples [start, start + n) of the ring with window Wp, into the
 // caller's buffers w[0..4] = per-window min, max, mean, EMA, EMA partial sums and w_nover, each [F][nw], nw = ceil(n / Wp).  With piv
@@ -286,7 +407,7 @@ int32_t gpud_ring_window_pass(gpud_ring* r, int64_t start, int64_t n, int Wp, do
 // select's grid is sized by the segments left open) and leaves the results on the device, valid until the next call on *st:
 // out [5][F n_seg] (MIN, MAX, MEAN, -, P99: no EMA), nover [F n_seg], part [F][n_seg seg_len / Wp] the sub-windows' EMA partial sums.
 struct gpud_seg_out { const double* out; const uint32_t* nover; const double* part; int64_t open; const int* reasons; };
-int32_t gpud_ring_segments(gpud_ring* r, gpud_range_state** st, int64_t start, int64_t seg_len, int64_t n_seg, int Wp, gpud_seg_out* out);
+int32_t gpud_ring_segments(gpud_ring* r, std::unique_ptr<gpud_range_state>& st, int64_t start, int64_t seg_len, int64_t n_seg, int Wp, gpud_seg_out* out);
 
 // gpud_ring_reduce_ranges and gpud_rings_reduce_range_sets (ranges.cu, DESIGN.md §2 "Ranges", "Range sets", "Box sets").  A set of
 // several ranges, or of one range in a ring other than the home ring, reads its samples through the call's piece table: piece i of a
@@ -371,8 +492,4 @@ int32_t gpud_kmsg_dedup_run(gpud_ctx* ctx, gpud_kmsg_dedup* dd, const uint8_t* d
                             int64_t now_unix, const uint32_t* d_chunk_local, const unsigned long long* d_tile_base, int64_t n_units, cudaStream_t st,
                             uint8_t* dropped);
 
-void gpud_scan_state_free(gpud_scan_state*);
-void gpud_comm_state_free(gpud_comm_state*);
-void gpud_range_state_free(gpud_range_state*);
-void gpud_ranges_state_free(gpud_ranges_state*);
 void gpud_parallel_memcpy(void* dst, const void* src, size_t n);

@@ -211,49 +211,33 @@ inline unsigned blocks_for(int64_t n) { return (unsigned)std::max<int64_t>(1, (n
 }  // namespace
 
 struct gpud_kmsg_dedup {
+  gpud_stream stream;                // gpud_kmsg_dedup_stats; a scan call runs on the scan's stream
   gpud_ctx* ctx = nullptr;
   int dev = 0;
   int64_t ttl = 900;
   int32_t trunc = 60;
   unsigned long long hash_mask = ~0ull;
   // the table: `slots` (a power of two) words / first units / entries, and the arena of the keys' bytes
-  unsigned long long* d_word = nullptr;
-  unsigned* d_first = nullptr;
-  Entry* d_ent = nullptr;
-  uint8_t* d_arena = nullptr;
-  size_t slots = 0, arena_cap = 0;
+  gpud_buf<unsigned long long> d_word;
+  gpud_buf<unsigned> d_first;
+  gpud_buf<Entry> d_ent;
+  gpud_buf<uint8_t> d_arena;
+  size_t slots = 0;
   int64_t n_occ = 0;                 // occupied slots (live or expired, until the next rebuild)
   int64_t arena_used = 0;
   int64_t rebuilds = 0;
   bool have_now = false;
   int64_t last_now = 0;
   // per-unit scratch of a call
-  int64_t* d_start = nullptr; size_t start_cap = 0;
-  UnitKey* d_keys = nullptr; size_t keys_cap = 0;
-  unsigned long long* d_uslot = nullptr; size_t uslot_cap = 0;
-  uint8_t* d_dropped = nullptr; size_t dropped_cap = 0;
-  Counters* d_cnt = nullptr;
-  Counters* h_cnt = nullptr;         // pinned
-  cudaStream_t stream = nullptr;     // gpud_kmsg_dedup_stats; a scan call runs on the scan's stream
-  cudaEvent_t ev[2] = {nullptr, nullptr};
+  gpud_buf<int64_t> d_start;
+  gpud_buf<UnitKey> d_keys;
+  gpud_buf<unsigned long long> d_uslot;
+  gpud_buf<uint8_t> d_dropped;
+  gpud_buf<Counters> d_cnt;
+  gpud_pinned<Counters> h_cnt;
+  gpud_event ev[2];
   bool timed = false;
 };
-
-static void dedup_free_table(gpud_kmsg_dedup* d) {
-  cudaFree(d->d_word); cudaFree(d->d_first); cudaFree(d->d_ent); cudaFree(d->d_arena);
-  d->d_word = nullptr; d->d_first = nullptr; d->d_ent = nullptr; d->d_arena = nullptr;
-}
-
-static void dedup_free(gpud_kmsg_dedup* d) {
-  if (!d) return;
-  cudaSetDevice(d->dev);
-  dedup_free_table(d);
-  cudaFree(d->d_start); cudaFree(d->d_keys); cudaFree(d->d_uslot); cudaFree(d->d_dropped); cudaFree(d->d_cnt);
-  if (d->h_cnt) cudaFreeHost(d->h_cnt);
-  for (auto& e : d->ev) if (e) cudaEventDestroy(e);
-  if (d->stream) cudaStreamDestroy(d->stream);
-  delete d;
-}
 
 // keys alive at `now` and their bytes, on stream st (synchronises)
 static cudaError_t live_count(gpud_kmsg_dedup* d, int64_t now, cudaStream_t st, unsigned long long* live, unsigned long long* bytes) {
@@ -277,30 +261,26 @@ static int32_t rebuild(gpud_ctx* ctx, gpud_kmsg_dedup* d, int64_t now, int64_t u
   size_t slots = 1024;
   while (slots < 4 * ((size_t)live + (size_t)units)) slots <<= 1;
   const size_t arena_cap = std::max<size_t>(1 << 16, 2 * ((size_t)live_bytes + (size_t)bytes));
-  unsigned long long* word = nullptr;
-  unsigned* first = nullptr;
-  Entry* ent = nullptr;
-  uint8_t* arena = nullptr;
-  cudaError_t e = cudaMalloc(&word, slots * sizeof *word);
-  if (e == cudaSuccess) e = cudaMalloc(&first, slots * sizeof *first);
-  if (e == cudaSuccess) e = cudaMalloc(&ent, slots * sizeof *ent);
-  if (e == cudaSuccess) e = cudaMalloc(&arena, arena_cap);
-  if (e == cudaSuccess) e = cudaMemsetAsync(word, 0, slots * sizeof *word, st);
+  gpud_buf<unsigned long long> word;
+  gpud_buf<unsigned> first;
+  gpud_buf<Entry> ent;
+  gpud_buf<uint8_t> arena;
+  cudaError_t e = word.alloc(slots);
+  if (e == cudaSuccess) e = first.alloc(slots);
+  if (e == cudaSuccess) e = ent.alloc(slots);
+  if (e == cudaSuccess) e = arena.alloc(arena_cap);
+  if (e == cudaSuccess) e = cudaMemsetAsync(word, 0, slots * sizeof(unsigned long long), st);
   if (e == cudaSuccess) e = cudaMemsetAsync(&d->d_cnt->arena_used, 0, sizeof(unsigned long long), st);
   if (e == cudaSuccess && d->slots) {
     k_rebuild<<<blocks_for((int64_t)d->slots), 256, 0, st>>>(d->d_word, d->d_ent, d->slots, d->d_arena, now, word, ent, slots - 1, arena, d->d_cnt);
     e = cudaGetLastError();
   }
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  if (e != cudaSuccess) {
-    cudaFree(word); cudaFree(first); cudaFree(ent); cudaFree(arena);
+  if (e != cudaSuccess)
     return gpud_fail(ctx, e == cudaErrorMemoryAllocation ? GPUD_E_NOMEM : GPUD_E_CUDA, "kmsg dedup table of %zu slots: %s", slots, cudaGetErrorString(e));
-  }
   if (d->slots) ++d->rebuilds;
-  dedup_free_table(d);
-  d->d_word = word; d->d_first = first; d->d_ent = ent; d->d_arena = arena;
+  d->d_word = std::move(word); d->d_first = std::move(first); d->d_ent = std::move(ent); d->d_arena = std::move(arena);
   d->slots = slots;
-  d->arena_cap = arena_cap;
   d->n_occ = (int64_t)live;
   d->arena_used = (int64_t)live_bytes;
   return GPUD_OK;
@@ -311,14 +291,14 @@ int32_t gpud_kmsg_dedup_run(gpud_ctx* ctx, gpud_kmsg_dedup* d, const uint8_t* d_
                             uint8_t* dropped) {
   if (n_units >= (int64_t)kOld - 1) return gpud_fail(ctx, GPUD_E_INVALID, "kmsg dedup: %lld units in one call", (long long)n_units);
   const bool raw = (mode & 0xff) == GPUD_SCAN_RAW_KMSG;
-  if (2 * (d->n_occ + n_units) > (int64_t)d->slots || d->arena_used + len > (int64_t)d->arena_cap) {
+  if (2 * (d->n_occ + n_units) > (int64_t)d->slots || d->arena_used + len > (int64_t)d->d_arena.cap()) {
     const int32_t rc = rebuild(ctx, d, now_unix, n_units, len, st);
     if (rc) return rc;
   }
-  GPUD_CUDA(ctx, gpud_grow(&d->d_start, &d->start_cap, (size_t)n_units + 1));
-  GPUD_CUDA(ctx, gpud_grow(&d->d_keys, &d->keys_cap, (size_t)n_units));
-  GPUD_CUDA(ctx, gpud_grow(&d->d_uslot, &d->uslot_cap, (size_t)n_units));
-  GPUD_CUDA(ctx, gpud_grow(&d->d_dropped, &d->dropped_cap, (size_t)n_units));
+  GPUD_CUDA(ctx, d->d_start.grow((size_t)n_units + 1));
+  GPUD_CUDA(ctx, d->d_keys.grow((size_t)n_units));
+  GPUD_CUDA(ctx, d->d_uslot.grow((size_t)n_units));
+  GPUD_CUDA(ctx, d->d_dropped.grow((size_t)n_units));
   GPUD_CUDA(ctx, cudaEventRecord(d->ev[0], st));
   GPUD_CUDA(ctx, cudaMemsetAsync(d->d_first, 0xff, d->slots * sizeof(unsigned), st));
   GPUD_CUDA(ctx, cudaMemsetAsync(&d->d_cnt->new_slots, 0, sizeof(unsigned long long), st));
@@ -358,25 +338,27 @@ extern "C" int32_t gpud_kmsg_dedup_create(gpud_ctx* ctx, int32_t dev, int64_t tt
   *out = nullptr;
   if (gpud_dev_slot(ctx, dev) < 0) return gpud_fail(ctx, GPUD_E_INVALID, "device %d is not part of this ctx", dev);
   GPUD_CUDA(ctx, cudaSetDevice(dev));
-  gpud_kmsg_dedup* d = new gpud_kmsg_dedup();
+  auto d = std::make_unique<gpud_kmsg_dedup>();
   d->ctx = ctx;
   d->dev = dev;
   d->ttl = ttl_seconds > 0 ? ttl_seconds : 15 * 60;          // defaultCacheExpiration
   d->trunc = truncate_seconds > 0 ? truncate_seconds : 60;   // WithCacheKeyTruncateSeconds ignores values <= 0
-  cudaError_t e = cudaMalloc(&d->d_cnt, sizeof(Counters));
+  cudaError_t e = d->d_cnt.alloc(1);
   if (e == cudaSuccess) e = cudaMemset(d->d_cnt, 0, sizeof(Counters));
-  if (e == cudaSuccess) e = cudaMallocHost(&d->h_cnt, sizeof(Counters));
-  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&d->stream, cudaStreamNonBlocking);
-  for (auto& ev : d->ev) if (e == cudaSuccess) e = cudaEventCreate(&ev);
-  if (e != cudaSuccess) {
-    dedup_free(d);
+  if (e == cudaSuccess) e = d->h_cnt.alloc(1);
+  if (e == cudaSuccess) e = d->stream.make();
+  for (auto& ev : d->ev) if (e == cudaSuccess) e = ev.make();
+  if (e != cudaSuccess)
     return gpud_fail(ctx, e == cudaErrorMemoryAllocation ? GPUD_E_NOMEM : GPUD_E_CUDA, "kmsg dedup on device %d: %s", dev, cudaGetErrorString(e));
-  }
-  *out = d;
+  *out = d.release();
   return GPUD_OK;
 }
 
-extern "C" void gpud_kmsg_dedup_destroy(gpud_kmsg_dedup* dd) { dedup_free(dd); }
+extern "C" void gpud_kmsg_dedup_destroy(gpud_kmsg_dedup* dd) {
+  if (!dd) return;
+  cudaSetDevice(dd->dev);
+  delete dd;
+}
 
 extern "C" int32_t gpud_kmsg_dedup_stats(gpud_kmsg_dedup* dd, int64_t* out4, float* dedup_ms) {
   if (!dd || !out4) return GPUD_E_INVALID;

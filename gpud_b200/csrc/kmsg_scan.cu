@@ -1589,58 +1589,24 @@ struct ScanCounters {
   unsigned long long fam_pos[kSortBins];      // per-family cursors of k_cand_scatter
 };
 
-struct gpud_scan_state {
-  int dev = 0;
-  gpud_tables* d_tables = nullptr;
-  uint8_t* d_buf = nullptr; size_t buf_cap = 0;
-  uint32_t* d_chunk_sep = nullptr; uint32_t* d_chunk_local = nullptr; unsigned long long* d_tile_base = nullptr; size_t chunk_sep_cap = 0, chunk_local_cap = 0, tile_cap = 0;
-  unsigned long long* d_cands = nullptr; size_t cand_cap = 0;
-  unsigned long long* d_side = nullptr; size_t side_cap = 0;   // family-sorted copy of short candidate lists
-  gpud_xid_hit* d_hits = nullptr; size_t hit_cap = 0;
-  ScanCounters* d_counters = nullptr;
-  ScanCounters* h_counters = nullptr;         // pinned
-  cudaStream_t stream = nullptr;
-  cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};   // around filter / prefix / match of the last scan
-  bool phase_timing = false;                                  // record ev[1], ev[2] too (and give up the overlapped launches, see launch_chain)
-  bool last_phased = false;                                   // what the last scan recorded
-  uint8_t* h_stage[2] = {nullptr, nullptr};                    // pinned staging for pageable caller buffers
-  gpud_xid_hit* h_hits = nullptr; size_t h_hits_cap = 0;      // pinned landing buffer of the hit list
-  cudaEvent_t ev_stage[2] = {nullptr, nullptr};
-};
-
-void gpud_scan_state_free(gpud_scan_state* s) {
-  if (!s) return;
-  cudaFree(s->d_tables); cudaFree(s->d_buf); cudaFree(s->d_chunk_sep); cudaFree(s->d_chunk_local); cudaFree(s->d_tile_base); cudaFree(s->d_cands); cudaFree(s->d_side);
-  cudaFree(s->d_hits); cudaFree(s->d_counters);
-  if (s->h_counters) cudaFreeHost(s->h_counters);
-  if (s->h_hits) cudaFreeHost(s->h_hits);
-  for (auto& e : s->ev) if (e) cudaEventDestroy(e);
-  for (int i = 0; i < 2; ++i) { if (s->h_stage[i]) cudaFreeHost(s->h_stage[i]); if (s->ev_stage[i]) cudaEventDestroy(s->ev_stage[i]); }
-  if (s->stream) cudaStreamDestroy(s->stream);
-  delete s;
-}
-
 static int32_t scan_state_get(gpud_ctx* ctx, int dev, gpud_scan_state** out) {
   const int slot = gpud_dev_slot(ctx, dev);
   if (slot < 0) return gpud_fail(ctx, GPUD_E_INVALID, "device %d is not part of this ctx", dev);
   GPUD_CUDA(ctx, cudaSetDevice(dev));
   if (!ctx->scan[slot]) {
-    // built locally, published only when every allocation has succeeded (a half-built state must never be picked up later)
-    gpud_scan_state* s = new gpud_scan_state();
+    auto s = std::make_unique<gpud_scan_state>();
     s->dev = dev;
-    cudaError_t e = cudaMalloc(&s->d_tables, sizeof(gpud_tables));
+    cudaError_t e = s->d_tables.alloc(1);
     if (e == cudaSuccess) e = cudaMemcpy(s->d_tables, gpud_host_tables(), sizeof(gpud_tables), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMalloc(&s->d_counters, sizeof(ScanCounters));
-    if (e == cudaSuccess) e = cudaMallocHost(&s->h_counters, sizeof(ScanCounters));
-    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
-    for (auto& ev : s->ev) if (e == cudaSuccess) e = cudaEventCreate(&ev);
-    if (e != cudaSuccess) {
-      gpud_scan_state_free(s);
+    if (e == cudaSuccess) e = s->d_counters.alloc(1);
+    if (e == cudaSuccess) e = s->h_counters.alloc(1);
+    if (e == cudaSuccess) e = s->stream.make();
+    for (auto& ev : s->ev) if (e == cudaSuccess) e = ev.make();
+    if (e != cudaSuccess)
       return gpud_fail(ctx, e == cudaErrorMemoryAllocation ? GPUD_E_NOMEM : GPUD_E_CUDA, "scan state on device %d: %s", dev, cudaGetErrorString(e));
-    }
-    ctx->scan[slot] = s;
+    ctx->scan[slot] = std::move(s);
   }
-  *out = ctx->scan[slot];
+  *out = ctx->scan[slot].get();
   return GPUD_OK;
 }
 
@@ -1759,7 +1725,7 @@ static bool scan_mode_ok(int32_t mode) {
 
 // one kernel of the scan's chain; `overlap`: allow it to be scheduled while its predecessor on the stream drains (see pdl_wait)
 template <typename... P, typename... A>
-static cudaError_t launch_chain(bool overlap, void (*kernel)(P...), dim3 grid, dim3 block, cudaStream_t st, A... args) {
+static cudaError_t launch_chain(bool overlap, void (*kernel)(P...), dim3 grid, dim3 block, cudaStream_t st, A&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
@@ -1776,13 +1742,13 @@ static int32_t scan_launch(gpud_ctx* ctx, gpud_scan_state* s, const uint8_t* d_b
                            cudaStream_t st) {
   const int64_t n_chunks = std::max<int64_t>(1, (len + kChunk - 1) / kChunk);
   const int64_t n_tiles = (n_chunks + 1023) / 1024;
-  GPUD_CUDA(ctx, gpud_grow(&s->d_chunk_sep, &s->chunk_sep_cap, (size_t)n_chunks));
-  GPUD_CUDA(ctx, gpud_grow(&s->d_chunk_local, &s->chunk_local_cap, (size_t)n_chunks));
-  GPUD_CUDA(ctx, gpud_grow(&s->d_tile_base, &s->tile_cap, (size_t)n_chunks / 1024 + 2));
-  GPUD_CUDA(ctx, gpud_grow(&s->d_cands, &s->cand_cap, (size_t)(len / 4 + 1024)));
-  GPUD_CUDA(ctx, gpud_grow(&s->d_hits, &s->hit_cap, (size_t)std::max<int64_t>(hit_cap_req, 1024)));
+  GPUD_CUDA(ctx, s->d_chunk_sep.grow((size_t)n_chunks));
+  GPUD_CUDA(ctx, s->d_chunk_local.grow((size_t)n_chunks));
+  GPUD_CUDA(ctx, s->d_tile_base.grow((size_t)n_chunks / 1024 + 2));
+  GPUD_CUDA(ctx, s->d_cands.grow((size_t)(len / 4 + 1024)));
+  GPUD_CUDA(ctx, s->d_hits.grow((size_t)std::max<int64_t>(hit_cap_req, 1024)));
   GPUD_CUDA(ctx, cudaMemsetAsync(s->d_counters, 0, sizeof(ScanCounters), st));
-  GPUD_CUDA(ctx, gpud_grow(&s->d_side, &s->side_cap, std::min<size_t>(s->cand_cap, (size_t)1 << 20)));
+  GPUD_CUDA(ctx, s->d_side.grow(std::min<size_t>(s->d_cands.cap(), (size_t)1 << 20)));
   if (len == 0) {
     GPUD_CUDA(ctx, cudaMemsetAsync(s->d_chunk_sep, 0, sizeof(uint32_t), st));
   }
@@ -1798,7 +1764,7 @@ static int32_t scan_launch(gpud_ctx* ctx, gpud_scan_state* s, const uint8_t* d_b
   const auto filter = fm ? k_scan_filter<GPUD_SCAN_FM_LOG, false>
                          : mode == GPUD_SCAN_LINES ? (ext ? k_scan_filter<GPUD_SCAN_LINES, true> : k_scan_filter<GPUD_SCAN_LINES, false>)
                                                    : (ext ? k_scan_filter<GPUD_SCAN_RAW_KMSG, true> : k_scan_filter<GPUD_SCAN_RAW_KMSG, false>);
-  GPUD_CUDA(ctx, launch_chain(false, filter, dim3(grid), dim3(256), st, b, s->d_chunk_sep, s->d_cands, &c->n_cand, (unsigned long long)s->cand_cap,
+  GPUD_CUDA(ctx, launch_chain(false, filter, dim3(grid), dim3(256), st, b, s->d_chunk_sep, s->d_cands, &c->n_cand, (unsigned long long)s->d_cands.cap(),
                               c->fam_cnt, fm ? fm_tab() : ext_tab()));
   // phase timing off (the default): no event between the kernels, so each launch may carry the programmatic-serialization attribute
   // (pdl_wait / pdl_release in the kernels); on: ev[1], ev[2] split the scan into filter / prefix / match and the launches are plain.
@@ -1809,9 +1775,9 @@ static int32_t scan_launch(gpud_ctx* ctx, gpud_scan_state* s, const uint8_t* d_b
                               n_tiles, &c->n_sep, &c->ticket));
   if (phased) cudaEventRecord(s->ev[2], st);
   // candidates sorted by matcher family before the match step: faster on 100 MiB buffers, most with all 22 families switched on
-  const unsigned long long side_cap = (unsigned long long)s->side_cap;
+  const unsigned long long side_cap = (unsigned long long)s->d_side.cap();
   GPUD_CUDA(ctx, launch_chain(!phased, k_cand_scatter, dim3(64), dim3(256), st, (const unsigned long long*)s->d_cands, &c->n_cand,
-                              (unsigned long long)s->cand_cap, (unsigned long long)s->side_cap, c->fam_cnt, c->fam_pos, s->d_side));
+                              (unsigned long long)s->d_cands.cap(), (unsigned long long)s->d_side.cap(), c->fam_cnt, c->fam_pos, s->d_side));
   const auto occupancy = [](auto kernel) {
     int nb = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kernel, 128, 0) != cudaSuccess || nb < 1) nb = 4;
@@ -1821,10 +1787,10 @@ static int32_t scan_launch(gpud_ctx* ctx, gpud_scan_state* s, const uint8_t* d_b
   GPUD_CUDA(ctx, launch_chain(!phased, fm ? k_scan_match<true> : k_scan_match<false>, dim3((unsigned)(ctx->sm_count * (fm ? fm_match_blocks : match_blocks))),
                               dim3(128), st, b, (int)mode,
                               (const unsigned long long*)s->d_cands, (const unsigned long long*)s->d_side, side_cap, &c->n_cand,
-                              (unsigned long long)s->cand_cap, (const uint32_t*)s->d_chunk_local, (const unsigned long long*)s->d_tile_base, (const gpud_tables*)s->d_tables,
-                              s->d_hits, (unsigned long long)s->hit_cap, &c->n_hits));
+                              (unsigned long long)s->d_cands.cap(), (const uint32_t*)s->d_chunk_local, (const unsigned long long*)s->d_tile_base, (const gpud_tables*)s->d_tables,
+                              s->d_hits, (unsigned long long)s->d_hits.cap(), &c->n_hits));
   GPUD_CUDA(ctx, launch_chain(!phased, k_scan_finish, dim3((unsigned)(ctx->sm_count * 16)), dim3(256), st, b, (int)mode, (const uint32_t*)s->d_chunk_local,
-                              (const unsigned long long*)s->d_tile_base, (const gpud_tables*)s->d_tables, s->d_hits, &c->n_hits, (unsigned long long)s->hit_cap));
+                              (const unsigned long long*)s->d_tile_base, (const gpud_tables*)s->d_tables, s->d_hits, &c->n_hits, (unsigned long long)s->d_hits.cap()));
   cudaEventRecord(s->ev[3], st);
   GPUD_CUDA(ctx, cudaMemcpyAsync(s->h_counters, c, offsetof(ScanCounters, fam_cnt), cudaMemcpyDeviceToHost, st));
   return GPUD_OK;
@@ -1838,7 +1804,7 @@ static int32_t scan_run(gpud_ctx* ctx, gpud_scan_state* s, const uint8_t* d_buf,
   if (rc) return rc;
   GPUD_CUDA(ctx, cudaStreamSynchronize(st));
   const int64_t found = (int64_t)s->h_counters->n_hits;
-  if (found <= (int64_t)s->hit_cap) return GPUD_OK;
+  if (found <= (int64_t)s->d_hits.cap()) return GPUD_OK;
   rc = scan_launch(ctx, s, d_buf, len, mode, found, st);
   if (rc) return rc;
   GPUD_CUDA(ctx, cudaStreamSynchronize(st));
@@ -1852,16 +1818,9 @@ static int32_t scan_collect(gpud_ctx* ctx, gpud_scan_state* s, gpud_xid_hit* hit
   const int64_t found = (int64_t)c.n_hits;
   if (n_hits) *n_hits = found;
   if (n_units) *n_units = (int64_t)c.n_sep + 1;
-  if (c.n_cand > s->cand_cap) return gpud_fail(ctx, GPUD_E_CAPACITY, "candidate list overflow (%llu)", c.n_cand);
+  if (c.n_cand > s->d_cands.cap()) return gpud_fail(ctx, GPUD_E_CAPACITY, "candidate list overflow (%llu)", c.n_cand);
   // hits land in a pinned host buffer; only 24-byte keys are sorted, each 288-byte record moves once
-  if ((size_t)found > s->h_hits_cap) {
-    if (s->h_hits) cudaFreeHost(s->h_hits);
-    s->h_hits = nullptr;
-    s->h_hits_cap = 0;
-    const size_t want = std::max<size_t>((size_t)found, 4096);
-    GPUD_CUDA(ctx, cudaMallocHost(&s->h_hits, want * sizeof(gpud_xid_hit)));
-    s->h_hits_cap = want;
-  }
+  if ((size_t)found > s->h_hits.cap()) GPUD_CUDA(ctx, s->h_hits.alloc(std::max<size_t>((size_t)found, 4096)));
   if (found) {
     GPUD_CUDA(ctx, cudaMemcpyAsync(s->h_hits, s->d_hits, (size_t)found * sizeof(gpud_xid_hit), cudaMemcpyDeviceToHost, st));
     GPUD_CUDA(ctx, cudaStreamSynchronize(st));
@@ -1907,7 +1866,7 @@ extern "C" int32_t gpud_kmsg_scan_device(gpud_ctx* ctx, int32_t dev, const uint8
 
 // the caller's host bytes into s->d_buf, on s->stream
 static int32_t stage_host(gpud_ctx* ctx, gpud_scan_state* s, const uint8_t* buf, int64_t len) {
-  GPUD_CUDA(ctx, gpud_grow(&s->d_buf, &s->buf_cap, (size_t)len + 64));
+  GPUD_CUDA(ctx, s->d_buf.grow((size_t)len + 64));
   if (len) {
     cudaPointerAttributes attr;
     bool pinned = false;
@@ -1918,11 +1877,10 @@ static int32_t stage_host(gpud_ctx* ctx, gpud_scan_state* s, const uint8_t* buf,
     } else {
       // pageable caller memory (a Go []byte): stage through two pinned buffers so the CPU copy of piece k+1 overlaps the DMA of piece k
       const size_t piece = 8u << 20;
-      for (int i = 0; i < 2; ++i)
-        if (!s->h_stage[i]) {
-          GPUD_CUDA(ctx, cudaMallocHost(&s->h_stage[i], piece));
-          GPUD_CUDA(ctx, cudaEventCreateWithFlags(&s->ev_stage[i], cudaEventDisableTiming));
-        }
+      for (int i = 0; i < 2; ++i) {
+        GPUD_CUDA(ctx, s->h_stage[i].grow(piece));
+        GPUD_CUDA(ctx, s->ev_stage[i].make(cudaEventDisableTiming));
+      }
       int k = 0;
       for (size_t off = 0; off < (size_t)len; off += piece, k ^= 1) {
         const size_t n = std::min(piece, (size_t)len - off);
@@ -2056,7 +2014,7 @@ extern "C" int32_t gpud_xid_classify(gpud_ctx* ctx, int32_t dev, gpud_xid_hit* h
   gpud_scan_state* s;
   int32_t rc = scan_state_get(ctx, dev, &s);
   if (rc) return rc;
-  GPUD_CUDA(ctx, gpud_grow(&s->d_hits, &s->hit_cap, (size_t)std::max<int64_t>(n, 1024)));
+  GPUD_CUDA(ctx, s->d_hits.grow((size_t)std::max<int64_t>(n, 1024)));
   GPUD_CUDA(ctx, cudaMemcpyAsync(s->d_hits, hits, (size_t)n * sizeof(gpud_xid_hit), cudaMemcpyHostToDevice, s->stream));
   k_classify<<<(unsigned)((n + 3) / 4), 128, 0, s->stream>>>(s->d_tables, s->d_hits, n);   // one warp per hit
   GPUD_CUDA(ctx, cudaGetLastError());

@@ -118,14 +118,14 @@ struct gpud_poller {
   gpud_ring* ring = nullptr;
   int dev = 0;
   nvmlDevice_t h = nullptr;
-  uint32_t* rows = nullptr;      // pinned [cap_rows][GPUD_POLL_N_FIELDS]
+  gpud_pinned<uint32_t> rows;    // [cap_rows][GPUD_POLL_N_FIELDS]
   int64_t cap_rows = 0, n_rows = 0;
   double last_poll_s = 0.0;      // wall time of the last gpud_poller_poll call
   uint32_t held[GPUD_POLL_N_FIELDS] = {0};       // last good value per column (what a failed getter's column repeats)
   uint32_t fail_mask = 0;                        // columns that failed at least once since create
   int32_t last_rc[GPUD_POLL_N_FIELDS] = {0};     // the NVML return code of each column's last failure
   uint64_t n_failed[GPUD_POLL_N_FIELDS] = {0};
-  uint64_t* field_rows = nullptr;                // pinned [cap_rows][GPUD_FIELD_ROW_N] (gpud_poller_poll_fields)
+  gpud_pinned<uint64_t> field_rows;              // [cap_rows][GPUD_FIELD_ROW_N] (gpud_poller_poll_fields)
   uint64_t field_held[GPUD_FIELD_ROW_N] = {0};
   double gpm_held[GPUD_GPM_N] = {0};
 };
@@ -140,21 +140,15 @@ extern "C" int32_t gpud_poller_create(gpud_ctx* ctx, int32_t dev, gpud_ring* rin
   nvmlDevice_t h;
   const nvmlReturn_t rc = N->by_pci(bus, &h);
   if (rc != 0) return gpud_fail(ctx, GPUD_E_UNSUPPORTED, "nvmlDeviceGetHandleByPciBusId(%s): %s", bus, N->err ? N->err(rc) : "error");
-  gpud_poller* p = new gpud_poller();
+  auto p = std::make_unique<gpud_poller>();
   p->ctx = ctx; p->ring = ring; p->dev = dev; p->h = h;
   p->cap_rows = 1 << 14;
-  if (cudaMallocHost(&p->rows, (size_t)p->cap_rows * GPUD_POLL_N_FIELDS * sizeof(uint32_t)) != cudaSuccess) {
-    delete p;
-    return gpud_fail(ctx, GPUD_E_CUDA, "pinned poll buffer");
-  }
-  *out = p;
+  if (p->rows.alloc((size_t)p->cap_rows * GPUD_POLL_N_FIELDS) != cudaSuccess) return gpud_fail(ctx, GPUD_E_CUDA, "pinned poll buffer");
+  *out = p.release();
   return GPUD_OK;
 }
 
 extern "C" void gpud_poller_destroy(gpud_poller* p) {
-  if (!p) return;
-  if (p->rows) cudaFreeHost(p->rows);
-  if (p->field_rows) cudaFreeHost(p->field_rows);
   delete p;
 }
 
@@ -654,7 +648,7 @@ extern "C" int32_t gpud_poller_poll_fields(gpud_poller* p, gpud_ring* ring, int6
   if (!N || !N->field_values) return GPUD_E_UNSUPPORTED;
   if (ring->F != GPUD_FIELD_ROW_N) return gpud_fail(p->ctx, GPUD_E_INVALID, "the field-row source needs a ring of %d fields (this one has %d)", GPUD_FIELD_ROW_N, ring->F);
   if (!p->field_rows) {
-    if (cudaMallocHost(&p->field_rows, (size_t)p->cap_rows * GPUD_FIELD_ROW_N * sizeof(uint64_t)) != cudaSuccess) return gpud_fail(p->ctx, GPUD_E_CUDA, "pinned field rows");
+    if (p->field_rows.alloc((size_t)p->cap_rows * GPUD_FIELD_ROW_N) != cudaSuccess) return gpud_fail(p->ctx, GPUD_E_CUDA, "pinned field rows");
   }
   timespec t0, t1;
   clock_gettime(CLOCK_MONOTONIC, &t0);

@@ -116,16 +116,6 @@ static void tile_pieces(const gpud_range_geo& g, const gpud_piece* p, int64_t* t
   }
 }
 
-void gpud_ranges_state_free(gpud_ranges_state* s) {
-  if (!s) return;
-  gpud_range_state_free(s->seg);
-  cudaFree(s->d_short); cudaFree(s->d_pieces); cudaFree(s->d_srcs); cudaFree(s->d_tile); cudaFree(s->d_tile_piece); cudaFree(s->d_out); cudaFree(s->d_nover);
-  cudaFree(s->d_vring); cudaFree(s->d_vsmp); cudaFree(s->d_rows); cudaFree(s->d_vdir); cudaFree(s->d_voffs); cudaFree(s->d_runs); cudaFree(s->d_vsum);
-  for (auto& ev : s->ev) if (ev) cudaEventDestroy(ev);
-  for (auto& ev : s->ev_dec) if (ev) cudaEventDestroy(ev);
-  delete s;
-}
-
 namespace {
 // one batch's long results [5][F n_long] / [F n_long] (segment f n_long + j) into the call's [5][F][n_out] / [F][n_out], column geo[j].id
 __global__ void k_ranges_scatter(const double* __restrict__ seg_out, const uint32_t* __restrict__ seg_nover, const gpud_range_geo* __restrict__ geo, int64_t n_long,
@@ -169,12 +159,11 @@ static int32_t rings_ready(const gpud_ring_view& v, gpud_ring* const* rings, int
   for (int i = 1; i < n_rings; ++i) {
     gpud_ring* o = rings[i];
     if (o->stream == v.stream) continue;
-    cudaEvent_t ev = nullptr;
+    gpud_event ev;                     // released once the wait has been satisfied
     GPUD_CUDA(v.ctx, cudaSetDevice(o->dev));
-    GPUD_CUDA(v.ctx, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    GPUD_CUDA(v.ctx, ev.make(cudaEventDisableTiming));
     cudaError_t e = cudaEventRecord(ev, o->stream);
     if (e == cudaSuccess) e = cudaStreamWaitEvent(v.stream, ev, 0);
-    cudaEventDestroy(ev);              // released once the wait has been satisfied
     if (e != cudaSuccess) return gpud_fail(v.ctx, GPUD_E_CUDA, "ring %d: waiting for its stream: %s", i, cudaGetErrorString(e));
   }
   GPUD_CUDA(v.ctx, cudaSetDevice(v.dev));
@@ -183,10 +172,10 @@ static int32_t rings_ready(const gpud_ring_view& v, gpud_ring* const* rings, int
 
 // The call behind the entry points, after their argument checks (and, for several rings, rings_check): every refusal comes from
 // ranges_plan, or the peer check after it, before any launch.  The kernels run on the home ring's device and stream, read through the
-// view v (the ring itself, or a buffer laid out as one: a slot of a virtual box) and the ring table t, with the scratch *state (created
+// view v (the ring itself, or a buffer laid out as one: a slot of a virtual box) and the ring table t, with the scratch `state` (created
 // on first use): the home ring's own, or a box query's (gpud_box_query), which must leave the ring's untouched.
 int32_t reduce_sets(const gpud_ring_view& v, const RingTable& t, const int32_t* ring_of, const int64_t* first, const int64_t* len, int64_t n_ranges,
-                    const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over, gpud_ranges_state** state) {
+                    const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over, std::unique_ptr<gpud_ranges_state>& state) {
   const int n_rings = t.n();
   std::vector<gpud_ring_src> src(t.src);
   src[0] = {v.d_ring, v.d_sample};
@@ -198,30 +187,30 @@ int32_t reduce_sets(const gpud_ring_view& v, const RingTable& t, const int32_t* 
   bool multi = false;
   for (const gpud_piece& q : pl.pieces) multi |= gpud_piece_ring(q) != 0;
   GPUD_CUDA(v.ctx, cudaSetDevice(v.dev));
-  if (!*state) *state = new gpud_ranges_state();
-  gpud_ranges_state* rs = *state;
-  if (!rs->seg) rs->seg = new gpud_range_state();
+  if (!state) state = std::make_unique<gpud_ranges_state>();
+  gpud_ranges_state* rs = state.get();
+  if (!rs->seg) rs->seg = std::make_unique<gpud_range_state>();
   rs->timed = false;
   rs->seg_last = false;
   rs->open = 0;
   std::fill(rs->reasons, rs->reasons + GPUD_RANGE_N_OPEN_REASONS, 0);
   const size_t plane = (size_t)v.F * n_sets;
-  GPUD_CUDA(v.ctx, gpud_grow(&rs->d_out, &rs->out_cap, 5 * plane));
-  GPUD_CUDA(v.ctx, gpud_grow(&rs->d_nover, &rs->nover_cap, plane));
-  GPUD_CUDA(v.ctx, gpud_grow(&rs->d_short, &rs->short_cap, std::max<size_t>(1, pl.shorts.size())));
+  GPUD_CUDA(v.ctx, rs->d_out.grow(5 * plane));
+  GPUD_CUDA(v.ctx, rs->d_nover.grow(plane));
+  GPUD_CUDA(v.ctx, rs->d_short.grow(std::max<size_t>(1, pl.shorts.size())));
   const gpud_piece* d_pieces = nullptr;
   if (!pl.pieces.empty()) {
-    GPUD_CUDA(v.ctx, gpud_grow(&rs->d_pieces, &rs->pieces_cap, pl.pieces.size()));
-    if (multi) GPUD_CUDA(v.ctx, gpud_grow(&rs->d_srcs, &rs->srcs_cap, (size_t)n_rings));
+    GPUD_CUDA(v.ctx, rs->d_pieces.grow(pl.pieces.size()));
+    if (multi) GPUD_CUDA(v.ctx, rs->d_srcs.grow((size_t)n_rings));
     d_pieces = rs->d_pieces;
   }
-  for (auto& ev : rs->ev) if (!ev) GPUD_CUDA(v.ctx, cudaEventCreate(&ev));
+  for (auto& ev : rs->ev) GPUD_CUDA(v.ctx, ev.make());
   GPUD_CUDA(v.ctx, cudaEventRecord(rs->ev[0], v.stream));
   if (d_pieces) {
     GPUD_CUDA(v.ctx, cudaMemcpyAsync(rs->d_pieces, pl.pieces.data(), pl.pieces.size() * sizeof(gpud_piece), cudaMemcpyHostToDevice, v.stream));
     if (multi) GPUD_CUDA(v.ctx, cudaMemcpyAsync(rs->d_srcs, src.data(), n_rings * sizeof(gpud_ring_src), cudaMemcpyHostToDevice, v.stream));
   }
-  const gpud_ring_src* d_srcs = multi ? rs->d_srcs : nullptr;
+  const gpud_ring_src* d_srcs = multi ? rs->d_srcs.get() : nullptr;
   if (!pl.shorts.empty()) {
     GPUD_CUDA(v.ctx, cudaMemcpyAsync(rs->d_short, pl.shorts.data(), pl.shorts.size() * sizeof(gpud_short_range), cudaMemcpyHostToDevice, v.stream));
     GPUD_CUDA(v.ctx, gpud_ranges_short(v, rs->d_short, (int)pl.shorts.size(), d_pieces, d_srcs, n_sets, rs->d_out, rs->d_nover));
@@ -240,16 +229,16 @@ int32_t reduce_sets(const gpud_ring_view& v, const RingTable& t, const int32_t* 
         tile_pieces(g, pl.pieces.data() + pl.p0[g0 + j], tile_piece.data() + g.tile0);
       }
     }
-    GPUD_CUDA(v.ctx, gpud_grow(&rs->d_tile, &rs->tile_cap, (size_t)n_tiles));
+    GPUD_CUDA(v.ctx, rs->d_tile.grow((size_t)n_tiles));
     GPUD_CUDA(v.ctx, cudaMemcpyAsync(rs->d_tile, tile.data(), n_tiles * sizeof(int32_t), cudaMemcpyHostToDevice, v.stream));
     if (!tile_piece.empty()) {
-      GPUD_CUDA(v.ctx, gpud_grow(&rs->d_tile_piece, &rs->tile_piece_cap, (size_t)n_tiles));
+      GPUD_CUDA(v.ctx, rs->d_tile_piece.grow((size_t)n_tiles));
       GPUD_CUDA(v.ctx, cudaMemcpyAsync(rs->d_tile_piece, tile_piece.data(), n_tiles * sizeof(int64_t), cudaMemcpyHostToDevice, v.stream));
     }
-    gpud_range_state* s = rs->seg;
+    gpud_range_state* s = rs->seg.get();
     const bool pieces = !tile_piece.empty();   // a set with pieces in this batch
     { int32_t rc = run_select(v, nullptr, s, pl.geo.data() + g0, n_long, GPUD_MAX_WINDOW, true, true, rs->d_tile, nullptr, nullptr, pieces ? d_pieces : nullptr,
-                              pl.p0.data() + g0, pieces ? rs->d_tile_piece : nullptr, pieces ? d_srcs : nullptr); if (rc) return rc; }
+                              pl.p0.data() + g0, pieces ? rs->d_tile_piece.get() : nullptr, pieces ? d_srcs : nullptr); if (rc) return rc; }
     rs->seg_last = true;
     rs->open += s->fields_open;
     for (int i = 0; i < GPUD_RANGE_N_OPEN_REASONS; ++i) rs->reasons[i] += s->reasons[i];
@@ -371,7 +360,7 @@ static void tier_scatter(const std::vector<double>& f64, const std::vector<uint3
 }
 
 int32_t reduce_subset(const gpud_ring_view& v, const RingTable& t, const std::vector<int64_t>& ids, const int32_t* ring_of, const int64_t* first,
-                      const int64_t* len, const int64_t* set_off, gpud_ranges_state** state, std::vector<double>& f64, std::vector<uint32_t>& nov) {
+                      const int64_t* len, const int64_t* set_off, std::unique_ptr<gpud_ranges_state>& state, std::vector<double>& f64, std::vector<uint32_t>& nov) {
   std::vector<int64_t> sf, sl, so(1, 0);
   std::vector<int32_t> sr;
   for (int64_t s : ids) {
@@ -391,8 +380,8 @@ int32_t reduce_subset(const gpud_ring_view& v, const RingTable& t, const std::ve
 
 // Device scratch of the virtual box, grown on the home ring: a failed allocation is GPUD_E_CUDA and leaves every ring usable.
 template <typename T>
-static int32_t vbox_grow(gpud_ctx* ctx, T** p, size_t* cap, size_t need) {
-  const cudaError_t e = gpud_grow(p, cap, std::max<size_t>(1, need));
+static int32_t vbox_grow(gpud_ctx* ctx, gpud_buf<T>& b, size_t need) {
+  const cudaError_t e = b.grow(std::max<size_t>(1, need));
   if (e == cudaSuccess) return GPUD_OK;
   cudaGetLastError();
   return gpud_fail(ctx, GPUD_E_CUDA, "reduce_range_sets: the virtual box's %zu-element scratch: %s", need, cudaGetErrorString(e));
@@ -419,7 +408,7 @@ static int32_t reduce_box(gpud_ring* const* rings, int n_rings, const int32_t* r
   }
   TierSplit sp;
   if (tiered) { int32_t rc = tier_split(ctx, rg, h->cap, ring_of, first, len, n_ranges, set_off, n_sets, &sp); if (rc) return rc; }
-  if (sp.ring.empty()) return reduce_sets(gpud_view(h), rt, ring_of, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over, &h->ranges);
+  if (sp.ring.empty()) return reduce_sets(gpud_view(h), rt, ring_of, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over, h->ranges);
   { int32_t rc = rings_ready(gpud_view(h), rings, n_rings); if (rc) return rc; }
   rt.rings = nullptr;                              // ready: the subsets below wait for nothing more
   std::vector<int64_t> ids[2];
@@ -447,19 +436,18 @@ static int32_t reduce_box(gpud_ring* const* rings, int n_rings, const int32_t* r
     r0[v + 1] = (int64_t)runs.size();
   }
   GPUD_CUDA(ctx, cudaSetDevice(h->dev));
-  if (!h->ranges) h->ranges = new gpud_ranges_state();
-  gpud_ranges_state* rs = h->ranges;
-  { int32_t rc = vbox_grow(ctx, &rs->d_vring, &rs->vring_cap, (size_t)ns * G * vcap); if (rc) return rc; }
-  { int32_t rc = vbox_grow(ctx, &rs->d_vsmp, &rs->vsmp_cap, (size_t)ns * G * smp_slots); if (rc) return rc; }
-  { int32_t rc = vbox_grow(ctx, &rs->d_rows, &rs->rows_cap, drows.size()); if (rc) return rc; }
-  { int32_t rc = vbox_grow(ctx, &rs->d_vdir, &rs->vdir_cap, (size_t)G * drows.size()); if (rc) return rc; }
-  { int32_t rc = vbox_grow(ctx, &rs->d_voffs, &rs->voffs_cap, (size_t)G * drows.size()); if (rc) return rc; }
-  { int32_t rc = vbox_grow(ctx, &rs->d_runs, &rs->runs_cap, runs.size()); if (rc) return rc; }
-  { int32_t rc = vbox_grow(ctx, &rs->d_vsum, &rs->vsum_cap, (size_t)G); if (rc) return rc; }
-  for (auto& e : rs->ev_dec) if (!e) GPUD_CUDA(ctx, cudaEventCreate(&e));
-  cudaEvent_t ev[2] = {};
-  for (auto& e : ev) GPUD_CUDA(ctx, cudaEventCreate(&e));
-  struct EvFree { cudaEvent_t* e; ~EvFree() { for (int i = 0; i < 2; ++i) if (e[i]) cudaEventDestroy(e[i]); } } ev_free{ev};
+  if (!h->ranges) h->ranges = std::make_unique<gpud_ranges_state>();
+  gpud_ranges_state* rs = h->ranges.get();
+  { int32_t rc = vbox_grow(ctx, rs->d_vring, (size_t)ns * G * vcap); if (rc) return rc; }
+  { int32_t rc = vbox_grow(ctx, rs->d_vsmp, (size_t)ns * G * smp_slots); if (rc) return rc; }
+  { int32_t rc = vbox_grow(ctx, rs->d_rows, drows.size()); if (rc) return rc; }
+  { int32_t rc = vbox_grow(ctx, rs->d_vdir, (size_t)G * drows.size()); if (rc) return rc; }
+  { int32_t rc = vbox_grow(ctx, rs->d_voffs, (size_t)G * drows.size()); if (rc) return rc; }
+  { int32_t rc = vbox_grow(ctx, rs->d_runs, runs.size()); if (rc) return rc; }
+  { int32_t rc = vbox_grow(ctx, rs->d_vsum, (size_t)G); if (rc) return rc; }
+  for (auto& e : rs->ev_dec) GPUD_CUDA(ctx, e.make());
+  gpud_event ev[2];
+  for (auto& e : ev) GPUD_CUDA(ctx, e.make());
   GPUD_CUDA(ctx, cudaEventRecord(ev[0], h->stream));
   if (!drows.empty()) GPUD_CUDA(ctx, cudaMemcpyAsync(rs->d_rows, drows.data(), drows.size() * sizeof(int64_t), cudaMemcpyHostToDevice, h->stream));
   if (!runs.empty()) GPUD_CUDA(ctx, cudaMemcpyAsync(rs->d_runs, runs.data(), runs.size() * sizeof(gpud_tier_run), cudaMemcpyHostToDevice, h->stream));
@@ -472,7 +460,7 @@ static int32_t reduce_box(gpud_ring* const* rings, int n_rings, const int32_t* r
   std::vector<double> f64;
   std::vector<uint32_t> nov;
   if (!ids[0].empty()) {
-    int32_t rc = reduce_subset(gpud_view(h), rt, ids[0], ring_of, first, len, set_off, &h->ranges, f64, nov);
+    int32_t rc = reduce_subset(gpud_view(h), rt, ids[0], ring_of, first, len, set_off, h->ranges, f64, nov);
     if (rc) return rc;
     tier_scatter(f64, nov, ids[0], 0, F, F, n_sets, out_f64, out_n_over);
     tally();
@@ -504,7 +492,7 @@ static int32_t reduce_box(gpud_ring* const* rings, int n_rings, const int32_t* r
     vv.d_sample = vs[0].sample;
     vv.smp_shift = smp_shift;
     vv.smp_slots = smp_slots;
-    int32_t rc = reduce_subset(vv, vt, ids[1], ns > 1 ? sp.vslot.data() : nullptr, sp.vfirst.data(), len, set_off, &h->ranges, f64, nov);
+    int32_t rc = reduce_subset(vv, vt, ids[1], ns > 1 ? sp.vslot.data() : nullptr, sp.vfirst.data(), len, set_off, h->ranges, f64, nov);
     if (rc) return rc;
     float ms = 0.f;
     GPUD_CUDA(ctx, cudaEventElapsedTime(&ms, rs->ev_dec[0], rs->ev_dec[1]));
@@ -622,7 +610,7 @@ extern "C" int32_t gpud_ring_reduce_range_sets(gpud_ring* r, const int64_t* firs
 
 extern "C" int32_t gpud_ring_ranges_stats(gpud_ring* r, float* device_ms, int64_t* segments_by_radix, int32_t* reasons) {
   if (!r || !device_ms) return GPUD_E_INVALID;
-  const gpud_ranges_state* rs = r->ranges;
+  const gpud_ranges_state* rs = r->ranges.get();
   if (!rs || !rs->timed) return gpud_fail(r->ctx, GPUD_E_STATE, "no gpud_ring_reduce_ranges has run to the end on this ring");
   GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
   GPUD_CUDA(r->ctx, cudaEventSynchronize(rs->ev[1]));
@@ -642,11 +630,11 @@ extern "C" int32_t gpudh_ring_segment_scratch(gpud_ring* r, gpud_ring_windows* h
   if (h) {
     if (h->L <= GPUD_MAX_WINDOW || !h->seg || !h->seg->timed)
       return gpud_fail(r->ctx, GPUD_E_STATE, "no reduce of this handle has run the segment select to the end");
-    s = h->seg;
+    s = h->seg.get();
   } else {
     if (!r->ranges || !r->ranges->timed || !r->ranges->seg_last)
       return gpud_fail(r->ctx, GPUD_E_STATE, "the last reduce_ranges (if any) had no long range");
-    s = r->ranges->seg;
+    s = r->ranges->seg.get();
   }
   GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
   if (piv) GPUD_CUDA(r->ctx, cudaMemcpyAsync(piv, s->d_piv, 2 * s->n_segs * sizeof(double), cudaMemcpyDeviceToHost, r->stream));

@@ -18,7 +18,7 @@
 #include <algorithm>
 
 #include "../../include/gpud_b200_hooks.h"
-#include "internal.h"
+#include "segsel.h"
 
 namespace {
 
@@ -1130,40 +1130,36 @@ extern "C" int32_t gpud_ring_create(gpud_ctx* ctx, int32_t dev, const gpud_ring_
   if (qn == 0 && qd == 0) { qn = 99; qd = 100; }
   if (qn < 0 || qd <= 0 || qn > qd) return gpud_fail(ctx, GPUD_E_INVALID, "quantile q_num/q_den must satisfy 0 <= num <= den");
   GPUD_CUDA(ctx, cudaSetDevice(dev));
-  gpud_ring* r = new gpud_ring();
+  auto r = std::make_unique<gpud_ring>();
   r->ctx = ctx; r->dev = dev; r->F = cfg->n_fields; r->W = cfg->window; r->cap = cfg->capacity; r->alpha = alpha;
   r->q_num = qn; r->q_den = qd;
   r->sm_count = ctx->sm_count;
   r->nw_max = (r->cap + r->W - 1) / r->W;
-  const size_t ring_bytes = (size_t)r->F * r->cap * sizeof(double) + 64;   // slack: the 16-byte load of a window's last odd element
-  const size_t res_bytes = (size_t)r->F * r->nw_max * sizeof(double);
+  const size_t ring_len = (size_t)r->F * r->cap + 8;   // slack: the 16-byte load of a window's last odd element
+  const size_t res_len = (size_t)r->F * r->nw_max;
   while (((r->cap + (1ll << r->smp_shift) - 1) >> r->smp_shift) > GPUD_RANGE_SAMPLE_MAX) ++r->smp_shift;
   r->smp_slots = (r->cap + (1ll << r->smp_shift) - 1) >> r->smp_shift;
-  cudaError_t e = cudaMalloc(&r->d_ring, ring_bytes);
-  if (e == cudaSuccess) e = cudaMemsetAsync(r->d_ring, 0, ring_bytes, 0);
-  if (e == cudaSuccess) e = cudaMalloc(&r->d_sample, (size_t)r->F * r->smp_slots * sizeof(double));
+  cudaError_t e = r->d_ring.alloc(ring_len);
+  if (e == cudaSuccess) e = cudaMemsetAsync(r->d_ring, 0, ring_len * sizeof(double), 0);
+  if (e == cudaSuccess) e = r->d_sample.alloc((size_t)r->F * r->smp_slots);
   if (e == cudaSuccess) e = cudaMemsetAsync(r->d_sample, 0, (size_t)r->F * r->smp_slots * sizeof(double), 0);
-  if (e == cudaSuccess) e = cudaMalloc(&r->d_thr, r->F * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc(&r->d_pw, 127 * sizeof(double));
-  for (int i = 0; i < 5 && e == cudaSuccess; ++i) e = cudaMalloc(&r->d_res[i], res_bytes);
-  if (e == cudaSuccess) e = cudaMalloc(&r->d_nover, (size_t)r->F * r->nw_max * sizeof(uint32_t));
-  if (e == cudaSuccess) e = cudaMalloc(&r->d_part, res_bytes);
-  if (e == cudaSuccess) e = cudaMalloc(&r->d_cursor, 4 * sizeof(unsigned long long));
-  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&r->own_stream, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&r->copy_stream, cudaStreamNonBlocking);
+  if (e == cudaSuccess) e = r->d_thr.alloc(r->F);
+  if (e == cudaSuccess) e = r->d_pw.alloc(127);
+  for (int i = 0; i < 5 && e == cudaSuccess; ++i) e = r->d_res[i].alloc(res_len);
+  if (e == cudaSuccess) e = r->d_nover.alloc(res_len);
+  if (e == cudaSuccess) e = r->d_part.alloc(res_len);
+  if (e == cudaSuccess) e = r->d_cursor.alloc(4);
+  if (e == cudaSuccess) e = r->own_stream.make();
+  if (e == cudaSuccess) e = r->copy_stream.make();
   r->stage_rows = std::max<int64_t>(1, (int64_t)(kStageBytes / (sizeof(double) * r->F)));
   for (int i = 0; i < 2 && e == cudaSuccess; ++i) {
-    e = cudaMallocHost(&r->h_stage[i], (size_t)r->stage_rows * r->F * sizeof(double));
-    if (e == cudaSuccess) e = cudaMalloc(&r->d_stage[i], (size_t)r->stage_rows * r->F * sizeof(double));
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&r->ev_stage[i], cudaEventDisableTiming);
-    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&r->ev_copied[i], cudaEventDisableTiming);
+    e = r->h_stage[i].alloc((size_t)r->stage_rows * r->F);
+    if (e == cudaSuccess) e = r->d_stage[i].alloc((size_t)r->stage_rows * r->F);
+    if (e == cudaSuccess) e = r->ev_stage[i].make(cudaEventDisableTiming);
+    if (e == cudaSuccess) e = r->ev_copied[i].make(cudaEventDisableTiming);
   }
-  for (int i = 0; i < 3 && e == cudaSuccess; ++i) e = cudaEventCreate(&r->ev_k[i]);
-  if (e != cudaSuccess) {
-    int32_t rc = gpud_fail(ctx, e == cudaErrorMemoryAllocation ? GPUD_E_NOMEM : GPUD_E_CUDA, "ring_create: %s", cudaGetErrorString(e));
-    gpud_ring_destroy(r);
-    return rc;
-  }
+  for (int i = 0; i < 3 && e == cudaSuccess; ++i) e = r->ev_k[i].make();
+  if (e != cudaSuccess) return gpud_fail(ctx, e == cudaErrorMemoryAllocation ? GPUD_E_NOMEM : GPUD_E_CUDA, "ring_create: %s", cudaGetErrorString(e));
   r->stream = r->own_stream;
   std::vector<double> thr(r->F, INFINITY), pw(127);
   if (cfg->thresholds) std::copy(cfg->thresholds, cfg->thresholds + r->F, thr.begin());
@@ -1172,40 +1168,15 @@ extern "C" int32_t gpud_ring_create(gpud_ctx* ctx, int32_t dev, const gpud_ring_
   GPUD_CUDA(ctx, cudaMemcpy(r->d_pw, pw.data(), 127 * sizeof(double), cudaMemcpyHostToDevice));
   GPUD_CUDA(ctx, cudaDeviceSynchronize());
   r->thr = thr;
-  *out = r;
+  *out = r.release();
   return GPUD_OK;
-}
-
-static void windows_free(gpud_ring_windows* s) {
-  if (!s) return;
-  cudaFree(s->d_hist); cudaFree(s->d_hist_nover); cudaFree(s->d_ema); cudaFree(s->d_sc); cudaFree(s->d_sc_nover);
-  cudaFree(s->d_eq); cudaFree(s->d_eq_nover);
-  gpud_range_state_free(s->seg);
-  for (auto& ev : s->ev) if (ev) cudaEventDestroy(ev);
-  delete s;
 }
 
 extern "C" int32_t gpud_ring_destroy(gpud_ring* r) {
   if (!r) return GPUD_E_INVALID;
   cudaSetDevice(r->dev);
-  if (r->own_stream) cudaStreamSynchronize(r->own_stream);
-  cudaFree(r->d_ring); cudaFree(r->d_sample); cudaFree(r->d_thr); cudaFree(r->d_pw); cudaFree(r->d_nover); cudaFree(r->d_part);
-  cudaFree(r->d_cursor);
-  for (auto& p : r->d_res) cudaFree(p);
-  gpud_range_state_free(r->range);
-  gpud_ranges_state_free(r->ranges);
-  gpud_tier_free(r->tier);
-  windows_free(r->swin);
-  for (gpud_ring_windows* w : r->handles) windows_free(w);
-  for (int i = 0; i < 2; ++i) {
-    if (r->h_stage[i]) cudaFreeHost(r->h_stage[i]);
-    cudaFree(r->d_stage[i]);
-    if (r->ev_stage[i]) cudaEventDestroy(r->ev_stage[i]);
-    if (r->ev_copied[i]) cudaEventDestroy(r->ev_copied[i]);
-  }
-  for (auto& ev : r->ev_k) if (ev) cudaEventDestroy(ev);
-  if (r->copy_stream) { cudaStreamSynchronize(r->copy_stream); cudaStreamDestroy(r->copy_stream); }
-  if (r->own_stream) cudaStreamDestroy(r->own_stream);
+  cudaStreamSynchronize(r->own_stream);
+  cudaStreamSynchronize(r->copy_stream);
   delete r;
   return GPUD_OK;
 }
@@ -1304,7 +1275,7 @@ extern "C" int32_t gpud_ring_push_raw(gpud_ring* r, const void* host_rows_v, int
     if (!pinned) {
       GPUD_CUDA(r->ctx, cudaEventSynchronize(r->ev_copied[buf]));   // the previous H2D out of this pinned piece has finished
       gpud_parallel_memcpy(r->h_stage[buf], src, bytes);           // pageable caller memory: stage through pinned
-      src = (const char*)r->h_stage[buf];
+      src = (const char*)r->h_stage[buf].get();
     }
     GPUD_CUDA(r->ctx, cudaStreamWaitEvent(r->copy_stream, r->ev_stage[buf], 0));   // the append that last read d_stage[buf] is done
     GPUD_CUDA(r->ctx, cudaMemcpyAsync(r->d_stage[buf], src, bytes, cudaMemcpyHostToDevice, r->copy_stream));
@@ -1588,7 +1559,7 @@ extern "C" int32_t gpudh_ring_hop_plan(int64_t total, int64_t cap, int32_t W, in
   return (int32_t)n_ph;
 }
 
-static int32_t windows_open(gpud_ring* r, int64_t span, int64_t hop, int64_t history_windows, gpud_ring_windows** out) {
+static int32_t windows_open(gpud_ring* r, int64_t span, int64_t hop, int64_t history_windows, std::unique_ptr<gpud_ring_windows>* out) {
   if (span < 1 || span > r->cap / r->W)
     return gpud_fail(r->ctx, GPUD_E_INVALID, "windows of span %lld x %d samples do not fit the ring's %lld", (long long)span, r->W, (long long)r->cap);
   if (hop < 1 || hop > span || span % hop != 0)
@@ -1597,7 +1568,7 @@ static int32_t windows_open(gpud_ring* r, int64_t span, int64_t hop, int64_t his
   const int64_t H = history_windows > 0 ? history_windows : (r->cap + P - 1) / P;
   if (H > ((int64_t)1 << 40) / r->F) return gpud_fail(r->ctx, GPUD_E_INVALID, "history of %lld windows is too long", (long long)H);
   GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
-  gpud_ring_windows* s = new gpud_ring_windows();
+  auto s = std::make_unique<gpud_ring_windows>();
   s->ring = r;
   s->span = span;
   s->hop = hop;
@@ -1607,33 +1578,28 @@ static int32_t windows_open(gpud_ring* r, int64_t span, int64_t hop, int64_t his
   s->Wq = sub_window(r->W, hop);
   s->H = H;
   s->first = s->next = stream_plan(r->total, r->cap, L, P, H, 0, 0).reducible_from;
-  cudaError_t e = cudaMalloc(&s->d_hist, (size_t)5 * r->F * H * sizeof(double));
-  if (e == cudaSuccess) e = cudaMalloc(&s->d_hist_nover, (size_t)r->F * H * sizeof(uint32_t));
-  if (e == cudaSuccess) e = cudaMalloc(&s->d_ema, (size_t)r->F * sizeof(double));
+  cudaError_t e = s->d_hist.alloc((size_t)5 * r->F * H);
+  if (e == cudaSuccess) e = s->d_hist_nover.alloc((size_t)r->F * H);
+  if (e == cudaSuccess) e = s->d_ema.alloc((size_t)r->F);
   if (L <= GPUD_MAX_WINDOW) {
     s->sc_cols = (r->cap + L - 1) / L;
-    if (e == cudaSuccess) e = cudaMalloc(&s->d_sc, (size_t)5 * r->F * s->sc_cols * sizeof(double));
-    if (e == cudaSuccess) e = cudaMalloc(&s->d_sc_nover, (size_t)r->F * s->sc_cols * sizeof(uint32_t));
+    if (e == cudaSuccess) e = s->d_sc.alloc((size_t)5 * r->F * s->sc_cols);
+    if (e == cudaSuccess) e = s->d_sc_nover.alloc((size_t)r->F * s->sc_cols);
   }
   if (P < L) {
     s->eq_cols = (r->cap + s->Wq - 1) / s->Wq;
-    if (e == cudaSuccess) e = cudaMalloc(&s->d_eq, (size_t)4 * r->F * s->eq_cols * sizeof(double));
-    if (e == cudaSuccess) e = cudaMalloc(&s->d_eq_nover, (size_t)r->F * s->eq_cols * sizeof(uint32_t));
+    if (e == cudaSuccess) e = s->d_eq.alloc((size_t)4 * r->F * s->eq_cols);
+    if (e == cudaSuccess) e = s->d_eq_nover.alloc((size_t)r->F * s->eq_cols);
   }
-  for (int i = 0; i < 2 && e == cudaSuccess; ++i) e = cudaEventCreate(&s->ev[i]);
-  if (e != cudaSuccess) {
-    windows_free(s);
-    return gpud_fail(r->ctx, e == cudaErrorMemoryAllocation ? GPUD_E_NOMEM : GPUD_E_CUDA, "windows_open: %s", cudaGetErrorString(e));
-  }
-  *out = s;
+  for (int i = 0; i < 2 && e == cudaSuccess; ++i) e = s->ev[i].make();
+  if (e != cudaSuccess) return gpud_fail(r->ctx, e == cudaErrorMemoryAllocation ? GPUD_E_NOMEM : GPUD_E_CUDA, "windows_open: %s", cudaGetErrorString(e));
+  *out = std::move(s);
   return GPUD_OK;
 }
 
-int32_t gpud_ring_windows_new(gpud_ring* r, int64_t span, int64_t hop, int64_t history_windows, gpud_ring_windows** out) {
+int32_t gpud_ring_windows_new(gpud_ring* r, int64_t span, int64_t hop, int64_t history_windows, std::unique_ptr<gpud_ring_windows>* out) {
   return windows_open(r, span, hop, history_windows, out);
 }
-
-void gpud_ring_windows_free(gpud_ring_windows* s) { windows_free(s); }
 
 // The device work of a tumbling handle of span s on n consecutive windows of L from physical column start: their aggregates, and
 // the EMA partials of their sub-windows of Wp, in scratch that stays valid until the handle's next phase.
@@ -1652,7 +1618,7 @@ static int32_t reduce_phase(gpud_ring_windows* s, int64_t start, int64_t n, Phas
   } else {
     // every window of every field is one segment of the range pass, which runs in sub-windows of Wp samples
     gpud_seg_out o;
-    { int32_t rc = gpud_ring_segments(r, &s->seg, start, s->L, n, s->Wp, &o); if (rc) return rc; }
+    { int32_t rc = gpud_ring_segments(r, s->seg, start, s->L, n, s->Wp, &o); if (rc) return rc; }
     po->stride = (int64_t)r->F * n;
     po->sc = o.out; po->nover = o.nover; po->part = o.part;
     s->seg_open += o.open;
@@ -1727,7 +1693,7 @@ static int32_t windows_read(const gpud_ring_windows* s, int32_t op, int64_t firs
   const size_t need = (size_t)r->F * n * el;
   if ((size_t)out_bytes < need) return gpud_fail(r->ctx, GPUD_E_CAPACITY, "need %zu bytes", need);
   GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
-  const char* src = op == GPUD_OP_NOVER ? (const char*)s->d_hist_nover : (const char*)(s->d_hist + (size_t)op * r->F * s->H);
+  const char* src = op == GPUD_OP_NOVER ? (const char*)s->d_hist_nover.get() : (const char*)(s->d_hist + (size_t)op * r->F * s->H);
   // the windows sit in slots first_window % H onwards, wrapping at most once: two strided copies of F rows
   const int64_t slot = n ? first_window % s->H : 0, n1 = std::min(n, s->H - slot);
   if (n1 > 0)
@@ -1750,29 +1716,29 @@ extern "C" int32_t gpud_ring_stream_open(gpud_ring* r, int64_t history_windows) 
 extern "C" int32_t gpud_ring_stream_reduce(gpud_ring* r, int64_t* n_new, int64_t* n_lost) {
   if (!r) return GPUD_E_INVALID;
   if (!r->swin) return gpud_fail(r->ctx, GPUD_E_STATE, "stream windows are not open");
-  return windows_reduce(r->swin, n_new, n_lost);
+  return windows_reduce(r->swin.get(), n_new, n_lost);
 }
 
 extern "C" int32_t gpud_ring_stream_counts(gpud_ring* r, int64_t* first, int64_t* next, int64_t* lost_total) {
   if (!r) return GPUD_E_INVALID;
   if (!r->swin) return gpud_fail(r->ctx, GPUD_E_STATE, "stream windows are not open");
-  return gpud_ring_windows_counts(r->swin, first, next, lost_total);
+  return gpud_ring_windows_counts(r->swin.get(), first, next, lost_total);
 }
 
 extern "C" int32_t gpud_ring_stream_read(gpud_ring* r, int32_t op, int64_t first_window, int64_t n, void* out, int64_t out_bytes) {
   if (!r || !out || op < 0 || op >= GPUD_N_OPS || n < 0) return GPUD_E_INVALID;
   if (!r->swin) return gpud_fail(r->ctx, GPUD_E_STATE, "stream windows are not open");
-  return windows_read(r->swin, op, first_window, n, out, out_bytes);
+  return windows_read(r->swin.get(), op, first_window, n, out, out_bytes);
 }
 
 // gpud_ring_windows_*: handles of any span and hop
 extern "C" int32_t gpud_ring_windows_open_hop(gpud_ring* r, int64_t span, int64_t hop, int64_t history_windows, gpud_ring_windows** out) {
   if (!r || !out) return GPUD_E_INVALID;
-  gpud_ring_windows* s = nullptr;
+  std::unique_ptr<gpud_ring_windows> s;
   { int32_t rc = windows_open(r, span, hop, history_windows, &s); if (rc) return rc; }
-  r->handles.push_back(s);
+  *out = s.get();
+  r->handles.push_back(std::move(s));
   ++r->handle_gen;
-  *out = s;
   return GPUD_OK;
 }
 
@@ -1783,13 +1749,12 @@ extern "C" int32_t gpud_ring_windows_open(gpud_ring* r, int64_t span, int64_t hi
 extern "C" int32_t gpud_ring_windows_close(gpud_ring_windows* w) {
   if (!w) return GPUD_E_INVALID;
   gpud_ring* r = w->ring;
-  auto it = std::find(r->handles.begin(), r->handles.end(), w);
+  auto it = std::find_if(r->handles.begin(), r->handles.end(), [w](const std::unique_ptr<gpud_ring_windows>& h) { return h.get() == w; });
   if (it == r->handles.end()) return gpud_fail(r->ctx, GPUD_E_INVALID, "not an open windows handle of this ring");
-  r->handles.erase(it);
   ++r->handle_gen;
   cudaSetDevice(r->dev);
   cudaStreamSynchronize(r->stream);   // no launch of this handle's is still running when its memory goes
-  windows_free(w);
+  r->handles.erase(it);
   return GPUD_OK;
 }
 

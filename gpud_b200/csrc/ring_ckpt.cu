@@ -209,8 +209,8 @@ int64_t handle_body_bytes(int64_t F, int64_t n) { return 40 * F * n + pad8(4 * F
 // The handles a checkpoint records, in its order: the stream handle, then the windows handles in open order.
 std::vector<gpud_ring_windows*> ckpt_handles(const gpud_ring* r) {
   std::vector<gpud_ring_windows*> v;
-  if (r->swin) v.push_back(r->swin);
-  v.insert(v.end(), r->handles.begin(), r->handles.end());
+  if (r->swin) v.push_back(r->swin.get());
+  for (const auto& h : r->handles) v.push_back(h.get());
   return v;
 }
 
@@ -267,7 +267,7 @@ int32_t copy_history(gpud_ring* r, gpud_ring_windows* s, int64_t from, uint8_t* 
     const int32_t rc = part((char*)(s->d_hist + (size_t)op * F * H), sizeof(double), body + op * F * n * 8);
     if (rc) return rc;
   }
-  const int32_t rc = part((char*)s->d_hist_nover, sizeof(uint32_t), body + 40 * F * n);
+  const int32_t rc = part((char*)s->d_hist_nover.get(), sizeof(uint32_t), body + 40 * F * n);
   if (rc) return rc;
   GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));   // pageable caller memory: the copies have landed / been consumed
   return GPUD_OK;
@@ -297,12 +297,11 @@ int32_t read_handle_body(gpud_ring* r, gpud_ring_windows* s, int64_t from, const
 // Encode of the samples of g: size() runs pass 1 and the scan (every block's mode, width and offset, the field checksums and the
 // payload's words); pack() runs pass 2 and copies the payload into the caller's bytes.
 struct Encoder {
-  CallScratch sc;
   CkGeo g{};
   int64_t units = 0, words = 0;
-  uint8_t* d_dir = nullptr;
-  unsigned long long *d_words = nullptr, *d_offs = nullptr, *d_csum = nullptr, *d_payload = nullptr;
-  cudaEvent_t ev[4];
+  gpud_buf<uint8_t> d_dir;
+  gpud_buf<unsigned long long> d_words, d_offs, d_csum, d_payload;
+  gpud_event ev[4];
   std::vector<uint8_t> dir;
   std::vector<uint64_t> csum;
   float ms = 0.f;     // device ms of both passes
@@ -314,21 +313,21 @@ struct Encoder {
     if (units > INT32_MAX) return gpud_fail(r->ctx, GPUD_E_INVALID, "%s: %lld blocks", what, (long long)units);
     dir.assign(units, 0);
     csum.assign(F, 0);
-    for (auto& e : ev) GPUD_CUDA(r->ctx, sc.event(&e));
+    for (auto& e : ev) GPUD_CUDA(r->ctx, e.make());
     if (units == 0) return GPUD_OK;
     size_t tmp_bytes = 0;
-    GPUD_CUDA(r->ctx, cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_words, d_offs, (int)units, r->stream));
-    void* d_tmp = nullptr;
-    cudaError_t e = sc.alloc(&d_dir, units);
-    if (e == cudaSuccess) e = sc.alloc(&d_words, units);
-    if (e == cudaSuccess) e = sc.alloc(&d_offs, units);
-    if (e == cudaSuccess) e = sc.alloc(&d_csum, F);
-    if (e == cudaSuccess) e = sc.alloc((char**)&d_tmp, tmp_bytes);
+    GPUD_CUDA(r->ctx, cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, d_words.get(), d_offs.get(), (int)units, r->stream));
+    gpud_buf<char> d_tmp;
+    cudaError_t e = d_dir.alloc(units);
+    if (e == cudaSuccess) e = d_words.alloc(units);
+    if (e == cudaSuccess) e = d_offs.alloc(units);
+    if (e == cudaSuccess) e = d_csum.alloc(F);
+    if (e == cudaSuccess) e = d_tmp.alloc(tmp_bytes);
     if (e != cudaSuccess) return scratch_fail(r, e, what);
     GPUD_CUDA(r->ctx, cudaMemsetAsync(d_csum, 0, F * sizeof(unsigned long long), r->stream));
     GPUD_CUDA(r->ctx, cudaEventRecord(ev[0], r->stream));
     GPUD_CUDA(r->ctx, launch_size(r, g, d_dir, d_words, d_csum));
-    GPUD_CUDA(r->ctx, cub::DeviceScan::ExclusiveSum(d_tmp, tmp_bytes, d_words, d_offs, (int)units, r->stream));
+    GPUD_CUDA(r->ctx, cub::DeviceScan::ExclusiveSum(d_tmp.get(), tmp_bytes, d_words.get(), d_offs.get(), (int)units, r->stream));
     GPUD_CUDA(r->ctx, cudaEventRecord(ev[1], r->stream));
     unsigned long long last[2];
     GPUD_CUDA(r->ctx, cudaMemcpyAsync(&last[0], d_offs + units - 1, 8, cudaMemcpyDeviceToHost, r->stream));
@@ -340,7 +339,7 @@ struct Encoder {
 
   int32_t pack(gpud_ring* r, uint8_t* out_payload, bool pinned, const char* what) {
     if (units == 0) return GPUD_OK;
-    const cudaError_t e = sc.alloc(&d_payload, words);
+    const cudaError_t e = d_payload.alloc(words);
     if (e != cudaSuccess) return scratch_fail(r, e, what);
     GPUD_CUDA(r->ctx, cudaEventRecord(ev[2], r->stream));
     GPUD_CUDA(r->ctx, launch_pack(r, g, d_dir, d_offs, d_payload));
@@ -390,21 +389,20 @@ int32_t read_directory(gpud_ctx* ctx, const uint8_t* dir, int64_t units, int64_t
 
 // The decode's device inputs: the directory, the block offsets the host computed from it, the payload and zeroed field sums.
 struct Decoder {
-  CallScratch sc;
-  uint8_t* d_dir = nullptr;
-  unsigned long long *d_offs = nullptr, *d_payload = nullptr, *d_csum = nullptr;
-  cudaEvent_t ev[4];
+  gpud_buf<uint8_t> d_dir;
+  gpud_buf<unsigned long long> d_offs, d_payload, d_csum;
+  gpud_event ev[4];
 
   int32_t stage(gpud_ring* r, const uint8_t* dir, const std::vector<unsigned long long>& offs, const uint8_t* payload, int64_t pay_bytes,
                 const char* what) {
     const int64_t units = (int64_t)offs.size();
     bool pinned = false;
     { const int32_t rc = host_pinned(r, payload, &pinned); if (rc) return rc; }
-    cudaError_t e = sc.alloc(&d_dir, units);
-    if (e == cudaSuccess) e = sc.alloc(&d_offs, units);
-    if (e == cudaSuccess) e = sc.alloc(&d_payload, pay_bytes / 8);
-    if (e == cudaSuccess) e = sc.alloc(&d_csum, r->F);
-    for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = sc.event(&ev[i]);
+    cudaError_t e = d_dir.alloc(units);
+    if (e == cudaSuccess) e = d_offs.alloc(units);
+    if (e == cudaSuccess) e = d_payload.alloc(pay_bytes / 8);
+    if (e == cudaSuccess) e = d_csum.alloc(r->F);
+    for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = ev[i].make();
     if (e != cudaSuccess) return scratch_fail(r, e, what);
     GPUD_CUDA(r->ctx, cudaMemcpyAsync(d_dir, dir, units, cudaMemcpyHostToDevice, r->stream));
     GPUD_CUDA(r->ctx, cudaMemcpyAsync(d_offs, offs.data(), units * 8, cudaMemcpyHostToDevice, r->stream));
@@ -472,7 +470,7 @@ int32_t write_blob(gpud_ring* r, bool delta, void* out_v, int64_t cap, int64_t* 
   std::vector<int64_t> heads;
   for (gpud_ring_windows* s : hs) {
     const int64_t from = body_from(s, delta);
-    const int64_t head[10] = {s == r->swin ? kKindStream : kKindWindows, s->span, s->hop, s->H, s->first, s->next, s->lost, s->reseed ? 1 : 0,
+    const int64_t head[10] = {s == r->swin.get() ? kKindStream : kKindWindows, s->span, s->hop, s->H, s->first, s->next, s->lost, s->reseed ? 1 : 0,
                               s->ck_next, from};
     memcpy(out + off, head, 8 * nh);
     heads.insert(heads.end(), head, head + nh);
@@ -556,7 +554,7 @@ int32_t full_record_ok(gpud_ring* r, const CkHandle& h, uint32_t i, int64_t tota
 
 // A delta's record i: the successor of the ring's handle s.
 int32_t delta_record_ok(gpud_ring* r, const gpud_ring_windows* s, const CkHandle& h, uint32_t i, int64_t total) {
-  const bool same = h.kind == (s == r->swin ? kKindStream : kKindWindows) && h.span == s->span && h.hop == s->hop && h.H == s->H;
+  const bool same = h.kind == (s == r->swin.get() ? kKindStream : kKindWindows) && h.span == s->span && h.hop == s->hop && h.H == s->H;
   const int64_t complete = total < s->L ? 0 : (total - s->L) / s->P + 1;
   const bool hist_ok = h.prev_next == s->ck_next && h.first >= s->first && h.first <= h.next && h.next - h.first <= h.H && h.next >= h.prev_next &&
                        h.from == std::max(h.first, h.prev_next) && h.next <= complete && h.lost >= 0 && (h.reseed == 0 || h.reseed == 1);
@@ -715,17 +713,16 @@ extern "C" int32_t gpud_ring_restore(gpud_ring* r, const void* in_v, int64_t n_b
   float ms = 0.f;
   { const int32_t rc = load_samples(r, fr, false, &ms); if (rc) return rc; }
   // the handles, re-created; a failure leaves the ring as created
-  std::vector<gpud_ring_windows*> made;
+  std::vector<std::unique_ptr<gpud_ring_windows>> made;
   for (const CkHandle& h : fr.recs) {
-    gpud_ring_windows* s = nullptr;
+    std::unique_ptr<gpud_ring_windows> s;
     int32_t rc = gpud_ring_windows_new(r, h.span, h.hop, h.H, &s);
     if (rc == GPUD_OK) {
-      made.push_back(s);
       s->first = h.first; s->next = h.next; s->lost = h.lost; s->reseed = h.reseed != 0;
-      rc = read_handle_body(r, s, h.first, in + h.off, "restore");
+      rc = read_handle_body(r, s.get(), h.first, in + h.off, "restore");
+      made.push_back(std::move(s));
     }
     if (rc) {
-      for (gpud_ring_windows* x : made) gpud_ring_windows_free(x);
       r->total = 0;
       zero_ring(r);
       return rc;
@@ -734,10 +731,10 @@ extern "C" int32_t gpud_ring_restore(gpud_ring* r, const void* in_v, int64_t n_b
   int32_t k = 0;
   for (size_t i = 0; i < fr.recs.size(); ++i) {
     if (fr.recs[i].kind == kKindStream) {
-      r->swin = made[i];
+      r->swin = std::move(made[i]);
     } else {
-      r->handles.push_back(made[i]);
-      handles[k++] = made[i];
+      handles[k++] = made[i].get();
+      r->handles.push_back(std::move(made[i]));
     }
   }
   return finish_restore(r, fr, ms);

@@ -37,21 +37,21 @@ __host__ __device__ __forceinline__ bool sel_in_list(unsigned long long kmin, un
 // Everything a segment select keeps between selects: gpud_ring_reduce_range's (gpud_ring::range), a handle's (gpud_ring_windows::seg),
 // the long route's of the range calls (gpud_ranges_state::seg) and a box query's.  Every buffer is grown on demand (sel_reserve) and kept.
 struct gpud_range_state {
-  gpud_range_geo* d_geo = nullptr;  size_t geo_cap = 0;         // the table of its segments [n_geo]
-  double* d_win[5] = {};  size_t win_cap[5] = {};              // the pass, per row [F][n_rows]: min, max, mean, EMA, EMA partial sums
-  uint32_t* d_win_nover = nullptr;  size_t win_nover_cap = 0;  //   and n_over
-  uint4* d_cls = nullptr;  size_t cls_cap = 0;                  // sampled pass: per-row class counts [F][n_rows]
-  unsigned long long* d_lists = nullptr;  size_t lists_cap = 0; // sampled pass: the keys between the pivots [F][list_row]
-  double* d_piv = nullptr;  size_t piv_cap = 0;                 // sampled pass: pivots [segments][2] lo, hi
-  unsigned* d_fill = nullptr;  size_t fill_cap = 0;             // sampled pass: list fill counters [segments]
-  double* d_out = nullptr;  size_t out_cap = 0;                 // the select's result [5][segments]
-  uint32_t* d_nover = nullptr;  size_t nover_cap = 0;           //   and n_over [segments]
-  SelState* d_st = nullptr;  size_t st_cap = 0;                 // radix select state [segments]
-  unsigned* d_open = nullptr;  size_t open_cap = 0;             // [0] = number of segments left open by k_range_finish, [1..] = their ids
-  unsigned* d_hist = nullptr;  size_t hist_cap = 0;             // radix select: digit histograms [segments selected][kBins]
-  unsigned long long* d_cand = nullptr;  size_t cand_cap = 0;   // radix select: candidate lists [segments selected][kCollectMax]
-  int64_t* d_p0 = nullptr;  size_t p0_cap = 0;                  // sets of several ranges: each entry's first piece [n_geo]
-  cudaEvent_t ev[3] = {};         // before the pivots / after the pass and carry / after the finish
+  gpud_buf<gpud_range_geo> d_geo;        // the table of its segments [n_geo]
+  gpud_buf<double> d_win[5];             // the pass, per row [F][n_rows]: min, max, mean, EMA, EMA partial sums
+  gpud_buf<uint32_t> d_win_nover;        //   and n_over
+  gpud_buf<uint4> d_cls;                 // sampled pass: per-row class counts [F][n_rows]
+  gpud_buf<unsigned long long> d_lists;  // sampled pass: the keys between the pivots [F][list_row]
+  gpud_buf<double> d_piv;                // sampled pass: pivots [segments][2] lo, hi
+  gpud_buf<unsigned> d_fill;             // sampled pass: list fill counters [segments]
+  gpud_buf<double> d_out;                // the select's result [5][segments]
+  gpud_buf<uint32_t> d_nover;            //   and n_over [segments]
+  gpud_buf<SelState> d_st;               // radix select state [segments]
+  gpud_buf<unsigned> d_open;             // [0] = number of segments left open by k_range_finish, [1..] = their ids
+  gpud_buf<unsigned> d_hist;             // radix select: digit histograms [segments selected][kBins]
+  gpud_buf<unsigned long long> d_cand;   // radix select: candidate lists [segments selected][kCollectMax]
+  gpud_buf<int64_t> d_p0;                // sets of several ranges: each entry's first piece [n_geo]
+  gpud_event ev[3];                      // before the pivots / after the pass and carry / after the finish
   bool timed = false;             // the last select was sampled (and ran to the end)
   int reasons[GPUD_RANGE_N_OPEN_REASONS] = {};   // its open segments by reason
   int fields_open = 0;            // segments it handed to the radix select
@@ -120,15 +120,15 @@ int32_t ranges_plan(gpud_ctx* ctx, const int64_t* totals, int n_rings, const int
 
 // Everything gpud_ring_reduce_ranges / _range_sets keep between calls (gpud_ring::ranges), grown on demand.
 struct gpud_ranges_state {
-  gpud_range_state* seg = nullptr;                              // the long route's segment select (apart from gpud_ring_reduce_range's)
-  gpud_short_range* d_short = nullptr;  size_t short_cap = 0;
-  gpud_piece* d_pieces = nullptr;  size_t pieces_cap = 0;       // the call's piece table
-  gpud_ring_src* d_srcs = nullptr;  size_t srcs_cap = 0;        // ... and ring table (internal.h)
-  int32_t* d_tile = nullptr;  size_t tile_cap = 0;              // the long set of each tile of one batch
-  int64_t* d_tile_piece = nullptr;  size_t tile_piece_cap = 0;  // ... and the piece of its first sample (sets of several ranges)
-  double* d_out = nullptr;  size_t out_cap = 0;                 // the call's result [5][F][n_sets]
-  uint32_t* d_nover = nullptr;  size_t nover_cap = 0;           //   and n_over [F][n_sets]
-  cudaEvent_t ev[2] = {};
+  std::unique_ptr<gpud_range_state> seg;  // the long route's segment select (apart from gpud_ring_reduce_range's)
+  gpud_buf<gpud_short_range> d_short;
+  gpud_buf<gpud_piece> d_pieces;          // the call's piece table
+  gpud_buf<gpud_ring_src> d_srcs;         // ... and ring table (internal.h)
+  gpud_buf<int32_t> d_tile;               // the long set of each tile of one batch
+  gpud_buf<int64_t> d_tile_piece;         // ... and the piece of its first sample (sets of several ranges)
+  gpud_buf<double> d_out;                 // the call's result [5][F][n_sets]
+  gpud_buf<uint32_t> d_nover;             //   and n_over [F][n_sets]
+  gpud_event ev[2];
   bool timed = false;
   bool seg_last = false;          // seg holds the last batch of the last call (that call had a long set)
   int64_t open = 0;
@@ -136,14 +136,14 @@ struct gpud_ranges_state {
   // The virtual box of a call that reaches a tier (ranges.cu, DESIGN.md §2 "Tier"): its slots' samples [slots][G][vcap] and sample
   // rings [slots][G][smp_slots], the tier rows to decode and their directories and block offsets, the ring runs to copy, the decode's
   // unread field sums, and events around each group's decode.
-  double* d_vring = nullptr;  size_t vring_cap = 0;
-  double* d_vsmp = nullptr;  size_t vsmp_cap = 0;
-  int64_t* d_rows = nullptr;  size_t rows_cap = 0;
-  uint8_t* d_vdir = nullptr;  size_t vdir_cap = 0;
-  unsigned long long* d_voffs = nullptr;  size_t voffs_cap = 0;
-  gpud_tier_run* d_runs = nullptr;  size_t runs_cap = 0;
-  unsigned long long* d_vsum = nullptr;  size_t vsum_cap = 0;
-  cudaEvent_t ev_dec[2] = {};
+  gpud_buf<double> d_vring;
+  gpud_buf<double> d_vsmp;
+  gpud_buf<int64_t> d_rows;
+  gpud_buf<uint8_t> d_vdir;
+  gpud_buf<unsigned long long> d_voffs;
+  gpud_buf<gpud_tier_run> d_runs;
+  gpud_buf<unsigned long long> d_vsum;
+  gpud_event ev_dec[2];
 };
 
 // The ring table of a call: slot k's samples and sample ring (slot 0: the view's own, which the table's entry 0 need not repeat) and
@@ -159,12 +159,12 @@ struct RingTable {
 RingTable ring_table(gpud_ring* const* rings, int n_rings);
 
 // The sets of a call over table t (slot 0 the view v's ring), into out_f64 [5][F][n_sets] / out_n_over [F][n_sets], on the scratch
-// *state (created on first use).  ranges.cu says the rest.
+// `state` (created on first use).  ranges.cu says the rest.
 int32_t reduce_sets(const gpud_ring_view& v, const RingTable& t, const int32_t* ring_of, const int64_t* first, const int64_t* len, int64_t n_ranges,
-                    const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over, gpud_ranges_state** state);
-// The sets ids[] of a call (set_off NULL: every range a set) reduced as a call of their own over v and table t, on *state: range i in
+                    const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over, std::unique_ptr<gpud_ranges_state>& state);
+// The sets ids[] of a call (set_off NULL: every range a set) reduced as a call of their own over v and table t, on `state`: range i in
 // slot ring_of[i] (ring_of NULL: all in slot 0) from sample first[i], len[i] samples, into f64 [5][F][ids] / nov [F][ids].
 int32_t reduce_subset(const gpud_ring_view& v, const RingTable& t, const std::vector<int64_t>& ids, const int32_t* ring_of, const int64_t* first,
-                      const int64_t* len, const int64_t* set_off, gpud_ranges_state** state, std::vector<double>& f64, std::vector<uint32_t>& nov);
+                      const int64_t* len, const int64_t* set_off, std::unique_ptr<gpud_ranges_state>& state, std::vector<double>& f64, std::vector<uint32_t>& nov);
 // The results of a select's n_long segments (s->d_out [5][F n_long], s->d_nover) into columns geo[j].id of out [5][F][n_out] / nover [F][n_out].
 cudaError_t ranges_scatter(const gpud_ring_view& v, const gpud_range_state* s, int64_t n_long, int64_t n_out, double* out, uint32_t* nover);

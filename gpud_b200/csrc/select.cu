@@ -506,34 +506,25 @@ __global__ void __launch_bounds__(kSelThreads) k_sel_final(const SelState* __res
 }
 
 }  // namespace
-void gpud_range_state_free(gpud_range_state* s) {
-  if (!s) return;
-  for (auto* p : s->d_win) cudaFree(p);
-  cudaFree(s->d_geo); cudaFree(s->d_win_nover); cudaFree(s->d_cls); cudaFree(s->d_lists); cudaFree(s->d_piv); cudaFree(s->d_fill);
-  cudaFree(s->d_out); cudaFree(s->d_nover); cudaFree(s->d_st); cudaFree(s->d_open); cudaFree(s->d_hist); cudaFree(s->d_cand); cudaFree(s->d_p0);
-  for (auto& ev : s->ev) if (ev) cudaEventDestroy(ev);
-  delete s;
-}
-
 // ---- the stages of a segment select (segsel.h says what goes in and out) ----------------------------------------------------------
 cudaError_t sel_reserve(const gpud_ring_view& v, gpud_range_state* s, const gpud_range_geo* geo, int64_t n_geo, int64_t rows, int64_t list_row,
                         bool sampled, const int64_t* seg_p0) {
   const int64_t n_segs = (int64_t)v.F * n_geo;
   const size_t per = (size_t)v.F * rows;
-  cudaError_t e = gpud_grow(&s->d_geo, &s->geo_cap, (size_t)n_geo);
-  for (int i = 0; i < 5 && e == cudaSuccess; ++i) e = gpud_grow(&s->d_win[i], &s->win_cap[i], per);
-  if (e == cudaSuccess) e = gpud_grow(&s->d_win_nover, &s->win_nover_cap, per);
+  cudaError_t e = s->d_geo.grow((size_t)n_geo);
+  for (int i = 0; i < 5 && e == cudaSuccess; ++i) e = s->d_win[i].grow(per);
+  if (e == cudaSuccess) e = s->d_win_nover.grow(per);
   if (e == cudaSuccess && sampled) {
-    e = gpud_grow(&s->d_cls, &s->cls_cap, per);
-    if (e == cudaSuccess) e = gpud_grow(&s->d_lists, &s->lists_cap, (size_t)v.F * list_row);
-    if (e == cudaSuccess) e = gpud_grow(&s->d_piv, &s->piv_cap, 2 * (size_t)n_segs);
-    if (e == cudaSuccess) e = gpud_grow(&s->d_fill, &s->fill_cap, (size_t)n_segs);
+    e = s->d_cls.grow(per);
+    if (e == cudaSuccess) e = s->d_lists.grow((size_t)v.F * list_row);
+    if (e == cudaSuccess) e = s->d_piv.grow(2 * (size_t)n_segs);
+    if (e == cudaSuccess) e = s->d_fill.grow((size_t)n_segs);
   }
-  if (e == cudaSuccess) e = gpud_grow(&s->d_out, &s->out_cap, 5 * (size_t)n_segs);
-  if (e == cudaSuccess) e = gpud_grow(&s->d_nover, &s->nover_cap, (size_t)n_segs);
-  if (e == cudaSuccess) e = gpud_grow(&s->d_st, &s->st_cap, (size_t)n_segs);
-  if (e == cudaSuccess) e = gpud_grow(&s->d_open, &s->open_cap, 1 + (size_t)n_segs);
-  if (e == cudaSuccess && seg_p0) e = gpud_grow(&s->d_p0, &s->p0_cap, (size_t)n_geo);
+  if (e == cudaSuccess) e = s->d_out.grow(5 * (size_t)n_segs);
+  if (e == cudaSuccess) e = s->d_nover.grow((size_t)n_segs);
+  if (e == cudaSuccess) e = s->d_st.grow((size_t)n_segs);
+  if (e == cudaSuccess) e = s->d_open.grow(1 + (size_t)n_segs);
+  if (e == cudaSuccess && seg_p0) e = s->d_p0.grow((size_t)n_geo);
   if (e != cudaSuccess) return e;
   s->n_segs = n_segs;
   s->n_rows = (int64_t)per;
@@ -563,8 +554,8 @@ cudaError_t sel_finish(const gpud_ring_view& v, gpud_range_state* s, int64_t n_g
   s->fields_open = 0;
   if (ids) ids->clear();
   k_range_finish<<<(unsigned)n_segs, kSelThreads, 0, stream>>>((int)n_segs, Wp, s->d_geo, n_geo, rows, list_row, s->d_win[0], s->d_win[1], s->d_win[2],
-                                                              ema ? s->d_win[3] : nullptr, s->d_win_nover, sampled ? 1 : 0, sampled ? s->d_piv : nullptr,
-                                                              sampled ? s->d_fill : nullptr, sampled ? s->d_cls : nullptr, sampled ? s->d_lists : nullptr,
+                                                              ema ? s->d_win[3].get() : nullptr, s->d_win_nover, sampled ? 1 : 0, sampled ? s->d_piv.get() : nullptr,
+                                                              sampled ? s->d_fill.get() : nullptr, sampled ? s->d_cls.get() : nullptr, sampled ? s->d_lists.get() : nullptr,
                                                               s->d_out, s->d_nover, s->d_st, s->d_open, reinterpret_cast<int*>(s->d_open + 1));
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess && done) e = cudaEventRecord(done, stream);
@@ -594,8 +585,8 @@ cudaError_t sel_finish(const gpud_ring_view& v, gpud_range_state* s, int64_t n_g
 }
 
 cudaError_t sel_radix_reserve(gpud_range_state* s, int n_sel) {
-  const cudaError_t e = gpud_grow(&s->d_hist, &s->hist_cap, (size_t)n_sel * kBins);
-  return e == cudaSuccess ? gpud_grow(&s->d_cand, &s->cand_cap, (size_t)n_sel * kCollectMax) : e;
+  const cudaError_t e = s->d_hist.grow((size_t)n_sel * kBins);
+  return e == cudaSuccess ? s->d_cand.grow((size_t)n_sel * kCollectMax) : e;
 }
 
 // the radix select's blocks per segment: enough CTAs to fill the machine a few times over, each streaming >= 16 Ki keys
@@ -694,16 +685,16 @@ int32_t run_select(const gpud_ring_view& v, gpud_ring* ring, gpud_range_state* s
 
   GPUD_CUDA(ctx, cudaSetDevice(v.dev));
   s->timed = false;                    // until this select has run to the end: a failed grow may free the last one's scratch
-  for (auto& ev : s->ev) if (!ev) GPUD_CUDA(ctx, cudaEventCreate(&ev));
+  for (auto& ev : s->ev) GPUD_CUDA(ctx, ev.make());
   cudaError_t e = sel_reserve(v, s, geo, n_geo, rows, list_row, sampled, d_pieces ? seg_p0 : nullptr);
-  const int64_t* d_p0 = d_pieces ? s->d_p0 : nullptr;
+  const int64_t* d_p0 = d_pieces ? s->d_p0.get() : nullptr;
   if (e == cudaSuccess) e = cudaEventRecord(s->ev[0], stream);
   if (e == cudaSuccess && sampled) e = sel_pivots(v, s, geo, n_geo, s->d_fill, d_pieces, d_p0, d_srcs);
-  const double* piv = sampled ? s->d_piv : nullptr;
-  unsigned* fill = sampled ? s->d_fill : nullptr;
-  uint4* cls = sampled ? s->d_cls : nullptr;
-  unsigned long long* lists = sampled ? s->d_lists : nullptr;
-  double* const w[5] = {s->d_win[0], s->d_win[1], s->d_win[2], ema ? s->d_win[3] : nullptr, s->d_win[4]};
+  const double* piv = sampled ? s->d_piv.get() : nullptr;
+  unsigned* fill = sampled ? s->d_fill.get() : nullptr;
+  uint4* cls = sampled ? s->d_cls.get() : nullptr;
+  unsigned long long* lists = sampled ? s->d_lists.get() : nullptr;
+  double* const w[5] = {s->d_win[0], s->d_win[1], s->d_win[2], ema ? s->d_win[3].get() : nullptr, s->d_win[4]};
   if (e == cudaSuccess && d_tile) {
     e = gpud_ranges_tiles(v, s->d_geo, n_geo, d_tile, rows, piv, w, s->d_win_nover, cls, lists, list_row, fill, d_pieces, d_p0, d_tile_piece, d_srcs);
     if (e == cudaSuccess && ema) e = gpud_ranges_ema(v, s->d_geo, n_geo, w[4], rows, w[3], d_pieces, d_p0, d_srcs);
@@ -739,9 +730,9 @@ extern "C" int32_t gpud_ring_reduce_range(gpud_ring* ring, int64_t last_n, doubl
   g.smp = (g.n >> ring->smp_shift) >= 2048;
   g.lcap = (unsigned)std::min<int64_t>(kListCap, g.n);
   const bool sampled = g.n >= kSampledMin;
-  if (!ring->range) ring->range = new gpud_range_state();
-  const gpud_range_state* s = ring->range;
-  { int32_t rc = run_select(gpud_view(ring), ring, ring->range, &g, 1, (int)std::min<int64_t>(GPUD_MAX_WINDOW, g.n), sampled, true, nullptr, out_f64, out_n_over); if (rc) return rc; }
+  if (!ring->range) ring->range = std::make_unique<gpud_range_state>();
+  const gpud_range_state* s = ring->range.get();
+  { int32_t rc = run_select(gpud_view(ring), ring, ring->range.get(), &g, 1, (int)std::min<int64_t>(GPUD_MAX_WINDOW, g.n), sampled, true, nullptr, out_f64, out_n_over); if (rc) return rc; }
   // what the select's synchronisation did not bring: every result of an unsampled call, the p99 of the fields the radix select took
   const size_t F = (size_t)ring->F;
   cudaError_t e = cudaSuccess;
@@ -758,7 +749,7 @@ extern "C" int32_t gpud_ring_reduce_range(gpud_ring* ring, int64_t last_n, doubl
 
 // Stream windows of L = seg_len > GPUD_MAX_WINDOW samples (internal.h): one sampled select over n_seg segments per field, each under
 // the rule of seg_sample, at the rows, lists, pivots and fill counters the window kernel's seg_sub mapping gives it.
-int32_t gpud_ring_segments(gpud_ring* r, gpud_range_state** st, int64_t start, int64_t seg_len, int64_t n_seg, int Wp, gpud_seg_out* out) {
+int32_t gpud_ring_segments(gpud_ring* r, std::unique_ptr<gpud_range_state>& st, int64_t start, int64_t seg_len, int64_t n_seg, int Wp, gpud_seg_out* out) {
   gpud_range_geo g{};
   g.n = seg_len;
   g.k = gpud_rank_from_top(seg_len, r->q_num, r->q_den);
@@ -769,8 +760,8 @@ int32_t gpud_ring_segments(gpud_ring* r, gpud_range_state** st, int64_t start, i
     geo[j].tile0 = j * (seg_len / Wp);
     geo[j].list0 = j * (int64_t)g.lcap;
   }
-  if (!*st) *st = new gpud_range_state();
-  gpud_range_state* s = *st;
+  if (!st) st = std::make_unique<gpud_range_state>();
+  gpud_range_state* s = st.get();
   { int32_t rc = run_select(gpud_view(r), r, s, geo.data(), n_seg, Wp, true, false, nullptr, nullptr, nullptr); if (rc) return rc; }
   out->out = s->d_out;
   out->nover = s->d_nover;
@@ -782,7 +773,7 @@ int32_t gpud_ring_segments(gpud_ring* r, gpud_range_state** st, int64_t start, i
 
 extern "C" int32_t gpud_ring_range_stats(gpud_ring* r, float* pass_ms, float* total_ms, int32_t* fields_by_histogram, int32_t* reasons) {
   if (!r || !pass_ms || !total_ms || !fields_by_histogram) return GPUD_E_INVALID;
-  const gpud_range_state* s = r->range;
+  const gpud_range_state* s = r->range.get();
   if (!s || !s->timed) return gpud_fail(r->ctx, GPUD_E_STATE, "the last reduce_range (if any) did not take the sampled single pass");
   GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
   GPUD_CUDA(r->ctx, cudaEventSynchronize(s->ev[2]));
@@ -797,7 +788,7 @@ extern "C" int32_t gpud_ring_range_stats(gpud_ring* r, float* pass_ms, float* to
 // its list fill counter (which may exceed the list's capacity) and, when cls is given, its per-window class counts.
 extern "C" int32_t gpudh_ring_range_scratch(gpud_ring* r, double* piv, uint32_t* fill, uint32_t* cls, int64_t* nw) {
   if (!r || !piv || !fill || !nw) return GPUD_E_INVALID;
-  const gpud_range_state* s = r->range;
+  const gpud_range_state* s = r->range.get();
   if (!s || !s->timed) return gpud_fail(r->ctx, GPUD_E_STATE, "the last reduce_range (if any) did not take the sampled single pass");
   const size_t F = (size_t)r->F;
   GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));

@@ -146,18 +146,19 @@ CkGeo rows_geo(int64_t F, int64_t n) {
 // uploads an identity row list and the table; run gathers rows [q0, q0 + m)'s directories and block offsets (k_tier_gather) and
 // decodes them with nothing stored (k_ckpt_unpack<false>), adding their field checksums into csum [F].
 struct RowCheck {
-  int64_t n = 0, *d_rows = nullptr;              // the identity row list [n], then the slot table [n][2]
-  uint8_t* d_dir = nullptr;
-  unsigned long long* d_offs = nullptr;
+  int64_t n = 0;
+  gpud_buf<int64_t> d_rows;               // the identity row list [n], then the slot table [n][2]
+  gpud_buf<uint8_t> d_dir;
+  gpud_buf<unsigned long long> d_offs;
 
-  int32_t init(gpud_ring* r, CallScratch& sc, const std::vector<int64_t>& slot, const char* what) {
+  int32_t init(gpud_ring* r, const std::vector<int64_t>& slot, const char* what) {
     n = (int64_t)slot.size() / 2;
     std::vector<int64_t> rows(n);
     for (int64_t q = 0; q < n; ++q) rows[q] = q;
     rows.insert(rows.end(), slot.begin(), slot.end());
-    cudaError_t e = sc.alloc(&d_rows, 3 * n);
-    if (e == cudaSuccess) e = sc.alloc(&d_dir, r->F * n);
-    if (e == cudaSuccess) e = sc.alloc(&d_offs, r->F * n);
+    cudaError_t e = d_rows.alloc(3 * n);
+    if (e == cudaSuccess) e = d_dir.alloc(r->F * n);
+    if (e == cudaSuccess) e = d_offs.alloc(r->F * n);
     if (e != cudaSuccess) return scratch_fail(r, e, what);
     if (n > 0) GPUD_CUDA(r->ctx, cudaMemcpyAsync(d_rows, rows.data(), 24 * n, cudaMemcpyHostToDevice, r->stream));
     return GPUD_OK;
@@ -222,14 +223,6 @@ cudaError_t launch_copy(const gpud_ring* r, const TierCopy* rows, int64_t n_rows
 
 }  // namespace
 
-void gpud_tier_free(gpud_tier* t) {
-  if (!t) return;
-  cudaFree(t->d_buf); cudaFree(t->d_slot); cudaFree(t->d_ctl); cudaFree(t->d_dir); cudaFree(t->d_words); cudaFree(t->d_offs); cudaFree(t->d_csum);
-  cudaFree(t->d_rowsz);
-  for (auto& e : t->ev_enc) if (e) cudaEventDestroy(e);
-  delete t;
-}
-
 // The rows the tier can hold at most: every row at least its record and F anchors.
 static int64_t tier_slots(int64_t B, int64_t F) { return B / (tier_rec_bytes(F) + 8 * F) + 1; }
 // The largest row: its record and every block coded at 64 bits.
@@ -254,7 +247,7 @@ static int32_t tier_encode(gpud_ring* r, gpud_tier* t, int64_t row0, int64_t nb,
 }
 
 int32_t gpud_tier_push(gpud_ring* r) {
-  gpud_tier* t = r->tier;
+  gpud_tier* t = r->tier.get();
   bool clear = false;
   const int64_t row0 = tier_loss(&t->next, &t->lost, &clear, r->total, r->cap);
   if (row0 == t->next && !clear) return GPUD_OK;
@@ -271,7 +264,7 @@ int32_t gpud_tier_read_ctl(gpud_ring* r, gpud_tier_ctl* c) {
 cudaError_t gpud_tier_decode(const gpud_ring* h, const gpud_ring* o, const int64_t* d_rows, int64_t n, int f0, int G, const gpud_vslot& s,
                              int64_t vcol0, uint8_t* dir, unsigned long long* offs, unsigned long long* csum) {
   if (n == 0) return cudaSuccess;
-  const gpud_tier* t = o->tier;
+  const gpud_tier* t = o->tier.get();
   // the gather and the unpack run on h; every ring of a call has h's F, so o's records have h's layout
   const cudaError_t e = launch_gather(h, d_rows, n, f0, G, t->d_buf, t->d_slot, t->slots, dir, offs);
   if (e != cudaSuccess) return e;
@@ -300,30 +293,30 @@ static int32_t tier_size_ok(gpud_ctx* ctx, int64_t cap, int64_t F, int64_t tier_
 }
 
 // A tier of tier_bytes for the ring, its control word set to c0; nothing is placed or encoded.  On failure nothing stays allocated.
-static int32_t tier_new(gpud_ring* r, int64_t tier_bytes, const gpud_tier_ctl& c0, gpud_tier** out, const char* what) {
+static int32_t tier_new(gpud_ring* r, int64_t tier_bytes, const gpud_tier_ctl& c0, std::unique_ptr<gpud_tier>* out, const char* what) {
   const int64_t F = r->F, B = tier_bytes & ~(int64_t)7;
-  gpud_tier* t = new gpud_tier();
+  auto t = std::make_unique<gpud_tier>();
   t->bytes = B;
   t->rec_bytes = tier_rec_bytes(F);
   t->slots = tier_slots(B, F);
   t->units_cap = F * (r->cap / kBlock + 1);
-  cudaError_t e = cudaMalloc(&t->d_buf, (size_t)(B + tier_row_max(F)));
-  if (e == cudaSuccess) e = cudaMalloc(&t->d_slot, (size_t)t->slots * 2 * sizeof(int64_t));
-  if (e == cudaSuccess) e = cudaMalloc(&t->d_ctl, sizeof(gpud_tier_ctl));
-  if (e == cudaSuccess) e = cudaMalloc(&t->d_dir, (size_t)t->units_cap);
-  if (e == cudaSuccess) e = cudaMalloc(&t->d_words, (size_t)t->units_cap * 8);
-  if (e == cudaSuccess) e = cudaMalloc(&t->d_offs, (size_t)t->units_cap * 8);
-  if (e == cudaSuccess) e = cudaMalloc(&t->d_csum, (size_t)F * 8);
-  if (e == cudaSuccess) e = cudaMalloc(&t->d_rowsz, (size_t)(r->cap / kBlock + 1) * 8);
-  for (int i = 0; i < 2 && e == cudaSuccess; ++i) e = cudaEventCreate(&t->ev_enc[i]);
+  cudaError_t e = t->d_buf.alloc((size_t)(B + tier_row_max(F)) / 8);
+  if (e == cudaSuccess) e = t->d_slot.alloc((size_t)t->slots * 2);
+  if (e == cudaSuccess) e = t->d_ctl.alloc(1);
+  if (e == cudaSuccess) e = t->d_dir.alloc((size_t)t->units_cap);
+  if (e == cudaSuccess) e = t->d_words.alloc((size_t)t->units_cap);
+  if (e == cudaSuccess) e = t->d_offs.alloc((size_t)t->units_cap);
+  if (e == cudaSuccess) e = t->d_csum.alloc((size_t)F);
+  if (e == cudaSuccess) e = t->d_rowsz.alloc((size_t)(r->cap / kBlock + 1));
+  for (int i = 0; i < 2 && e == cudaSuccess; ++i) e = t->ev_enc[i].make();
   if (e == cudaSuccess) e = cudaMemcpyAsync(t->d_ctl, &c0, sizeof c0, cudaMemcpyHostToDevice, r->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(r->stream);
   if (e != cudaSuccess) {
-    gpud_tier_free(t);
+    t.reset();
     cudaGetLastError();
     return scratch_fail(r, e, what);
   }
-  *out = t;
+  *out = std::move(t);
   return GPUD_OK;
 }
 
@@ -334,10 +327,10 @@ extern "C" int32_t gpud_ring_tier_open(gpud_ring* r, int64_t tier_bytes) {
   GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
   // the tier starts at the first row wholly in the ring: the rows the ring already completed are encoded now, as a push would
   const int64_t whole = first_whole_row(r->total, r->cap);
-  gpud_tier* t = nullptr;
+  std::unique_ptr<gpud_tier> t;
   { const int32_t rc = tier_new(r, tier_bytes, gpud_tier_ctl{whole, whole, 0, 0, 0, 0, 0, 0}, &t, "tier_open"); if (rc) return rc; }
   t->next = whole;
-  r->tier = t;
+  r->tier = std::move(t);
   return gpud_tier_push(r);
 }
 
@@ -355,7 +348,7 @@ extern "C" int32_t gpud_ring_tier_counts(gpud_ring* r, int64_t* first_sample, in
 
 extern "C" int32_t gpud_ring_tier_stats(gpud_ring* r, float* encode_ms, float* decode_ms, int64_t* blocks_by_mode) {
   if (!r) return GPUD_E_INVALID;
-  gpud_tier* t = r->tier;
+  gpud_tier* t = r->tier.get();
   if (!t) return gpud_fail(r->ctx, GPUD_E_STATE, "tier_stats: the ring has no tier");
   gpud_tier_ctl c;
   { const int32_t rc = gpud_tier_read_ctl(r, &c); if (rc) return rc; }
@@ -370,7 +363,7 @@ extern "C" int32_t gpud_ring_tier_stats(gpud_ring* r, float* encode_ms, float* d
 // Test hooks (include/gpud_b200_hooks.h).
 extern "C" int32_t gpudh_ring_tier_row(gpud_ring* r, int64_t row, void* out, int64_t cap, int64_t* n_bytes) {
   if (!r || !n_bytes || cap < 0 || (cap > 0 && !out)) return GPUD_E_INVALID;
-  gpud_tier* t = r->tier;
+  gpud_tier* t = r->tier.get();
   if (!t) return gpud_fail(r->ctx, GPUD_E_STATE, "the ring has no tier");
   gpud_tier_ctl c;
   { const int32_t rc = gpud_tier_read_ctl(r, &c); if (rc) return rc; }
@@ -380,7 +373,7 @@ extern "C" int32_t gpudh_ring_tier_row(gpud_ring* r, int64_t row, void* out, int
   GPUD_CUDA(r->ctx, cudaMemcpy(s, t->d_slot + 2 * (row % t->slots), sizeof s, cudaMemcpyDeviceToHost));
   *n_bytes = s[1];
   if (cap < s[1]) return GPUD_E_CAPACITY;
-  GPUD_CUDA(r->ctx, cudaMemcpy(out, reinterpret_cast<const uint8_t*>(t->d_buf) + s[0], s[1], cudaMemcpyDeviceToHost));
+  GPUD_CUDA(r->ctx, cudaMemcpy(out, reinterpret_cast<const uint8_t*>(t->d_buf.get()) + s[0], s[1], cudaMemcpyDeviceToHost));
   return GPUD_OK;
 }
 
@@ -446,7 +439,7 @@ struct TierSpan {
 };
 
 int32_t tier_span_of(gpud_ring* r, bool delta, TierSpan* s, const char* what) {
-  gpud_tier* t = r->tier;
+  gpud_tier* t = r->tier.get();
   if (!t) return gpud_fail(r->ctx, GPUD_E_STATE, "%s: the ring has no tier", what);
   if (delta && !t->ck_marked)
     return gpud_fail(r->ctx, GPUD_E_STATE, "%s: no tier checkpoint written or restored on this ring yet: write a full tier checkpoint", what);
@@ -488,7 +481,7 @@ int32_t write_tier_blob(gpud_ring* r, bool delta, void* out_v, int64_t cap, int6
   const char* what = delta ? "tier_checkpoint_delta" : "tier_checkpoint";
   TierSpan s;
   { const int32_t rc = tier_span_of(r, delta, &s, what); if (rc) return rc; }
-  gpud_tier* t = r->tier;
+  gpud_tier* t = r->tier.get();
   const int64_t F = r->F, n = s.next - s.from, size = kHeaderBytes + s.rows_len + 8 * F;
   *n_bytes = size;
   if (cap < size) return gpud_fail(r->ctx, GPUD_E_CAPACITY, "%s needs %lld bytes", what, (long long)size);
@@ -496,21 +489,20 @@ int32_t write_tier_blob(gpud_ring* r, bool delta, void* out_v, int64_t cap, int6
   { const int32_t rc = host_pinned(r, out, &pinned); if (rc) return rc; }
   std::vector<uint64_t> csum(F, 0);
   float ms = 0.f;
-  CallScratch sc;
-  unsigned long long *d_rows_sec = nullptr, *d_csum = nullptr;
   if (n > 0) {
     // the check pass's slot table: row j (numbered from 0) at its section offset
     std::vector<int64_t> slot;
     for (const TierCopy& c : s.rows) slot.insert(slot.end(), {c.dst, c.n});
-    TierCopy* d_copy = nullptr;
+    gpud_buf<unsigned long long> d_rows_sec, d_csum;
+    gpud_buf<TierCopy> d_copy;
     RowCheck check;
-    cudaEvent_t ev[2];
-    cudaError_t e = sc.alloc(&d_rows_sec, s.rows_len / 8);
-    if (e == cudaSuccess) e = sc.alloc(&d_copy, n);
-    if (e == cudaSuccess) e = sc.alloc(&d_csum, F);
-    for (int i = 0; i < 2 && e == cudaSuccess; ++i) e = sc.event(&ev[i]);
+    gpud_event ev[2];
+    cudaError_t e = d_rows_sec.alloc(s.rows_len / 8);
+    if (e == cudaSuccess) e = d_copy.alloc(n);
+    if (e == cudaSuccess) e = d_csum.alloc(F);
+    for (int i = 0; i < 2 && e == cudaSuccess; ++i) e = ev[i].make();
     if (e != cudaSuccess) return scratch_fail(r, e, what);
-    { const int32_t rc = check.init(r, sc, slot, what); if (rc) return rc; }
+    { const int32_t rc = check.init(r, slot, what); if (rc) return rc; }
     GPUD_CUDA(r->ctx, cudaMemcpyAsync(d_copy, s.rows.data(), n * sizeof(TierCopy), cudaMemcpyHostToDevice, r->stream));
     GPUD_CUDA(r->ctx, cudaMemsetAsync(d_csum, 0, F * 8, r->stream));
     GPUD_CUDA(r->ctx, cudaEventRecord(ev[0], r->stream));
@@ -698,19 +690,18 @@ extern "C" int32_t gpud_ring_tier_restore(gpud_ring* r, int64_t tier_bytes, cons
   // the rows held by both the chain and the ring: [ov0, last next), staged rows q_ov.. of the last blobs
   const int64_t ov0 = std::max(p.whole, last.first), n_ov = last.next - ov0;
   const int64_t q_ov = n_ov > 0 ? p.staged[ov0 - last.first] : 0;
-  CallScratch sc;
   RowCheck check;
-  unsigned long long *d_stage = nullptr, *d_csum = nullptr;
-  cudaEvent_t ev[4];
-  cudaError_t e = sc.alloc(&d_stage, stage_bytes_all / 8);
-  if (e == cudaSuccess) e = sc.alloc(&d_csum, F * (n_blobs + 2));
-  for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = sc.event(&ev[i]);
+  gpud_buf<unsigned long long> d_stage, d_csum;
+  gpud_event ev[4];
+  cudaError_t e = d_stage.alloc(stage_bytes_all / 8);
+  if (e == cudaSuccess) e = d_csum.alloc(F * (n_blobs + 2));
+  for (int i = 0; i < 4 && e == cudaSuccess; ++i) e = ev[i].make();
   if (e != cudaSuccess) return scratch_fail(r, e, what);
-  { const int32_t rc = check.init(r, sc, sslot, what); if (rc) return rc; }
+  { const int32_t rc = check.init(r, sslot, what); if (rc) return rc; }
   for (int32_t i = 0; i < n_blobs; ++i) {
     bool pinned = false;
     { const int32_t rc = host_pinned(r, p.blobs[i].rows, &pinned); if (rc) return rc; }
-    { const int32_t rc = copy_in(r, (uint8_t*)d_stage + blob_at[i], p.blobs[i].rows, (size_t)p.blobs[i].rows_len, pinned); if (rc) return rc; }
+    { const int32_t rc = copy_in(r, (uint8_t*)d_stage.get() + blob_at[i], p.blobs[i].rows, (size_t)p.blobs[i].rows_len, pinned); if (rc) return rc; }
   }
   GPUD_CUDA(r->ctx, cudaMemsetAsync(d_csum, 0, F * (n_blobs + 2) * 8, r->stream));
   // the check pass: each blob's rows decoded against its checksums, and the rows the ring also holds decoded and re-encoded from it
@@ -741,10 +732,10 @@ extern "C" int32_t gpud_ring_tier_restore(gpud_ring* r, int64_t tier_bytes, cons
     const int64_t a = k - last.first, q = p.staged[a];
     kept.push_back(TierCopy{sslot[2 * q], p.place[a], sslot[2 * q + 1]});
   }
-  TierCopy* d_kept = nullptr;
-  e = sc.alloc(&d_kept, kept.size());
+  gpud_buf<TierCopy> d_kept;
+  e = d_kept.alloc(kept.size());
   if (e != cudaSuccess) return scratch_fail(r, e, what);
-  gpud_tier* t = nullptr;
+  std::unique_ptr<gpud_tier> t;
   { const int32_t rc = tier_new(r, tier_bytes, p.c, &t, what); if (rc) return rc; }
   e = cudaMemcpyAsync(t->d_slot, p.slot.data(), p.slot.size() * 8, cudaMemcpyHostToDevice, r->stream);
   if (e == cudaSuccess && !kept.empty()) e = cudaMemcpyAsync(d_kept, kept.data(), kept.size() * sizeof(TierCopy), cudaMemcpyHostToDevice, r->stream);
@@ -753,10 +744,7 @@ extern "C" int32_t gpud_ring_tier_restore(gpud_ring* r, int64_t tier_bytes, cons
   if (e == cudaSuccess) e = cudaEventRecord(ev[3], r->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(r->stream);
   if (e == cudaSuccess) e = cudaEventElapsedTime(&ms_load, ev[2], ev[3]);
-  if (e != cudaSuccess) {
-    gpud_tier_free(t);
-    return gpud_fail(r->ctx, GPUD_E_CUDA, "%s: %s", what, cudaGetErrorString(e));
-  }
+  if (e != cudaSuccess) return gpud_fail(r->ctx, GPUD_E_CUDA, "%s: %s", what, cudaGetErrorString(e));
   t->next = last.next;
   t->lost = last.lost;
   t->ck_marked = true;
@@ -765,7 +753,7 @@ extern "C" int32_t gpud_ring_tier_restore(gpud_ring* r, int64_t tier_bytes, cons
   t->ck_timed = true;
   t->ck_decode_ms = ms_check + ms_load;
   t->ck_rows = (int64_t)kept.size();
-  r->tier = t;
+  r->tier = std::move(t);
   // rows [last next, total / 1024) from the ring, as the open encodes them
   return gpud_tier_push(r);
 }

@@ -169,6 +169,8 @@ int32_t gpudh_box_query_plan(int32_t n_ranks, const int64_t* totals, int64_t cap
 /* The pivots {lo, hi} of the last batch of long spread sets a finished box query reduced, [F][n_long] in the order of the sets: *n
  * = F x n_long.  GPUD_E_STATE when it reduced none, GPUD_E_CAPACITY when *n > cap. */
 int32_t gpudh_box_query_pivots(gpud_box_query* q, double* piv, int64_t cap, int64_t* n);
+/* The CUDA objects the library owns now: out[4] = {device buffers, pinned host buffers, events, streams}.  Host counters; no device call. */
+void gpudh_cuda_objects(int64_t out[4]);
 
 #ifdef __cplusplus
 }
