@@ -755,7 +755,7 @@ class FabricVerdict(C.Structure):
 SYMBOLS = ["gpud_abi_version", "gpud_sizeof", "gpud_ctx_create", "gpud_ctx_destroy", "gpud_last_error", "gpud_host_alloc",
            "gpud_host_free", "gpud_ring_create", "gpud_ring_destroy", "gpud_ring_set_stream", "gpud_ring_push",
            "gpud_ring_push_device", "gpud_ring_push_raw", "gpud_clock_event_reasons", "gpud_hw_slowdown_event_message", "gpud_hw_slowdown_check", "gpud_store_insert_hw_slowdown", "gpud_store_open", "gpud_store_close", "gpud_store_last_error", "gpud_store_event_table", "gpud_store_insert_event", "gpud_store_insert_xid_hits", "gpud_store_metrics_table", "gpud_store_record_metrics", "gpud_kmsg_syncer_create", "gpud_kmsg_syncer_destroy", "gpud_kmsg_syncer_feed", "gpud_store_find_event", "gpud_store_record_reboot", "gpud_xid_state_from_store", "gpud_sxid_state_from_store", "gpud_store_get_events", "gpud_store_latest_event", "gpud_store_purge_events", "gpud_kmsg_syncer_configure", "gpud_kmsg_syncer_configure_component", "gpud_kmsg_syncer_offer", "gpud_ib_scan", "gpud_ib_reason", "gpud_poller_create", "gpud_poller_destroy", "gpud_poller_poll", "gpud_poller_last_rows", "gpud_poller_errors", "gpud_poll_row_hold", "gpud_nvml_devices", "gpud_nvml_devices_arg", "gpud_nvml_bus_id", "gpud_poller_remapped_rows", "gpud_remapped_rows_check", "gpud_poller_ecc_errors", "gpud_poller_field_row", "gpud_poller_poll_fields", "gpud_poller_gpm_supported", "gpud_poller_gpm_metrics", "gpud_poller_poll_gpm", "gpud_gpm_check", "gpud_poller_fabric_raw", "gpud_poller_product_name", "gpud_poller_temperature", "gpud_temperature_check", "gpud_temperature_reason", "gpud_poller_counters", "gpud_ring_counts", "gpud_ring_reduce", "gpud_ring_sync", "gpud_ring_kernel_ms", "gpud_ring_read",
-           "gpud_ring_result_ptr", "gpud_ring_stream_open", "gpud_ring_stream_reduce", "gpud_ring_stream_counts", "gpud_ring_stream_read", "gpud_ring_windows_open", "gpud_ring_windows_open_hop", "gpud_ring_windows_close", "gpud_ring_windows_reduce", "gpud_ring_windows_counts", "gpud_ring_windows_read", "gpud_ring_windows_stats", "gpud_ring_reduce_range", "gpud_ring_range_stats", "gpud_ring_reduce_ranges", "gpud_ring_reduce_range_sets", "gpud_rings_reduce_range_sets", "gpud_ring_ranges_stats", "gpud_box_query_create", "gpud_box_query_step", "gpud_box_query_result", "gpud_box_query_stats", "gpud_box_query_destroy", "gpud_ring_set_cta_reserve", "gpud_kmsg_scan", "gpud_kmsg_scan_sharded", "gpud_kmsg_scan_device", "gpud_kmsg_scan_kernel_ms", "gpud_kmsg_scan_phase_timing", "gpud_kmsg_scan_stats", "gpud_xid_classify",
+           "gpud_ring_result_ptr", "gpud_ring_stream_open", "gpud_ring_stream_reduce", "gpud_ring_stream_counts", "gpud_ring_stream_read", "gpud_ring_windows_open", "gpud_ring_windows_open_hop", "gpud_ring_windows_close", "gpud_ring_windows_reduce", "gpud_ring_windows_counts", "gpud_ring_windows_read", "gpud_ring_windows_stats", "gpud_ring_reduce_range", "gpud_ring_range_stats", "gpud_ring_reduce_ranges", "gpud_ring_reduce_range_sets", "gpud_rings_reduce_range_sets", "gpud_rings_reduce_range_sets_fields", "gpud_ring_ranges_stats", "gpud_box_query_create", "gpud_box_query_step", "gpud_box_query_result", "gpud_box_query_stats", "gpud_box_query_destroy", "gpud_ring_set_cta_reserve", "gpud_kmsg_scan", "gpud_kmsg_scan_sharded", "gpud_kmsg_scan_device", "gpud_kmsg_scan_kernel_ms", "gpud_kmsg_scan_phase_timing", "gpud_kmsg_scan_stats", "gpud_xid_classify",
            "gpud_hit_detail_json", "gpud_xid_description", "gpud_xid_mnemonic", "gpud_sxid_name", "gpud_nvlink_rule_hint", "gpud_sxid_reason", "gpud_sxid_get_detail", "gpud_store_insert_sxid_hits", "gpud_product_mem_caps", "gpud_product_fm_supported", "gpud_product_fabric_state_supported", "gpud_xid_get_detail", "gpud_xid_detail", "gpud_xid_build_message", "gpud_xid_hit_message", "gpud_xid_device_matches_bus_id", "gpud_kmsg_event_name", "gpud_kmsg_event_message", "gpud_kmsg_component", "gpud_kmsg_hit_message", "gpud_kmsg_stateful_create", "gpud_kmsg_stateful_destroy", "gpud_kmsg_stateful_feed", "gpud_component_create", "gpud_component_destroy", "gpud_component_name", "gpud_component_start", "gpud_component_check", "gpud_component_last_health_states", "gpud_component_events", "gpud_component_close", "gpud_component_checks", "gpud_component_xid_set_source", "gpud_component_xid_set_healthy", "gpud_component_xid_add_reboot", "gpud_component_xid_set_devices", "gpud_component_ring", "gpud_kmsg_stateful_feed_units", "gpud_kmsg_deduper_create", "gpud_kmsg_deduper_destroy", "gpud_kmsg_dedup_units",
            "gpud_kmsg_dedup_create", "gpud_kmsg_dedup_destroy", "gpud_kmsg_scan_dedup", "gpud_kmsg_dedup_stats",
            "gpud_fabric_issues", "gpud_fabric_suggest_reboot", "gpud_set_nvml_error_string", "gpud_nvml_error_strings_from_driver", "gpud_fabric_reason", "gpud_fabric_report_reason", "gpud_fabric_pack", "gpud_fabric_verdict_device", "gpud_comm_unique_id", "gpud_comm_init", "gpud_fabric_gather",
@@ -825,6 +825,7 @@ def lib() -> C.CDLL:
         "gpud_ring_reduce_ranges": (i32, [vp, vp, vp, i64, vp, vp]),
         "gpud_ring_reduce_range_sets": (i32, [vp, vp, vp, i64, vp, i64, vp, vp]),
         "gpud_rings_reduce_range_sets": (i32, [vp, i32, vp, vp, vp, i64, vp, i64, vp, vp]),
+        "gpud_rings_reduce_range_sets_fields": (i32, [vp, i32, vp, vp, i32, vp, vp, i64, vp, i64, vp, vp]),
         "gpud_ring_ranges_stats": (i32, [vp, C.POINTER(C.c_float), C.POINTER(i64), vp]),
         "gpud_box_query_create": (i32, [vp, i32, i32, vp, vp, vp, i64, vp, i64, C.POINTER(vp)]),
         "gpud_box_query_step": (i32, [vp, vp, C.POINTER(vp), C.POINTER(i64)]), "gpud_box_query_result": (i32, [vp, vp, vp]),
@@ -1079,11 +1080,12 @@ def comm_unique_id() -> bytes:
     return b.raw
 
 
-def rings_reduce_range_sets(rings, ring_of, first, length, set_off) -> dict:
+def rings_reduce_range_sets(rings, ring_of, first, length, set_off, fields=None) -> dict:
     """Range sets over several rings of one Context (gpud_rings_reduce_range_sets): range i is samples [first[i], first[i] + length[i])
     of rings[ring_of[i]] in that ring's own push order, set s is ranges set_off[s] .. set_off[s + 1] - 1, its samples theirs
     concatenated in that order, whichever rings hold them.  rings[0] is the home ring whose device runs the call.  {op: [F][n_sets]}
-    as Ring.reduce_range_sets returns."""
+    as Ring.reduce_range_sets returns; with a list of fields, only those are read (gpud_rings_reduce_range_sets_fields) and row g
+    of each result is field fields[g]: {op: [len(fields)][n_sets]}."""
     rings = list(rings)
     assert len(rings) >= 1
     home = rings[0]
@@ -1094,12 +1096,27 @@ def rings_reduce_range_sets(rings, ring_of, first, length, set_off) -> dict:
     assert first.shape == length.shape == ring_of.shape and set_off.shape[0] >= 1
     n_sets = set_off.shape[0] - 1
     hs = (C.c_void_p * len(rings))(*[r._h.value if r is not None else None for r in rings])
+    if fields is not None:
+        return _range_sets_fields(home, C.cast(hs, C.c_void_p), len(rings), C.c_void_p(ring_of.ctypes.data), fields, first, length, set_off)
     f64 = np.empty((5, home.F, n_sets), dtype=np.float64)
     nov = np.empty((home.F, n_sets), dtype=np.uint32)
     home.ctx._check(home._L.gpud_rings_reduce_range_sets(C.cast(hs, C.c_void_p), len(rings), C.c_void_p(ring_of.ctypes.data),
                                                          C.c_void_p(first.ctypes.data), C.c_void_p(length.ctypes.data), first.shape[0],
                                                          C.c_void_p(set_off.ctypes.data), n_sets, C.c_void_p(f64.ctypes.data),
                                                          C.c_void_p(nov.ctypes.data)))
+    return {"min": f64[0], "max": f64[1], "mean": f64[2], "ema": f64[3], "p99": f64[4], "n_over": nov}
+
+
+def _range_sets_fields(home, rings_p, n_rings, ring_of_p, fields, first, length, set_off) -> dict:
+    """gpud_rings_reduce_range_sets_fields over the rings at rings_p (ring_of_p: NULL for one ring): {op: [len(fields)][n_sets]}"""
+    fields = np.ascontiguousarray(fields, dtype=np.int32).reshape(-1)
+    n_sets = set_off.shape[0] - 1
+    f64 = np.empty((5, fields.shape[0], n_sets), dtype=np.float64)
+    nov = np.empty((fields.shape[0], n_sets), dtype=np.uint32)
+    home.ctx._check(home._L.gpud_rings_reduce_range_sets_fields(rings_p, n_rings, ring_of_p, C.c_void_p(fields.ctypes.data), fields.shape[0],
+                                                                C.c_void_p(first.ctypes.data), C.c_void_p(length.ctypes.data), first.shape[0],
+                                                                C.c_void_p(set_off.ctypes.data), n_sets, C.c_void_p(f64.ctypes.data),
+                                                                C.c_void_p(nov.ctypes.data)))
     return {"min": f64[0], "max": f64[1], "mean": f64[2], "ema": f64[3], "p99": f64[4], "n_over": nov}
 
 
@@ -1315,27 +1332,34 @@ class Ring:
         self.range_open_reasons = {k: int(why[i]) for i, k in enumerate(("", "short", "nan", "pivots", "above", "below", "overflow")) if i and why[i]}
         return float(a.value), float(b.value), int(n.value)
 
-    def reduce_ranges(self, first, length) -> dict:
+    def reduce_ranges(self, first, length, fields=None) -> dict:
         """Aggregates of samples [first[i], first[i] + length[i]) of the push order (sample 0 = the first ever pushed), each range one
-        window with the definitions of reduce_range: {op: [F][n]}"""
+        window with the definitions of reduce_range: {op: [F][n]}; with a list of fields, only those ({op: [len(fields)][n]}, row g
+        field fields[g], as reduce_range_sets(fields=...) over one range per set)"""
         first = np.ascontiguousarray(first, dtype=np.int64).reshape(-1)
         length = np.ascontiguousarray(length, dtype=np.int64).reshape(-1)
         assert first.shape == length.shape
         n = first.shape[0]
+        if fields is not None:
+            return self.reduce_range_sets(first, length, np.arange(n + 1, dtype=np.int64), fields=fields)
         f64 = np.empty((5, self.F, n), dtype=np.float64)
         nov = np.empty((self.F, n), dtype=np.uint32)
         self.ctx._check(self._L.gpud_ring_reduce_ranges(self._h, C.c_void_p(first.ctypes.data), C.c_void_p(length.ctypes.data), n,
                                                         C.c_void_p(f64.ctypes.data), C.c_void_p(nov.ctypes.data)))
         return {"min": f64[0], "max": f64[1], "mean": f64[2], "ema": f64[3], "p99": f64[4], "n_over": nov}
 
-    def reduce_range_sets(self, first, length, set_off) -> dict:
+    def reduce_range_sets(self, first, length, set_off, fields=None) -> dict:
         """Aggregates of sets of ranges: set s is ranges set_off[s] .. set_off[s + 1] - 1 of (first, length), its samples theirs
         concatenated in that order, reduced as one window with the definitions of reduce_range (the EMA runs across the joins):
-        {op: [F][n_sets]}"""
+        {op: [F][n_sets]}; with a list of fields, only those are read (gpud_rings_reduce_range_sets_fields on this ring alone) and
+        row g is field fields[g]: {op: [len(fields)][n_sets]}"""
         first = np.ascontiguousarray(first, dtype=np.int64).reshape(-1)
         length = np.ascontiguousarray(length, dtype=np.int64).reshape(-1)
         set_off = np.ascontiguousarray(set_off, dtype=np.int64).reshape(-1)
         assert first.shape == length.shape and set_off.shape[0] >= 1
+        if fields is not None:
+            hs = (C.c_void_p * 1)(self._h.value)
+            return _range_sets_fields(self, C.cast(hs, C.c_void_p), 1, None, fields, first, length, set_off)
         n_sets = set_off.shape[0] - 1
         f64 = np.empty((5, self.F, n_sets), dtype=np.float64)
         nov = np.empty((self.F, n_sets), dtype=np.uint32)

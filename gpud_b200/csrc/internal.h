@@ -257,16 +257,17 @@ int32_t gpud_tier_read_ctl(gpud_ring* r, gpud_tier_ctl* c);
 struct gpud_vslot { double* ring; double* sample; int64_t vcap; int smp_shift; int64_t smp_slots; };
 // tier.cu: fields [f0, f0 + G) of rows d_rows[0, n) of ring o's tier (each held, ascending) decoded into virtual columns
 // [vcol0, vcol0 + 1024 n) of slot s, on ring h's device and stream: o's coded rows are read in place (through the peer mapping when
-// o lives on another device), dir / offs [G n] are h's scratch and csum [G] takes the field sums no one reads.
-cudaError_t gpud_tier_decode(const gpud_ring* h, const gpud_ring* o, const int64_t* d_rows, int64_t n, int f0, int G, const gpud_vslot& s,
-                             int64_t vcol0, uint8_t* dir, unsigned long long* offs, unsigned long long* csum);
+// o lives on another device), dir / offs [G n] are h's scratch and csum [G] takes the field sums no one reads.  With fmap (device
+// memory, G entries) the slot's field f is the ring's field fmap[f] instead of f0 + f.
+cudaError_t gpud_tier_decode(const gpud_ring* h, const gpud_ring* o, const int64_t* d_rows, int64_t n, int f0, int G, const int32_t* fmap,
+                             const gpud_vslot& s, int64_t vcol0, uint8_t* dir, unsigned long long* offs, unsigned long long* csum);
 // A run of samples copied from a ring into its virtual slot: samples [first, first + n) of the ring's push order to virtual columns
 // vcol.., where n is the next run's off minus this one's (the last: up to n_samples); off counts the samples of the runs before it.
 struct gpud_tier_run { int64_t first, vcol, off; };
-// tier.cu: fields [f0, f0 + G) of the n_runs runs d_runs (n_samples samples in all) from ring o into slot s, in one launch on ring h's
-// device and stream, the sample ring by k_ring_append's rule.
+// tier.cu: fields [f0, f0 + G) (fmap: the ring's fields fmap[0, G)) of the n_runs runs d_runs (n_samples samples in all) from ring o
+// into slot s, in one launch on ring h's device and stream, the sample ring by k_ring_append's rule.
 cudaError_t gpud_tier_copy_runs(const gpud_ring* h, const gpud_ring* o, const gpud_tier_run* d_runs, int64_t n_runs, int64_t n_samples, int f0, int G,
-                                const gpud_vslot& s);
+                                const int32_t* fmap, const gpud_vslot& s);
 // The placement of one row of s bytes (host plan and device encode): the oldest rows go until [off, off + s) overlaps none held.
 __host__ __device__ inline int64_t gpud_tier_place(gpud_tier_ctl& c, int64_t* slot, int64_t R, int64_t B, int64_t s) {
   for (;;) {
@@ -322,15 +323,18 @@ struct gpud_ring_windows {
 
 // What the range launchers (ring.cu, select.cu, ranges.cu, box_query.cu) read of a ring; owns nothing.  gpud_view gives a real ring's;
 // a slot of a range call's virtual box (rows decoded from tiers or copied from rings) and the box query's dense and pivot buffers are
-// views of their own, with the ring's config.
+// views of their own, with the ring's config.  The field map d_fmap [F] (device memory; NULL: the identity) makes the view's field f
+// the ring's field d_fmap[f] wherever the range kernels read ring data - samples, sample ring, thresholds - while their results and
+// scratch keep the view's numbering: a call over chosen fields (gpud_rings_reduce_range_sets_fields) has F = the fields it names.
 struct gpud_ring_view {
   gpud_ctx* ctx; int dev; cudaStream_t stream; int sm_count;                         // where the launches run
   int F; int64_t cap; double alpha; int q_num, q_den;                                // the ring's config
   const double *d_ring, *d_thr, *d_pw, *d_sample; int smp_shift; int64_t smp_slots;  // samples [F][cap], thresholds, EMA powers, sample ring
+  const int32_t* d_fmap;                                                             // the ring field of each view field (NULL: f itself)
 };
 inline gpud_ring_view gpud_view(const gpud_ring* r) {
   return {r->ctx, r->dev, r->stream, r->sm_count, r->F, r->cap, r->alpha, r->q_num, r->q_den, r->d_ring, r->d_thr, r->d_pw, r->d_sample, r->smp_shift,
-          r->smp_slots};
+          r->smp_slots, nullptr};
 }
 
 inline int64_t ring_count(const gpud_ring* r) { return r->total < r->cap ? r->total : r->cap; }

@@ -174,8 +174,10 @@ static int32_t rings_ready(const gpud_ring_view& v, gpud_ring* const* rings, int
 // ranges_plan, or the peer check after it, before any launch.  The kernels run on the home ring's device and stream, read through the
 // view v (the ring itself, or a buffer laid out as one: a slot of a virtual box) and the ring table t, with the scratch `state` (created
 // on first use): the home ring's own, or a box query's (gpud_box_query), which must leave the ring's untouched.
-int32_t reduce_sets(const gpud_ring_view& v, const RingTable& t, const int32_t* ring_of, const int64_t* first, const int64_t* len, int64_t n_ranges,
-                    const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over, std::unique_ptr<gpud_ranges_state>& state) {
+int32_t reduce_sets(const gpud_ring_view& v0, const RingTable& t, const int32_t* ring_of, const int64_t* first, const int64_t* len, int64_t n_ranges,
+                    const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over, std::unique_ptr<gpud_ranges_state>& state,
+                    const int32_t* fields) {
+  gpud_ring_view v = v0;
   const int n_rings = t.n();
   std::vector<gpud_ring_src> src(t.src);
   src[0] = {v.d_ring, v.d_sample};
@@ -195,6 +197,11 @@ int32_t reduce_sets(const gpud_ring_view& v, const RingTable& t, const int32_t* 
   rs->open = 0;
   std::fill(rs->reasons, rs->reasons + GPUD_RANGE_N_OPEN_REASONS, 0);
   const size_t plane = (size_t)v.F * n_sets;
+  if (fields) {                                    // one launch chain for any list of fields: every kernel reads through the map
+    GPUD_CUDA(v.ctx, rs->d_fmap.grow((size_t)v.F));
+    GPUD_CUDA(v.ctx, cudaMemcpyAsync(rs->d_fmap, fields, v.F * sizeof(int32_t), cudaMemcpyHostToDevice, v.stream));
+    v.d_fmap = rs->d_fmap;
+  }
   GPUD_CUDA(v.ctx, rs->d_out.grow(5 * plane));
   GPUD_CUDA(v.ctx, rs->d_nover.grow(plane));
   GPUD_CUDA(v.ctx, rs->d_short.grow(std::max<size_t>(1, pl.shorts.size())));
@@ -360,7 +367,8 @@ static void tier_scatter(const std::vector<double>& f64, const std::vector<uint3
 }
 
 int32_t reduce_subset(const gpud_ring_view& v, const RingTable& t, const std::vector<int64_t>& ids, const int32_t* ring_of, const int64_t* first,
-                      const int64_t* len, const int64_t* set_off, std::unique_ptr<gpud_ranges_state>& state, std::vector<double>& f64, std::vector<uint32_t>& nov) {
+                      const int64_t* len, const int64_t* set_off, std::unique_ptr<gpud_ranges_state>& state, std::vector<double>& f64, std::vector<uint32_t>& nov,
+                      const int32_t* fields) {
   std::vector<int64_t> sf, sl, so(1, 0);
   std::vector<int32_t> sr;
   for (int64_t s : ids) {
@@ -375,7 +383,7 @@ int32_t reduce_subset(const gpud_ring_view& v, const RingTable& t, const std::ve
   const int64_t m = (int64_t)ids.size();
   f64.assign(5 * (size_t)v.F * m, 0.0);
   nov.assign((size_t)v.F * m, 0u);
-  return reduce_sets(v, t, ring_of ? sr.data() : nullptr, sf.data(), sl.data(), (int64_t)sf.size(), so.data(), m, f64.data(), nov.data(), state);
+  return reduce_sets(v, t, ring_of ? sr.data() : nullptr, sf.data(), sl.data(), (int64_t)sf.size(), so.data(), m, f64.data(), nov.data(), state, fields);
 }
 
 // Device scratch of the virtual box, grown on the home ring: a failed allocation is GPUD_E_CUDA and leaves every ring usable.
@@ -390,10 +398,14 @@ static int32_t vbox_grow(gpud_ctx* ctx, gpud_buf<T>& b, size_t need) {
 // The call behind gpud_rings_reduce_range_sets, and behind the one-ring calls as its n_rings = 1 case (set_off NULL: every range is a
 // set, n_sets = n_ranges), after their argument checks and rings_check.  A call none of whose rings has a tier is reduce_sets; so is a
 // call with no set that reaches a tier, once each tiered ring's control word has been read (one synchronisation of its stream).
+// fields (gpud_rings_reduce_range_sets_fields; NULL: every field): the call's field f is the rings' field fields[f] of n_fields, its
+// output [5][n_fields][n_sets]; the virtual box decodes and copies only those fields, in groups of the named fields.
 static int32_t reduce_box(gpud_ring* const* rings, int n_rings, const int32_t* ring_of, const int64_t* first, const int64_t* len, int64_t n_ranges,
-                          const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over) {
+                          const int64_t* set_off, int64_t n_sets, const int32_t* fields, int n_fields, double* out_f64, uint32_t* out_n_over) {
   gpud_ring* h = rings[0];
   gpud_ctx* ctx = h->ctx;
+  gpud_ring_view hv = gpud_view(h);                // the home ring, over the call's fields
+  if (fields) hv.F = n_fields;
   RingTable rt = ring_table(rings, n_rings);
   std::vector<SplitRing> rg(n_rings);
   bool tiered = false;
@@ -408,12 +420,12 @@ static int32_t reduce_box(gpud_ring* const* rings, int n_rings, const int32_t* r
   }
   TierSplit sp;
   if (tiered) { int32_t rc = tier_split(ctx, rg, h->cap, ring_of, first, len, n_ranges, set_off, n_sets, &sp); if (rc) return rc; }
-  if (sp.ring.empty()) return reduce_sets(gpud_view(h), rt, ring_of, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over, h->ranges);
-  { int32_t rc = rings_ready(gpud_view(h), rings, n_rings); if (rc) return rc; }
+  if (sp.ring.empty()) return reduce_sets(hv, rt, ring_of, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over, h->ranges, fields);
+  { int32_t rc = rings_ready(hv, rings, n_rings); if (rc) return rc; }
   rt.rings = nullptr;                              // ready: the subsets below wait for nothing more
   std::vector<int64_t> ids[2];
   for (int64_t s = 0; s < n_sets; ++s) ids[sp.route[s]].push_back(s);
-  const int F = h->F, ns = (int)sp.ring.size();
+  const int F = hv.F, ns = (int)sp.ring.size();
   // the virtual box's geometry and field groups
   const int64_t vcap = sp.vcap;
   const int smp_shift = ring_smp_shift(vcap);
@@ -445,12 +457,22 @@ static int32_t reduce_box(gpud_ring* const* rings, int n_rings, const int32_t* r
   { int32_t rc = vbox_grow(ctx, rs->d_voffs, (size_t)G * drows.size()); if (rc) return rc; }
   { int32_t rc = vbox_grow(ctx, rs->d_runs, runs.size()); if (rc) return rc; }
   { int32_t rc = vbox_grow(ctx, rs->d_vsum, (size_t)G); if (rc) return rc; }
+  std::vector<double> thr;                         // chosen fields: the box's thresholds and the ring field of each of its fields
+  if (fields) {
+    { int32_t rc = vbox_grow(ctx, rs->d_vthr, (size_t)F); if (rc) return rc; }
+    { int32_t rc = vbox_grow(ctx, rs->d_fmap, (size_t)F); if (rc) return rc; }
+    for (int f = 0; f < F; ++f) thr.push_back(h->thr[fields[f]]);
+  }
   for (auto& e : rs->ev_dec) GPUD_CUDA(ctx, e.make());
   gpud_event ev[2];
   for (auto& e : ev) GPUD_CUDA(ctx, e.make());
   GPUD_CUDA(ctx, cudaEventRecord(ev[0], h->stream));
   if (!drows.empty()) GPUD_CUDA(ctx, cudaMemcpyAsync(rs->d_rows, drows.data(), drows.size() * sizeof(int64_t), cudaMemcpyHostToDevice, h->stream));
   if (!runs.empty()) GPUD_CUDA(ctx, cudaMemcpyAsync(rs->d_runs, runs.data(), runs.size() * sizeof(gpud_tier_run), cudaMemcpyHostToDevice, h->stream));
+  if (fields) {
+    GPUD_CUDA(ctx, cudaMemcpyAsync(rs->d_vthr, thr.data(), F * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    GPUD_CUDA(ctx, cudaMemcpyAsync(rs->d_fmap, fields, F * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
+  }
   int64_t open = 0;
   int reasons[GPUD_RANGE_N_OPEN_REASONS] = {};
   auto tally = [&]() {
@@ -460,7 +482,7 @@ static int32_t reduce_box(gpud_ring* const* rings, int n_rings, const int32_t* r
   std::vector<double> f64;
   std::vector<uint32_t> nov;
   if (!ids[0].empty()) {
-    int32_t rc = reduce_subset(gpud_view(h), rt, ids[0], ring_of, first, len, set_off, h->ranges, f64, nov);
+    int32_t rc = reduce_subset(hv, rt, ids[0], ring_of, first, len, set_off, h->ranges, f64, nov, fields);
     if (rc) return rc;
     tier_scatter(f64, nov, ids[0], 0, F, F, n_sets, out_f64, out_n_over);
     tally();
@@ -479,16 +501,17 @@ static int32_t reduce_box(gpud_ring* const* rings, int n_rings, const int32_t* r
     GPUD_CUDA(ctx, cudaEventRecord(rs->ev_dec[0], h->stream));
     for (int v = 0; v < ns; ++v) {
       const gpud_ring* o = rings[sp.ring[v]];
-      GPUD_CUDA(ctx, gpud_tier_decode(h, o, rs->d_rows + d0[v], d0[v + 1] - d0[v], f0, g, vs[v], dcol[v], rs->d_vdir + (size_t)g * d0[v],
+      const int32_t* fmap = fields ? rs->d_fmap + f0 : nullptr;
+      GPUD_CUDA(ctx, gpud_tier_decode(h, o, rs->d_rows + d0[v], d0[v + 1] - d0[v], f0, g, fmap, vs[v], dcol[v], rs->d_vdir + (size_t)g * d0[v],
                                       rs->d_voffs + (size_t)g * d0[v], rs->d_vsum));
-      GPUD_CUDA(ctx, gpud_tier_copy_runs(h, o, rs->d_runs + r0[v], r0[v + 1] - r0[v], rn[v], f0, g, vs[v]));
+      GPUD_CUDA(ctx, gpud_tier_copy_runs(h, o, rs->d_runs + r0[v], r0[v + 1] - r0[v], rn[v], f0, g, fmap, vs[v]));
     }
     GPUD_CUDA(ctx, cudaEventRecord(rs->ev_dec[1], h->stream));
-    gpud_ring_view vv = gpud_view(h);   // the box: fields [f0, f0 + g) of every slot, slot 0 the view's own
+    gpud_ring_view vv = gpud_view(h);   // the box: the call's fields [f0, f0 + g) of every slot, slot 0 the view's own
     vv.F = g;
     vv.cap = vcap;
     vv.d_ring = vs[0].ring;
-    vv.d_thr = h->d_thr + f0;
+    vv.d_thr = (fields ? rs->d_vthr.get() : h->d_thr.get()) + f0;
     vv.d_sample = vs[0].sample;
     vv.smp_shift = smp_shift;
     vv.smp_slots = smp_slots;
@@ -569,7 +592,7 @@ extern "C" int32_t gpud_ring_reduce_ranges(gpud_ring* r, const int64_t* first, c
   if (!first || !len || !out_f64 || !out_n_over) return GPUD_E_INVALID;
   if (n_ranges > GPUD_RANGES_MAX_SEGMENTS / r->F)
     return gpud_fail(r->ctx, GPUD_E_INVALID, "%d fields x %lld ranges exceed GPUD_RANGES_MAX_SEGMENTS", r->F, (long long)n_ranges);
-  return reduce_box(&r, 1, nullptr, first, len, n_ranges, nullptr, n_ranges, out_f64, out_n_over);
+  return reduce_box(&r, 1, nullptr, first, len, n_ranges, nullptr, n_ranges, nullptr, 0, out_f64, out_n_over);
 }
 
 // The refusals of a call over several rings beyond those of one ring (DESIGN.md §2 "Box sets"): one ctx and the home ring's config bit
@@ -600,7 +623,27 @@ extern "C" int32_t gpud_rings_reduce_range_sets(gpud_ring* const* rings, int32_t
   if (n_sets > GPUD_RANGES_MAX_SEGMENTS / r->F)
     return gpud_fail(r->ctx, GPUD_E_INVALID, "%d fields x %lld sets exceed GPUD_RANGES_MAX_SEGMENTS", r->F, (long long)n_sets);
   { int32_t rc = rings_check(rings, n_rings); if (rc) return rc; }
-  return reduce_box(rings, n_rings, ring_of, first, len, n_ranges, set_off, n_sets, out_f64, out_n_over);
+  return reduce_box(rings, n_rings, ring_of, first, len, n_ranges, set_off, n_sets, nullptr, 0, out_f64, out_n_over);
+}
+
+// The same call over the fields the caller names (DESIGN.md §2 "Field selection"): field g of the call is the rings' field fields[g],
+// read and, in a tier, decoded alone; every other refusal is gpud_rings_reduce_range_sets', with the segment limit on n_fields.
+extern "C" int32_t gpud_rings_reduce_range_sets_fields(gpud_ring* const* rings, int32_t n_rings, const int32_t* ring_of, const int32_t* fields,
+                                                       int32_t n_fields, const int64_t* first, const int64_t* len, int64_t n_ranges,
+                                                       const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over) {
+  if (!rings || n_rings < 1 || n_rings > GPUD_PIECE_RINGS || !rings[0] || n_ranges < 0 || n_sets < 0) return GPUD_E_INVALID;
+  gpud_ring* r = rings[0];
+  if (n_sets == 0) return GPUD_OK;
+  if (!first || !len || !set_off || !out_f64 || !out_n_over || (n_rings > 1 && !ring_of)) return GPUD_E_INVALID;
+  if (!fields) return gpud_fail(r->ctx, GPUD_E_INVALID, "fields is NULL");
+  if (n_fields < 1) return gpud_fail(r->ctx, GPUD_E_INVALID, "n_fields is %d, not at least 1", n_fields);
+  for (int32_t g = 0; g < n_fields; ++g)
+    if (fields[g] < 0 || fields[g] >= r->F)
+      return gpud_fail(r->ctx, GPUD_E_INVALID, "fields[%d] is %d, not a field of the ring's %d", g, fields[g], r->F);
+  if (n_sets > GPUD_RANGES_MAX_SEGMENTS / n_fields)
+    return gpud_fail(r->ctx, GPUD_E_INVALID, "n_fields %d x %lld sets exceed GPUD_RANGES_MAX_SEGMENTS", n_fields, (long long)n_sets);
+  { int32_t rc = rings_check(rings, n_rings); if (rc) return rc; }
+  return reduce_box(rings, n_rings, ring_of, first, len, n_ranges, set_off, n_sets, fields, n_fields, out_f64, out_n_over);
 }
 
 extern "C" int32_t gpud_ring_reduce_range_sets(gpud_ring* r, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets,

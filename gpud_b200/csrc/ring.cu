@@ -963,13 +963,15 @@ __device__ __forceinline__ RunPass run_pass(const double2 (&v)[16], uint4* my_ro
 // Short route: one warp per (field, short set).  The order statistic: the k-th largest lane maximum bounds it from below, the keys
 // above that bound are gathered and selected from (the window kernel's medium path); a rank deeper than 32, or more than 32 keys
 // above the bound, takes the MSB-first bit search over the rows.  The EMA starts at the set's first sample.  MULTI: the call's pieces
-// lie in several rings (srcs), and a set of one range outside the home ring has one piece.
-template <bool MULTI>
+// lie in several rings (srcs), and a set of one range outside the home ring has one piece.  FMAP: field f of the call reads the rings'
+// field fmap[f] (samples and threshold); its results keep index f.
+template <bool MULTI, bool FMAP>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, kCtasPerSM) k_ranges_short(const double* __restrict__ ring, int64_t cap, int F, const gpud_short_range* __restrict__ rs,
                                                                      int n_short, const gpud_piece* __restrict__ pieces, int64_t n_out,
                                                                      const double* __restrict__ thr, const double* __restrict__ pw,
                                                                      double q64, double alpha, int q_num, int q_den, double* __restrict__ out,
-                                                                     uint32_t* __restrict__ out_nover, const gpud_ring_src* __restrict__ srcs) {
+                                                                     uint32_t* __restrict__ out_nover, const gpud_ring_src* __restrict__ srcs,
+                                                                     const int32_t* __restrict__ fmap) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   unsigned char* wbase = smem_raw + (size_t)warp * kWarpSmemBytes;
@@ -983,12 +985,13 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, kCtasPerSM) k_ranges_shor
     const int f = (int)(u / n_short);
     const gpud_short_range q = rs[u - (int64_t)f * n_short];
     const int m = q.len;
-    const int64_t fo = (int64_t)f * cap;
+    const int rf = FMAP ? __ldg(fmap + f) : f;   // the rings' field
+    const int64_t fo = (int64_t)rf * cap;
     const double* __restrict__ base = (MULTI && q.np ? gpud_piece_data(srcs, pieces[q.p0], ring) : ring) + fo;   // the ring of the set's first sample
     double2 v[16];
     if (q.np > 1) load_pieces<MULTI>(v, my_row4, srcs, ring, fo, cap, pieces + q.p0, q.np, 0, m, lane);
     else load_run(v, base, cap, q.start, m, lane);
-    const RunPass rp = run_pass<false>(v, my_row4, m, __ldg(thr + f), q64, alpha, pw, 0.0, 0.0, lane);
+    const RunPass rp = run_pass<false>(v, my_row4, m, __ldg(thr + rf), q64, alpha, pw, 0.0, 0.0, lane);
     const unsigned mh = (unsigned)(rp.kmax >> 32), ml = (unsigned)rp.kmax;   // the lane's largest key
     const K64 wmax = warp_max_k64(mh, ml);
     const int k = (int)gpud_rank_from_top(m, q_num, q_den);
@@ -1034,8 +1037,8 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, kCtasPerSM) k_ranges_shor
 // Long route, the tile pass: one warp per (field, tile) of the flat tile list of the long sets.  What k_range_finish folds per
 // segment: min, max, mean, EMA partial, n_over and the class counts of classify_window against the segment's pivots, whose list
 // receives the keys strictly between them.  A set of several ranges is cut into tiles over its concatenated samples: a tile inside
-// one piece loads as one run, a tile across joins through the piece table.  MULTI: as k_ranges_short.
-template <bool MULTI>
+// one piece loads as one run, a tile across joins through the piece table.  MULTI, FMAP: as k_ranges_short.
+template <bool MULTI, bool FMAP>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, kCtasPerSM) k_ranges_tiles(const double* __restrict__ ring, int64_t cap, int F, const gpud_range_geo* __restrict__ geo,
                                                                      int64_t n_long, const int32_t* __restrict__ tile_range, int64_t n_tiles,
                                                                      const double* __restrict__ thr, const double* __restrict__ pw, double q64, double alpha,
@@ -1044,7 +1047,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, kCtasPerSM) k_ranges_tile
                                                                      uint4* __restrict__ t_cls, unsigned long long* __restrict__ lists, int64_t list_row,
                                                                      unsigned* __restrict__ fill, const gpud_piece* __restrict__ pieces,
                                                                      const int64_t* __restrict__ seg_p0, const int64_t* __restrict__ tile_piece,
-                                                                     const gpud_ring_src* __restrict__ srcs) {
+                                                                     const gpud_ring_src* __restrict__ srcs, const int32_t* __restrict__ fmap) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   unsigned char* wbase = smem_raw + (size_t)warp * kWarpSmemBytes;
@@ -1058,7 +1061,8 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, kCtasPerSM) k_ranges_tile
     const gpud_range_geo& g = geo[j];
     const int64_t off = (t - g.tile0) * GPUD_MAX_WINDOW;
     const int m = (int)min((int64_t)GPUD_MAX_WINDOW, g.n - off);
-    const int64_t fo = (int64_t)f * cap;
+    const int rf = FMAP ? __ldg(fmap + f) : f;
+    const int64_t fo = (int64_t)rf * cap;
     const int64_t sg = (int64_t)f * n_long + j;
     const double lo = __ldg(piv + 2 * sg), hi = __ldg(piv + 2 * sg + 1);
     double2 v[16];
@@ -1073,7 +1077,7 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, kCtasPerSM) k_ranges_tile
       if (p0 >= cap) p0 -= cap;
       load_run(v, ring + fo, cap, p0, m, lane);
     }
-    const RunPass rp = run_pass<true>(v, my_row4, m, __ldg(thr + f), q64, alpha, pw, lo, hi, lane);
+    const RunPass rp = run_pass<true>(v, my_row4, m, __ldg(thr + rf), q64, alpha, pw, lo, hi, lane);
     const bool lo_zero = __reduce_or_sync(kFull, rp.lor) == 0u;
     WinParams lp{};
     lp.fill = fill + sg;
@@ -1095,12 +1099,12 @@ __global__ void __launch_bounds__(kWarpsPerBlock * 32, kCtasPerSM) k_ranges_tile
 }
 
 // Long route, the EMA: one 128-thread CTA per segment, the carry's scan over the segment's tiles from its first sample (MULTI: in
-// its first piece's ring), into its last tile's row of ema [F][n_tiles].
-template <bool GUARD, bool MULTI>
+// its first piece's ring; FMAP: in the rings' field fmap[f]), into its last tile's row of ema [F][n_tiles].
+template <bool GUARD, bool MULTI, bool FMAP>
 __global__ void __launch_bounds__(128) k_ranges_ema(const double* __restrict__ part, int64_t n_tiles, const gpud_range_geo* __restrict__ geo, int64_t n_long,
                                                      const double* __restrict__ ring, int64_t cap, double d_full, double* __restrict__ ema,
                                                      const gpud_piece* __restrict__ pieces, const int64_t* __restrict__ seg_p0,
-                                                     const gpud_ring_src* __restrict__ srcs) {
+                                                     const gpud_ring_src* __restrict__ srcs, const int32_t* __restrict__ fmap) {
   __shared__ double s_warp[4];
   __shared__ double s_carry;
   const int64_t sg = blockIdx.x;
@@ -1109,8 +1113,9 @@ __global__ void __launch_bounds__(128) k_ranges_ema(const double* __restrict__ p
   const gpud_range_geo& g = geo[j];
   const int nw = (int)((g.n + GPUD_MAX_WINDOW - 1) / GPUD_MAX_WINDOW);
   const double* __restrict__ P = part + (int64_t)f * n_tiles + g.tile0;
+  const int64_t rf = FMAP ? __ldg(fmap + f) : f;
   decayed_scan<GUARD>(P, nw - 1, d_full, s_warp, s_carry,
-                      [&] { return (MULTI && g.np ? gpud_piece_data(srcs, pieces[seg_p0[j]], ring) : ring)[(int64_t)f * cap + g.start]; }, [](int, double) {});
+                      [&] { return (MULTI && g.np ? gpud_piece_data(srcs, pieces[seg_p0[j]], ring) : ring)[rf * cap + g.start]; }, [](int, double) {});
   if (threadIdx.x == 0) ema[(int64_t)f * n_tiles + g.tile0 + nw - 1] = decay_fma<GUARD>(g.d_last, s_carry, __ldg(P + nw - 1));
 }
 
@@ -1812,23 +1817,25 @@ static int ranges_grid(const gpud_ring_view& v, int64_t units) {
 
 cudaError_t gpud_ranges_short(const gpud_ring_view& v, const gpud_short_range* rs, int n_short, const gpud_piece* pieces, const gpud_ring_src* srcs,
                               int64_t n_out, double* out, uint32_t* nover) {
-  const auto k = srcs ? k_ranges_short<true> : k_ranges_short<false>;
+  const auto k = srcs ? (v.d_fmap ? k_ranges_short<true, true> : k_ranges_short<true, false>)
+                      : (v.d_fmap ? k_ranges_short<false, true> : k_ranges_short<false, false>);
   const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kBlockSmemBytes);
   if (e != cudaSuccess) return e;
   k<<<ranges_grid(v, (int64_t)v.F * n_short), kWarpsPerBlock * 32, kBlockSmemBytes, v.stream>>>(
-      v.d_ring, v.cap, v.F, rs, n_short, pieces, n_out, v.d_thr, v.d_pw, pow(1.0 - v.alpha, 64.0), v.alpha, v.q_num, v.q_den, out, nover, srcs);
+      v.d_ring, v.cap, v.F, rs, n_short, pieces, n_out, v.d_thr, v.d_pw, pow(1.0 - v.alpha, 64.0), v.alpha, v.q_num, v.q_den, out, nover, srcs, v.d_fmap);
   return cudaGetLastError();
 }
 
 cudaError_t gpud_ranges_tiles(const gpud_ring_view& v, const gpud_range_geo* geo, int64_t n_long, const int32_t* tile_range, int64_t n_tiles, const double* piv,
                               double* const w[5], uint32_t* w_nover, uint4* w_cls, unsigned long long* lists, int64_t list_row, unsigned* fill,
                               const gpud_piece* pieces, const int64_t* seg_p0, const int64_t* tile_piece, const gpud_ring_src* srcs) {
-  const auto k = srcs ? k_ranges_tiles<true> : k_ranges_tiles<false>;
+  const auto k = srcs ? (v.d_fmap ? k_ranges_tiles<true, true> : k_ranges_tiles<true, false>)
+                      : (v.d_fmap ? k_ranges_tiles<false, true> : k_ranges_tiles<false, false>);
   const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kBlockSmemBytes);
   if (e != cudaSuccess) return e;
   k<<<ranges_grid(v, (int64_t)v.F * n_tiles), kWarpsPerBlock * 32, kBlockSmemBytes, v.stream>>>(
       v.d_ring, v.cap, v.F, geo, n_long, tile_range, n_tiles, v.d_thr, v.d_pw, pow(1.0 - v.alpha, 64.0), v.alpha, piv, w[0], w[1], w[2], w[4],
-      w_nover, w_cls, lists, list_row, fill, pieces, seg_p0, tile_piece, srcs);
+      w_nover, w_cls, lists, list_row, fill, pieces, seg_p0, tile_piece, srcs, v.d_fmap);
   return cudaGetLastError();
 }
 
@@ -1838,7 +1845,10 @@ cudaError_t gpud_ranges_ema(const gpud_ring_view& v, const gpud_range_geo* geo, 
   const double d_full = pow(1.0 - v.alpha, (double)GPUD_MAX_WINDOW);
   const unsigned grid = (unsigned)((int64_t)v.F * n_long);
   const bool guard = pow(d_full, 128.0) < 0x1p-900;
-  const auto k = srcs ? (guard ? k_ranges_ema<true, true> : k_ranges_ema<false, true>) : (guard ? k_ranges_ema<true, false> : k_ranges_ema<false, false>);
-  k<<<grid, 128, 0, v.stream>>>(part, n_tiles, geo, n_long, v.d_ring, v.cap, d_full, ema, pieces, seg_p0, srcs);
+  using K = decltype(&k_ranges_ema<false, false, false>);
+  const K ks[2][2][2] = {{{k_ranges_ema<false, false, false>, k_ranges_ema<false, false, true>}, {k_ranges_ema<false, true, false>, k_ranges_ema<false, true, true>}},
+                         {{k_ranges_ema<true, false, false>, k_ranges_ema<true, false, true>}, {k_ranges_ema<true, true, false>, k_ranges_ema<true, true, true>}}};
+  const K k = ks[guard][srcs != nullptr][v.d_fmap != nullptr];
+  k<<<grid, 128, 0, v.stream>>>(part, n_tiles, geo, n_long, v.d_ring, v.cap, d_full, ema, pieces, seg_p0, srcs, v.d_fmap);
   return cudaGetLastError();
 }

@@ -128,6 +128,7 @@ struct gpud_ranges_state {
   gpud_buf<int64_t> d_tile_piece;         // ... and the piece of its first sample (sets of several ranges)
   gpud_buf<double> d_out;                 // the call's result [5][F][n_sets]
   gpud_buf<uint32_t> d_nover;             //   and n_over [F][n_sets]
+  gpud_buf<int32_t> d_fmap;               // a call over chosen fields: the ring field of each (gpud_ring_view::d_fmap)
   gpud_event ev[2];
   bool timed = false;
   bool seg_last = false;          // seg holds the last batch of the last call (that call had a long set)
@@ -143,6 +144,7 @@ struct gpud_ranges_state {
   gpud_buf<unsigned long long> d_voffs;
   gpud_buf<gpud_tier_run> d_runs;
   gpud_buf<unsigned long long> d_vsum;
+  gpud_buf<double> d_vthr;                // a call over chosen fields: their thresholds, the box's in its field order
   gpud_event ev_dec[2];
 };
 
@@ -159,12 +161,16 @@ struct RingTable {
 RingTable ring_table(gpud_ring* const* rings, int n_rings);
 
 // The sets of a call over table t (slot 0 the view v's ring), into out_f64 [5][F][n_sets] / out_n_over [F][n_sets], on the scratch
-// `state` (created on first use).  ranges.cu says the rest.
+// `state` (created on first use).  fields (host memory, v.F of them; NULL: none): the view's field f is the rings' field fields[f],
+// uploaded to the scratch as the view's field map once the plan has passed.  ranges.cu says the rest.
 int32_t reduce_sets(const gpud_ring_view& v, const RingTable& t, const int32_t* ring_of, const int64_t* first, const int64_t* len, int64_t n_ranges,
-                    const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over, std::unique_ptr<gpud_ranges_state>& state);
+                    const int64_t* set_off, int64_t n_sets, double* out_f64, uint32_t* out_n_over, std::unique_ptr<gpud_ranges_state>& state,
+                    const int32_t* fields = nullptr);
 // The sets ids[] of a call (set_off NULL: every range a set) reduced as a call of their own over v and table t, on `state`: range i in
-// slot ring_of[i] (ring_of NULL: all in slot 0) from sample first[i], len[i] samples, into f64 [5][F][ids] / nov [F][ids].
+// slot ring_of[i] (ring_of NULL: all in slot 0) from sample first[i], len[i] samples, into f64 [5][F][ids] / nov [F][ids] (fields: as
+// reduce_sets).
 int32_t reduce_subset(const gpud_ring_view& v, const RingTable& t, const std::vector<int64_t>& ids, const int32_t* ring_of, const int64_t* first,
-                      const int64_t* len, const int64_t* set_off, std::unique_ptr<gpud_ranges_state>& state, std::vector<double>& f64, std::vector<uint32_t>& nov);
+                      const int64_t* len, const int64_t* set_off, std::unique_ptr<gpud_ranges_state>& state, std::vector<double>& f64, std::vector<uint32_t>& nov,
+                      const int32_t* fields = nullptr);
 // The results of a select's n_long segments (s->d_out [5][F n_long], s->d_nover) into columns geo[j].id of out [5][F][n_out] / nover [F][n_out].
 cudaError_t ranges_scatter(const gpud_ring_view& v, const gpud_range_state* s, int64_t n_long, int64_t n_out, double* out, uint32_t* nover);

@@ -177,14 +177,14 @@ __device__ __forceinline__ const gpud_range_geo& seg_geo(const gpud_range_geo* g
 // contiguous memory per field, kept current by the append kernel), else from g.S strided reads of the ring itself (one 32-byte sector
 // each; PIECES: a set with pieces, entry j's pieces from seg_p0[j] on, maps each read's concatenated position to its piece and ring,
 // and - MULTI, a call over several rings - a piece's samples and a set of one range in another ring's sample ring come from the
-// call's ring table srcs).  One block per segment; 32 registers, so that four blocks fit an SM when the sample is small (a handle's
-// many segments).
-template <bool PIECES, bool MULTI>
+// call's ring table srcs).  FMAP: segment field f reads the ring field fmap[f] (its samples and its sample ring).  One block per
+// segment; 32 registers, so that four blocks fit an SM when the sample is small (a handle's many segments).
+template <bool PIECES, bool MULTI, bool FMAP>
 __global__ void __launch_bounds__(kSelThreads, 4) k_range_pivots(const double* __restrict__ ring, int64_t cap, const gpud_range_geo* __restrict__ geo, int64_t n_geo,
                                                        double* __restrict__ piv, unsigned* __restrict__ fill,
                                                        const double* __restrict__ sample, int smp_shift, int64_t smp_slots,
                                                        const gpud_piece* __restrict__ pieces, const int64_t* __restrict__ seg_p0,
-                                                       const gpud_ring_src* __restrict__ srcs) {
+                                                       const gpud_ring_src* __restrict__ srcs, const int32_t* __restrict__ fmap) {
   extern __shared__ __align__(16) unsigned long long s_keys[];
   __shared__ unsigned s_hist[512];
   __shared__ unsigned long long s_red[2 * kSelThreads / 32];
@@ -195,11 +195,12 @@ __global__ void __launch_bounds__(kSelThreads, 4) k_range_pivots(const double* _
   int f;
   const gpud_range_geo& g = seg_geo(geo, n_geo, sg, &f);
   const int64_t start = g.start, n = g.n, stride = g.stride;
+  const int64_t rf = FMAP ? __ldg(fmap + f) : f;   // the ring field
   int S = g.S;
   if (g.smp) {
     if (t == 0) s_cnt = 0;
     __syncthreads();
-    const double* __restrict__ sb = (MULTI && g.np ? srcs[gpud_piece_ring(pieces[seg_p0[sg - (int64_t)f * n_geo]])].sample : sample) + (int64_t)f * smp_slots;
+    const double* __restrict__ sb = (MULTI && g.np ? srcs[gpud_piece_ring(pieces[seg_p0[sg - (int64_t)f * n_geo]])].sample : sample) + rf * smp_slots;
     const int64_t half = (1ll << smp_shift) >> 1;
     for (int64_t s0 = 0; s0 < smp_slots; s0 += kSelThreads) {             // slots compacted with one ballot + one counter bump per warp
       const int64_t sl = s0 + t;
@@ -219,14 +220,14 @@ __global__ void __launch_bounds__(kSelThreads, 4) k_range_pivots(const double* _
     __syncthreads();
     S = s_cnt;
   } else {
-    const double* __restrict__ base = ring + (int64_t)f * cap;
+    const double* __restrict__ base = ring + rf * cap;
     if (PIECES && (MULTI ? g.np > 0 : g.np > 1)) {
       const gpud_piece* __restrict__ p = pieces + seg_p0[sg - (int64_t)f * n_geo];
       const int64_t np = g.np;
       for (int j = t; j < S; j += kSelThreads) {
         const int64_t c = (int64_t)j * stride + (stride >> 1);
         const gpud_piece& q = p[gpud_piece_at(p, 0, np, c)];
-        const double* __restrict__ src = MULTI ? gpud_piece_data(srcs, q, ring) + (int64_t)f * cap : base;
+        const double* __restrict__ src = MULTI ? gpud_piece_data(srcs, q, ring) + rf * cap : base;
         s_keys[j] = gpud_f64_key((unsigned long long)__double_as_longlong(__ldg(src + gpud_piece_col<MULTI>(q, c, cap))));
       }
     } else {
@@ -418,13 +419,13 @@ __global__ void __launch_bounds__(kSelThreads) k_range_finish(int F, int Wp, con
   }
 }
 
-// grid (blocks_per_segment, segments): histogram of the next digit over the keys that match the segment's prefix (PIECES, MULTI: as
-// k_range_pivots)
-template <bool PIECES, bool MULTI>
+// grid (blocks_per_segment, segments): histogram of the next digit over the keys that match the segment's prefix (PIECES, MULTI,
+// FMAP: as k_range_pivots)
+template <bool PIECES, bool MULTI, bool FMAP>
 __global__ void __launch_bounds__(256) k_sel_hist(const double* __restrict__ ring, int64_t cap, const gpud_range_geo* __restrict__ geo, int64_t n_geo,
                                                    const SelState* __restrict__ st, unsigned* __restrict__ hist, const int* __restrict__ ids,
                                                    const gpud_piece* __restrict__ pieces, const int64_t* __restrict__ seg_p0,
-                                                   const gpud_ring_src* __restrict__ srcs) {
+                                                   const gpud_ring_src* __restrict__ srcs, const int32_t* __restrict__ fmap) {
   __shared__ unsigned s_hist[kBins];
   const int f = ids ? ids[blockIdx.y] : blockIdx.y;   // the segment
   const SelState s = st[f];
@@ -438,11 +439,12 @@ __global__ void __launch_bounds__(256) k_sel_hist(const double* __restrict__ rin
   const int64_t n = g.n;
   const int64_t per = (((n + gridDim.x - 1) / gridDim.x) + 1) & ~(int64_t)1;   // even, so aligned slices stay aligned
   const int64_t b = min(n, (int64_t)blockIdx.x * per), e = min(n, b + per);
+  const int64_t fo = (FMAP ? (int64_t)__ldg(fmap + fld) : (int64_t)fld) * cap;
   auto bin = [&](unsigned long long key) {
     if (key_matches(key, s)) atomicAdd(&s_hist[(unsigned)(key >> shift) & mask], 1u);
   };
-  if (PIECES && (MULTI ? g.np > 0 : g.np > 1)) for_each_piece_key<MULTI>(srcs, ring + (int64_t)fld * cap, (int64_t)fld * cap, cap, g, pieces + seg_p0[f - (int64_t)fld * n_geo], b, e, bin);
-  else for_each_key(ring + (int64_t)fld * cap, cap, g.start, b, e, bin);
+  if (PIECES && (MULTI ? g.np > 0 : g.np > 1)) for_each_piece_key<MULTI>(srcs, ring + fo, fo, cap, g, pieces + seg_p0[f - (int64_t)fld * n_geo], b, e, bin);
+  else for_each_key(ring + fo, cap, g.start, b, e, bin);
   __syncthreads();
   for (int i = threadIdx.x; i < kBins; i += blockDim.x)
     if (s_hist[i]) atomicAdd(&hist[(int64_t)blockIdx.y * kBins + i], s_hist[i]);
@@ -469,12 +471,12 @@ __global__ void __launch_bounds__(kSelThreads) k_sel_pick(unsigned* __restrict__
 }
 
 // grid (blocks_per_segment, segments): compact the keys that still match into the segment's candidate list (<= kCollectMax of them;
-// PIECES, MULTI: as k_range_pivots)
-template <bool PIECES, bool MULTI>
+// PIECES, MULTI, FMAP: as k_range_pivots)
+template <bool PIECES, bool MULTI, bool FMAP>
 __global__ void __launch_bounds__(256) k_sel_collect(const double* __restrict__ ring, int64_t cap, const gpud_range_geo* __restrict__ geo, int64_t n_geo,
                                                       SelState* __restrict__ st, unsigned long long* __restrict__ lists, const int* __restrict__ ids,
                                                       const gpud_piece* __restrict__ pieces, const int64_t* __restrict__ seg_p0,
-                                                      const gpud_ring_src* __restrict__ srcs) {
+                                                      const gpud_ring_src* __restrict__ srcs, const int32_t* __restrict__ fmap) {
   const int f = ids ? ids[blockIdx.y] : blockIdx.y;   // the segment
   const SelState s = st[f];
   if (s.nbits == 64) return;
@@ -485,14 +487,15 @@ __global__ void __launch_bounds__(256) k_sel_collect(const double* __restrict__ 
   const int64_t b = min(n, (int64_t)blockIdx.x * per), e = min(n, b + per);
   unsigned long long* __restrict__ list = lists + (int64_t)blockIdx.y * kCollectMax;
   unsigned* fill = &st[f].collected;
+  const int64_t fo = (FMAP ? (int64_t)__ldg(fmap + fld) : (int64_t)fld) * cap;
   auto keep = [&](unsigned long long key) {
     if (key_matches(key, s)) {
       const unsigned pos = atomicAdd(fill, 1u);
       if (pos < (unsigned)kCollectMax) list[pos] = key;
     }
   };
-  if (PIECES && (MULTI ? g.np > 0 : g.np > 1)) for_each_piece_key<MULTI>(srcs, ring + (int64_t)fld * cap, (int64_t)fld * cap, cap, g, pieces + seg_p0[f - (int64_t)fld * n_geo], b, e, keep);
-  else for_each_key(ring + (int64_t)fld * cap, cap, g.start, b, e, keep);
+  if (PIECES && (MULTI ? g.np > 0 : g.np > 1)) for_each_piece_key<MULTI>(srcs, ring + fo, fo, cap, g, pieces + seg_p0[f - (int64_t)fld * n_geo], b, e, keep);
+  else for_each_key(ring + fo, cap, g.start, b, e, keep);
 }
 
 // one block per field: its answer, selected from its (<= kCollectMax) collected keys unless the histogram passes finished it
@@ -538,11 +541,12 @@ cudaError_t sel_pivots(const gpud_ring_view& v, gpud_range_state* s, const gpud_
                        const int64_t* seg_p0, const gpud_ring_src* srcs) {
   size_t smem = 0;                     // the largest sample of the table
   for (int64_t j = 0; j < n_geo; ++j) smem = std::max(smem, (geo[j].smp ? (size_t)GPUD_RANGE_SAMPLE_MAX : (size_t)geo[j].S) * sizeof(unsigned long long));
-  const auto k = srcs ? k_range_pivots<true, true> : pieces ? k_range_pivots<true, false> : k_range_pivots<false, false>;
+  const auto k = v.d_fmap ? (srcs ? k_range_pivots<true, true, true> : pieces ? k_range_pivots<true, false, true> : k_range_pivots<false, false, true>)
+                          : (srcs ? k_range_pivots<true, true, false> : pieces ? k_range_pivots<true, false, false> : k_range_pivots<false, false, false>);
   const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(GPUD_RANGE_SAMPLE_MAX * sizeof(unsigned long long)));
   if (e != cudaSuccess) return e;
   k<<<(unsigned)(v.F * n_geo), kSelThreads, smem, v.stream>>>(v.d_ring, v.cap, s->d_geo, n_geo, s->d_piv, fill, v.d_sample, v.smp_shift, v.smp_slots,
-                                                              pieces, seg_p0, srcs);
+                                                              pieces, seg_p0, srcs, v.d_fmap);
   return cudaGetLastError();
 }
 
@@ -596,8 +600,9 @@ static int sel_blocks(const gpud_ring_view& v, int64_t n_max, int n_sel) {
 
 cudaError_t sel_hist(const gpud_ring_view& v, const gpud_range_state* s, const gpud_range_geo* geo, int64_t n_geo, int64_t n_max, const int* ids, int n_sel,
                      unsigned* hist, const gpud_piece* pieces, const int64_t* seg_p0, const gpud_ring_src* srcs) {
-  const auto k = srcs ? k_sel_hist<true, true> : pieces ? k_sel_hist<true, false> : k_sel_hist<false, false>;
-  k<<<dim3(sel_blocks(v, n_max, n_sel), n_sel), 256, 0, v.stream>>>(v.d_ring, v.cap, geo, n_geo, s->d_st, hist, ids, pieces, seg_p0, srcs);
+  const auto k = v.d_fmap ? (srcs ? k_sel_hist<true, true, true> : pieces ? k_sel_hist<true, false, true> : k_sel_hist<false, false, true>)
+                          : (srcs ? k_sel_hist<true, true, false> : pieces ? k_sel_hist<true, false, false> : k_sel_hist<false, false, false>);
+  k<<<dim3(sel_blocks(v, n_max, n_sel), n_sel), 256, 0, v.stream>>>(v.d_ring, v.cap, geo, n_geo, s->d_st, hist, ids, pieces, seg_p0, srcs, v.d_fmap);
   return cudaGetLastError();
 }
 
@@ -608,8 +613,9 @@ cudaError_t sel_pick(const gpud_ring_view& v, gpud_range_state* s, const int* id
 
 cudaError_t sel_collect(const gpud_ring_view& v, gpud_range_state* s, const gpud_range_geo* geo, int64_t n_geo, int64_t n_max, const int* ids, int n_sel,
                         const gpud_piece* pieces, const int64_t* seg_p0, const gpud_ring_src* srcs) {
-  const auto k = srcs ? k_sel_collect<true, true> : pieces ? k_sel_collect<true, false> : k_sel_collect<false, false>;
-  k<<<dim3(sel_blocks(v, n_max, n_sel), n_sel), 256, 0, v.stream>>>(v.d_ring, v.cap, geo, n_geo, s->d_st, s->d_cand, ids, pieces, seg_p0, srcs);
+  const auto k = v.d_fmap ? (srcs ? k_sel_collect<true, true, true> : pieces ? k_sel_collect<true, false, true> : k_sel_collect<false, false, true>)
+                          : (srcs ? k_sel_collect<true, true, false> : pieces ? k_sel_collect<true, false, false> : k_sel_collect<false, false, false>);
+  k<<<dim3(sel_blocks(v, n_max, n_sel), n_sel), 256, 0, v.stream>>>(v.d_ring, v.cap, geo, n_geo, s->d_st, s->d_cand, ids, pieces, seg_p0, srcs, v.d_fmap);
   return cudaGetLastError();
 }
 

@@ -93,26 +93,30 @@ __global__ void __launch_bounds__(kPlaceThreads) k_tier_place(const uint8_t* __r
   }
 }
 
-// Decode inputs of fields [f0, f0 + G) of rows[0, n): unit u = f n + j (k_ckpt_unpack's numbering) from row rows[j]'s record.
+// Decode inputs of fields [f0, f0 + G) (FMAP: the fields fmap[0, G)) of rows[0, n): unit u = f n + j (k_ckpt_unpack's numbering) from
+// row rows[j]'s record.  Each field's block is coded on its own, so any list of fields decodes alone.
+template <bool FMAP>
 __global__ void __launch_bounds__(256) k_tier_gather(const int64_t* __restrict__ rows, int64_t n, int f0, int G, int F, const unsigned long long* __restrict__ buf,
                                                      const int64_t* __restrict__ slot, int64_t R, int64_t rec_bytes, uint8_t* __restrict__ dir,
-                                                     unsigned long long* __restrict__ offs) {
+                                                     unsigned long long* __restrict__ offs, const int32_t* __restrict__ fmap) {
   const int64_t units = (int64_t)G * n;
   for (int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; u < units; u += (int64_t)gridDim.x * blockDim.x) {
     const int64_t f = u / n, j = u - f * n;
+    const int64_t rf = FMAP ? (int64_t)__ldg(fmap + f) : f0 + f;   // the ring field
     const int64_t off = slot[2 * (rows[j] % R)];
     const uint8_t* rec = reinterpret_cast<const uint8_t*>(buf) + off;
-    dir[u] = rec[kTierRecHead + f0 + f];
-    offs[u] = (unsigned long long)((off + rec_bytes) / 8) + reinterpret_cast<const uint32_t*>(rec + kTierRecHead + pad8(F))[f0 + f];
+    dir[u] = rec[kTierRecHead + rf];
+    offs[u] = (unsigned long long)((off + rec_bytes) / 8) + reinterpret_cast<const uint32_t*>(rec + kTierRecHead + pad8(F))[rf];
   }
 }
 
-// Ring samples into a virtual slot: the n samples of the runs (gpud_tier_run, ascending off) of fields [f0, f0 + G) from the ring to
-// their virtual columns, with the sample ring kept as k_ring_append keeps it.  The newest row, not yet coded, is one run; an untiered
-// ring's rows, or rows a tier does not hold, are the others.
+// Ring samples into a virtual slot: the n samples of the runs (gpud_tier_run, ascending off) of fields [f0, f0 + G) (FMAP: the fields
+// fmap[0, G)) from the ring to their virtual columns, with the sample ring kept as k_ring_append keeps it.  The newest row, not yet
+// coded, is one run; an untiered ring's rows, or rows a tier does not hold, are the others.
+template <bool FMAP>
 __global__ void __launch_bounds__(256) k_tier_ring_runs(const double* __restrict__ ring, int64_t cap, const gpud_tier_run* __restrict__ runs, int64_t n_runs,
                                                         int64_t n, int f0, int G, double* __restrict__ vring, int64_t vcap, double* __restrict__ vsmp,
-                                                        int smp_shift, int64_t smp_half, int64_t smp_slots) {
+                                                        int smp_shift, int64_t smp_half, int64_t smp_slots, const int32_t* __restrict__ fmap) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < (int64_t)G * n; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t f = i / n, t = i - f * n;
     int64_t lo = 0, hi = n_runs;                   // the run of sample t: the last whose off <= t
@@ -121,16 +125,18 @@ __global__ void __launch_bounds__(256) k_tier_ring_runs(const double* __restrict
       if (__ldg(&runs[mid].off) <= t) lo = mid; else hi = mid;
     }
     const int64_t d = t - __ldg(&runs[lo].off), c = __ldg(&runs[lo].vcol) + d;
-    const double x = ring[(f0 + f) * cap + (__ldg(&runs[lo].first) + d) % cap];
+    const int64_t rf = FMAP ? (int64_t)__ldg(fmap + f) : f0 + f;
+    const double x = ring[rf * cap + (__ldg(&runs[lo].first) + d) % cap];
     vring[f * vcap + c] = x;
     if ((c & ((1ll << smp_shift) - 1)) == smp_half) vsmp[f * smp_slots + (c >> smp_shift)] = x;
   }
 }
 
-cudaError_t launch_gather(const gpud_ring* r, const int64_t* rows, int64_t n, int f0, int G, const unsigned long long* buf, const int64_t* slot,
-                          int64_t R, uint8_t* dir, unsigned long long* offs) {
+cudaError_t launch_gather(const gpud_ring* r, const int64_t* rows, int64_t n, int f0, int G, const int32_t* fmap, const unsigned long long* buf,
+                          const int64_t* slot, int64_t R, uint8_t* dir, unsigned long long* offs) {
   const int grid = (int)std::min<int64_t>(((int64_t)G * n + 255) / 256, (int64_t)r->sm_count * 8);
-  k_tier_gather<<<grid, 256, 0, r->stream>>>(rows, n, f0, G, r->F, buf, slot, R, tier_rec_bytes(r->F), dir, offs);
+  const auto k = fmap ? k_tier_gather<true> : k_tier_gather<false>;
+  k<<<grid, 256, 0, r->stream>>>(rows, n, f0, G, r->F, buf, slot, R, tier_rec_bytes(r->F), dir, offs, fmap);
   return cudaGetLastError();
 }
 
@@ -166,7 +172,7 @@ struct RowCheck {
 
   cudaError_t run(const gpud_ring* r, const unsigned long long* buf, int64_t q0, int64_t m, unsigned long long* csum) const {
     if (m == 0) return cudaSuccess;
-    const cudaError_t e = launch_gather(r, d_rows + q0, m, 0, r->F, buf, d_rows + n, n, d_dir + r->F * q0, d_offs + r->F * q0);
+    const cudaError_t e = launch_gather(r, d_rows + q0, m, 0, r->F, nullptr, buf, d_rows + n, n, d_dir + r->F * q0, d_offs + r->F * q0);
     return e != cudaSuccess ? e : launch_unpack(r, false, rows_geo(r->F, m), d_dir + r->F * q0, d_offs + r->F * q0, buf, csum);
   }
 };
@@ -261,12 +267,12 @@ int32_t gpud_tier_read_ctl(gpud_ring* r, gpud_tier_ctl* c) {
   return GPUD_OK;
 }
 
-cudaError_t gpud_tier_decode(const gpud_ring* h, const gpud_ring* o, const int64_t* d_rows, int64_t n, int f0, int G, const gpud_vslot& s,
-                             int64_t vcol0, uint8_t* dir, unsigned long long* offs, unsigned long long* csum) {
+cudaError_t gpud_tier_decode(const gpud_ring* h, const gpud_ring* o, const int64_t* d_rows, int64_t n, int f0, int G, const int32_t* fmap,
+                             const gpud_vslot& s, int64_t vcol0, uint8_t* dir, unsigned long long* offs, unsigned long long* csum) {
   if (n == 0) return cudaSuccess;
   const gpud_tier* t = o->tier.get();
   // the gather and the unpack run on h; every ring of a call has h's F, so o's records have h's layout
-  const cudaError_t e = launch_gather(h, d_rows, n, f0, G, t->d_buf, t->d_slot, t->slots, dir, offs);
+  const cudaError_t e = launch_gather(h, d_rows, n, f0, G, fmap, t->d_buf, t->d_slot, t->slots, dir, offs);
   if (e != cudaSuccess) return e;
   CkGeo g = rows_geo(G, n);
   g.ring = s.ring; g.sample = s.sample; g.cap = s.vcap; g.start = vcol0;
@@ -275,11 +281,12 @@ cudaError_t gpud_tier_decode(const gpud_ring* h, const gpud_ring* o, const int64
 }
 
 cudaError_t gpud_tier_copy_runs(const gpud_ring* h, const gpud_ring* o, const gpud_tier_run* d_runs, int64_t n_runs, int64_t n_samples, int f0, int G,
-                                const gpud_vslot& s) {
+                                const int32_t* fmap, const gpud_vslot& s) {
   if (n_runs == 0 || n_samples == 0) return cudaSuccess;
   const int grid = (int)std::min<int64_t>(((int64_t)G * n_samples + 255) / 256, (int64_t)h->sm_count * 8);
-  k_tier_ring_runs<<<grid, 256, 0, h->stream>>>(o->d_ring, o->cap, d_runs, n_runs, n_samples, f0, G, s.ring, s.vcap, s.sample, s.smp_shift,
-                                                (1ll << s.smp_shift) >> 1, s.smp_slots);
+  const auto k = fmap ? k_tier_ring_runs<true> : k_tier_ring_runs<false>;
+  k<<<grid, 256, 0, h->stream>>>(o->d_ring, o->cap, d_runs, n_runs, n_samples, f0, G, s.ring, s.vcap, s.sample, s.smp_shift, (1ll << s.smp_shift) >> 1,
+                                 s.smp_slots, fmap);
   return cudaGetLastError();
 }
 

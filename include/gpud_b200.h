@@ -336,6 +336,20 @@ int32_t gpud_ring_reduce_range_sets(gpud_ring* ring, const int64_t* first, const
 int32_t gpud_rings_reduce_range_sets(gpud_ring* const* rings, int32_t n_rings, const int32_t* ring_of, const int64_t* first,
                                      const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets,
                                      double* out_f64 /*[5][F][n_sets]*/, uint32_t* out_n_over /*[F][n_sets]*/);
+/* Range sets over chosen fields (DESIGN.md §2 "Field selection"): gpud_rings_reduce_range_sets over the fields fields[0, n_fields) of
+ * the rings only, in any order, repeats allowed.  Column g of the output is field fields[g]: it equals row fields[g] of
+ * gpud_rings_reduce_range_sets over the same rings, ranges and sets, bit for bit in all six outputs.  Only the named fields are read,
+ * and a set that reaches a tier decodes only their blocks, so the work, the scratch and the segment limit scale with n_fields, not F.
+ * A one-ring call passes n_rings = 1 and ring_of = NULL; a call over plain ranges passes set_off = 0 .. n_ranges.  Every refusal of
+ * gpud_rings_reduce_range_sets applies, with the segment limit on n_fields x n_sets instead of F x n_sets; beyond them fields == NULL,
+ * n_fields < 1 and a field outside [0, F) give GPUD_E_INVALID; every refusal comes before any launch, writes nothing and names the
+ * argument in gpud_last_error.  n_sets = 0 returns 0 and touches nothing.  Shares the range calls' scratch and gpud_ring_ranges_stats
+ * (which report this call: its segments are the named fields'), and gpud_ring_tier_stats' decode time covers the named fields' decode;
+ * what gpud_rings_reduce_range_sets leaves reading the same, this call does too.  Synchronous. */
+int32_t gpud_rings_reduce_range_sets_fields(gpud_ring* const* rings, int32_t n_rings, const int32_t* ring_of, const int32_t* fields,
+                                            int32_t n_fields, const int64_t* first, const int64_t* len, int64_t n_ranges,
+                                            const int64_t* set_off, int64_t n_sets, double* out_f64 /*[5][n_fields][n_sets]*/,
+                                            uint32_t* out_n_over /*[n_fields][n_sets]*/);
 /* Box sets across processes (DESIGN.md §2 "Box sets across processes"): the range sets of gpud_rings_reduce_range_sets when each ring
  * belongs to its own process, rank r of a group of n_ranks owning ring r.  Every rank creates the query with the same arguments
  * (rank_of[i]: the rank whose ring holds range i; first / len in that ring's own push order; set_off) and passes only its own ring.
