@@ -755,7 +755,7 @@ class FabricVerdict(C.Structure):
 SYMBOLS = ["gpud_abi_version", "gpud_sizeof", "gpud_ctx_create", "gpud_ctx_destroy", "gpud_last_error", "gpud_host_alloc",
            "gpud_host_free", "gpud_ring_create", "gpud_ring_destroy", "gpud_ring_set_stream", "gpud_ring_push",
            "gpud_ring_push_device", "gpud_ring_push_raw", "gpud_clock_event_reasons", "gpud_hw_slowdown_event_message", "gpud_hw_slowdown_check", "gpud_store_insert_hw_slowdown", "gpud_store_open", "gpud_store_close", "gpud_store_last_error", "gpud_store_event_table", "gpud_store_insert_event", "gpud_store_insert_xid_hits", "gpud_store_metrics_table", "gpud_store_record_metrics", "gpud_kmsg_syncer_create", "gpud_kmsg_syncer_destroy", "gpud_kmsg_syncer_feed", "gpud_store_find_event", "gpud_store_record_reboot", "gpud_xid_state_from_store", "gpud_sxid_state_from_store", "gpud_store_get_events", "gpud_store_latest_event", "gpud_store_purge_events", "gpud_kmsg_syncer_configure", "gpud_kmsg_syncer_configure_component", "gpud_kmsg_syncer_offer", "gpud_ib_scan", "gpud_ib_reason", "gpud_poller_create", "gpud_poller_destroy", "gpud_poller_poll", "gpud_poller_last_rows", "gpud_poller_errors", "gpud_poll_row_hold", "gpud_nvml_devices", "gpud_nvml_devices_arg", "gpud_nvml_bus_id", "gpud_poller_remapped_rows", "gpud_remapped_rows_check", "gpud_poller_ecc_errors", "gpud_poller_field_row", "gpud_poller_poll_fields", "gpud_poller_gpm_supported", "gpud_poller_gpm_metrics", "gpud_poller_poll_gpm", "gpud_gpm_check", "gpud_poller_fabric_raw", "gpud_poller_product_name", "gpud_poller_temperature", "gpud_temperature_check", "gpud_temperature_reason", "gpud_poller_counters", "gpud_ring_counts", "gpud_ring_reduce", "gpud_ring_sync", "gpud_ring_kernel_ms", "gpud_ring_read",
-           "gpud_ring_result_ptr", "gpud_ring_stream_open", "gpud_ring_stream_reduce", "gpud_ring_stream_counts", "gpud_ring_stream_read", "gpud_ring_windows_open", "gpud_ring_windows_open_hop", "gpud_ring_windows_close", "gpud_ring_windows_reduce", "gpud_ring_windows_counts", "gpud_ring_windows_read", "gpud_ring_windows_stats", "gpud_ring_reduce_range", "gpud_ring_range_stats", "gpud_ring_reduce_ranges", "gpud_ring_reduce_range_sets", "gpud_rings_reduce_range_sets", "gpud_rings_reduce_range_sets_fields", "gpud_ring_ranges_stats", "gpud_box_query_create", "gpud_box_query_step", "gpud_box_query_result", "gpud_box_query_stats", "gpud_box_query_destroy", "gpud_ring_set_cta_reserve", "gpud_kmsg_scan", "gpud_kmsg_scan_sharded", "gpud_kmsg_scan_device", "gpud_kmsg_scan_kernel_ms", "gpud_kmsg_scan_phase_timing", "gpud_kmsg_scan_stats", "gpud_xid_classify",
+           "gpud_ring_result_ptr", "gpud_ring_stream_open", "gpud_ring_stream_reduce", "gpud_ring_stream_counts", "gpud_ring_stream_read", "gpud_ring_windows_open", "gpud_ring_windows_open_hop", "gpud_ring_windows_close", "gpud_ring_windows_reduce", "gpud_ring_windows_counts", "gpud_ring_windows_read", "gpud_ring_windows_stats", "gpud_ring_windows_open_fields", "gpud_ring_windows_fields", "gpud_ring_reduce_range", "gpud_ring_range_stats", "gpud_ring_reduce_ranges", "gpud_ring_reduce_range_sets", "gpud_rings_reduce_range_sets", "gpud_rings_reduce_range_sets_fields", "gpud_ring_ranges_stats", "gpud_box_query_create", "gpud_box_query_step", "gpud_box_query_result", "gpud_box_query_stats", "gpud_box_query_destroy", "gpud_ring_set_cta_reserve", "gpud_kmsg_scan", "gpud_kmsg_scan_sharded", "gpud_kmsg_scan_device", "gpud_kmsg_scan_kernel_ms", "gpud_kmsg_scan_phase_timing", "gpud_kmsg_scan_stats", "gpud_xid_classify",
            "gpud_hit_detail_json", "gpud_xid_description", "gpud_xid_mnemonic", "gpud_sxid_name", "gpud_nvlink_rule_hint", "gpud_sxid_reason", "gpud_sxid_get_detail", "gpud_store_insert_sxid_hits", "gpud_product_mem_caps", "gpud_product_fm_supported", "gpud_product_fabric_state_supported", "gpud_xid_get_detail", "gpud_xid_detail", "gpud_xid_build_message", "gpud_xid_hit_message", "gpud_xid_device_matches_bus_id", "gpud_kmsg_event_name", "gpud_kmsg_event_message", "gpud_kmsg_component", "gpud_kmsg_hit_message", "gpud_kmsg_stateful_create", "gpud_kmsg_stateful_destroy", "gpud_kmsg_stateful_feed", "gpud_component_create", "gpud_component_destroy", "gpud_component_name", "gpud_component_start", "gpud_component_check", "gpud_component_last_health_states", "gpud_component_events", "gpud_component_close", "gpud_component_checks", "gpud_component_xid_set_source", "gpud_component_xid_set_healthy", "gpud_component_xid_add_reboot", "gpud_component_xid_set_devices", "gpud_component_ring", "gpud_kmsg_stateful_feed_units", "gpud_kmsg_deduper_create", "gpud_kmsg_deduper_destroy", "gpud_kmsg_dedup_units",
            "gpud_kmsg_dedup_create", "gpud_kmsg_dedup_destroy", "gpud_kmsg_scan_dedup", "gpud_kmsg_dedup_stats",
            "gpud_fabric_issues", "gpud_fabric_suggest_reboot", "gpud_set_nvml_error_string", "gpud_nvml_error_strings_from_driver", "gpud_fabric_reason", "gpud_fabric_report_reason", "gpud_fabric_pack", "gpud_fabric_verdict_device", "gpud_comm_unique_id", "gpud_comm_init", "gpud_fabric_gather",
@@ -839,6 +839,8 @@ def lib() -> C.CDLL:
         "gpud_ring_windows_counts": (i32, [vp, C.POINTER(i64), C.POINTER(i64), C.POINTER(i64)]),
         "gpud_ring_windows_read": (i32, [vp, i32, i64, i64, vp, i64]),
         "gpud_ring_windows_stats": (i32, [vp, C.POINTER(C.c_float), C.POINTER(i64), vp]),
+        "gpud_ring_windows_open_fields": (i32, [vp, i64, i64, i64, vp, i32, C.POINTER(vp)]),
+        "gpud_ring_windows_fields": (i32, [vp, vp, i32, C.POINTER(i32)]),
         "gpud_ring_checkpoint_bound": (i32, [vp, C.POINTER(i64)]), "gpud_ring_checkpoint": (i32, [vp, vp, i64, C.POINTER(i64)]),
         "gpud_ring_restore": (i32, [vp, vp, i64, vp, i32, C.POINTER(C.c_int32)]),
         "gpud_ring_checkpoint_stats": (i32, [vp, C.POINTER(C.c_float), C.POINTER(C.c_float), vp]),
@@ -1312,10 +1314,11 @@ class Ring:
         self.ctx._check(self._L.gpud_ring_stream_read(self._h, OPS[op], first, n, C.c_void_p(out.ctypes.data), out.nbytes))
         return out
 
-    def windows(self, span: int, history: int = 0, hop: int = None) -> "RingWindows":
+    def windows(self, span: int, history: int = 0, hop: int = None, fields=None) -> "RingWindows":
         """stream windows of span x window samples each, one every hop x window samples (gpud_ring_windows_open_hop; hop None or
-        span: tumbling windows); history <= 0: ceil(capacity / (hop x window))"""
-        return RingWindows(self, span, history, hop)
+        span: tumbling windows); history <= 0: ceil(capacity / (hop x window)).  With a list of fields the handle reduces, keeps and
+        checkpoints only those (gpud_ring_windows_open_fields): its row g is field fields[g]."""
+        return RingWindows(self, span, history, hop, fields)
 
     def reduce_range(self, last_n: int = 0) -> dict:
         f64 = np.empty((5, self.F), dtype=np.float64)
@@ -1405,11 +1408,11 @@ class Ring:
         windows handles in the order they had been opened.  The stream handle, if there was one, is open again on the ring."""
         mv, src = _blob_ptr(blob)
         recs = checkpoint_handles(mv)
-        cap = sum(1 for kind, _, _ in recs if kind == 1)
+        cap = sum(1 for kind, _, _ in recs if kind != 0)
         hs = (C.c_void_p * max(1, cap))()
         n = C.c_int32()
         self.ctx._check(self._L.gpud_ring_restore(self._h, src, len(mv), hs, cap, C.byref(n)))
-        wins = [(span, hop) for kind, span, hop in recs if kind == 1]
+        wins = [(span, hop) for kind, span, hop in recs if kind != 0]
         return [RingWindows._adopt(self, hs[i], span, hop) for i, (span, hop) in enumerate(wins[:n.value])]
 
     # ---- delta checkpoints: only what changed since the last checkpoint written or loaded, full or delta ----
@@ -1507,8 +1510,9 @@ def _blob_ptr(blob):
 
 
 def checkpoint_handles(blob) -> List[tuple]:
-    """(kind, span, hop) of each handle record of a checkpoint (kind 0: the stream handle, 1: a windows handle), read from its header
-    and handle section (DESIGN.md "Ring checkpoint format"); [] for bytes too short to hold them"""
+    """(kind, span, hop) of each handle record of a checkpoint (kind 0: the stream handle, 1: a windows handle, 2: a windows handle
+    over chosen fields), read from its header and handle section (DESIGN.md "Ring checkpoint format"); [] for bytes too short to hold
+    them"""
     import struct
     mv = memoryview(blob).cast("B")
     if len(mv) < 128:
@@ -1520,9 +1524,15 @@ def checkpoint_handles(blob) -> List[tuple]:
         if off < 0 or off + 64 > len(mv):
             break
         kind, span, hop, _, first, nxt = struct.unpack_from("<6q", mv, off)
-        n = nxt - first
+        n, nf = nxt - first, F
         out.append((kind, span, hop))
-        off += 64 + 40 * F * n + ((4 * F * n + 7) & ~7) + 8 * F
+        off += 64
+        if kind == 2:
+            if off + 8 > len(mv):
+                break
+            nf = struct.unpack_from("<q", mv, off)[0]
+            off += 8 + ((4 * nf + 7) & ~7)
+        off += 40 * nf * n + ((4 * nf * n + 7) & ~7) + 8 * nf
     return out
 
 
@@ -1533,16 +1543,21 @@ class RingWindows:
     """gpud_ring_windows: window k = samples [kP, kP + L) of the ring's push order, L = span x window, P = hop x window, reduced once
     into a history.  The ring frees a handle that is still open when it is closed itself."""
 
-    def __init__(self, ring: Ring, span: int, history: int = 0, hop: int = None):
+    def __init__(self, ring: Ring, span: int, history: int = 0, hop: int = None, fields=None):
         self.ring, self.ctx, self._L = ring, ring.ctx, ring._L
         self.hop = span if hop is None else hop
         self.span, self.L, self.P = span, span * ring.W, self.hop * ring.W
         h = C.c_void_p()
-        if hop is None:
+        if fields is not None:
+            f = np.ascontiguousarray(fields, dtype=np.int32).reshape(-1)
+            self.ctx._check(self._L.gpud_ring_windows_open_fields(ring._h, span, self.hop, history, C.c_void_p(f.ctypes.data),
+                                                                  f.shape[0], C.byref(h)))
+        elif hop is None:
             self.ctx._check(self._L.gpud_ring_windows_open(ring._h, span, history, C.byref(h)))
         else:
             self.ctx._check(self._L.gpud_ring_windows_open_hop(ring._h, span, hop, history, C.byref(h)))
         self._h = h
+        self.n_fields = ring.F if fields is None else len(f)
 
     @classmethod
     def _adopt(cls, ring: Ring, handle, span: int, hop: int) -> "RingWindows":
@@ -1551,7 +1566,18 @@ class RingWindows:
         self.ring, self.ctx, self._L = ring, ring.ctx, ring._L
         self.span, self.hop, self.L, self.P = span, hop, span * ring.W, hop * ring.W
         self._h = C.c_void_p(handle)
+        self.n_fields = len(self.fields())
         return self
+
+    def fields(self) -> np.ndarray:
+        """the ring field of each row of the history (gpud_ring_windows_fields): the list of a handle over chosen fields, else 0 .. F - 1"""
+        n = C.c_int32()
+        rc = self._L.gpud_ring_windows_fields(self._h, None, 0, C.byref(n))
+        if rc not in (0, -4):
+            self.ctx._check(rc)
+        out = np.empty(n.value, dtype=np.int32)
+        self.ctx._check(self._L.gpud_ring_windows_fields(self._h, C.c_void_p(out.ctypes.data), n.value, C.byref(n)))
+        return out
 
     def close(self):
         if self._h and self.ring._h:
@@ -1571,8 +1597,8 @@ class RingWindows:
         return a.value, b.value, c.value
 
     def read(self, op: str, first: int, n: int) -> np.ndarray:
-        """windows [first, first + n) of one aggregate of the history, [F][n]"""
-        out = np.empty((self.ring.F, n), dtype=np.uint32 if op == "n_over" else np.float64)
+        """windows [first, first + n) of one aggregate of the history, [n_fields][n] (n_fields = F for an all-field handle)"""
+        out = np.empty((self.n_fields, n), dtype=np.uint32 if op == "n_over" else np.float64)
         self.ctx._check(self._L.gpud_ring_windows_read(self._h, OPS[op], first, n, C.c_void_p(out.ctypes.data), out.nbytes))
         return out
 

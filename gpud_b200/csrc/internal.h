@@ -292,9 +292,14 @@ __host__ __device__ inline int64_t gpud_tier_place(gpud_tier_ctl& c, int64_t* sl
 }
 
 // Stream windows of a ring (ring.cu, DESIGN.md §2): the aggregates of windows [first, next) of the sample stream, window k =
-// samples [kP, kP + L) with L = span * W and P = hop * W (hop = span: tumbling windows), in history slot k % H.
+// samples [kP, kP + L) with L = span * W and P = hop * W (hop = span: tumbling windows), in history slot k % H.  A handle over
+// chosen fields (DESIGN.md §2 "Field selection") has nf of them: its field g is the ring's field fields[g] wherever ring data is read
+// (samples, sample ring, thresholds, the EMA seed), and every array below counts nf fields; an all-field handle has nf = F.
 struct gpud_ring_windows {
   gpud_ring* ring = nullptr;
+  int nf = 0;                          // the handle's fields
+  std::vector<int32_t> fields;         // ... a handle over chosen fields: their ring fields (empty: every field, in order)
+  gpud_buf<int32_t> d_fmap;            // ... and the same on the device (gpud_ring_view::d_fmap; NULL for an all-field handle)
   int64_t span = 1, hop = 1, L = 0, P = 0;
   int Wp = 0;                          // L > GPUD_MAX_WINDOW: sub-window of the range pass (W times the largest divisor g of span with W g <= 1024)
   int Wq = 0;                          // sub-window of the EMA partials: P up to GPUD_MAX_WINDOW, else W g for the largest divisor g of hop with
@@ -303,9 +308,9 @@ struct gpud_ring_windows {
   int64_t first = 0, next = 0, lost = 0;
   bool reseed = true;                  // the next commit seeds the EMA with the ring's sample at window next's start (open, loss)
   int64_t ck_next = 0;                 // `next` at the ring's chain marker (ring_ckpt.cu)
-  gpud_buf<double> d_hist;             // [5][F][H] f64, aggregate GPUD_OP_MIN..GPUD_OP_P99
-  gpud_buf<uint32_t> d_hist_nover;     // [F][H]
-  gpud_buf<double> d_ema;              // [F] EMA at the last sample of window next - 1
+  gpud_buf<double> d_hist;             // [5][nf][H] f64, aggregate GPUD_OP_MIN..GPUD_OP_P99
+  gpud_buf<uint32_t> d_hist_nover;     // [nf][H]
+  gpud_buf<double> d_ema;              // [nf] EMA at the last sample of window next - 1
   gpud_buf<double> d_sc;               // L <= GPUD_MAX_WINDOW: [5][F][ceil(CAP / L)] window-pass output of the new windows: MIN, MAX,
                                        // MEAN, P99 and, in slot GPUD_OP_EMA, the EMA partials; [F][n_new] packed at the start of each
   gpud_buf<uint32_t> d_sc_nover;       // [F][ceil(CAP / L)]
@@ -390,28 +395,33 @@ __host__ __device__ __forceinline__ long long gpud_rank_from_top(long long n, in
 }
 #endif
 
-// ring.cu: open a windows handle of the ring (gpud_ring_windows_open_hop's checks, history_windows <= 0: the default) without
-// registering it anywhere.  ring_ckpt.cu re-creates a checkpoint's handles through it.
-int32_t gpud_ring_windows_new(gpud_ring* r, int64_t span, int64_t hop, int64_t history_windows, std::unique_ptr<gpud_ring_windows>* out);
+// ring.cu: open a windows handle of the ring (gpud_ring_windows_open_hop's checks, history_windows <= 0: the default; fields non-NULL:
+// gpud_ring_windows_open_fields' checks and a handle over fields[0, n_fields)) without registering it anywhere.  ring_ckpt.cu
+// re-creates a checkpoint's handles through it.
+int32_t gpud_ring_windows_new(gpud_ring* r, int64_t span, int64_t hop, int64_t history_windows, const int32_t* fields, int32_t n_fields,
+                              std::unique_ptr<gpud_ring_windows>* out);
 
-// ring.cu: the window pass and the EMA carry over chronological samples [start, start + n) of the ring with window Wp, into the
-// caller's buffers w[0..4] = per-window min, max, mean, EMA, EMA partial sums and w_nover, each [F][nw], nw = ceil(n / Wp).  With piv
+// ring.cu: the window pass and the EMA carry over chronological samples [start, start + n) of F fields of the ring with window Wp, into
+// the caller's buffers w[0..4] = per-window min, max, mean, EMA, EMA partial sums and w_nover, each [F][nw], nw = ceil(n / Wp).  F is
+// the ring's and fmap NULL, or fmap [F] (device memory) names the ring field of each pass field (no EMA carry then).  With piv
 // the pass also classifies every sample against the field's pivots lo = piv[2f], hi = piv[2f + 1]: class counts {above hi, == hi,
 // == lo, strictly inside} per window into w_cls, the keys strictly inside into lists [F][list_cap] behind the counters fill [F].
 // Segments: with seg_sub > 0 every seg_sub consecutive windows of a field form one segment, window w of field f uses segment
 // sg = f (nw / seg_sub) + w / seg_sub's pivots, fill counter and list [sg list_cap, (sg + 1) list_cap); seg_sub = 0 is one segment
 // per field.  These are the rows and lists of the segment select's table for n_geo = nw / seg_sub equal segments (gpud_range_geo
 // below: tile0 = j seg_sub, list0 = j list_cap).  w[3] == NULL: no EMA carry.
-int32_t gpud_ring_window_pass(gpud_ring* r, int64_t start, int64_t n, int Wp, double* const w[5], uint32_t* w_nover,
+int32_t gpud_ring_window_pass(gpud_ring* r, int F, const int32_t* fmap, int64_t start, int64_t n, int Wp, double* const w[5], uint32_t* w_nover,
                               const double* piv, uint4* w_cls, unsigned long long* lists, unsigned* fill, unsigned list_cap, int seg_sub);
 
-// select.cu: exact aggregates of n_seg consecutive segments of seg_len samples of every field, from physical ring column `start`
-// on: a segment select whose table entry j is samples [start + j seg_len, start + (j + 1) seg_len), for every field.  The window pass
+// select.cu: exact aggregates of n_seg consecutive segments of seg_len samples of every field of the view v of ring r (v.F fields, its
+// d_fmap naming their ring fields), from physical ring column `start` on: a segment select whose table entry j is samples
+// [start + j seg_len, start + (j + 1) seg_len), for every field.  The window pass
 // runs in sub-windows of Wp samples (Wp divides seg_len, Wp <= GPUD_MAX_WINDOW).  Synchronises the ring's stream once (the radix
 // select's grid is sized by the segments left open) and leaves the results on the device, valid until the next call on *st:
 // out [5][F n_seg] (MIN, MAX, MEAN, -, P99: no EMA), nover [F n_seg], part [F][n_seg seg_len / Wp] the sub-windows' EMA partial sums.
 struct gpud_seg_out { const double* out; const uint32_t* nover; const double* part; int64_t open; const int* reasons; };
-int32_t gpud_ring_segments(gpud_ring* r, std::unique_ptr<gpud_range_state>& st, int64_t start, int64_t seg_len, int64_t n_seg, int Wp, gpud_seg_out* out);
+int32_t gpud_ring_segments(const gpud_ring_view& v, gpud_ring* r, std::unique_ptr<gpud_range_state>& st, int64_t start, int64_t seg_len, int64_t n_seg,
+                           int Wp, gpud_seg_out* out);
 
 // gpud_ring_reduce_ranges and gpud_rings_reduce_range_sets (ranges.cu, DESIGN.md §2 "Ranges", "Range sets", "Box sets").  A set of
 // several ranges, or of one range in a ring other than the home ring, reads its samples through the call's piece table: piece i of a

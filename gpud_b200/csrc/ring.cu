@@ -16,6 +16,7 @@
 #include <stdarg.h>
 
 #include <algorithm>
+#include <type_traits>
 
 #include "../../include/gpud_b200_hooks.h"
 #include "segsel.h"
@@ -65,6 +66,9 @@ struct WinParams {
   // RANGE over segments: window w of field f belongs to segment f * (nw / seg_sub) + w / seg_sub, and piv / lists / fill are per
   // segment instead of per field (seg_sub = nw: one segment per field).  Last member: the other instantiations' parameter offsets stay.
   int seg_sub;
+  // FMAP instantiations only (a windows handle over chosen fields): field f of the launch reads the ring's field fmap[f] - its
+  // samples and threshold - while every output keeps index f.  After seg_sub for the same reason.
+  const int32_t* fmap;   // [F]
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -323,6 +327,9 @@ __device__ __forceinline__ unsigned extreme_lo(const unsigned long long* sk, uns
 }
 
 struct WinUnit { int f, w, m; int64_t p0; };
+struct WinUnitF : WinUnit { int rf; };   // FMAP: and the ring field of f
+__device__ __forceinline__ int ring_field(const WinUnit& q) { return q.f; }
+__device__ __forceinline__ int ring_field(const WinUnitF& q) { return q.rf; }
 // streaming 128-bit load: read-only path, no L1 allocation, 256-byte L2 sector promotion
 __device__ __forceinline__ double2 ld_stream(const double2* p) {
   double2 r;
@@ -398,9 +405,10 @@ __device__ __forceinline__ uint4 classify_window(const WinParams& p, const unsig
 }
 
 // The warp loop of k_window_reduce: reduces the units it claims from the work cursor until the cursor runs out and returns how
-// many it reduced.  TAIL: the units are the w_skip[0..n_tail) windows of every field (claimed from cursor[1]).
+// many it reduced.  TAIL: the units are the w_skip[0..n_tail) windows of every field (claimed from cursor[1]).  FMAP: the unit's
+// samples and threshold are the ring field p.fmap[f]'s, looked up once per unit when it is fetched.
 // Nothing reads the count.  It stays because without it ptxas (CUDA 12.9) emits pass 1's four accumulator zeroings in another order.
-template <bool ALIGNED, int JF, bool RANGE, bool TAIL>
+template <bool ALIGNED, int JF, bool RANGE, bool TAIL, bool FMAP>
 __device__ __forceinline__ int window_loop(const WinParams& p) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   const int lane = threadIdx.x & 31;
@@ -445,11 +453,12 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
   };
   int n_done = 0;
 
+  using Unit = std::conditional_t<FMAP, WinUnitF, WinUnit>;
   constexpr int PF = (ALIGNED && JF >= 0) ? kPrefetchPairs : 16;
   double2 v[16];                 // the window in flight: loaded for the NEXT unit while the current one is post-processed
   double thr_next = 0.0, lo_next = 0.0, hi_next = 0.0;
-  auto load_unaligned = [&](const WinUnit& q) {
-    const double* __restrict__ base = p.ring + (int64_t)q.f * p.cap;
+  auto load_unaligned = [&](const Unit& q) {
+    const double* __restrict__ base = p.ring + (int64_t)ring_field(q) * p.cap;
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
       const int t0 = 64 * j + 2 * lane;
@@ -459,8 +468,8 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
     }
   };
   // register pairs [j0, j1) of an aligned window.  The loop walks all 16 pairs: starting it at j0 moves registers in <true, 15, false>.
-  auto load_pairs = [&](const WinUnit& q, int j0, int j1) {
-    const double2* __restrict__ b2 = reinterpret_cast<const double2*>(p.ring + (int64_t)q.f * p.cap + q.p0) + lane;
+  auto load_pairs = [&](const Unit& q, int j0, int j1) {
+    const double2* __restrict__ b2 = reinterpret_cast<const double2*>(p.ring + (int64_t)ring_field(q) * p.cap + q.p0) + lane;
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
       if (j < j0 || j >= j1) continue;
@@ -473,7 +482,7 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
   // slower: choosing the next unit BEFORE pass 1 (its address/threshold registers live through pass 1) and issuing each
   // pair's load inside pass 1 right after the pair is consumed.  TAIL loads nothing ahead: a warp reduces at most a few tail
   // units, and without a window in flight during the post-processing the tail loop fits the hot kernel's 128 registers.
-  auto fetch = [&](WinUnit& q) -> bool {
+  auto fetch = [&](Unit& q) -> bool {
     for (;;) {
       if (u >= u_end && !take_run()) return false;
       q.f = uf;
@@ -486,7 +495,8 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
     q.m = JF >= 0 ? p.W : (int)min((int64_t)p.W, p.count - c0);
     q.p0 = p.start + c0;
     if (q.p0 >= p.cap) q.p0 -= p.cap;
-    thr_next = __ldg(p.thr + q.f);
+    if constexpr (FMAP) q.rf = __ldg(p.fmap + q.f);
+    thr_next = __ldg(p.thr + ring_field(q));
     if (RANGE) {
       // the segment is computed again where the classification needs it: a variable carried to there reorders pass 1's
       // accumulator zeroings in the RANGE = false instantiations (ptxas, CUDA 12.9)
@@ -498,12 +508,12 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
     return true;
   };
 
-  auto fetch_rest = [&](const WinUnit& q) {
+  auto fetch_rest = [&](const Unit& q) {
     if (TAIL) load_unaligned(q);
     if (PF < 16) load_pairs(q, PF, 16);
   };
 
-  WinUnit cur, nxt;
+  Unit cur, nxt;
   bool have = fetch(cur);
   while (have) {
     ++n_done;
@@ -742,11 +752,12 @@ __device__ __forceinline__ int window_loop(const WinParams& p) {
 
 // The trailing partial window and the window that wraps the physical end of the ring (w_skip) need the generic code; an aligned
 // launch reduces them itself once its cursor has run out (n_tail > 0), through the same loop instantiated for them.
-template <bool ALIGNED, int JF, bool RANGE>
+// FMAP: a windows handle over chosen fields (WinParams::fmap).
+template <bool ALIGNED, int JF, bool RANGE, bool FMAP>
 __global__ void __launch_bounds__(kWarpsPerBlock * 32, kCtasPerSM) k_window_reduce(const WinParams p) {
-  window_loop<ALIGNED, JF, RANGE, false>(p);
+  window_loop<ALIGNED, JF, RANGE, false, FMAP>(p);
   if constexpr (ALIGNED) {
-    if (p.n_tail > 0) window_loop<false, -1, RANGE, true>(p);
+    if (p.n_tail > 0) window_loop<false, -1, RANGE, true, FMAP>(p);
   }
 }
 
@@ -819,14 +830,16 @@ __global__ void __launch_bounds__(128) k_ema_carry(const double* __restrict__ pa
 // EMA (n_part > 0): part [F][n_part] holds the EMA partials of consecutive sub-windows, each with the decay d_full.  The EMA is the
 // carry's scan over all of them from the field's stored state, or, when reseed is set (open, loss), from the ring's sample at
 // physical column seed_col.  Sub-windows e_first, e_first + e_step, ... end windows ek0, ek0 + 1, ...: their scan values are
-// those windows' EMAs, written into slot (ek0 + j) % H.  n_part = 0: no scan, the stored state stays.
-template <bool GUARD>
+// those windows' EMAs, written into slot (ek0 + j) % H.  n_part = 0: no scan, the stored state stays.  FMAP: a handle over chosen
+// fields, whose field f re-seeds from the ring's field fmap[f].
+template <bool GUARD, bool FMAP>
 __global__ void __launch_bounds__(128) k_stream_commit(const double* __restrict__ sc, const uint32_t* __restrict__ sc_nover, int64_t sc_stride,
                                                         int n_sc, int n_skip, int64_t k0, int64_t k_step,
                                                         const double* __restrict__ part, int n_part, int e_first, int e_step, int64_t ek0,
                                                         const double* __restrict__ ring, int64_t cap, int64_t seed_col, int reseed,
                                                         int64_t H, double d_full,
-                                                        double* __restrict__ ema_state, double* __restrict__ hist, uint32_t* __restrict__ hist_nover, int F) {
+                                                        double* __restrict__ ema_state, double* __restrict__ hist, uint32_t* __restrict__ hist_nover, int F,
+                                                        const int32_t* __restrict__ fmap) {
   __shared__ double s_warp[4];
   __shared__ double s_carry;
   const int f = blockIdx.x, t = threadIdx.x;
@@ -844,7 +857,7 @@ __global__ void __launch_bounds__(128) k_stream_commit(const double* __restrict_
   if (n_part == 0) return;
   double* __restrict__ O = hist + GPUD_OP_EMA * hop + fh;
   decayed_scan<GUARD>(part + (int64_t)f * n_part, n_part, d_full, s_warp, s_carry,
-                      [&] { return reseed ? ring[(int64_t)f * cap + seed_col] : ema_state[f]; },
+                      [&] { return reseed ? ring[(int64_t)(FMAP ? __ldg(fmap + f) : f) * cap + seed_col] : ema_state[f]; },
                       [&](int v, double e) {
                         const int j = (v - e_first) / e_step;
                         if (v >= e_first && v - j * e_step == e_first) O[(ek0 + j) % H] = e;
@@ -1334,16 +1347,22 @@ static void set_schedule(WinParams& p, int64_t units, int64_t warps) {
   p.n_runs = kRunWindows > 1 ? std::max<int64_t>(0, (units - warps * kRunWindows / 2) / kRunWindows) : 0;
 }
 
-template <bool ALIGNED, int JF, bool RANGE>
-static cudaError_t launch_one(gpud_ring* r, WinParams p, int64_t units) {
+template <bool ALIGNED, int JF, bool RANGE, bool FMAP>
+static cudaError_t launch_kernel(gpud_ring* r, WinParams p, int64_t units) {
   // persistent grid: kCtasPerSM CTAs of kWarpsPerBlock warps per SM, a whole number of waves
   // 72 KB of dynamic shared memory per CTA (8 warps x (32 x 272 B key rows + candidate list)): opt in above 48 KB
-  cudaError_t e = cudaFuncSetAttribute(k_window_reduce<ALIGNED, JF, RANGE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBlockSmemBytes);
+  cudaError_t e = cudaFuncSetAttribute(k_window_reduce<ALIGNED, JF, RANGE, FMAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBlockSmemBytes);
   if (e != cudaSuccess) return e;
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((units + kWarpsPerBlock - 1) / kWarpsPerBlock, (int64_t)r->sm_count * kCtasPerSM - r->cta_reserve));
   set_schedule(p, units, (int64_t)grid * kWarpsPerBlock);
-  k_window_reduce<ALIGNED, JF, RANGE><<<grid, kWarpsPerBlock * 32, kBlockSmemBytes, r->stream>>>(p);
+  k_window_reduce<ALIGNED, JF, RANGE, FMAP><<<grid, kWarpsPerBlock * 32, kBlockSmemBytes, r->stream>>>(p);
   return cudaGetLastError();
+}
+
+// p.fmap picks the instantiation: a pass over a handle's chosen fields, or over every field of the ring
+template <bool ALIGNED, int JF, bool RANGE>
+static cudaError_t launch_one(gpud_ring* r, const WinParams& p, int64_t units) {
+  return p.fmap ? launch_kernel<ALIGNED, JF, RANGE, true>(r, p, units) : launch_kernel<ALIGNED, JF, RANGE, false>(r, p, units);
 }
 
 template <bool RANGE>
@@ -1564,17 +1583,24 @@ extern "C" int32_t gpudh_ring_hop_plan(int64_t total, int64_t cap, int32_t W, in
   return (int32_t)n_ph;
 }
 
-static int32_t windows_open(gpud_ring* r, int64_t span, int64_t hop, int64_t history_windows, std::unique_ptr<gpud_ring_windows>* out) {
+int32_t gpud_ring_windows_new(gpud_ring* r, int64_t span, int64_t hop, int64_t history_windows, const int32_t* fields, int32_t n_fields,
+                              std::unique_ptr<gpud_ring_windows>* out) {
   if (span < 1 || span > r->cap / r->W)
     return gpud_fail(r->ctx, GPUD_E_INVALID, "windows of span %lld x %d samples do not fit the ring's %lld", (long long)span, r->W, (long long)r->cap);
   if (hop < 1 || hop > span || span % hop != 0)
     return gpud_fail(r->ctx, GPUD_E_INVALID, "hop %lld must divide span %lld", (long long)hop, (long long)span);
+  if (fields && n_fields < 1) return gpud_fail(r->ctx, GPUD_E_INVALID, "windows over fields: n_fields %d, at least 1", n_fields);
+  for (int32_t g = 0; fields && g < n_fields; ++g)
+    if (fields[g] < 0 || fields[g] >= r->F)
+      return gpud_fail(r->ctx, GPUD_E_INVALID, "windows over fields: fields[%d] = %d is not a field of the ring's %d", g, fields[g], r->F);
+  const int nf = fields ? n_fields : r->F;
   const int64_t L = span * r->W, P = hop * r->W;
   const int64_t H = history_windows > 0 ? history_windows : (r->cap + P - 1) / P;
-  if (H > ((int64_t)1 << 40) / r->F) return gpud_fail(r->ctx, GPUD_E_INVALID, "history of %lld windows is too long", (long long)H);
+  if (H > ((int64_t)1 << 40) / nf) return gpud_fail(r->ctx, GPUD_E_INVALID, "history of %lld windows is too long", (long long)H);
   GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
   auto s = std::make_unique<gpud_ring_windows>();
   s->ring = r;
+  s->nf = nf;
   s->span = span;
   s->hop = hop;
   s->L = L;
@@ -1583,27 +1609,28 @@ static int32_t windows_open(gpud_ring* r, int64_t span, int64_t hop, int64_t his
   s->Wq = sub_window(r->W, hop);
   s->H = H;
   s->first = s->next = stream_plan(r->total, r->cap, L, P, H, 0, 0).reducible_from;
-  cudaError_t e = s->d_hist.alloc((size_t)5 * r->F * H);
-  if (e == cudaSuccess) e = s->d_hist_nover.alloc((size_t)r->F * H);
-  if (e == cudaSuccess) e = s->d_ema.alloc((size_t)r->F);
+  cudaError_t e = s->d_hist.alloc((size_t)5 * nf * H);
+  if (e == cudaSuccess) e = s->d_hist_nover.alloc((size_t)nf * H);
+  if (e == cudaSuccess) e = s->d_ema.alloc((size_t)nf);
   if (L <= GPUD_MAX_WINDOW) {
     s->sc_cols = (r->cap + L - 1) / L;
-    if (e == cudaSuccess) e = s->d_sc.alloc((size_t)5 * r->F * s->sc_cols);
-    if (e == cudaSuccess) e = s->d_sc_nover.alloc((size_t)r->F * s->sc_cols);
+    if (e == cudaSuccess) e = s->d_sc.alloc((size_t)5 * nf * s->sc_cols);
+    if (e == cudaSuccess) e = s->d_sc_nover.alloc((size_t)nf * s->sc_cols);
   }
   if (P < L) {
     s->eq_cols = (r->cap + s->Wq - 1) / s->Wq;
-    if (e == cudaSuccess) e = s->d_eq.alloc((size_t)4 * r->F * s->eq_cols);
-    if (e == cudaSuccess) e = s->d_eq_nover.alloc((size_t)r->F * s->eq_cols);
+    if (e == cudaSuccess) e = s->d_eq.alloc((size_t)4 * nf * s->eq_cols);
+    if (e == cudaSuccess) e = s->d_eq_nover.alloc((size_t)nf * s->eq_cols);
+  }
+  if (fields) {
+    s->fields.assign(fields, fields + nf);
+    if (e == cudaSuccess) e = s->d_fmap.alloc((size_t)nf);
+    if (e == cudaSuccess) e = cudaMemcpy(s->d_fmap, fields, (size_t)nf * sizeof(int32_t), cudaMemcpyHostToDevice);
   }
   for (int i = 0; i < 2 && e == cudaSuccess; ++i) e = s->ev[i].make();
   if (e != cudaSuccess) return gpud_fail(r->ctx, e == cudaErrorMemoryAllocation ? GPUD_E_NOMEM : GPUD_E_CUDA, "windows_open: %s", cudaGetErrorString(e));
   *out = std::move(s);
   return GPUD_OK;
-}
-
-int32_t gpud_ring_windows_new(gpud_ring* r, int64_t span, int64_t hop, int64_t history_windows, std::unique_ptr<gpud_ring_windows>* out) {
-  return windows_open(r, span, hop, history_windows, out);
 }
 
 // The device work of a tumbling handle of span s on n consecutive windows of L from physical column start: their aggregates, and
@@ -1614,8 +1641,10 @@ static int32_t reduce_phase(gpud_ring_windows* s, int64_t start, int64_t n, Phas
   gpud_ring* r = s->ring;
   if (s->L <= GPUD_MAX_WINDOW) {
     // the windows are one range of the ring: the window pass runs on it as on any other, into the handle's scratch
-    po->stride = (int64_t)r->F * s->sc_cols;
+    po->stride = (int64_t)s->nf * s->sc_cols;
     WinParams p = win_params(r, start, n * s->L, (int)s->L, r->d_cursor);
+    p.F = s->nf;
+    p.fmap = s->d_fmap;
     p.out_min = s->d_sc + GPUD_OP_MIN * po->stride; p.out_max = s->d_sc + GPUD_OP_MAX * po->stride; p.out_mean = s->d_sc + GPUD_OP_MEAN * po->stride;
     p.out_p99 = s->d_sc + GPUD_OP_P99 * po->stride; p.part = s->d_sc + GPUD_OP_EMA * po->stride; p.out_nover = s->d_sc_nover; p.do_select = 1;
     { int32_t rc = launch_windows<false>(r, p); if (rc) return rc; }
@@ -1623,8 +1652,11 @@ static int32_t reduce_phase(gpud_ring_windows* s, int64_t start, int64_t n, Phas
   } else {
     // every window of every field is one segment of the range pass, which runs in sub-windows of Wp samples
     gpud_seg_out o;
-    { int32_t rc = gpud_ring_segments(r, s->seg, start, s->L, n, s->Wp, &o); if (rc) return rc; }
-    po->stride = (int64_t)r->F * n;
+    gpud_ring_view v = gpud_view(r);
+    v.F = s->nf;
+    v.d_fmap = s->d_fmap;
+    { int32_t rc = gpud_ring_segments(v, r, s->seg, start, s->L, n, s->Wp, &o); if (rc) return rc; }
+    po->stride = (int64_t)s->nf * n;
     po->sc = o.out; po->nover = o.nover; po->part = o.part;
     s->seg_open += o.open;
     for (int i = 0; i < GPUD_RANGE_N_OPEN_REASONS; ++i) s->seg_reasons[i] += o.reasons[i];
@@ -1648,9 +1680,9 @@ static int32_t windows_reduce(gpud_ring_windows* s, int64_t* n_new, int64_t* n_l
     const int64_t p = s->L / s->P;
     const double* part = nullptr;
     if (p > 1) {
-      const int64_t c = (int64_t)r->F * s->eq_cols;
+      const int64_t c = (int64_t)s->nf * s->eq_cols;
       double* const w[5] = {s->d_eq, s->d_eq + c, s->d_eq + 2 * c, nullptr, s->d_eq + 3 * c};
-      { int32_t rc = gpud_ring_window_pass(r, ep.start, ep.n, s->Wq, w, s->d_eq_nover, nullptr, nullptr, nullptr, nullptr, 0, 0); if (rc) return rc; }
+      { int32_t rc = gpud_ring_window_pass(r, s->nf, s->d_fmap, ep.start, ep.n, s->Wq, w, s->d_eq_nover, nullptr, nullptr, nullptr, nullptr, 0, 0); if (rc) return rc; }
       part = w[4];
     }
     s->seg_open = 0;
@@ -1665,14 +1697,11 @@ static int32_t windows_reduce(gpud_ring_windows* s, int64_t* n_new, int64_t* n_l
       { int32_t rc = reduce_phase(s, ph.start, ph.n, &o); if (rc) return rc; }
       if (p == 1) part = o.part;
       const int n_part = i == n_ph - 1 ? (int)(ep.n / s->Wq) : 0;
-      if (guard)
-        k_stream_commit<true><<<r->F, 128, 0, r->stream>>>(o.sc, o.nover, o.stride, (int)ph.n, (int)ph.n_skip, ph.k, p, part, n_part, (int)ep.e_first,
-                                                           (int)ep.e_step, pl.write_from, r->d_ring, r->cap, ep.start, reseed, s->H, d_full,
-                                                           s->d_ema, s->d_hist, s->d_hist_nover, r->F);
-      else
-        k_stream_commit<false><<<r->F, 128, 0, r->stream>>>(o.sc, o.nover, o.stride, (int)ph.n, (int)ph.n_skip, ph.k, p, part, n_part, (int)ep.e_first,
-                                                            (int)ep.e_step, pl.write_from, r->d_ring, r->cap, ep.start, reseed, s->H, d_full,
-                                                            s->d_ema, s->d_hist, s->d_hist_nover, r->F);
+      using K = decltype(&k_stream_commit<false, false>);
+      const K ks[2][2] = {{k_stream_commit<false, false>, k_stream_commit<false, true>}, {k_stream_commit<true, false>, k_stream_commit<true, true>}};
+      ks[guard][s->d_fmap.get() != nullptr]<<<s->nf, 128, 0, r->stream>>>(o.sc, o.nover, o.stride, (int)ph.n, (int)ph.n_skip, ph.k, p, part, n_part,
+                                                                         (int)ep.e_first, (int)ep.e_step, pl.write_from, r->d_ring, r->cap, ep.start,
+                                                                         reseed, s->H, d_full, s->d_ema, s->d_hist, s->d_hist_nover, s->nf, s->d_fmap);
       GPUD_CUDA(r->ctx, cudaGetLastError());
     }
     GPUD_CUDA(r->ctx, cudaEventRecord(s->ev[1], r->stream));
@@ -1695,16 +1724,16 @@ static int32_t windows_read(const gpud_ring_windows* s, int32_t op, int64_t firs
     return gpud_fail(r->ctx, GPUD_E_INVALID, "windows [%lld, %lld) are not all in the history [%lld, %lld)", (long long)first_window,
                      (long long)(first_window + n), (long long)s->first, (long long)s->next);
   const size_t el = op == GPUD_OP_NOVER ? sizeof(uint32_t) : sizeof(double);
-  const size_t need = (size_t)r->F * n * el;
+  const size_t need = (size_t)s->nf * n * el;
   if ((size_t)out_bytes < need) return gpud_fail(r->ctx, GPUD_E_CAPACITY, "need %zu bytes", need);
   GPUD_CUDA(r->ctx, cudaSetDevice(r->dev));
-  const char* src = op == GPUD_OP_NOVER ? (const char*)s->d_hist_nover.get() : (const char*)(s->d_hist + (size_t)op * r->F * s->H);
-  // the windows sit in slots first_window % H onwards, wrapping at most once: two strided copies of F rows
+  const char* src = op == GPUD_OP_NOVER ? (const char*)s->d_hist_nover.get() : (const char*)(s->d_hist + (size_t)op * s->nf * s->H);
+  // the windows sit in slots first_window % H onwards, wrapping at most once: two strided copies of the handle's rows
   const int64_t slot = n ? first_window % s->H : 0, n1 = std::min(n, s->H - slot);
   if (n1 > 0)
-    GPUD_CUDA(r->ctx, cudaMemcpy2DAsync(out, n * el, src + slot * el, s->H * el, n1 * el, r->F, cudaMemcpyDeviceToHost, r->stream));
+    GPUD_CUDA(r->ctx, cudaMemcpy2DAsync(out, n * el, src + slot * el, s->H * el, n1 * el, s->nf, cudaMemcpyDeviceToHost, r->stream));
   if (n > n1)
-    GPUD_CUDA(r->ctx, cudaMemcpy2DAsync((char*)out + n1 * el, n * el, src, s->H * el, (n - n1) * el, r->F, cudaMemcpyDeviceToHost, r->stream));
+    GPUD_CUDA(r->ctx, cudaMemcpy2DAsync((char*)out + n1 * el, n * el, src, s->H * el, (n - n1) * el, s->nf, cudaMemcpyDeviceToHost, r->stream));
   GPUD_CUDA(r->ctx, cudaStreamSynchronize(r->stream));
   return GPUD_OK;
 }
@@ -1713,7 +1742,7 @@ static int32_t windows_read(const gpud_ring_windows* s, int32_t op, int64_t firs
 extern "C" int32_t gpud_ring_stream_open(gpud_ring* r, int64_t history_windows) {
   if (!r) return GPUD_E_INVALID;
   if (r->swin) return gpud_fail(r->ctx, GPUD_E_STATE, "the ring's stream windows are already open");
-  { int32_t rc = windows_open(r, 1, 1, history_windows, &r->swin); if (rc) return rc; }
+  { int32_t rc = gpud_ring_windows_new(r, 1, 1, history_windows, nullptr, 0, &r->swin); if (rc) return rc; }
   ++r->handle_gen;   // a delta checkpoint cannot span a change of the handle set
   return GPUD_OK;
 }
@@ -1737,18 +1766,39 @@ extern "C" int32_t gpud_ring_stream_read(gpud_ring* r, int32_t op, int64_t first
 }
 
 // gpud_ring_windows_*: handles of any span and hop
-extern "C" int32_t gpud_ring_windows_open_hop(gpud_ring* r, int64_t span, int64_t hop, int64_t history_windows, gpud_ring_windows** out) {
-  if (!r || !out) return GPUD_E_INVALID;
+static int32_t windows_register(gpud_ring* r, int64_t span, int64_t hop, int64_t history_windows, const int32_t* fields, int32_t n_fields,
+                                 gpud_ring_windows** out) {
   std::unique_ptr<gpud_ring_windows> s;
-  { int32_t rc = windows_open(r, span, hop, history_windows, &s); if (rc) return rc; }
+  { int32_t rc = gpud_ring_windows_new(r, span, hop, history_windows, fields, n_fields, &s); if (rc) return rc; }
   *out = s.get();
   r->handles.push_back(std::move(s));
   ++r->handle_gen;
   return GPUD_OK;
 }
 
+extern "C" int32_t gpud_ring_windows_open_hop(gpud_ring* r, int64_t span, int64_t hop, int64_t history_windows, gpud_ring_windows** out) {
+  if (!r || !out) return GPUD_E_INVALID;
+  return windows_register(r, span, hop, history_windows, nullptr, 0, out);
+}
+
 extern "C" int32_t gpud_ring_windows_open(gpud_ring* r, int64_t span, int64_t history_windows, gpud_ring_windows** out) {
   return gpud_ring_windows_open_hop(r, span, span, history_windows, out);
+}
+
+// Handles over chosen fields (DESIGN.md §2 "Field selection"): the handle's column g is the ring's field fields[g]
+extern "C" int32_t gpud_ring_windows_open_fields(gpud_ring* r, int64_t span, int64_t hop, int64_t history_windows, const int32_t* fields,
+                                                 int32_t n_fields, gpud_ring_windows** out) {
+  if (!r || !out) return GPUD_E_INVALID;
+  if (!fields) return gpud_fail(r->ctx, GPUD_E_INVALID, "windows over fields: fields is NULL");
+  return windows_register(r, span, hop, history_windows, fields, n_fields, out);
+}
+
+extern "C" int32_t gpud_ring_windows_fields(gpud_ring_windows* w, int32_t* fields, int32_t cap, int32_t* n_fields) {
+  if (!w || !n_fields || cap < 0 || (cap > 0 && !fields)) return GPUD_E_INVALID;
+  *n_fields = w->nf;
+  if (w->nf > cap) return gpud_fail(w->ring->ctx, GPUD_E_CAPACITY, "windows_fields: %d fields, room for %d", w->nf, cap);
+  for (int32_t g = 0; g < w->nf; ++g) fields[g] = w->fields.empty() ? g : w->fields[g];
+  return GPUD_OK;
 }
 
 extern "C" int32_t gpud_ring_windows_close(gpud_ring_windows* w) {
@@ -1794,9 +1844,12 @@ extern "C" int32_t gpud_ring_windows_stats(gpud_ring_windows* w, float* device_m
 }
 
 // The window pass of the whole-range reduce and of the segment select (select.cu); internal.h says what goes in and out.
-int32_t gpud_ring_window_pass(gpud_ring* r, int64_t start, int64_t n, int Wp, double* const w[5], uint32_t* w_nover,
+int32_t gpud_ring_window_pass(gpud_ring* r, int F, const int32_t* fmap, int64_t start, int64_t n, int Wp, double* const w[5], uint32_t* w_nover,
                               const double* piv, uint4* w_cls, unsigned long long* lists, unsigned* fill, unsigned list_cap, int seg_sub) {
+  if (fmap && w[3]) return gpud_fail(r->ctx, GPUD_E_INVALID, "window_pass: no EMA carry over chosen fields");
   WinParams p = win_params(r, start, n, Wp, r->d_cursor + 2);
+  p.F = F;
+  p.fmap = fmap;
   p.out_min = w[0]; p.out_max = w[1]; p.out_mean = w[2]; p.out_nover = w_nover; p.part = w[4]; p.do_select = 0;
   p.piv = piv; p.w_cls = w_cls; p.lists = lists; p.fill = fill; p.list_cap = list_cap;
   p.seg_sub = seg_sub > 0 ? seg_sub : p.nw;

@@ -29,7 +29,7 @@ constexpr unsigned kFull = 0xffffffffu;
 constexpr int kCkThreads = 256;                     // k_ckpt_size / k_ckpt_unpack: 8 warps, one block each at a time
 constexpr int kPackWarps = 4;                       // k_ckpt_pack: 8 KB of residuals per warp in shared memory
 constexpr char kMagic[2][8] = {{'G', 'P', 'U', 'D', 'R', 'C', 'K', '1'}, {'G', 'P', 'U', 'D', 'R', 'C', 'D', '1'}};   // [delta]
-enum { kKindStream = 0, kKindWindows = 1 };
+enum { kKindStream = 0, kKindWindows = 1, kKindFields = 2 };   // kKindFields: windows over chosen fields
 
 __device__ __forceinline__ uint64_t zigzag(uint64_t d) { return (d << 1) ^ (uint64_t)((int64_t)d >> 63); }
 __device__ __forceinline__ uint64_t unzigzag(uint64_t r) { return (r >> 1) ^ (0ull - (r & 1ull)); }
@@ -203,7 +203,8 @@ __global__ void __launch_bounds__(kCkThreads) k_ckpt_unpack(const CkGeo g, const
 }
 
 // ---- host ----
-// one handle's record after its head: [5][F][n] f64 history, [F][n] u32 n_over (padded to 8 bytes), [F] f64 EMA state
+// one handle's record after its head (and field list): [5][F][n] f64 history, [F][n] u32 n_over (padded to 8 bytes), [F] f64 EMA
+// state, F the handle's fields
 int64_t handle_body_bytes(int64_t F, int64_t n) { return 40 * F * n + pad8(4 * F * n) + 8 * F; }
 
 // The handles a checkpoint records, in its order: the stream handle, then the windows handles in open order.
@@ -225,9 +226,16 @@ int head_words(bool delta) { return delta ? 10 : 8; }
 int64_t blob_first(const gpud_ring* r, bool delta) { return std::max(delta ? r->ck_total : 0, r->total - r->cap); }
 int64_t body_from(const gpud_ring_windows* s, bool delta) { return delta ? std::max(s->first, s->ck_next) : s->first; }
 
+int64_t handle_kind(const gpud_ring* r, const gpud_ring_windows* s) {
+  return s == r->swin.get() ? kKindStream : s->fields.empty() ? kKindWindows : kKindFields;
+}
+// A kind-2 record's field list between its head words and its body: i64 n_fields, then the i32 ids zero-padded to 8 bytes
+int64_t list_bytes(int64_t nf) { return 8 + pad8(4 * nf); }
+
 int64_t handles_bytes(const gpud_ring* r, bool delta) {
   int64_t n = 0;
-  for (const gpud_ring_windows* s : ckpt_handles(r)) n += 8 * head_words(delta) + handle_body_bytes(r->F, s->next - body_from(s, delta));
+  for (const gpud_ring_windows* s : ckpt_handles(r))
+    n += 8 * head_words(delta) + (s->fields.empty() ? 0 : list_bytes(s->nf)) + handle_body_bytes(s->nf, s->next - body_from(s, delta));
   return n;
 }
 
@@ -248,7 +256,7 @@ int ckpt_grid(const gpud_ring* r, int64_t units, int warps_per_cta) {
 
 // Handle history [from, next) <-> n contiguous windows per field: slots from % H onwards, wrapping at most once.
 int32_t copy_history(gpud_ring* r, gpud_ring_windows* s, int64_t from, uint8_t* body, bool to_device) {
-  const int64_t F = r->F, n = s->next - from, H = s->H;
+  const int64_t F = s->nf, n = s->next - from, H = s->H;
   if (n == 0) return GPUD_OK;
   const int64_t slot = from % H, n1 = std::min(n, H - slot);
   auto part = [&](char* dev, size_t el, uint8_t* host) -> int32_t {
@@ -275,7 +283,7 @@ int32_t copy_history(gpud_ring* r, gpud_ring_windows* s, int64_t from, uint8_t* 
 
 // A handle's record body for windows [from, next) out of the device, and back into it.
 int32_t write_handle_body(gpud_ring* r, gpud_ring_windows* s, int64_t from, uint8_t* body) {
-  const int64_t F = r->F, n = s->next - from;
+  const int64_t F = s->nf, n = s->next - from;
   memset(body + 40 * F * n, 0, pad8(4 * F * n));   // the n_over rows' padding
   { const int32_t rc = copy_history(r, s, from, body, false); if (rc) return rc; }
   uint8_t* ema = body + 40 * F * n + pad8(4 * F * n);
@@ -286,7 +294,7 @@ int32_t write_handle_body(gpud_ring* r, gpud_ring_windows* s, int64_t from, uint
 }
 
 int32_t read_handle_body(gpud_ring* r, gpud_ring_windows* s, int64_t from, const uint8_t* body_c, const char* what) {
-  const int64_t F = r->F, n = s->next - from;
+  const int64_t F = s->nf, n = s->next - from;
   uint8_t* body = const_cast<uint8_t*>(body_c);      // copy_history only reads it in this direction
   { const int32_t rc = copy_history(r, s, from, body, true); if (rc) return rc; }
   if (cudaMemcpy(s->d_ema, body + 40 * F * n + pad8(4 * F * n), 8 * F, cudaMemcpyHostToDevice) != cudaSuccess)
@@ -470,12 +478,21 @@ int32_t write_blob(gpud_ring* r, bool delta, void* out_v, int64_t cap, int64_t* 
   std::vector<int64_t> heads;
   for (gpud_ring_windows* s : hs) {
     const int64_t from = body_from(s, delta);
-    const int64_t head[10] = {s == r->swin.get() ? kKindStream : kKindWindows, s->span, s->hop, s->H, s->first, s->next, s->lost, s->reseed ? 1 : 0,
-                              s->ck_next, from};
+    const int64_t head[10] = {handle_kind(r, s), s->span, s->hop, s->H, s->first, s->next, s->lost, s->reseed ? 1 : 0, s->ck_next, from};
     memcpy(out + off, head, 8 * nh);
     heads.insert(heads.end(), head, head + nh);
-    { const int32_t rc = write_handle_body(r, s, from, out + off + 8 * nh); if (rc) return rc; }
-    off += 8 * nh + handle_body_bytes(F, s->next - from);
+    off += 8 * nh;
+    if (!s->fields.empty()) {
+      // the list: n_fields, the ids zero-padded; the link folds its words after the head's
+      const int64_t lb = list_bytes(s->nf);
+      memset(out + off, 0, lb);
+      put<int64_t>(out, off, s->nf);
+      memcpy(out + off + 8, s->fields.data(), 4 * s->nf);
+      for (int64_t i = 0; i < lb; i += 8) heads.push_back(get<int64_t>(out, off + i));
+      off += lb;
+    }
+    { const int32_t rc = write_handle_body(r, s, from, out + off); if (rc) return rc; }
+    off += handle_body_bytes(s->nf, s->next - from);
   }
   en.stats(r);
   set_marker(r, r->total, link_fold(delta ? r->ck_link : 0, {r->total}, out + sum_off, F, heads));
@@ -490,7 +507,8 @@ int32_t blob_bound(gpud_ring* r, bool delta, int64_t* bytes) {
   return GPUD_OK;
 }
 
-struct CkHandle { int64_t kind, span, hop, H, first, next, lost, reseed, prev_next, from, off; };
+// off: where the body starts; nf: the record's fields (F, or kind 2's n_fields), ids: kind 2's list
+struct CkHandle { int64_t kind, span, hop, H, first, next, lost, reseed, prev_next, from, off, nf; std::vector<int32_t> ids; };
 
 // A blob whose frame checked out against the ring it goes into: its samples [first, total), where its sections are, and its handle
 // records, each with its head words for the chain link.
@@ -541,10 +559,10 @@ int32_t delta_target_ok(gpud_ring* r, const uint8_t* in, const std::vector<gpud_
 
 // A full checkpoint's record i: a handle this ring can hold, the stream handle only first.
 int32_t full_record_ok(gpud_ring* r, const CkHandle& h, uint32_t i, int64_t total) {
-  const bool kind_ok = h.kind == kKindWindows || (h.kind == kKindStream && i == 0 && h.span == 1 && h.hop == 1);
+  const bool kind_ok = h.kind == kKindWindows || h.kind == kKindFields || (h.kind == kKindStream && i == 0 && h.span == 1 && h.hop == 1);
   const bool shape_ok = h.span >= 1 && h.span <= r->cap / r->W && h.hop >= 1 && h.hop <= h.span && h.span % h.hop == 0;
   const int64_t L = h.span * r->W, P = h.hop * r->W, complete = total < L ? 0 : (total - L) / P + 1;
-  const bool hist_ok = h.H >= 1 && h.H <= ((int64_t)1 << 40) / r->F && h.first >= 0 && h.first <= h.next && h.next - h.first <= h.H &&
+  const bool hist_ok = h.H >= 1 && h.H <= ((int64_t)1 << 40) / h.nf && h.first >= 0 && h.first <= h.next && h.next - h.first <= h.H &&
                        h.next <= complete && h.lost >= 0 && (h.reseed == 0 || h.reseed == 1);
   if (!kind_ok || !shape_ok || !hist_ok)
     return gpud_fail(r->ctx, GPUD_E_INVALID, "restore: handle %u (kind %lld, span %lld, hop %lld, history %lld, windows [%lld, %lld)) is not one this ring can hold",
@@ -552,9 +570,9 @@ int32_t full_record_ok(gpud_ring* r, const CkHandle& h, uint32_t i, int64_t tota
   return GPUD_OK;
 }
 
-// A delta's record i: the successor of the ring's handle s.
+// A delta's record i: the successor of the ring's handle s, over the same fields.
 int32_t delta_record_ok(gpud_ring* r, const gpud_ring_windows* s, const CkHandle& h, uint32_t i, int64_t total) {
-  const bool same = h.kind == (s == r->swin.get() ? kKindStream : kKindWindows) && h.span == s->span && h.hop == s->hop && h.H == s->H;
+  const bool same = h.kind == handle_kind(r, s) && h.span == s->span && h.hop == s->hop && h.H == s->H && h.ids == s->fields;
   const int64_t complete = total < s->L ? 0 : (total - s->L) / s->P + 1;
   const bool hist_ok = h.prev_next == s->ck_next && h.first >= s->first && h.first <= h.next && h.next - h.first <= h.H && h.next >= h.prev_next &&
                        h.from == std::max(h.first, h.prev_next) && h.next <= complete && h.lost >= 0 && (h.reseed == 0 || h.reseed == 1);
@@ -615,12 +633,29 @@ int32_t read_frame(gpud_ring* r, const uint8_t* in, int64_t n_bytes, bool delta,
     int64_t v[10] = {};
     memcpy(v, in + off, 8 * nh);
     fr->heads.insert(fr->heads.end(), v, v + nh);
-    const CkHandle h{v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7], v[8], delta ? v[9] : v[4], off + 8 * nh};
+    CkHandle h{v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7], v[8], delta ? v[9] : v[4], off + 8 * nh, F, {}};
+    if (h.kind == kKindFields) {
+      // the list: n_fields in [1, what the bytes can hold], every id a field of the ring, zero padding
+      if (h.off + 8 > n_bytes) return gpud_fail(ctx, GPUD_E_INVALID, "%s: truncated handle %u", what, i);
+      const int64_t nf = get<int64_t>(in, h.off);
+      if (nf < 1 || nf > INT32_MAX || nf > (n_bytes - h.off - 8) / 4 || h.off + list_bytes(nf) > n_bytes)
+        return gpud_fail(ctx, GPUD_E_INVALID, "%s: handle %u has a list of %lld fields", what, i, (long long)nf);
+      h.nf = nf;
+      h.ids.resize(nf);
+      memcpy(h.ids.data(), in + h.off + 8, 4 * nf);
+      for (int64_t g = 0; g < nf; ++g)
+        if (h.ids[g] < 0 || h.ids[g] >= F)
+          return gpud_fail(ctx, GPUD_E_INVALID, "%s: handle %u names field %d, the ring has %lld", what, i, h.ids[g], (long long)F);
+      for (int64_t b = h.off + 8 + 4 * nf; b < h.off + list_bytes(nf); ++b)
+        if (in[b]) return gpud_fail(ctx, GPUD_E_INVALID, "%s: handle %u: field list padding is not zero", what, i);
+      for (int64_t b = 0; b < list_bytes(nf); b += 8) fr->heads.push_back(get<int64_t>(in, h.off + b));
+      h.off += list_bytes(nf);
+    }
     { const int32_t rc = delta ? delta_record_ok(r, fr->hs[i], h, i, fr->total) : full_record_ok(r, h, i, fr->total); if (rc) return rc; }
-    const int64_t body = handle_body_bytes(F, h.next - h.from);
+    const int64_t body = handle_body_bytes(h.nf, h.next - h.from);
     if (h.off + body > hnd_end) return gpud_fail(ctx, GPUD_E_INVALID, "%s: truncated handle %u", what, i);
     off = h.off + body;
-    fr->recs.push_back(h);
+    fr->recs.push_back(std::move(h));
   }
   if (off != hnd_end) return gpud_fail(ctx, GPUD_E_INVALID, "%s: the handle section has %lld bytes after its last handle", what, (long long)(hnd_end - off));
   return GPUD_OK;
@@ -707,7 +742,7 @@ extern "C" int32_t gpud_ring_restore(gpud_ring* r, const void* in_v, int64_t n_b
   const uint8_t* in = (const uint8_t*)in_v;
   Frame fr;
   { const int32_t rc = read_frame(r, in, n_bytes, false, &fr); if (rc) return rc; }
-  const int64_t n_win = std::count_if(fr.recs.begin(), fr.recs.end(), [](const CkHandle& h) { return h.kind == kKindWindows; });
+  const int64_t n_win = std::count_if(fr.recs.begin(), fr.recs.end(), [](const CkHandle& h) { return h.kind != kKindStream; });
   if (n_handles) *n_handles = (int32_t)n_win;
   if (n_win > cap_handles) return gpud_fail(r->ctx, GPUD_E_CAPACITY, "restore: %lld windows handles, room for %d", (long long)n_win, cap_handles);
   float ms = 0.f;
@@ -716,7 +751,7 @@ extern "C" int32_t gpud_ring_restore(gpud_ring* r, const void* in_v, int64_t n_b
   std::vector<std::unique_ptr<gpud_ring_windows>> made;
   for (const CkHandle& h : fr.recs) {
     std::unique_ptr<gpud_ring_windows> s;
-    int32_t rc = gpud_ring_windows_new(r, h.span, h.hop, h.H, &s);
+    int32_t rc = gpud_ring_windows_new(r, h.span, h.hop, h.H, h.ids.empty() ? nullptr : h.ids.data(), (int32_t)h.ids.size(), &s);
     if (rc == GPUD_OK) {
       s->first = h.first; s->next = h.next; s->lost = h.lost; s->reseed = h.reseed != 0;
       rc = read_handle_body(r, s.get(), h.first, in + h.off, "restore");

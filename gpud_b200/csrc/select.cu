@@ -706,7 +706,7 @@ int32_t run_select(const gpud_ring_view& v, gpud_ring* ring, gpud_range_state* s
     if (e == cudaSuccess && ema) e = gpud_ranges_ema(v, s->d_geo, n_geo, w[4], rows, w[3], d_pieces, d_p0, d_srcs);
   } else if (e == cudaSuccess) {
     // segment j's windows are rows j rows / n_geo .. of its field's rows: the window kernel's seg_sub mapping
-    int32_t rc = gpud_ring_window_pass(ring, geo[0].start, n_geo * geo[0].n, Wp, w, s->d_win_nover, piv, cls, lists, fill, geo[0].lcap, (int)(rows / n_geo));
+    int32_t rc = gpud_ring_window_pass(ring, v.F, v.d_fmap, geo[0].start, n_geo * geo[0].n, Wp, w, s->d_win_nover, piv, cls, lists, fill, geo[0].lcap, (int)(rows / n_geo));
     if (rc) return rc;
   }
   if (e == cudaSuccess) e = cudaEventRecord(s->ev[1], stream);
@@ -755,7 +755,8 @@ extern "C" int32_t gpud_ring_reduce_range(gpud_ring* ring, int64_t last_n, doubl
 
 // Stream windows of L = seg_len > GPUD_MAX_WINDOW samples (internal.h): one sampled select over n_seg segments per field, each under
 // the rule of seg_sample, at the rows, lists, pivots and fill counters the window kernel's seg_sub mapping gives it.
-int32_t gpud_ring_segments(gpud_ring* r, std::unique_ptr<gpud_range_state>& st, int64_t start, int64_t seg_len, int64_t n_seg, int Wp, gpud_seg_out* out) {
+int32_t gpud_ring_segments(const gpud_ring_view& v, gpud_ring* r, std::unique_ptr<gpud_range_state>& st, int64_t start, int64_t seg_len, int64_t n_seg,
+                           int Wp, gpud_seg_out* out) {
   gpud_range_geo g{};
   g.n = seg_len;
   g.k = gpud_rank_from_top(seg_len, r->q_num, r->q_den);
@@ -768,7 +769,7 @@ int32_t gpud_ring_segments(gpud_ring* r, std::unique_ptr<gpud_range_state>& st, 
   }
   if (!st) st = std::make_unique<gpud_range_state>();
   gpud_range_state* s = st.get();
-  { int32_t rc = run_select(gpud_view(r), r, s, geo.data(), n_seg, Wp, true, false, nullptr, nullptr, nullptr); if (rc) return rc; }
+  { int32_t rc = run_select(v, r, s, geo.data(), n_seg, Wp, true, false, nullptr, nullptr, nullptr); if (rc) return rc; }
   out->out = s->d_out;
   out->nover = s->d_nover;
   out->part = s->d_win[4];

@@ -264,6 +264,20 @@ int32_t gpud_ring_windows_read(gpud_ring_windows* w, int32_t op, int64_t first_w
  * stream), and for L > 1024 how many (field, window) segments went to the radix select, by reason (reasons[GPUD_RANGE_OPEN_*],
  * may be NULL; all 0 for L <= 1024), summed over the reduce's phases.  GPUD_E_STATE before the first such reduce. */
 int32_t gpud_ring_windows_stats(gpud_ring_windows* w, float* device_ms, int64_t* segments_by_radix, int32_t* reasons);
+/* Windows over chosen fields (DESIGN.md §2 "Field selection"): a handle of gpud_ring_windows_open_hop that reduces, keeps and
+ * checkpoints only the ring's fields fields[0, n_fields), in any order, repeats allowed.  Column g of its history is field fields[g]:
+ * it equals row fields[g] of an all-field handle with the same span, hop and history opened at the same moment and reduced after the
+ * same pushes, bit for bit in all six aggregates, through loss, restart and re-seed.  Its reads, scratch and history scale with
+ * n_fields, not F, and gpud_ring_windows_read returns [n_fields][n].  Every refusal of gpud_ring_windows_open_hop applies, with the
+ * history limit counted on n_fields; beyond them fields == NULL, n_fields < 1 and a field outside [0, F) give GPUD_E_INVALID; every
+ * refusal comes before any allocation and names the argument in gpud_last_error.  _reduce, _counts, _read, _stats and _close take it
+ * like any handle; gpud_ring_stream_* stays all-field. */
+int32_t gpud_ring_windows_open_fields(gpud_ring* ring, int64_t span, int64_t hop, int64_t history_windows, const int32_t* fields,
+                                      int32_t n_fields, gpud_ring_windows** out);
+/* The ring field of each column of handle w into fields[0, *n_fields): a handle over chosen fields gives its list (one restored from a
+ * checkpoint, the list the checkpoint recorded), an all-field handle 0 .. F - 1.  *n_fields is set either way; cap below it gives
+ * GPUD_E_CAPACITY with nothing written (fields may be NULL when cap = 0). */
+int32_t gpud_ring_windows_fields(gpud_ring_windows* w, int32_t* fields, int32_t cap, int32_t* n_fields);
 
 /* Whole-range aggregates of the most recent `last_n` samples of every field (last_n = 0 => whole ring, i.e. the W = CAP order
  * statistic of BASELINE configs[3]); exact.  Ranges of >= 64 Ki samples read HBM once (sampled pivots + classification fused into
