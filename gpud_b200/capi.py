@@ -755,7 +755,7 @@ class FabricVerdict(C.Structure):
 SYMBOLS = ["gpud_abi_version", "gpud_sizeof", "gpud_ctx_create", "gpud_ctx_destroy", "gpud_last_error", "gpud_host_alloc",
            "gpud_host_free", "gpud_ring_create", "gpud_ring_destroy", "gpud_ring_set_stream", "gpud_ring_push",
            "gpud_ring_push_device", "gpud_ring_push_raw", "gpud_clock_event_reasons", "gpud_hw_slowdown_event_message", "gpud_hw_slowdown_check", "gpud_store_insert_hw_slowdown", "gpud_store_open", "gpud_store_close", "gpud_store_last_error", "gpud_store_event_table", "gpud_store_insert_event", "gpud_store_insert_xid_hits", "gpud_store_metrics_table", "gpud_store_record_metrics", "gpud_kmsg_syncer_create", "gpud_kmsg_syncer_destroy", "gpud_kmsg_syncer_feed", "gpud_store_find_event", "gpud_store_record_reboot", "gpud_xid_state_from_store", "gpud_sxid_state_from_store", "gpud_store_get_events", "gpud_store_latest_event", "gpud_store_purge_events", "gpud_kmsg_syncer_configure", "gpud_kmsg_syncer_configure_component", "gpud_kmsg_syncer_offer", "gpud_ib_scan", "gpud_ib_reason", "gpud_poller_create", "gpud_poller_destroy", "gpud_poller_poll", "gpud_poller_last_rows", "gpud_poller_errors", "gpud_poll_row_hold", "gpud_nvml_devices", "gpud_nvml_devices_arg", "gpud_nvml_bus_id", "gpud_poller_remapped_rows", "gpud_remapped_rows_check", "gpud_poller_ecc_errors", "gpud_poller_field_row", "gpud_poller_poll_fields", "gpud_poller_gpm_supported", "gpud_poller_gpm_metrics", "gpud_poller_poll_gpm", "gpud_gpm_check", "gpud_poller_fabric_raw", "gpud_poller_product_name", "gpud_poller_temperature", "gpud_temperature_check", "gpud_temperature_reason", "gpud_poller_counters", "gpud_ring_counts", "gpud_ring_reduce", "gpud_ring_sync", "gpud_ring_kernel_ms", "gpud_ring_read",
-           "gpud_ring_result_ptr", "gpud_ring_stream_open", "gpud_ring_stream_reduce", "gpud_ring_stream_counts", "gpud_ring_stream_read", "gpud_ring_windows_open", "gpud_ring_windows_open_hop", "gpud_ring_windows_close", "gpud_ring_windows_reduce", "gpud_ring_windows_counts", "gpud_ring_windows_read", "gpud_ring_windows_stats", "gpud_ring_windows_open_fields", "gpud_ring_windows_fields", "gpud_ring_reduce_range", "gpud_ring_range_stats", "gpud_ring_reduce_ranges", "gpud_ring_reduce_range_sets", "gpud_rings_reduce_range_sets", "gpud_rings_reduce_range_sets_fields", "gpud_ring_ranges_stats", "gpud_box_query_create", "gpud_box_query_step", "gpud_box_query_result", "gpud_box_query_stats", "gpud_box_query_destroy", "gpud_ring_set_cta_reserve", "gpud_kmsg_scan", "gpud_kmsg_scan_sharded", "gpud_kmsg_scan_device", "gpud_kmsg_scan_kernel_ms", "gpud_kmsg_scan_phase_timing", "gpud_kmsg_scan_stats", "gpud_xid_classify",
+           "gpud_ring_result_ptr", "gpud_ring_stream_open", "gpud_ring_stream_reduce", "gpud_ring_stream_counts", "gpud_ring_stream_read", "gpud_ring_windows_open", "gpud_ring_windows_open_hop", "gpud_ring_windows_close", "gpud_ring_windows_reduce", "gpud_ring_windows_counts", "gpud_ring_windows_read", "gpud_ring_windows_stats", "gpud_ring_windows_open_fields", "gpud_ring_windows_fields", "gpud_ring_reduce_range", "gpud_ring_range_stats", "gpud_ring_reduce_ranges", "gpud_ring_reduce_range_sets", "gpud_rings_reduce_range_sets", "gpud_rings_reduce_range_sets_fields", "gpud_ring_ranges_stats", "gpud_box_query_create", "gpud_box_query_create_fields", "gpud_box_query_step", "gpud_box_query_result", "gpud_box_query_stats", "gpud_box_query_destroy", "gpud_ring_set_cta_reserve", "gpud_kmsg_scan", "gpud_kmsg_scan_sharded", "gpud_kmsg_scan_device", "gpud_kmsg_scan_kernel_ms", "gpud_kmsg_scan_phase_timing", "gpud_kmsg_scan_stats", "gpud_xid_classify",
            "gpud_hit_detail_json", "gpud_xid_description", "gpud_xid_mnemonic", "gpud_sxid_name", "gpud_nvlink_rule_hint", "gpud_sxid_reason", "gpud_sxid_get_detail", "gpud_store_insert_sxid_hits", "gpud_product_mem_caps", "gpud_product_fm_supported", "gpud_product_fabric_state_supported", "gpud_xid_get_detail", "gpud_xid_detail", "gpud_xid_build_message", "gpud_xid_hit_message", "gpud_xid_device_matches_bus_id", "gpud_kmsg_event_name", "gpud_kmsg_event_message", "gpud_kmsg_component", "gpud_kmsg_hit_message", "gpud_kmsg_stateful_create", "gpud_kmsg_stateful_destroy", "gpud_kmsg_stateful_feed", "gpud_component_create", "gpud_component_destroy", "gpud_component_name", "gpud_component_start", "gpud_component_check", "gpud_component_last_health_states", "gpud_component_events", "gpud_component_close", "gpud_component_checks", "gpud_component_xid_set_source", "gpud_component_xid_set_healthy", "gpud_component_xid_add_reboot", "gpud_component_xid_set_devices", "gpud_component_ring", "gpud_kmsg_stateful_feed_units", "gpud_kmsg_deduper_create", "gpud_kmsg_deduper_destroy", "gpud_kmsg_dedup_units",
            "gpud_kmsg_dedup_create", "gpud_kmsg_dedup_destroy", "gpud_kmsg_scan_dedup", "gpud_kmsg_dedup_stats",
            "gpud_fabric_issues", "gpud_fabric_suggest_reboot", "gpud_set_nvml_error_string", "gpud_nvml_error_strings_from_driver", "gpud_fabric_reason", "gpud_fabric_report_reason", "gpud_fabric_pack", "gpud_fabric_verdict_device", "gpud_comm_unique_id", "gpud_comm_init", "gpud_fabric_gather",
@@ -828,10 +828,12 @@ def lib() -> C.CDLL:
         "gpud_rings_reduce_range_sets_fields": (i32, [vp, i32, vp, vp, i32, vp, vp, i64, vp, i64, vp, vp]),
         "gpud_ring_ranges_stats": (i32, [vp, C.POINTER(C.c_float), C.POINTER(i64), vp]),
         "gpud_box_query_create": (i32, [vp, i32, i32, vp, vp, vp, i64, vp, i64, C.POINTER(vp)]),
+        "gpud_box_query_create_fields": (i32, [vp, i32, i32, vp, vp, i32, vp, vp, i64, vp, i64, C.POINTER(vp)]),
         "gpud_box_query_step": (i32, [vp, vp, C.POINTER(vp), C.POINTER(i64)]), "gpud_box_query_result": (i32, [vp, vp, vp]),
         "gpud_box_query_stats": (i32, [vp, C.POINTER(C.c_float), C.POINTER(C.c_int32), C.POINTER(i64), C.POINTER(i64), vp]),
         "gpud_box_query_destroy": (None, [vp]),
         "gpudh_box_query_plan": (i32, [i32, vp, i64, i32, i32, i32, vp, vp, vp, i64, vp, i64, vp, vp, vp, vp, vp, vp, vp, C.c_char_p, i32]),
+        "gpudh_box_query_plan_fields": (i32, [i32, vp, i64, i32, vp, i32, i32, i32, vp, vp, vp, i64, vp, i64, vp, vp, vp, vp, vp, vp, vp, C.c_char_p, i32]),
         "gpudh_box_query_pivots": (i32, [vp, vp, i64, C.POINTER(i64)]),
         "gpud_ring_windows_open": (i32, [vp, i64, i64, C.POINTER(vp)]),
         "gpud_ring_windows_open_hop": (i32, [vp, i64, i64, i64, C.POINTER(vp)]), "gpud_ring_windows_close": (i32, [vp]),
@@ -1137,16 +1139,26 @@ class BoxQuery:
 
         send, nbytes = q.step()            # then, while nbytes: recv = all-gather of every rank's nbytes at send, in rank order
         send, nbytes = q.step(recv_ptr)    # recv_ptr: device memory on the ring's device, complete
-    and reads q.result() ({op: [F][n_sets]}, as rings_reduce_range_sets) and q.stats() at the end."""
+    and reads q.result() ({op: [F][n_sets]}, as rings_reduce_range_sets) and q.stats() at the end.  With a list of fields
+    (gpud_box_query_create_fields), only those are read and exchanged and row g of each result is field fields[g]:
+    {op: [len(fields)][n_sets]}."""
 
-    def __init__(self, ring, rank: int, n_ranks: int, rank_of, first, length, set_off):
+    def __init__(self, ring, rank: int, n_ranks: int, rank_of, first, length, set_off, fields=None):
         self.ring, self._L = ring, ring._L
         self._args = _box_args(rank_of, first, length, set_off)   # kept alive: the query copies them, but keep them for the caller
         ro, fi, ln, so = self._args
         self.n_sets = so.shape[0] - 1
+        self.G = ring.F
         h = C.c_void_p()
-        ring.ctx._check(self._L.gpud_box_query_create(ring._h, rank, n_ranks, C.c_void_p(ro.ctypes.data), C.c_void_p(fi.ctypes.data),
-                                                      C.c_void_p(ln.ctypes.data), fi.shape[0], C.c_void_p(so.ctypes.data), self.n_sets, C.byref(h)))
+        if fields is None:
+            ring.ctx._check(self._L.gpud_box_query_create(ring._h, rank, n_ranks, C.c_void_p(ro.ctypes.data), C.c_void_p(fi.ctypes.data),
+                                                          C.c_void_p(ln.ctypes.data), fi.shape[0], C.c_void_p(so.ctypes.data), self.n_sets, C.byref(h)))
+        else:
+            fl = np.ascontiguousarray(fields, dtype=np.int32).reshape(-1)
+            self.G = fl.shape[0]
+            ring.ctx._check(self._L.gpud_box_query_create_fields(ring._h, rank, n_ranks, C.c_void_p(ro.ctypes.data), C.c_void_p(fl.ctypes.data),
+                                                                 fl.shape[0], C.c_void_p(fi.ctypes.data), C.c_void_p(ln.ctypes.data), fi.shape[0],
+                                                                 C.c_void_p(so.ctypes.data), self.n_sets, C.byref(h)))
         self._h = h
 
     def step(self, recv_ptr: int = 0):
@@ -1156,9 +1168,8 @@ class BoxQuery:
         return (send.value or 0), nb.value
 
     def result(self) -> dict:
-        F = self.ring.F
-        f64 = np.empty((5, F, self.n_sets), dtype=np.float64)
-        nov = np.empty((F, self.n_sets), dtype=np.uint32)
+        f64 = np.empty((5, self.G, self.n_sets), dtype=np.float64)
+        nov = np.empty((self.G, self.n_sets), dtype=np.uint32)
         self.ring.ctx._check(self._L.gpud_box_query_result(self._h, C.c_void_p(f64.ctypes.data), C.c_void_p(nov.ctypes.data)))
         return {"min": f64[0], "max": f64[1], "mean": f64[2], "ema": f64[3], "p99": f64[4], "n_over": nov}
 
@@ -1171,12 +1182,12 @@ class BoxQuery:
                 "reasons": reasons[:len(RANGE_OPEN_REASONS)].copy()}
 
     def pivots(self) -> np.ndarray:
-        """the pivots {lo, hi} of the last batch of long spread sets, [F][n_long][2] (gpudh_box_query_pivots)"""
+        """the pivots {lo, hi} of the last batch of long spread sets, [F][n_long][2], or [len(fields)][n_long][2] (gpudh_box_query_pivots)"""
         n = C.c_int64()
         self._L.gpudh_box_query_pivots(self._h, None, 0, C.byref(n))
         out = np.empty(2 * max(n.value, 1), dtype=np.float64)
         self.ring.ctx._check(self._L.gpudh_box_query_pivots(self._h, C.c_void_p(out.ctypes.data), n.value, C.byref(n)))
-        return out[:2 * n.value].reshape(self.ring.F, -1, 2)
+        return out[:2 * n.value].reshape(self.G, -1, 2)
 
     def close(self):
         if self._h:
@@ -1190,9 +1201,10 @@ class BoxQuery:
             pass
 
 
-def box_query_plan(totals, cap, rank_of, first, length, set_off, F=4, q=(99, 100), headers=None):
+def box_query_plan(totals, cap, rank_of, first, length, set_off, F=4, q=(99, 100), headers=None, fields=None):
     """gpudh_box_query_plan: (rc, message, route [n_sets], owner [n_sets], send_bytes [3], consistent headers [n_ranks][16],
-    pivot reads per set [n_sets], the rank of each pivot read [n_sets][8192])"""
+    pivot reads per set [n_sets], the rank of each pivot read [n_sets][8192]); with a list of fields, gpudh_box_query_plan_fields for
+    a query over those fields of rings of F fields"""
     L = lib()
     totals = np.ascontiguousarray(totals, dtype=np.int64)
     ro, fi, ln, so = _box_args(rank_of, first, length, set_off)
@@ -1203,11 +1215,16 @@ def box_query_plan(totals, cap, rank_of, first, length, set_off, F=4, q=(99, 100
     piv_n = np.zeros(n_sets, np.int32)
     piv_owner = np.full((n_sets, 8192), -1, np.int32) if n_sets <= 4096 else None    # the owners only for calls of a few sets
     msg = C.create_string_buffer(512)
-    rc = L.gpudh_box_query_plan(totals.shape[0], C.c_void_p(totals.ctypes.data), cap, F, q[0], q[1], C.c_void_p(ro.ctypes.data),
-                                C.c_void_p(fi.ctypes.data), C.c_void_p(ln.ctypes.data), fi.shape[0], C.c_void_p(so.ctypes.data), n_sets,
-                                C.c_void_p(hdr.ctypes.data), C.c_void_p(hin.ctypes.data) if hin is not None else None,
-                                C.c_void_p(route.ctypes.data), C.c_void_p(owner.ctypes.data), C.c_void_p(sb.ctypes.data),
-                                C.c_void_p(piv_n.ctypes.data), C.c_void_p(piv_owner.ctypes.data) if piv_owner is not None else None, msg, 512)
+    rest = (C.c_void_p(ro.ctypes.data), C.c_void_p(fi.ctypes.data), C.c_void_p(ln.ctypes.data), fi.shape[0], C.c_void_p(so.ctypes.data), n_sets,
+            C.c_void_p(hdr.ctypes.data), C.c_void_p(hin.ctypes.data) if hin is not None else None,
+            C.c_void_p(route.ctypes.data), C.c_void_p(owner.ctypes.data), C.c_void_p(sb.ctypes.data),
+            C.c_void_p(piv_n.ctypes.data), C.c_void_p(piv_owner.ctypes.data) if piv_owner is not None else None, msg, 512)
+    if fields is None:
+        rc = L.gpudh_box_query_plan(totals.shape[0], C.c_void_p(totals.ctypes.data), cap, F, q[0], q[1], *rest)
+    else:
+        fl = np.ascontiguousarray(fields, dtype=np.int32).reshape(-1)
+        rc = L.gpudh_box_query_plan_fields(totals.shape[0], C.c_void_p(totals.ctypes.data), cap, F, C.c_void_p(fl.ctypes.data), fl.shape[0],
+                                           q[0], q[1], *rest)
     return rc, msg.value.decode(), route, owner, sb, hdr, piv_n, piv_owner
 
 

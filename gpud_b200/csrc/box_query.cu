@@ -36,18 +36,21 @@ struct BoxLp { int64_t tile0, nt, len, pos; };        // a rank's local piece of
 
 __device__ __forceinline__ double box_decay(double w, double c, double s) { return (w == 0.0 && isinf(c)) ? c + s : fma(w, c, s); }
 
-// one warp per (field, run): a rank's own samples of the short spread sets into its send rows [F][row]
+// one warp per (field, run): a rank's own samples of the short spread sets into its send rows [F][row].  FMAP: the query's field f
+// reads the ring's field fmap[f]; its send row stays f.
+template <bool FMAP>
 __global__ void k_box_pack(const double* __restrict__ ring, int64_t cap, int F, const BoxRun* __restrict__ runs, int64_t n_runs,
-                           double* __restrict__ send, int64_t row) {
+                           double* __restrict__ send, int64_t row, const int32_t* __restrict__ fmap) {
   const int lane = threadIdx.x & 31;
   const int64_t units = (int64_t)F * n_runs;
   for (int64_t u = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; u < units; u += ((int64_t)gridDim.x * blockDim.x) >> 5) {
     const int64_t f = u / n_runs;
+    const int64_t rf = FMAP ? __ldg(fmap + f) : f;   // the ring's field
     const BoxRun q = runs[u - f * n_runs];
     for (int64_t t = lane; t < q.len; t += 32) {
       int64_t a = q.col + t;
       if (a >= cap) a -= cap;
-      send[f * row + q.pos + t] = ring[f * cap + a];
+      send[f * row + q.pos + t] = ring[rf * cap + a];
     }
   }
 }
@@ -222,9 +225,10 @@ struct BoxBatch {
 
 // What every rank derives alike from the call's arguments and the gathered totals: each set's route (0: local to rank owner[s];
 // 1: spread over several ranks, at most GPUD_MAX_WINDOW samples; 2: spread and longer, in batch batch[s]), the local sets, the short
-// spread sets' dense layout, and the batches of long spread sets.
+// spread sets' dense layout, and the batches of long spread sets.  G: the columns the query reduces, the ring's F or its n_fields;
+// every round, buffer and batch counts G.
 struct BoxPlan {
-  int F = 0, n = 0;
+  int G = 0, n = 0;
   std::vector<int32_t> route, owner;
   std::vector<int64_t> local;                 // the local sets, in set order
   std::vector<int64_t> dense0;                // per short spread set: its first dense column
@@ -234,15 +238,16 @@ struct BoxPlan {
   int64_t row = 0;                            // the most short-spread samples any rank holds
   std::vector<BoxBatch> batches;
   int64_t samples_words(size_t b) const {     // round samples(b)
-    int64_t w = 2 + (batches.empty() ? 0 : (int64_t)F * batches[b].row_s);
-    if (b == 0) w += (int64_t)kBoxLocalWords * F * (int64_t)local.size() + (int64_t)F * row;
+    int64_t w = 2 + (batches.empty() ? 0 : (int64_t)G * batches[b].row_s);
+    if (b == 0) w += (int64_t)kBoxLocalWords * G * (int64_t)local.size() + (int64_t)G * row;
     return w;
   }
-  int64_t summary_words(size_t b) const { return 2 + (int64_t)F * (int64_t)batches[b].geo.size() * kBoxSumWords + (int64_t)F * batches[b].row_p; }
+  int64_t summary_words(size_t b) const { return 2 + (int64_t)G * (int64_t)batches[b].geo.size() * kBoxSumWords + (int64_t)G * batches[b].row_p; }
 };
 
-int32_t box_verdict(gpud_ctx* ctx, const int64_t* hdr, int n, const int32_t* rank_of, const int64_t* first, const int64_t* len, int64_t n_ranges,
-                    const int64_t* set_off, int64_t n_sets, BoxPlan* bp) {
+// fields (NULL: every field of the ring) / n_fields: the query's field list, the same on every rank once the argument hashes agree.
+int32_t box_verdict(gpud_ctx* ctx, const int64_t* hdr, int n, const int32_t* fields, int n_fields, const int32_t* rank_of, const int64_t* first,
+                    const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets, BoxPlan* bp) {
   const int64_t* h0 = hdr;
   for (int i = 0; i < n; ++i)
     if (hdr[i * kHdrWords + kHdrMagic] != kBoxMagic) return gpud_fail(ctx, GPUD_E_INVALID, "gather slot %d: not a box query header", i);
@@ -265,15 +270,18 @@ int32_t box_verdict(gpud_ctx* ctx, const int64_t* hdr, int n, const int32_t* ran
   for (int i = 1; i < n; ++i)
     for (int w = kHdrF; w <= kHdrThr; ++w)
       if (hdr[i * kHdrWords + w] != h0[w]) return gpud_fail(ctx, GPUD_E_INVALID, "rank %d: config field %s differs from rank 0's", i, kField[w]);
+  const int F = (int)h0[kHdrF];
+  for (int g = 0; fields && g < n_fields; ++g)   // here, not at create: F is now agreed, and every rank refuses at this step
+    if (fields[g] < 0 || fields[g] >= F) return gpud_fail(ctx, GPUD_E_INVALID, "fields[%d] is %d, not a field of the ring's %d", g, fields[g], F);
   for (int i = 0; i < n; ++i) {
     const int64_t st = hdr[i * kHdrWords + kHdrStatus];
     if (st) return gpud_fail(ctx, (int32_t)st, "rank %d could not start the query: %s", i,
                              st == GPUD_E_CUDA ? cudaGetErrorString((cudaError_t)hdr[i * kHdrWords + kHdrDetail]) : "its ring changed");
   }
-  const int F = (int)h0[kHdrF];
+  const int G = fields ? n_fields : F;
   const int64_t cap = h0[kHdrCap];
-  if (n_sets > GPUD_RANGES_MAX_SEGMENTS / F)
-    return gpud_fail(ctx, GPUD_E_INVALID, "%d fields x %lld sets exceed GPUD_RANGES_MAX_SEGMENTS", F, (long long)n_sets);
+  if (n_sets > GPUD_RANGES_MAX_SEGMENTS / G)
+    return gpud_fail(ctx, GPUD_E_INVALID, "%d fields x %lld sets exceed GPUD_RANGES_MAX_SEGMENTS", G, (long long)n_sets);
   for (int64_t i = 0; i < n_ranges; ++i)
     if (rank_of[i] < 0 || rank_of[i] >= n)
       return gpud_fail(ctx, GPUD_E_INVALID, "range %lld: rank_of is %d, not a rank of the group's %d", (long long)i, rank_of[i], n);
@@ -282,10 +290,10 @@ int32_t box_verdict(gpud_ctx* ctx, const int64_t* hdr, int n, const int32_t* ran
   double alpha;
   memcpy(&alpha, &h0[kHdrAlpha], 8);
   RangesPlan pl;   // the box-sets plan with ring slot = rank: the range and set refusals, routes, pivot reads and batches
-  { int32_t rc = ranges_plan(ctx, totals.data(), n, rank_of, cap, F, (int)h0[kHdrQNum], (int)h0[kHdrQDen], alpha, ring_smp_shift(cap), first, len, n_ranges,
+  { int32_t rc = ranges_plan(ctx, totals.data(), n, rank_of, cap, G, (int)h0[kHdrQNum], (int)h0[kHdrQDen], alpha, ring_smp_shift(cap), first, len, n_ranges,
                              set_off, n_sets, &pl); if (rc) return rc; }
   *bp = BoxPlan();
-  bp->F = F;
+  bp->G = G;
   bp->n = n;
   bp->route.assign(n_sets, 0);
   bp->owner.assign(n_sets, -1);
@@ -360,8 +368,9 @@ struct gpud_box_query {
   int rank = 0, n_ranks = 0;
   std::vector<int32_t> rank_of;
   std::vector<int64_t> first, len, set_off;
+  std::vector<int32_t> fields;         // a query over chosen fields: column g is the ring's field fields[g] (empty: every field)
   int64_t n_ranges = 0, n_sets = 0;
-  int64_t gen0 = 0;                    // the ring's generation at create: a push or restore since then fails the query on every rank
+  int64_t gen0 = 0;                   // the ring's generation at create: a push or restore since then fails the query on every rank
   enum { kHeader, kSamples, kSummaries, kLists, kHist, kCollect, kDone, kFailed } sent = kHeader;   // what the last step sent
   bool started = false;
   size_t b = 0;                        // the batch of the round in flight
@@ -388,12 +397,14 @@ struct gpud_box_query {
   gpud_buf<unsigned long long> d_llists;     // this rank's keys between the pivots [F][list_row]
   gpud_buf<unsigned> d_lfill;                // ... and their fill (the pivots' fill counters)
   gpud_buf<unsigned> d_u32;                  // summed fill, each rank's fill, list slots
-  gpud_buf<double> d_out;                    // the result [5][F][n_sets]
+  gpud_buf<double> d_out;                    // the result [5][G][n_sets]
   gpud_buf<uint32_t> d_nover;
+  gpud_buf<int32_t> d_fmap;                  // a query over chosen fields: the list (gpud_ring_view::d_fmap of the ring's views) ...
+  gpud_buf<double> d_vthr;                   // ... and their thresholds, the dense buffer's in its field order
   std::vector<int64_t> list_off;       // the lists round: each segment's place (-1: none)
   std::vector<int> ids;                // the segments the finish left open, sorted
   std::vector<int64_t> cand_off;       // the collect round: each open segment's place (-1: none)
-  std::vector<double> local_out;       // the local sets' results, [n_local][F][6]
+  std::vector<double> local_out;       // the local sets' results, [G][n_local][6]
   std::vector<double> out;
   std::vector<uint32_t> nover;
   gpud_event ev[2];
@@ -424,8 +435,10 @@ static void box_header(int F, int W, int64_t cap, double alpha, int q_num, int q
   h[kHdrStatus] = status; h[kHdrDetail] = detail;
 }
 
+// A query over chosen fields folds n_fields and the ids after the call's other words, so that ranks whose lists differ, or one with a
+// list and one without, are refused as arguments that differ; an all-field query's hash is what it always was.
 static uint64_t box_args_hash(int32_t n_ranks, const int32_t* rank_of, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off,
-                              int64_t n_sets) {
+                              int64_t n_sets, const int32_t* fields, int32_t n_fields) {
   uint64_t h = 0xcbf29ce484222325ull;
   h = box_hash(h, &n_ranks, sizeof n_ranks);
   h = box_hash(h, &n_ranges, sizeof n_ranges);
@@ -433,12 +446,15 @@ static uint64_t box_args_hash(int32_t n_ranks, const int32_t* rank_of, const int
   h = box_hash(h, rank_of, n_ranges * sizeof(int32_t));
   h = box_hash(h, first, n_ranges * sizeof(int64_t));
   h = box_hash(h, len, n_ranges * sizeof(int64_t));
-  return box_hash(h, set_off, (n_sets + 1) * sizeof(int64_t));
+  h = box_hash(h, set_off, (n_sets + 1) * sizeof(int64_t));
+  if (!fields) return h;
+  h = box_hash(h, &n_fields, sizeof n_fields);
+  return box_hash(h, fields, n_fields * sizeof(int32_t));
 }
 
-extern "C" int32_t gpud_box_query_create(gpud_ring* ring, int32_t rank, int32_t n_ranks, const int32_t* rank_of, const int64_t* first, const int64_t* len,
-                                         int64_t n_ranges, const int64_t* set_off, int64_t n_sets, gpud_box_query** out) {
-  if (!ring || !out || n_ranges < 0 || n_sets < 1 || !set_off || (n_ranges > 0 && (!rank_of || !first || !len))) return GPUD_E_INVALID;
+// fields NULL: every field of the ring; else the caller checked fields and n_fields >= 1.
+static int32_t box_create(gpud_ring* ring, int32_t rank, int32_t n_ranks, const int32_t* rank_of, const int32_t* fields, int32_t n_fields,
+                          const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets, gpud_box_query** out) {
   if (n_ranks < 1 || n_ranks > GPUD_PIECE_RINGS) return gpud_fail(ring->ctx, GPUD_E_INVALID, "n_ranks %d is outside [1, %d]", n_ranks, GPUD_PIECE_RINGS);
   gpud_box_query* q = new gpud_box_query();
   q->ring = ring;
@@ -448,11 +464,29 @@ extern "C" int32_t gpud_box_query_create(gpud_ring* ring, int32_t rank, int32_t 
   q->first.assign(first, first + n_ranges);
   q->len.assign(len, len + n_ranges);
   q->set_off.assign(set_off, set_off + n_sets + 1);
+  if (fields) q->fields.assign(fields, fields + n_fields);
   q->n_ranges = n_ranges;
   q->n_sets = n_sets;
   q->gen0 = ring->gen;
   *out = q;
   return GPUD_OK;
+}
+
+extern "C" int32_t gpud_box_query_create(gpud_ring* ring, int32_t rank, int32_t n_ranks, const int32_t* rank_of, const int64_t* first, const int64_t* len,
+                                         int64_t n_ranges, const int64_t* set_off, int64_t n_sets, gpud_box_query** out) {
+  if (!ring || !out || n_ranges < 0 || n_sets < 1 || !set_off || (n_ranges > 0 && (!rank_of || !first || !len))) return GPUD_E_INVALID;
+  return box_create(ring, rank, n_ranks, rank_of, nullptr, 0, first, len, n_ranges, set_off, n_sets, out);
+}
+
+// The same query over the fields the caller names (DESIGN.md §2 "Field selection" under "Box sets across processes").  A field
+// outside [0, F) is refused by the verdict, on every rank at the same step.
+extern "C" int32_t gpud_box_query_create_fields(gpud_ring* ring, int32_t rank, int32_t n_ranks, const int32_t* rank_of, const int32_t* fields,
+                                                int32_t n_fields, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off,
+                                                int64_t n_sets, gpud_box_query** out) {
+  if (!ring || !out || n_ranges < 0 || n_sets < 1 || !set_off || (n_ranges > 0 && (!rank_of || !first || !len))) return GPUD_E_INVALID;
+  if (!fields) return gpud_fail(ring->ctx, GPUD_E_INVALID, "fields is NULL");
+  if (n_fields < 1) return gpud_fail(ring->ctx, GPUD_E_INVALID, "n_fields is %d, not at least 1", n_fields);
+  return box_create(ring, rank, n_ranks, rank_of, fields, n_fields, first, len, n_ranges, set_off, n_sets, out);
 }
 
 #define BOX_CUDA(expr) do { const cudaError_t _e = (expr); if (_e != cudaSuccess) return _e; } while (0)
@@ -461,15 +495,39 @@ static inline unsigned box_grid(const gpud_ring* r, int64_t threads) {
   return (unsigned)std::max<int64_t>(1, std::min<int64_t>((threads + 255) / 256, (int64_t)r->sm_count * 16));
 }
 
-// buf [F][cap] read as a ring of this rank's config by the range launchers (no sample ring)
-static gpud_ring_view box_view(const gpud_ring* r, const double* buf, int64_t cap) {
-  gpud_ring_view v = gpud_view(r);
+// This rank's ring over the query's G columns: a query over chosen fields reads the ring's field fields[g] for column g.
+static gpud_ring_view ring_view(const gpud_box_query* q) {
+  gpud_ring_view v = gpud_view(q->ring);
+  v.F = q->plan.G;
+  if (!q->fields.empty()) v.d_fmap = q->d_fmap;
+  return v;
+}
+
+// buf [G][cap] read as a ring of this rank's config by the range launchers (no sample ring).  It is in the query's column numbering
+// already, so it has no field map, but the column thresholds of a query over chosen fields are the named fields'.
+static gpud_ring_view box_view(const gpud_box_query* q, const double* buf, int64_t cap) {
+  gpud_ring_view v = gpud_view(q->ring);
+  v.F = q->plan.G;
   v.cap = cap;
   v.d_ring = buf;
+  if (!q->fields.empty()) v.d_thr = q->d_vthr;
   v.d_sample = nullptr;
   v.smp_shift = 0;
   v.smp_slots = 0;
   return v;
+}
+
+// A query over chosen fields: its list and their thresholds to the device, once the verdict has checked the list against F.
+static cudaError_t box_fields_upload(gpud_box_query* q) {
+  const int G = (int)q->fields.size();
+  if (G == 0) return cudaSuccess;
+  gpud_ring* r = q->ring;
+  std::vector<double> thr(G);
+  for (int g = 0; g < G; ++g) thr[g] = r->thr[q->fields[g]];
+  BOX_CUDA(q->d_fmap.grow(G));
+  BOX_CUDA(q->d_vthr.grow(G));
+  BOX_CUDA(cudaMemcpyAsync(q->d_fmap, q->fields.data(), G * sizeof(int32_t), cudaMemcpyHostToDevice, r->stream));
+  return cudaMemcpyAsync(q->d_vthr, thr.data(), G * sizeof(double), cudaMemcpyHostToDevice, r->stream);
 }
 
 // this rank's status for the round it sends: GPUD_E_STATE once its ring was pushed into or restored, else cuda's failure if any
@@ -482,13 +540,14 @@ static cudaError_t box_send(gpud_box_query* q, int64_t words) {
   return cudaMemsetAsync(q->d_send, 0, 16, q->ring->stream);
 }
 
-// The one-ring call for the sets this rank holds alone, on the query's own scratch, into local_out [n_local][F][6].
+// The one-ring call for the sets this rank holds alone (over the query's fields), on the query's own scratch, into local_out
+// [G][n_local][6].
 static int32_t box_local_sets(gpud_box_query* q) {
   gpud_ring* r = q->ring;
   const BoxPlan& bp = q->plan;
-  const int F = r->F;
+  const int G = bp.G;
   const int64_t n_local = (int64_t)bp.local.size();
-  q->local_out.assign((size_t)n_local * F * kBoxLocalWords, 0.0);
+  q->local_out.assign((size_t)n_local * G * kBoxLocalWords, 0.0);
   std::vector<int64_t> mine, sets;
   for (int64_t j = 0; j < n_local; ++j)
     if (bp.owner[bp.local[j]] == q->rank) { mine.push_back(j); sets.push_back(bp.local[j]); }
@@ -496,12 +555,15 @@ static int32_t box_local_sets(gpud_box_query* q) {
   const int64_t nm = (int64_t)mine.size();
   std::vector<double> o;
   std::vector<uint32_t> nv;
-  const int32_t rc = reduce_subset(gpud_view(r), ring_table(&r, 1), sets, nullptr, q->first.data(), q->len.data(), q->set_off.data(), q->local, o, nv);
+  gpud_ring_view v = gpud_view(r);                 // reduce_sets installs its own copy of the field map
+  v.F = G;
+  const int32_t rc = reduce_subset(v, ring_table(&r, 1), sets, nullptr, q->first.data(), q->len.data(), q->set_off.data(), q->local, o, nv,
+                                   q->fields.empty() ? nullptr : q->fields.data());
   if (rc) return rc;
-  for (int f = 0; f < F; ++f)
+  for (int f = 0; f < G; ++f)
     for (int64_t k = 0; k < nm; ++k) {
       double* w = q->local_out.data() + ((size_t)f * n_local + mine[k]) * kBoxLocalWords;
-      for (int op = 0; op < 5; ++op) w[op] = o[((size_t)op * F + f) * nm + k];
+      for (int op = 0; op < 5; ++op) w[op] = o[((size_t)op * G + f) * nm + k];
       w[5] = (double)nv[(size_t)f * nm + k];
     }
   q->radix += q->local->open;
@@ -509,11 +571,19 @@ static int32_t box_local_sets(gpud_box_query* q) {
   return GPUD_OK;
 }
 
+// k_box_pack of this rank's n_runs runs at d_runs into send rows [G][row], through the query's field map if it has one.
+static void box_pack(gpud_box_query* q, size_t n_runs, double* send, int64_t row) {
+  const gpud_ring* r = q->ring;
+  const int G = q->plan.G;
+  const auto k = q->fields.empty() ? k_box_pack<false> : k_box_pack<true>;
+  k<<<box_grid(r, (int64_t)G * n_runs * 32), 256, 0, r->stream>>>(r->d_ring, r->cap, G, q->d_runs, (int64_t)n_runs, send, row, q->d_fmap);
+}
+
 // Round samples(b): batch 0 also carries the local results and the short spread samples; then this rank's pivot reads of batch b.
 static cudaError_t box_samples(gpud_box_query* q) {
   gpud_ring* r = q->ring;
   const BoxPlan& bp = q->plan;
-  const int F = r->F;
+  const int G = q->plan.G;
   BOX_CUDA(box_send(q, bp.samples_words(q->b)));
   double* send = reinterpret_cast<double*>(q->d_send.get()) + 2;
   if (q->b == 0) {
@@ -522,25 +592,25 @@ static cudaError_t box_samples(gpud_box_query* q) {
     send += nl;
     const std::vector<BoxRun>& runs = bp.runs[q->rank];
     if (bp.row > 0) {
-      BOX_CUDA(cudaMemsetAsync(send, 0, (size_t)F * bp.row * 8, r->stream));
+      BOX_CUDA(cudaMemsetAsync(send, 0, (size_t)G * bp.row * 8, r->stream));
       if (!runs.empty()) {
         BOX_CUDA(q->d_runs.grow(runs.size()));
         BOX_CUDA(cudaMemcpyAsync(q->d_runs, runs.data(), runs.size() * sizeof(BoxRun), cudaMemcpyHostToDevice, r->stream));
-        k_box_pack<<<box_grid(r, (int64_t)F * runs.size() * 32), 256, 0, r->stream>>>(r->d_ring, r->cap, F, q->d_runs, (int64_t)runs.size(), send, bp.row);
+        box_pack(q, runs.size(), send, bp.row);
         BOX_CUDA(cudaGetLastError());
       }
     }
-    send += (size_t)F * bp.row;
+    send += (size_t)G * bp.row;
   }
   if (!bp.batches.empty()) {
     const BoxBatch& B = bp.batches[q->b];
     std::vector<BoxRun> runs;
     for (size_t e = 0; e < B.eown.size(); ++e) if (B.eown[e] == q->rank) runs.push_back({B.ecol[e], B.epos[e], 1});
-    BOX_CUDA(cudaMemsetAsync(send, 0, (size_t)F * B.row_s * 8, r->stream));
+    BOX_CUDA(cudaMemsetAsync(send, 0, (size_t)G * B.row_s * 8, r->stream));
     if (!runs.empty()) {
       BOX_CUDA(q->d_runs.grow(runs.size()));
       BOX_CUDA(cudaMemcpyAsync(q->d_runs, runs.data(), runs.size() * sizeof(BoxRun), cudaMemcpyHostToDevice, r->stream));
-      k_box_pack<<<box_grid(r, (int64_t)F * runs.size() * 32), 256, 0, r->stream>>>(r->d_ring, r->cap, F, q->d_runs, (int64_t)runs.size(), send, B.row_s);
+      box_pack(q, runs.size(), send, B.row_s);
       BOX_CUDA(cudaGetLastError());
     }
   }
@@ -550,15 +620,15 @@ static cudaError_t box_samples(gpud_box_query* q) {
 // The local sets' results from the gathered samples(0): each set's from the rank that owns it, into local_out.
 static cudaError_t box_gather_local(gpud_box_query* q, const double* recv, int64_t wpr) {
   const BoxPlan& bp = q->plan;
-  const int F = q->ring->F, n = q->n_ranks;
-  const int64_t n_local = (int64_t)bp.local.size(), nl = (int64_t)kBoxLocalWords * F * n_local;
+  const int G = q->plan.G, n = q->n_ranks;
+  const int64_t n_local = (int64_t)bp.local.size(), nl = (int64_t)kBoxLocalWords * G * n_local;
   if (nl == 0) return cudaSuccess;
   std::vector<double> all((size_t)n * nl);
   q->local_out.resize((size_t)nl);
   BOX_CUDA(cudaMemcpy2D(all.data(), nl * 8, recv + 2, wpr * 8, nl * 8, n, cudaMemcpyDeviceToHost));
   for (int64_t j = 0; j < n_local; ++j) {
     const double* src = all.data() + (size_t)bp.owner[bp.local[j]] * nl;
-    for (int f = 0; f < F; ++f)
+    for (int f = 0; f < G; ++f)
       for (int w = 0; w < kBoxLocalWords; ++w) {
         const size_t o = ((size_t)f * n_local + j) * kBoxLocalWords + w;
         q->local_out[o] = src[o];
@@ -571,7 +641,7 @@ static cudaError_t box_gather_local(gpud_box_query* q, const double* recv, int64
 static cudaError_t box_shorts(gpud_box_query* q, const double* recv, int64_t wpr) {
   gpud_ring* r = q->ring;
   const BoxPlan& bp = q->plan;
-  const int F = r->F;
+  const int G = q->plan.G;
   std::vector<gpud_short_range> shorts;
   for (int64_t s = 0; s < q->n_sets; ++s)
     if (bp.route[s] == 1) {
@@ -580,16 +650,16 @@ static cudaError_t box_shorts(gpud_box_query* q, const double* recv, int64_t wpr
       shorts.push_back({bp.dense0[s], (int32_t)m, (int32_t)s, 0, 0u, 0});
     }
   if (shorts.empty()) return cudaSuccess;
-  const int64_t base = 2 + (int64_t)kBoxLocalWords * F * (int64_t)bp.local.size();
-  BOX_CUDA(q->d_dense.grow((size_t)F * bp.D + 8));   // slack: the 16-byte load of a set's last odd sample
+  const int64_t base = 2 + (int64_t)kBoxLocalWords * G * (int64_t)bp.local.size();
+  BOX_CUDA(q->d_dense.grow((size_t)G * bp.D + 8));   // slack: the 16-byte load of a set's last odd sample
   BOX_CUDA(q->d_picks.grow(bp.picks.size()));
   BOX_CUDA(q->d_short.grow(shorts.size()));
   BOX_CUDA(cudaMemcpyAsync(q->d_picks, bp.picks.data(), bp.picks.size() * sizeof(BoxPick), cudaMemcpyHostToDevice, r->stream));
   BOX_CUDA(cudaMemcpyAsync(q->d_short, shorts.data(), shorts.size() * sizeof(gpud_short_range), cudaMemcpyHostToDevice, r->stream));
-  k_box_assemble<<<box_grid(r, (int64_t)F * bp.picks.size() * 32), 256, 0, r->stream>>>(recv, wpr, base, F, bp.row, q->d_picks, (int64_t)bp.picks.size(),
+  k_box_assemble<<<box_grid(r, (int64_t)G * bp.picks.size() * 32), 256, 0, r->stream>>>(recv, wpr, base, G, bp.row, q->d_picks, (int64_t)bp.picks.size(),
                                                                                       q->d_dense, bp.D);
   BOX_CUDA(cudaGetLastError());
-  return gpud_ranges_short(box_view(r, q->d_dense, bp.D), q->d_short, (int)shorts.size(), nullptr, nullptr, q->n_sets, q->d_out, q->d_nover);
+  return gpud_ranges_short(box_view(q, q->d_dense, bp.D), q->d_short, (int)shorts.size(), nullptr, nullptr, q->n_sets, q->d_out, q->d_nover);
 }
 
 // Batch b from its gathered samples: the pivot buffer, the pivots (k_range_pivots over it, stride 1: the same sample, the same pair),
@@ -598,21 +668,21 @@ static cudaError_t box_shorts(gpud_box_query* q, const double* recv, int64_t wpr
 static cudaError_t box_local_pass(gpud_box_query* q, const double* recv, int64_t wpr, int64_t base) {
   gpud_ring* r = q->ring;
   const BoxBatch& B = q->plan.batches[q->b];
-  const int F = r->F;
-  const int64_t n_long = (int64_t)B.geo.size(), segs = (int64_t)F * n_long;
+  const int G = q->plan.G;
+  const int64_t n_long = (int64_t)B.geo.size(), segs = (int64_t)G * n_long;
   if (!q->seg) q->seg = std::make_unique<gpud_range_state>();
   gpud_range_state* s = q->seg.get();
-  // the pivot buffer [F][D] and the pivots
+  // the pivot buffer [G][D] and the pivots
   std::vector<BoxPick> picks;
   for (size_t e = 0; e < B.eown.size(); ++e) picks.push_back({B.eown[e], B.epos[e], (int64_t)e, 1});
-  BOX_CUDA(q->d_piv_smp.grow((size_t)F * B.D + 8));
+  BOX_CUDA(q->d_piv_smp.grow((size_t)G * B.D + 8));
   BOX_CUDA(q->d_picks.grow(picks.size()));
   BOX_CUDA(cudaMemcpyAsync(q->d_picks, picks.data(), picks.size() * sizeof(BoxPick), cudaMemcpyHostToDevice, r->stream));
-  k_box_assemble<<<box_grid(r, (int64_t)F * picks.size() * 32), 256, 0, r->stream>>>(recv, wpr, base, F, B.row_s, q->d_picks, (int64_t)picks.size(),
+  k_box_assemble<<<box_grid(r, (int64_t)G * picks.size() * 32), 256, 0, r->stream>>>(recv, wpr, base, G, B.row_s, q->d_picks, (int64_t)picks.size(),
                                                                                    q->d_piv_smp, B.D);
   BOX_CUDA(cudaGetLastError());
   BOX_CUDA(q->d_lfill.grow((size_t)segs));
-  const gpud_ring_view pv = box_view(r, q->d_piv_smp, B.D);
+  const gpud_ring_view pv = box_view(q, q->d_piv_smp, B.D);
   BOX_CUDA(sel_reserve(pv, s, B.geo.data(), n_long, B.rows, B.list_row, true, nullptr));
   BOX_CUDA(sel_pivots(pv, s, B.geo.data(), n_long, q->d_lfill, nullptr, nullptr, nullptr));
   // this rank's pieces, launch kk taking each set's kk-th own piece
@@ -645,11 +715,11 @@ static cudaError_t box_local_pass(gpud_box_query* q, const double* recv, int64_t
     lb[kk + 1] = lb[kk] + ln[kk];
   }
   const int64_t T = lb[n_launch];
-  const size_t per = (size_t)F * std::max<int64_t>(1, T);
+  const size_t per = (size_t)G * std::max<int64_t>(1, T);
   for (int i = 0; i < 5; ++i) if (i != 3) BOX_CUDA(q->d_t[i].grow(per));
   BOX_CUDA(q->d_t_nover.grow(per));
   BOX_CUDA(q->d_t_cls.grow(per));
-  BOX_CUDA(q->d_llists.grow((size_t)F * B.list_row));
+  BOX_CUDA(q->d_llists.grow((size_t)G * B.list_row));
   BOX_CUDA(q->d_lgeo.grow(std::max<size_t>(1, lgeo.size())));
   BOX_CUDA(q->d_tile.grow(std::max<size_t>(1, tile.size())));
   BOX_CUDA(q->d_lp.grow(std::max<size_t>(1, lp.size())));
@@ -662,16 +732,16 @@ static cudaError_t box_local_pass(gpud_box_query* q, const double* recv, int64_t
     BOX_CUDA(cudaMemcpyAsync(q->d_i64 + n_launch, ln.data(), n_launch * sizeof(int64_t), cudaMemcpyHostToDevice, r->stream));
   }
   for (int kk = 0; kk < n_launch; ++kk) {
-    const size_t o = (size_t)F * lb[kk];
+    const size_t o = (size_t)G * lb[kk];
     double* const w[5] = {q->d_t[0] + o, q->d_t[1] + o, q->d_t[2] + o, nullptr, q->d_t[4] + o};
-    BOX_CUDA(gpud_ranges_tiles(gpud_view(r), q->d_lgeo + (size_t)kk * n_long, n_long, q->d_tile + lb[kk], ln[kk], s->d_piv, w, q->d_t_nover + o, q->d_t_cls + o,
+    BOX_CUDA(gpud_ranges_tiles(ring_view(q), q->d_lgeo + (size_t)kk * n_long, n_long, q->d_tile + lb[kk], ln[kk], s->d_piv, w, q->d_t_nover + o, q->d_t_cls + o,
                                q->d_llists, B.list_row, q->d_lfill, nullptr, nullptr, nullptr, nullptr));
   }
   // the summaries round
   BOX_CUDA(box_send(q, q->plan.summary_words(q->b)));
   unsigned long long* send = reinterpret_cast<unsigned long long*>(q->d_send.get()) + 2;
-  BOX_CUDA(cudaMemsetAsync(send + segs * kBoxSumWords, 0, (size_t)F * B.row_p * 8, r->stream));
-  k_box_summarize<<<box_grid(r, segs), 256, 0, r->stream>>>(F, n_long, n_launch, q->d_i64, q->d_i64 + n_launch, q->d_lp, q->d_t[0], q->d_t[1], q->d_t[2],
+  BOX_CUDA(cudaMemsetAsync(send + segs * kBoxSumWords, 0, (size_t)G * B.row_p * 8, r->stream));
+  k_box_summarize<<<box_grid(r, segs), 256, 0, r->stream>>>(G, n_long, n_launch, q->d_i64, q->d_i64 + n_launch, q->d_lp, q->d_t[0], q->d_t[1], q->d_t[2],
                                                            q->d_t[4], q->d_t_nover, q->d_t_cls, q->d_lfill, r->alpha, send,
                                                            reinterpret_cast<double*>(send + segs * kBoxSumWords), B.row_p);
   return cudaGetLastError();
@@ -681,8 +751,8 @@ static cudaError_t box_local_pass(gpud_box_query* q, const double* recv, int64_t
 static cudaError_t box_fold(gpud_box_query* q, const unsigned long long* recv, int64_t wpr, int64_t* list_words) {
   gpud_ring* r = q->ring;
   const BoxBatch& B = q->plan.batches[q->b];
-  const int F = r->F, n = q->n_ranks;
-  const int64_t n_long = (int64_t)B.geo.size(), segs = (int64_t)F * n_long;
+  const int G = q->plan.G, n = q->n_ranks;
+  const int64_t n_long = (int64_t)B.geo.size(), segs = (int64_t)G * n_long;
   gpud_range_state* s = q->seg.get();
   BOX_CUDA(q->d_u32.grow((size_t)segs * (n + 1)));
   BOX_CUDA(q->d_pcs.grow(B.pcs.size()));
@@ -691,7 +761,7 @@ static cudaError_t box_fold(gpud_box_query* q, const unsigned long long* recv, i
   BOX_CUDA(cudaMemcpyAsync(q->d_i64, B.pp0.data(), B.pp0.size() * sizeof(int64_t), cudaMemcpyHostToDevice, r->stream));
   unsigned* rfill = q->d_u32;
   unsigned* slot = q->d_u32 + (size_t)segs * n;
-  k_box_fold<<<box_grid(r, segs), 256, 0, r->stream>>>(recv, wpr, n, F, n_long, s->d_geo, s->d_piv, q->d_piv_smp, B.D, q->d_i64, q->d_pcs, B.row_p, r->alpha,
+  k_box_fold<<<box_grid(r, segs), 256, 0, r->stream>>>(recv, wpr, n, G, n_long, s->d_geo, s->d_piv, q->d_piv_smp, B.D, q->d_i64, q->d_pcs, B.row_p, r->alpha,
                                                       B.rows, s->d_win[0], s->d_win[1], s->d_win[2], s->d_win[3], s->d_win_nover, s->d_cls, s->d_fill,
                                                       rfill, slot);
   BOX_CUDA(cudaGetLastError());
@@ -707,7 +777,7 @@ static cudaError_t box_fold(gpud_box_query* q, const unsigned long long* recv, i
 
 // The finish over the folded rows and (when gathered) the merged lists; the segments it leaves open, sorted, in q->ids.
 static cudaError_t box_finish(gpud_box_query* q) {
-  const gpud_ring_view v = gpud_view(q->ring);
+  const gpud_ring_view v = ring_view(q);
   const BoxBatch& B = q->plan.batches[q->b];
   gpud_range_state* s = q->seg.get();
   // the open segments sorted: the finish appends them in any order, and every rank must lay them out alike
@@ -721,7 +791,7 @@ static cudaError_t box_finish(gpud_box_query* q) {
 // The radix select's next need for the open segments: 1 a histogram round, 2 a collect round, 0 neither (every one is finished).
 static cudaError_t box_radix_need(gpud_box_query* q, int* need) {
   const BoxBatch& B = q->plan.batches[q->b];
-  const int64_t segs = (int64_t)q->ring->F * (int64_t)B.geo.size();
+  const int64_t segs = (int64_t)q->plan.G * (int64_t)B.geo.size();
   std::vector<SelState> st(segs);
   BOX_CUDA(cudaMemcpyAsync(st.data(), q->seg->d_st, segs * sizeof(SelState), cudaMemcpyDeviceToHost, q->ring->stream));   // after k_sel_pick
   BOX_CUDA(cudaStreamSynchronize(q->ring->stream));
@@ -781,7 +851,7 @@ static cudaError_t box_radix_round(gpud_box_query* q, int need) {
   const int* ids = reinterpret_cast<const int*>(s->d_open + 1);
   int64_t n_max = 0;
   BOX_CUDA(box_radix_geo(q, &n_max));
-  const gpud_ring_view v = gpud_view(r);
+  const gpud_ring_view v = ring_view(q);
   const int64_t words = q->send_bytes / 8;
   BOX_CUDA(box_send(q, words));
   unsigned long long* send = reinterpret_cast<unsigned long long*>(q->d_send.get()) + 2;
@@ -796,9 +866,9 @@ static cudaError_t box_radix_round(gpud_box_query* q, int need) {
   return cudaGetLastError();
 }
 
-// The batch's results into the call's [5][F][n_sets]: the open segments' answers (k_sel_final), then the scatter.
+// The batch's results into the call's [5][G][n_sets]: the open segments' answers (k_sel_final), then the scatter.
 static cudaError_t box_batch_end(gpud_box_query* q) {
-  const gpud_ring_view v = gpud_view(q->ring);
+  const gpud_ring_view v = ring_view(q);
   gpud_range_state* s = q->seg.get();
   const int64_t n_long = (int64_t)q->plan.batches[q->b].geo.size();
   if (!q->ids.empty())
@@ -825,8 +895,8 @@ static cudaError_t box_next_batch(gpud_box_query* q, bool* done) {
   *done = ++q->b >= q->plan.batches.size();
   if (!*done) return box_samples(q);
   const BoxPlan& bp = q->plan;
-  const int F = r->F;
-  const size_t plane = (size_t)F * q->n_sets;
+  const int G = q->plan.G;
+  const size_t plane = (size_t)G * q->n_sets;
   q->out.assign(5 * plane, 0.0);
   q->nover.assign(plane, 0u);
   BOX_CUDA(cudaMemcpyAsync(q->out.data(), q->d_out, 5 * plane * 8, cudaMemcpyDeviceToHost, r->stream));
@@ -835,7 +905,7 @@ static cudaError_t box_next_batch(gpud_box_query* q, bool* done) {
   const int64_t n_local = (int64_t)bp.local.size();
   for (int64_t j = 0; j < n_local; ++j) {
     const int64_t s = bp.local[j];
-    for (int f = 0; f < F; ++f) {
+    for (int f = 0; f < G; ++f) {
       const double* w = q->local_out.data() + ((size_t)f * n_local + j) * kBoxLocalWords;
       for (int op = 0; op < 5; ++op) q->out[(size_t)op * plane + (size_t)f * q->n_sets + s] = w[op];
       q->nover[(size_t)f * q->n_sets + s] = (uint32_t)w[5];
@@ -854,20 +924,21 @@ static int32_t box_advance(gpud_box_query* q, const void* recv, bool* done) {
   if (q->sent == gpud_box_query::kHeader) {
     std::vector<int64_t> hdr((size_t)q->n_ranks * kHdrWords);
     GPUD_CUDA(ctx, cudaMemcpy(hdr.data(), recv, hdr.size() * 8, cudaMemcpyDeviceToHost));
-    { int32_t rc = box_verdict(ctx, hdr.data(), q->n_ranks, q->rank_of.data(), q->first.data(), q->len.data(), q->n_ranges, q->set_off.data(), q->n_sets,
-                               &q->plan); if (rc) return rc; }
+    { int32_t rc = box_verdict(ctx, hdr.data(), q->n_ranks, q->fields.empty() ? nullptr : q->fields.data(), (int)q->fields.size(), q->rank_of.data(),
+                               q->first.data(), q->len.data(), q->n_ranges, q->set_off.data(), q->n_sets, &q->plan); if (rc) return rc; }
   } else {
     int32_t rc = box_statuses(q, recv, wpr);
     if (rc) return rc;
   }
-  const int F = r->F;
-  const size_t plane = (size_t)F * q->n_sets;
+  const int G = q->plan.G;
+  const size_t plane = (size_t)G * q->n_sets;
   cudaError_t e = cudaSuccess;
   int32_t local_rc = 0;
   switch (q->sent) {
     case gpud_box_query::kHeader:
-      if (!box_status(q)) local_rc = box_local_sets(q);
-      e = q->d_out.grow(5 * plane);
+      e = box_fields_upload(q);
+      if (e == cudaSuccess && !box_status(q)) local_rc = box_local_sets(q);
+      if (e == cudaSuccess) e = q->d_out.grow(5 * plane);
       if (e == cudaSuccess) e = q->d_nover.grow(plane);
       q->b = 0;
       if (e == cudaSuccess) e = box_samples(q);
@@ -879,7 +950,7 @@ static int32_t box_advance(gpud_box_query* q, const void* recv, bool* done) {
       if (q->b == 0 && e == cudaSuccess) e = box_shorts(q, rv, wpr);
       if (e != cudaSuccess) break;
       if (q->plan.batches.empty()) { e = box_next_batch(q, done); q->sent = gpud_box_query::kDone; break; }
-      const int64_t base = 2 + (q->b == 0 ? (int64_t)kBoxLocalWords * F * (int64_t)q->plan.local.size() + (int64_t)F * q->plan.row : 0);
+      const int64_t base = 2 + (q->b == 0 ? (int64_t)kBoxLocalWords * G * (int64_t)q->plan.local.size() + (int64_t)G * q->plan.row : 0);
       e = box_local_pass(q, rv, wpr, base);
       q->sent = gpud_box_query::kSummaries;
       break;
@@ -890,7 +961,7 @@ static int32_t box_advance(gpud_box_query* q, const void* recv, bool* done) {
       if (e != cudaSuccess) break;
       if (lw) {
         const BoxBatch& B = q->plan.batches[q->b];
-        const int64_t segs = (int64_t)F * (int64_t)B.geo.size();
+        const int64_t segs = (int64_t)G * (int64_t)B.geo.size();
         e = box_send(q, 2 + lw);
         if (e == cudaSuccess) e = q->d_i64.grow((size_t)segs);
         if (e == cudaSuccess) e = cudaMemcpyAsync(q->d_i64, q->list_off.data(), segs * sizeof(int64_t), cudaMemcpyHostToDevice, r->stream);
@@ -907,7 +978,7 @@ static int32_t box_advance(gpud_box_query* q, const void* recv, bool* done) {
     case gpud_box_query::kLists: {
       if (q->sent == gpud_box_query::kLists) {
         const BoxBatch& B = q->plan.batches[q->b];
-        const int64_t segs = (int64_t)F * (int64_t)B.geo.size();
+        const int64_t segs = (int64_t)G * (int64_t)B.geo.size();
         k_box_merge_lists<<<box_grid(r, segs * 32), 256, 0, r->stream>>>(static_cast<const unsigned long long*>(recv), wpr, q->n_ranks, segs,
                                                                        (int64_t)B.geo.size(), q->d_i64, q->d_u32, q->seg->d_geo, B.list_row, q->seg->d_lists);
         e = cudaGetLastError();
@@ -929,7 +1000,7 @@ static int32_t box_advance(gpud_box_query* q, const void* recv, bool* done) {
       k_box_sum_hist<<<box_grid(r, (int64_t)n_sel * kBins), 256, 0, r->stream>>>(static_cast<const unsigned*>(recv), wpr, q->n_ranks, (int64_t)n_sel * kBins,
                                                                                 s->d_hist);
       e = cudaGetLastError();
-      if (e == cudaSuccess) e = sel_pick(gpud_view(r), s, reinterpret_cast<const int*>(s->d_open + 1), n_sel);
+      if (e == cudaSuccess) e = sel_pick(ring_view(q), s, reinterpret_cast<const int*>(s->d_open + 1), n_sel);
       int need = 0;
       if (e == cudaSuccess) e = box_radix_need(q, &need);
       if (e != cudaSuccess) break;
@@ -983,7 +1054,8 @@ extern "C" int32_t gpud_box_query_step(gpud_box_query* q, const void* dev_recv, 
   if (!q->started) {
     for (auto& ev : q->ev) GPUD_CUDA(ctx, ev.make());
     int64_t hdr[kHdrWords];
-    const uint64_t args = box_args_hash(q->n_ranks, q->rank_of.data(), q->first.data(), q->len.data(), q->n_ranges, q->set_off.data(), q->n_sets);
+    const uint64_t args = box_args_hash(q->n_ranks, q->rank_of.data(), q->first.data(), q->len.data(), q->n_ranges, q->set_off.data(), q->n_sets,
+                                        q->fields.empty() ? nullptr : q->fields.data(), (int32_t)q->fields.size());
     GPUD_CUDA(ctx, q->d_send.grow(sizeof hdr));
     box_header(r->F, r->W, r->cap, r->alpha, r->q_num, r->q_den, r->thr.data(), r->total, q->rank, q->n_ranks, args, box_status(q), 0, hdr);
     GPUD_CUDA(ctx, cudaMemcpy(q->d_send, hdr, sizeof hdr, cudaMemcpyHostToDevice));
@@ -1029,34 +1101,35 @@ extern "C" int32_t gpud_box_query_stats(gpud_box_query* q, float* device_ms, int
   return GPUD_OK;
 }
 
-// Test hook (include/gpud_b200_hooks.h): the pivots {lo, hi} of the last batch of long spread sets the query finished, [F][n_long].
+// Test hook (include/gpud_b200_hooks.h): the pivots {lo, hi} of the last batch of long spread sets the query finished, [G][n_long].
 extern "C" int32_t gpudh_box_query_pivots(gpud_box_query* q, double* piv, int64_t cap, int64_t* n) {
   if (!q || !n) return GPUD_E_INVALID;
   if (q->sent != gpud_box_query::kDone || !q->seg || q->plan.batches.empty()) return gpud_fail(q->ring->ctx, GPUD_E_STATE, "no long spread set was reduced");
-  *n = (int64_t)q->ring->F * (int64_t)q->plan.batches.back().geo.size();
+  *n = (int64_t)q->plan.G * (int64_t)q->plan.batches.back().geo.size();
   if (*n > cap || !piv) return GPUD_E_CAPACITY;
   GPUD_CUDA(q->ring->ctx, cudaMemcpy(piv, q->seg->d_piv, 2 * *n * sizeof(double), cudaMemcpyDeviceToHost));
   return GPUD_OK;
 }
 
 // Test hook (include/gpud_b200_hooks.h): the plan of one box query over n_ranks rings of totals[] pushed samples, and the verdict
-// every rank reaches from the gathered headers.
-extern "C" int32_t gpudh_box_query_plan(int32_t n_ranks, const int64_t* totals, int64_t cap, int32_t n_fields, int32_t q_num, int32_t q_den,
-                                        const int32_t* rank_of, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off,
-                                        int64_t n_sets, int64_t* hdr_out, const int64_t* hdr_in, int32_t* route, int32_t* owner, int64_t* send_bytes,
-                                        int32_t* piv_n, int32_t* piv_owner, char* msg, int32_t msg_cap) {
-  if (n_ranks < 1 || n_ranks > GPUD_PIECE_RINGS || !totals || cap < 2 || (cap & 1) || n_fields < 1 || q_den <= 0 || q_num < 0 || q_num > q_den || n_ranges < 0 ||
-      n_sets < 1 || !set_off || (n_ranges > 0 && (!rank_of || !first || !len)))
+// every rank reaches from the gathered headers.  fields (NULL: every field) / n_sel: a query over chosen fields of rings of F fields.
+extern "C" int32_t gpudh_box_query_plan_fields(int32_t n_ranks, const int64_t* totals, int64_t cap, int32_t F, const int32_t* fields, int32_t n_sel,
+                                               int32_t q_num, int32_t q_den, const int32_t* rank_of, const int64_t* first, const int64_t* len,
+                                               int64_t n_ranges, const int64_t* set_off, int64_t n_sets, int64_t* hdr_out, const int64_t* hdr_in,
+                                               int32_t* route, int32_t* owner, int64_t* send_bytes, int32_t* piv_n, int32_t* piv_owner, char* msg,
+                                               int32_t msg_cap) {
+  if (n_ranks < 1 || n_ranks > GPUD_PIECE_RINGS || !totals || cap < 2 || (cap & 1) || F < 1 || q_den <= 0 || q_num < 0 || q_num > q_den || n_ranges < 0 ||
+      n_sets < 1 || !set_off || (n_ranges > 0 && (!rank_of || !first || !len)) || (fields && n_sel < 1))
     return GPUD_E_INVALID;
-  const std::vector<double> thr(n_fields, 0.0);
-  const uint64_t args = box_args_hash(n_ranks, rank_of, first, len, n_ranges, set_off, n_sets);
+  const std::vector<double> thr(F, 0.0);
+  const uint64_t args = box_args_hash(n_ranks, rank_of, first, len, n_ranges, set_off, n_sets, fields, n_sel);
   std::vector<int64_t> hdr((size_t)n_ranks * kHdrWords);
   for (int i = 0; i < n_ranks; ++i)
-    box_header(n_fields, 1, cap, 0.5, q_num, q_den, thr.data(), totals[i], i, n_ranks, args, 0, 0, hdr.data() + (size_t)i * kHdrWords);
+    box_header(F, 1, cap, 0.5, q_num, q_den, thr.data(), totals[i], i, n_ranks, args, 0, 0, hdr.data() + (size_t)i * kHdrWords);
   if (hdr_out) std::copy(hdr.begin(), hdr.end(), hdr_out);
   gpud_ctx ctx;
   BoxPlan bp;
-  const int32_t rc = box_verdict(&ctx, hdr_in ? hdr_in : hdr.data(), n_ranks, rank_of, first, len, n_ranges, set_off, n_sets, &bp);
+  const int32_t rc = box_verdict(&ctx, hdr_in ? hdr_in : hdr.data(), n_ranks, fields, n_sel, rank_of, first, len, n_ranges, set_off, n_sets, &bp);
   if (msg && msg_cap > 0) snprintf(msg, (size_t)msg_cap, "%s", rc ? ctx.last_error.c_str() : "");
   if (rc) return rc;
   if (route) std::copy(bp.route.begin(), bp.route.end(), route);
@@ -1069,4 +1142,12 @@ extern "C" int32_t gpudh_box_query_plan(int32_t n_ranks, const int64_t* totals, 
       for (int64_t t = 0; piv_owner && t < g.S; ++t) piv_owner[g.id * GPUD_RANGE_SAMPLE_MAX + t] = B.eown[g.start + t];
     }
   return GPUD_OK;
+}
+
+extern "C" int32_t gpudh_box_query_plan(int32_t n_ranks, const int64_t* totals, int64_t cap, int32_t n_fields, int32_t q_num, int32_t q_den,
+                                        const int32_t* rank_of, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off,
+                                        int64_t n_sets, int64_t* hdr_out, const int64_t* hdr_in, int32_t* route, int32_t* owner, int64_t* send_bytes,
+                                        int32_t* piv_n, int32_t* piv_owner, char* msg, int32_t msg_cap) {
+  return gpudh_box_query_plan_fields(n_ranks, totals, cap, n_fields, nullptr, 0, q_num, q_den, rank_of, first, len, n_ranges, set_off, n_sets, hdr_out,
+                                     hdr_in, route, owner, send_bytes, piv_n, piv_owner, msg, msg_cap);
 }

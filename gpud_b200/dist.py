@@ -78,18 +78,19 @@ class _DevBytes:
         self.__cuda_array_interface__ = {"shape": (n,), "typestr": "|u1", "data": (ptr, False), "version": 3}
 
 
-def box_range_sets(ring, rank_of, first, length, set_off, group=None) -> dict:
+def box_range_sets(ring, rank_of, first, length, set_off, group=None, fields=None) -> dict:
     """Range sets over the rings of every rank of the group, this process holding ring `rank` (gpud_box_query, DESIGN.md §2 "Box sets
     across processes"): every rank calls this with the same arguments and gets the same {op: [F][n_sets]} result, identical to
-    capi.rings_reduce_range_sets over all the rings in one process.  NCCL all-gathers device buffers; any other backend (gloo) stages
-    through host memory."""
+    capi.rings_reduce_range_sets over all the rings in one process.  With a list of fields (the same on every rank), only those are
+    read and exchanged, and row g is field fields[g]: {op: [len(fields)][n_sets]}.  NCCL all-gathers device buffers; any other
+    backend (gloo) stages through host memory."""
     import torch
     import torch.distributed as dist
     from .capi import BoxQuery
     rank, world = dist.get_rank(group), dist.get_world_size(group)
     dev = torch.device("cuda", ring.dev)
     nccl = dist.get_backend(group) == "nccl"
-    q = BoxQuery(ring, rank, world, rank_of, first, length, set_off)
+    q = BoxQuery(ring, rank, world, rank_of, first, length, set_off, fields=fields)
     try:
         send_ptr, nb = q.step()
         while nb:

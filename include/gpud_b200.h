@@ -386,7 +386,21 @@ int32_t gpud_rings_reduce_range_sets_fields(gpud_ring* const* rings, int32_t n_r
 typedef struct gpud_box_query gpud_box_query;
 int32_t gpud_box_query_create(gpud_ring* ring, int32_t rank, int32_t n_ranks, const int32_t* rank_of, const int64_t* first,
                               const int64_t* len, int64_t n_ranges, const int64_t* set_off, int64_t n_sets, gpud_box_query** out);
+/* The box query over chosen fields (DESIGN.md §2 "Box sets across processes", "Field selection"): gpud_box_query_create over the
+ * fields fields[0, n_fields) of each rank's ring only, in any order, repeats allowed.  Column g of every rank's result is field
+ * fields[g]: it equals row fields[g] of the all-field query over the same rings and arguments, bit for bit in all six outputs, so it
+ * carries that query's guarantees against gpud_rings_reduce_range_sets_fields in one process.  Only the named fields are read, sent,
+ * reduced and selected: every round after the header, the device work and the scratch scale with n_fields, not F.  Every rank passes
+ * the same list: lists that differ between ranks, or a list on one rank and none on another, are refused as arguments that differ.
+ * Refusals: those of gpud_box_query_create, with the segment limit on n_fields x n_sets; at create, fields == NULL or n_fields < 1
+ * (GPUD_E_INVALID, named in gpud_last_error); a field outside [0, F) is refused by the verdict, on every rank at the same step, naming
+ * its position and value.  step, stats and destroy take either kind of query; result gives [5][n_fields][n_sets] f64 and
+ * [n_fields][n_sets] u32. */
+int32_t gpud_box_query_create_fields(gpud_ring* ring, int32_t rank, int32_t n_ranks, const int32_t* rank_of, const int32_t* fields,
+                                     int32_t n_fields, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off,
+                                     int64_t n_sets, gpud_box_query** out);
 int32_t gpud_box_query_step(gpud_box_query* q, const void* dev_recv, const void** dev_send, int64_t* send_bytes);
+/* [5][F][n_sets] and [F][n_sets]; a query over chosen fields: [5][n_fields][n_sets] and [n_fields][n_sets] */
 int32_t gpud_box_query_result(gpud_box_query* q, double* out_f64 /*[5][F][n_sets]*/, uint32_t* out_n_over /*[F][n_sets]*/);
 /* After the last step: this rank's device ms (each step's own work, summed; not the caller's gathers), the exchanges it took part in
  * and the bytes it sent, and the segments that went to the radix select, by reason (reasons[GPUD_RANGE_OPEN_*], may be NULL): those of

@@ -166,8 +166,17 @@ int32_t gpudh_box_query_plan(int32_t n_ranks, const int64_t* totals, int64_t cap
                              const int32_t* rank_of, const int64_t* first, const int64_t* len, int64_t n_ranges, const int64_t* set_off,
                              int64_t n_sets, int64_t* hdr_out, const int64_t* hdr_in, int32_t* route, int32_t* owner, int64_t* send_bytes,
                              int32_t* piv_n, int32_t* piv_owner, char* msg, int32_t msg_cap);
-/* The pivots {lo, hi} of the last batch of long spread sets a finished box query reduced, [F][n_long] in the order of the sets: *n
- * = F x n_long.  GPUD_E_STATE when it reduced none, GPUD_E_CAPACITY when *n > cap. */
+/* gpudh_box_query_plan for a query over chosen fields (gpud_box_query_create_fields) of rings of F fields: fields[0, n_sel) (NULL:
+ * every field, the call above) fold into the argument hash of hdr_out, and the verdict checks them against F and counts the segment
+ * limit and send_bytes on n_sel columns. */
+int32_t gpudh_box_query_plan_fields(int32_t n_ranks, const int64_t* totals, int64_t cap, int32_t F, const int32_t* fields, int32_t n_sel,
+                                    int32_t q_num, int32_t q_den, const int32_t* rank_of, const int64_t* first, const int64_t* len,
+                                    int64_t n_ranges, const int64_t* set_off, int64_t n_sets, int64_t* hdr_out, const int64_t* hdr_in,
+                                    int32_t* route, int32_t* owner, int64_t* send_bytes, int32_t* piv_n, int32_t* piv_owner, char* msg,
+                                    int32_t msg_cap);
+/* The pivots {lo, hi} of the last batch of long spread sets a finished box query reduced, [G][n_long] in the order of the sets, G
+ * its columns (F, or n_fields of a query over chosen fields): *n = G x n_long.  GPUD_E_STATE when it reduced none, GPUD_E_CAPACITY
+ * when *n > cap. */
 int32_t gpudh_box_query_pivots(gpud_box_query* q, double* piv, int64_t cap, int64_t* n);
 /* The CUDA objects the library owns now: out[4] = {device buffers, pinned host buffers, events, streams}.  Host counters; no device call. */
 void gpudh_cuda_objects(int64_t out[4]);

@@ -3,7 +3,8 @@
     python tools/sass_diff.py OLD.o NEW.o [OLD.o NEW.o ...]
 
 Kernels are matched by name without their argument list.  A kernel that gained a trailing `bool` template parameter (an FMAP or
-similar switch whose `false` instantiation is meant to stay the parent's code) is matched by its old name plus `, false`.  Prints one line per kernel of the old object (same / DIFFERENT /
+similar switch whose `false` instantiation is meant to stay the parent's code) is matched by its old name plus `, false`, and a plain
+kernel that became a template of one such parameter by its old name plus `<false>`.  Prints one line per kernel of the old object (same / DIFFERENT /
 missing) and exits 1 if any is not the same.  Register counts come from `cuobjdump -res-usage`."""
 import re
 import subprocess
@@ -50,8 +51,8 @@ def regs(obj):
 
 
 def with_false(name):
-    """k<a, b> -> k<a, b, false>"""
-    return name[:-1] + ", (bool)0>" if name.endswith(">") else None
+    """k<a, b> -> k<a, b, false>; k -> k<false>"""
+    return name[:-1] + ", (bool)0>" if name.endswith(">") else "void %s<(bool)0>" % name
 
 
 def main(pairs):
